@@ -1,8 +1,8 @@
-"""easy_vitpose_b200: the ViTPose crop path of JunkyByte/easy_ViTPose on B200 (sm_100a).
+"""easy_vitpose_b200: the ViTPose crop path of JunkyByte/easy_ViTPose on H100 (sm_90a).
 
     crops [B,3,256,192] -> ViT -> TopdownHeatmapSimpleHead -> heatmaps [B,K,64,48] -> keypoints [B,K,3]
 
-csrc/ holds the hand-written CUDA (tcgen05 GEMM + attention, LayerNorm, gathers, decode) and the C ABI
+csrc/ holds the hand-written CUDA (wgmma GEMM + attention, LayerNorm, gathers, decode) and the C ABI
 (include/vitpose_b200.h); the Python modules mirror the reference's interface for this path:
 model.ViTPose, top_down_eval.keypoints_from_heatmaps, inference.install / B200PoseBackend.
 """

@@ -67,7 +67,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB) or is_stale():
             try:
-                build()                              # nvcc cross-compiles sm_100a anywhere; seconds
+                build()                              # nvcc cross-compiles sm_90a anywhere
             except Exception as exc:
                 # never load a library older than its sources: its ABI / kernels may no longer match the header and
                 # the argtypes below.  VPB_ALLOW_STALE=1 is the explicit escape hatch (e.g. a box without nvcc).

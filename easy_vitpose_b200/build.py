@@ -1,4 +1,4 @@
-"""Builds csrc/libvitpose_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds csrc/libvitpose_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import fcntl
@@ -10,9 +10,9 @@ import tempfile
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 LIB = os.path.join(CSRC, "libvitpose_b200.so")
 SOURCES = ["engine.cu"]
-HEADERS = ["ptx.cuh", "gemm.cuh", "chain.cuh", "attention.cuh", "attention_pack.cuh", "pointwise.cuh", "decode.cuh", "preprocess.cuh",
+HEADERS = ["ptx.cuh", "wgmma.cuh", "gemm.cuh", "chain.cuh", "attention.cuh", "pointwise.cuh", "decode.cuh", "preprocess.cuh",
            os.path.join("..", "..", "include", "vitpose_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC"]
 
 

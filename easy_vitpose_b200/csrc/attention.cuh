@@ -1,45 +1,26 @@
-// Fused multi-head attention for one ViTPose crop: T = 192 tokens, head_dim 32 / 64 / 80 (ViT-S / B,L / H), on chip.
+// Fused multi-head attention for ViTPose crops: T = 192 tokens, head_dim 32 / 64 / 80 (ViT-S / B,L / H), on chip.
 //
-// Work unit = one "step" = one 128-row M tile of an item (crop b, head h); an item has two: tokens 0..127 and 128..191.
-// The 2 * batch * heads steps of a launch are split into gridDim.x CONTIGUOUS, equally long ranges (one CTA per SM), so a
-// CTA may start or end in the middle of an item (it then loads that item's Q,K,V like any other: 72 KB) -- with whole items
-// per CTA 768 items over 148 SMs gave 5.19 -> 6 items on the slowest CTA; by steps it is 10.38 -> 11 (8 % shorter).
-// Steps run through a software pipeline with four kinds of warps:
-//   warp 12, one thread  TMA of Q,K [192 x hd] bf16 boxes straight out of the qkv activation [M, 3D] -> swizzled smem (double
-//                        buffered per item) and UMMA issue of S = Q K^T (M=128 x N=192, fp32 -> TMEM buffer step%2), ahead of the
-//                        softmax as far as the two S buffers allow.
-//   warp 13, one thread  TMA of V and UMMA issue of O = P V, in three 64-key slices as the softmax publishes P.  (Two issuing
-//                        threads: a tcgen05.mma costs its issuing thread ~100 cycles and a step has 16..29 of them.)
-//   warps 0..3 / 4..7    softmax groups A / B: group A owns the even steps (S buffer 0), group B the odd ones (buffer 1), ONE
-//                        thread per row.  A thread streams its 192 logits out of TMEM in 32-column chunks twice: a max pass, then
-//                        the exp2 pass (the MUFU, 16 ex2/clk/SM, bounds this stage) with the row sum, writing P back IN PLACE as
-//                        packed bf16 (tcgen05.st, columns [0,96) of the S buffer) -- P never touches shared memory, and no
-//                        value crosses threads: no smem exchange, no named barrier.  The two warps that share an SM
-//                        sub-partition (warp q of A and of B) are in different phases of different steps, so one's TMEM loads /
-//                        max pass / stores run under the other's exponentials (round 1: two threads per row, both warps of a
-//                        sub-partition in lock step, the MUFU idle during every non-exp phase: 3.2 k cycles per step).
-//   warps 8..11          epilogue: O (head_dim <= 64: its own TMEM columns [384 + 64*(step&1), +hd); head_dim 80: the dead S
-//                        columns [96, 96+hd) of the same buffer) / rowsum -> bf16 -> smem staging -> coalesced 16-byte stores
-//                        to attn_out[b*192 + t, h*hd + d].
-// O = P V takes A = P from TMEM and B = V as an MN-major smem operand, i.e. exactly the [token][dim] box TMA delivered.
-// Operand tiles: head_dim 64 -> one 128-byte-swizzled box per operand; 32 -> one 64-byte-swizzled box; 80 -> a
-// 128B-swizzled box of 64 dims plus a 32B-swizzled box of the last 16 (QK^T: 4+1 K steps; PV: an N=64 and an N=16 MMA).
-// The second M tile only has 64 live rows.  Even items take A rows 128..255 (live rows in TMEM lanes 0..63, the rest
-// reads past Q into K: UMMA rows are independent, they only feed lanes nobody reads); odd items take A rows 64..191
-// (live rows in lanes 64..127), so the half-tile work alternates between lane quarters 0-1 and 2-3.
+// Work unit = one item (crop b, head h).  The items of a launch are handed out statically (item = blockIdx.x + i * gridDim.x,
+// one CTA per SM); Q, K, V of an item arrive by TMA as [192 x hd] boxes straight out of the qkv activation [M, 3D] into one of
+// two smem stages, so the loads of item i + 1 run under the math of item i.  The 192 query rows are three warpgroups of 64:
+//   S = Q K^T      wgmma m64n192k16, A = Q rows and B = K from smem (both K-major), fp32 logits in registers (96 per thread);
+//   softmax        in registers: row max over the thread's 48 logits and its quad (the four lanes that share a row), then
+//                  P = bf16(exp2(s log2e - max log2e)) and the row sum of those rounded weights; P never touches shared memory;
+//   O = P V        wgmma m64nHDk16 with A = P from registers (the accumulator layout of S is the A-fragment layout, 16 keys per
+//                  step) and B = V from smem as an MN-major operand, i.e. exactly the [token][dim] box TMA delivered;
+//   epilogue       O / rowsum -> bf16 -> attn_out[b*192 + t, h*hd + d].
+// Operand tiles: head_dim 64 -> one 128-byte-swizzled box per operand; 32 -> one 64-byte-swizzled box; 80 -> a 128B-swizzled
+// box of 64 dims plus a 32B-swizzled box of the last 16 (Q K^T: 4+1 K steps; P V: an N = 64 and an N = 16 MMA per step).
 #pragma once
 #include <cuda.h>
 
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace vpb {
 
 constexpr int ATT_T = 192;
-constexpr int ATT_THREADS = 14 * 32;                          // 8 softmax warps, 4 epilogue warps, 2 issue warps (QK / PV)
-constexpr int ATT_TMEM_COLS = 512;                            // two S/P/O buffers of 192 columns
-constexpr int ATT_BUF_COLS = 192;
-constexpr int ATT_O_COL = 96;                                 // head_dim 80: O inside the S buffer, behind P
-constexpr int ATT_O_SEP_COL = 384;                            // head_dim <= 64: O in its own columns [384 + 64*(step&1), +hd)
+constexpr int ATT_THREADS = 3 * 128;                          // three warpgroups x 64 query rows
 
 template <int HD>
 struct AttCfg {
@@ -51,14 +32,8 @@ struct AttCfg {
   static constexpr int TAIL_BYTES = TAIL ? ATT_T * 32 : 0;    // 6144
   static constexpr int OPER_BYTES = MAIN_BYTES + TAIL_BYTES;  // one of Q / K / V
   static constexpr int STAGE_BYTES = 3 * OPER_BYTES;          // Q, K, V of one item
-  // The kernel is bound by a latency chain, not by a pipe (DESIGN.md section 7): softmax(t) -> PV(t) -> O drained -> QK(t+2) ->
-  // S(t+2).  Two things shorten it: PV is issued in three 64-key slices as the softmax publishes P (p_chunk barriers), so only
-  // the last four UMMAs trail the softmax; and for head_dim <= 64 O has its own TMEM columns, so the S buffer is released by
-  // PV's commit instead of by the epilogue's drain (2*192 + 2*80 columns do not fit: head_dim 80 keeps O behind P).
-  static constexpr bool O_SEP = HD <= 64;
-  static constexpr int OUT_PITCH = HD * 2 + 16;               // staging row pitch (bytes): conflict-free 16-byte accesses
-  static constexpr int OUT_STAGE = 4 * 32 * OUT_PITCH;        // 4 epilogue warps x 32 rows
-  static constexpr int SMEM = 2 * STAGE_BYTES + OUT_STAGE + 2048 /*row sums: 4 slots x 128 rows*/ + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int SMEM = 2 * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(OPER_BYTES % 1024 == 0 && MAIN_BYTES % 1024 == 0, "swizzled boxes keep 1024-byte alignment");
 };
 
 struct AttnParams {
@@ -66,333 +41,147 @@ struct AttnParams {
   int heads;
   int dim;                // D = heads * head_dim
   __nv_bfloat16* out;     // [batch*192, D]
-  long long* dbg;         // debug: per CTA [8] or nullptr: 0 lifetime, 1 softmax(group A, warp 0) wait S, 2 its busy cycles, 3 epilogue
-                          //        wait, 4 epilogue busy, 5 softmax(group B, warp 4) wait S, 6 its busy cycles, 7 steps of this CTA
+  long long* dbg;         // debug: per CTA [8] or nullptr: 0 lifetime (cycles), 1 wait for operands (thread 0), 7 items of this CTA
 };
-
-// P (A operand) from TMEM, V (B operand) from smem
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(static_cast<uint32_t>(accumulate))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // tmap_main: box [192 rows x MAIN cols] (swizzle = MAIN*2 bytes); tmap_tail: box [192 x 16] (32B swizzle), hd 80 only.
 // NPOLY of every 32 exponentials go through ex2_poly (FMA pipe) instead of the MUFU: 0 (all MUFU) or 8 (every 4th)
 template <int HD, int NPOLY = 0>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
-attention_tcgen05(const __grid_constant__ CUtensorMap tmap_main, const __grid_constant__ CUtensorMap tmap_tail, const AttnParams p) {
+attention_wgmma(const __grid_constant__ CUtensorMap tmap_main, const __grid_constant__ CUtensorMap tmap_tail, const AttnParams p) {
   using Cfg = AttCfg<HD>;
+  static_assert(NPOLY == 0 || NPOLY == 8, "NPOLY");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sOut = smem + 2 * Cfg::STAGE_BYTES;               // per-warp output staging (coalesced global stores)
-  float* s_sum = reinterpret_cast<float*>(sOut + Cfg::OUT_STAGE);   // [4 slots = step & 3][128 rows]: the softmax may run two
-                                                              // steps of its buffer ahead of the epilogue's read
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_sum + 512);
-  uint64_t* qk_full = bars;          // [2] Q,K of item stage landed            (TMA -> QK issuer)
-  uint64_t* v_full = bars + 2;       // [2] V landed                             (TMA -> PV issuer)
-  uint64_t* s_full = bars + 4;       // [2] S complete                           (MMA commit -> softmax group step&1)
-  uint64_t* p_ready = bars + 6;      // [2] row sums published                   (128 softmax threads -> epilogue)
-  uint64_t* o_full = bars + 8;       // [2] O complete                           (MMA commit -> epilogue, issuers)
-  uint64_t* s_free = bars + 10;      // [2] O drained                            (128 epilogue threads -> issuers)
-  uint64_t* p_chunk = bars + 12;     // [2][3] P keys 64c..64c+63 of all rows published (128 softmax threads -> PV issuer)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * Cfg::STAGE_BYTES);    // [2] Q, K, V of a stage landed
 
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);      // warp-uniform for the compiler (see elect_one)
-  const int lane = threadIdx.x & 31;
-  // this CTA's contiguous range of steps [u0, u1): step u = tile (u & 1) of item (u >> 1)
-  const long long steps_all = 2LL * p.batch * p.heads;
-  const int u0 = static_cast<int>(steps_all * blockIdx.x / gridDim.x);
-  const int u1 = static_cast<int>(steps_all * (blockIdx.x + 1) / gridDim.x);
-  const int T = u1 - u0;                                     // steps of this CTA
-  const int item0 = u0 >> 1;
-  const int n_items = T > 0 ? ((u1 - 1) >> 1) - item0 + 1 : 0;   // items this CTA touches (the first / last possibly half)
+  const int wg = threadIdx.x >> 7;                            // query rows 64 wg .. 64 wg + 63
+  const int tid = threadIdx.x & 127;
+  const int lane = threadIdx.x & 31, wq = tid >> 5;
+  const int items = p.batch * p.heads;
   const long long t_cta0 = p.dbg ? clock64() : 0;
+  long long t_wait = 0;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_main);
     if constexpr (Cfg::TAIL > 0) tma_prefetch_desc(&tmap_tail);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&qk_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_ready[i], 128);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&s_free[i], 128);
-      for (int c = 0; c < 3; ++c) mbar_init(&p_chunk[i * 3 + c], 128);
-    }
+    mbar_init(&full[0], 1);
+    mbar_init(&full[1], 1);
     fence_mbar_init();
   }
-  if (warp == 12) tmem_alloc(tmem_slot, ATT_TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = uniform_u32(*tmem_slot);
   pdl_launch_dependents();
-  pdl_wait();                                               // qkv from the previous GEMM is complete
+  pdl_wait();                                                 // qkv from the previous GEMM is complete
 
-  // shared by the two issuing threads
-  auto stage_ptr = [&](int q, int oper) { return smem + q * Cfg::STAGE_BYTES + oper * Cfg::OPER_BYTES; };
-  auto load_oper = [&](uint8_t* dst, uint64_t* bar, int col0, int row0) {
-    tma_load_2d(dst, &tmap_main, bar, col0, row0);
-    if constexpr (Cfg::TAIL > 0) tma_load_2d(dst + Cfg::MAIN_BYTES, &tmap_tail, bar, col0 + Cfg::MAIN, row0);
+  auto oper = [&](int q, int o) { return smem + q * Cfg::STAGE_BYTES + o * Cfg::OPER_BYTES; };
+  auto load_item = [&](int item, int q) {                     // thread 0 only
+    const int b = item / p.heads, h = item % p.heads;
+    mbar_expect_tx(&full[q], Cfg::STAGE_BYTES);
+#pragma unroll
+    for (int o = 0; o < 3; ++o) {
+      tma_load_2d(oper(q, o), &tmap_main, &full[q], o * p.dim + h * HD, b * ATT_T);
+      if constexpr (Cfg::TAIL > 0) tma_load_2d(oper(q, o) + Cfg::MAIN_BYTES, &tmap_tail, &full[q], o * p.dim + h * HD + Cfg::MAIN, b * ATT_T);
+    }
   };
-  // local step t -> global step u = u0 + t: item u >> 1 (local item li = item - item0, smem stage li & 1), tile mt = u & 1,
-  // TMEM buffer t & 1, n = t >> 1 = how many times that buffer was used before (barrier phase n & 1)
-
-  if (warp == 12) {
-    // ------------------------------------------------------------------ issue warp 1: TMA of Q,K and S = Q K^T
-    // (the whole warp runs the loop, one elected lane issues: see elect_one)
-    auto load_qk = [&](int li) {
-      const int item = item0 + li, b = item / p.heads, h = item % p.heads, q = li & 1;
-      if (elect_one()) {
-        mbar_expect_tx(&qk_full[q], 2 * Cfg::OPER_BYTES);
-        load_oper(stage_ptr(q, 0), &qk_full[q], h * HD, b * ATT_T);
-        load_oper(stage_ptr(q, 1), &qk_full[q], p.dim + h * HD, b * ATT_T);
-      }
-      __syncwarp();
-    };
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, ATT_T);
-    if (n_items > 0) load_qk(0);
-    if (n_items > 1) load_qk(1);
-    for (int t = 0; t < T; ++t) {                            // S runs ahead of the softmax as far as the two buffers allow
-      const int u = u0 + t, item = u >> 1, mt = u & 1, li = item - item0, q = li & 1, n = t >> 1;
-      const bool first_of_item = (t == 0) || (mt == 0);
-      // the S buffer was last used by step t-2: PV(t-2) has consumed P (O elsewhere), or the epilogue has drained O from it
-      if (t >= 2) mbar_wait(Cfg::O_SEP ? &o_full[t & 1] : &s_free[t & 1], (n - 1) & 1);
-      if (first_of_item) mbar_wait(&qk_full[q], (li >> 1) & 1);
-      tc_fence_after_sync();
-      {
-        const uint32_t sQ = smem_u32(stage_ptr(q, 0)), sK = smem_u32(stage_ptr(q, 1));
-        const int q_row0 = mt == 0 ? 0 : ((item & 1) ? 64 : 128);
-        const uint32_t d = tmem_base + (t & 1) * ATT_BUF_COLS;
-        const uint64_t qd = umma_desc_rows<Cfg::MAIN_ROW>(sQ + q_row0 * Cfg::MAIN_ROW);
-        const uint64_t kd = umma_desc_rows<Cfg::MAIN_ROW>(sK);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < Cfg::MAIN / 16; ++k) umma_bf16(d, qd + 2 * k, kd + 2 * k, idesc_s, k != 0);
-          if constexpr (Cfg::TAIL > 0)
-            umma_bf16(d, umma_desc_rows<32>(sQ + Cfg::MAIN_BYTES + q_row0 * 32), umma_desc_rows<32>(sK + Cfg::MAIN_BYTES), idesc_s, true);
-          umma_commit(&s_full[t & 1]);
-        }
-        __syncwarp();
-      }
-      if (first_of_item && li >= 1 && li + 1 < n_items) {
-        // local item li-1's last Q K^T (step t-1) was issued before this one and has retired by now or soon: its stage is free
-        mbar_wait(&s_full[(t - 1) & 1], ((t - 1) >> 1) & 1);
-        load_qk(li + 1);
-      }
-    }
-  } else if (warp == 13) {
-    // ------------------------------------------------------------------ issue warp 2: TMA of V and O = P V
-    auto load_v = [&](int li) {
-      const int item = item0 + li, b = item / p.heads, h = item % p.heads, q = li & 1;
-      if (elect_one()) {
-        mbar_expect_tx(&v_full[q], Cfg::OPER_BYTES);
-        load_oper(stage_ptr(q, 2), &v_full[q], 2 * p.dim + h * HD, b * ATT_T);
-      }
-      __syncwarp();
-    };
-    constexpr uint32_t idesc_o_main = umma_idesc_bf16(128, Cfg::MAIN, /*b_mn_major=*/true);
-    constexpr uint32_t idesc_o_tail = umma_idesc_bf16(128, 16, /*b_mn_major=*/true);
-    // O(step t) = P V, slice c = keys 64c..64c+63 (UMMA k-steps 4c..4c+3): P = packed bf16 in columns [0,96) of the buffer;
-    // O -> its own columns (head_dim <= 64) or columns [96, 96+hd) of the buffer
-    auto issue_pv_slice = [&](int t, int q, int c) {
-      const uint32_t sV = smem_u32(stage_ptr(q, 2));
-      const uint32_t buf = tmem_base + (t & 1) * ATT_BUF_COLS;
-      const uint32_t od = Cfg::O_SEP ? tmem_base + ATT_O_SEP_COL + (t & 1) * 64 : buf + ATT_O_COL;
-      if (elect_one()) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          // 16 keys = 8 packed TMEM columns of P; V (MN-major): 16 tokens = two 8-row groups of the box
-          const int kk = 4 * c + j;
-          const bool acc = kk != 0;
-          umma_bf16_ts(od, buf + kk * 8, umma_desc_rows<Cfg::MAIN_ROW>(sV + kk * 16 * Cfg::MAIN_ROW), idesc_o_main, acc);
-          if constexpr (Cfg::TAIL > 0)
-            umma_bf16_ts(od + Cfg::MAIN, buf + kk * 8, umma_desc_rows<32>(sV + Cfg::MAIN_BYTES + kk * 16 * 32), idesc_o_tail, acc);
-        }
-        if (c == 2) umma_commit(&o_full[t & 1]);
-      }
-      __syncwarp();
-    };
-    if (n_items > 0) load_v(0);
-    if (n_items > 1) load_v(1);
-    for (int t = 0; t < T; ++t) {
-      const int u = u0 + t, item = u >> 1, mt = u & 1, li = item - item0, q = li & 1, n = t >> 1, bf = t & 1;
-      if (t == 0 || mt == 0) mbar_wait(&v_full[q], (li >> 1) & 1);
-      if (Cfg::O_SEP && t >= 2) mbar_wait(&s_free[bf], (n - 1) & 1);      // O(t-2) has left this step parity's O columns
-      if constexpr (!Cfg::O_SEP) {
-        // head_dim 80: O accumulates in columns [96, 176) of the S buffer, which the softmax still READS (keys 96..191)
-        // while it publishes the first slices of P: issue nothing before the whole row of P is out
-        mbar_wait(&p_chunk[bf * 3 + 2], n & 1);
-      }
-#pragma unroll 1
-      for (int c = 0; c < 3; ++c) {
-        mbar_wait(&p_chunk[bf * 3 + c], n & 1);              // this slice of P(t) is in TMEM
-        tc_fence_after_sync();
-        issue_pv_slice(t, q, c);
-      }
-      if (mt == 1 && li + 2 < n_items) {
-        mbar_wait(&o_full[bf], n & 1);                       // the item's last P V has retired: its V stage is free
-        load_v(li + 2);
-      }
-    }
-  } else if (warp < 8) {
-    // -------------------------------------------------------------------- softmax (group A: warps 0..3, B: warps 4..7)
-    const int quarter = warp & 3;                           // TMEM lane quarter
-    const int grp = warp >> 2;                              // steps t = grp, grp + 2, ...; TMEM buffer grp
-    const int tl = quarter * 32 + lane;                     // TMEM lane = row of the M tile
-    const uint32_t buf = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + grp * ATT_BUF_COLS;
-    constexpr float kLog2e = 1.4426950408889634f;
-    long long w_wait = 0, w_busy = 0, c0 = 0;
-    for (int t = grp; t < T; t += 2) {
-      const int u = u0 + t, item = u >> 1, mt = u & 1, n = t >> 1;
-      const bool live = (mt == 0) || ((item & 1) ? quarter >= 2 : quarter < 2);   // warp-uniform
-      if (p.dbg) c0 = clock64();
-      mbar_wait(&s_full[grp], n & 1);
-      if (p.dbg) { w_wait += clock64() - c0; c0 = clock64(); }
-      tc_fence_after_sync();
-      if (live) {
-        uint32_t ra[32], rb[32];
-        // ---- pass 1: row maximum over the 192 logits, two 32-column loads in flight
-        float mx = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < 6; c += 2) {
-          tmem_ld32(buf + 32 * c, ra);
-          tmem_ld32(buf + 32 * c + 32, rb);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; j += 2)
-            mx = fmaxf(fmaxf(mx, fmaxf(__uint_as_float(ra[j]), __uint_as_float(ra[j + 1]))), fmaxf(__uint_as_float(rb[j]), __uint_as_float(rb[j + 1])));
-        }
-        const float mscaled = mx * kLog2e;
-        // ---- pass 2: P = exp2(s log2e - max log2e) as packed bf16 IN PLACE (chunk c = keys 32c..32c+31 -> packed columns
-        // [16c, 16c+16), which lie inside S chunks already consumed), the next chunk's load in flight under the exponentials
-        float sum = 0.0f;
-        auto exp_chunk = [&](const uint32_t (&r)[32], int c) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int j = 0; j < 32; j += 2) {
-            const float a0 = fmaf(__uint_as_float(r[j]), kLog2e, -mscaled), a1 = fmaf(__uint_as_float(r[j + 1]), kLog2e, -mscaled);
-            const float e0 = ex2_approx(a0);
-            const float e1 = (NPOLY > 0 && ((j >> 1) % (16 / (NPOLY > 0 ? NPOLY : 1)) == 0)) ? ex2_poly(a1) : ex2_approx(a1);
-            sum += e0 + e1;
-            pk[j >> 1] = pack_bf16(e0, e1);
-          }
-          tmem_st16(buf + 16 * c, pk);
-          if (c & 1) {                                        // a 64-key slice is complete: the PV issuer may start on it
-            tmem_st_wait();
-            tc_fence_before_sync();
-            mbar_arrive(&p_chunk[grp * 3 + (c >> 1)]);
-          }
-        };
-        tmem_ld32(buf, ra);
-        tmem_ld_wait();
-#pragma unroll
-        for (int c = 0; c < 6; c += 2) {
-          tmem_ld32(buf + 32 * (c + 1), rb);
-          exp_chunk(ra, c);
-          tmem_ld_wait();
-          if (c + 2 < 6) tmem_ld32(buf + 32 * (c + 2), ra);
-          exp_chunk(rb, c + 1);
-          if (c + 2 < 6) tmem_ld_wait();
-        }
-        s_sum[(t & 3) * 128 + tl] = sum;
-      } else {
-        tc_fence_before_sync();
-#pragma unroll
-        for (int c = 0; c < 3; ++c) mbar_arrive(&p_chunk[grp * 3 + c]);
-      }
-      // The epilogue waits on p_ready[grp] by phase parity, and nothing else keeps this group from finishing step t while the
-      // epilogue has not yet looked at step t-2 of the same buffer (S(t) only needs P V(t-2) to have retired): completing
-      // two phases ahead of a waiter would leave it waiting on the wrong phase forever.  s_free[grp] of step t-2 is arrived
-      // by the epilogue after it passed that wait -- almost always long before this point.
-      if (t >= 2) mbar_wait(&s_free[grp], (n - 1) & 1);
-      mbar_arrive(&p_ready[grp]);                           // row sum published (release: visible to the epilogue's acquire)
-      if (p.dbg) w_busy += clock64() - c0;
-    }
-    if (p.dbg && lane == 0 && quarter == 0) { p.dbg[blockIdx.x * 8 + 1 + 4 * grp] = w_wait; p.dbg[blockIdx.x * 8 + 2 + 4 * grp] = w_busy; }
-  } else if (warp < 12) {
-    // -------------------------------------------------------------------- epilogue (warps 8..11)
-    const int quarter = warp - 8;
-    const int tl = quarter * 32 + lane;
-    const uint32_t lane_base = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    long long w_wait = 0, w_busy = 0, c0 = 0;
-    for (int t = 0; t < T; ++t) {
-      const int u = u0 + t, item = u >> 1, mt = u & 1, n = t >> 1, bf = t & 1;
-      const int b = item / p.heads, h = item % p.heads;
-      const bool live = (mt == 0) || ((item & 1) ? quarter >= 2 : quarter < 2);   // warp-uniform
-      int token;                                            // token of this thread's row
-      if (mt == 0) token = tl;
-      else if (item & 1) token = 64 + tl;                   // A rows 64..191 -> lanes 64..127 hold tokens 128..191
-      else token = 128 + tl;                                // A rows 128..255 -> lanes 0..63 hold tokens 128..191
-      if (p.dbg) c0 = clock64();
-      mbar_wait(&p_ready[bf], n & 1);                       // row sums are visible
-      mbar_wait(&o_full[bf], n & 1);
-      if (p.dbg) { w_wait += clock64() - c0; c0 = clock64(); }
-      tc_fence_after_sync();
-      constexpr int OCH = HD / 16;                          // 16-column chunks of O
-      uint32_t o[OCH][16];
-      float sum = 1.0f;
-      if (live) {
-#pragma unroll
-        for (int qq = 0; qq < OCH; ++qq)
-          tmem_ld16(lane_base + (Cfg::O_SEP ? ATT_O_SEP_COL + bf * 64 : bf * ATT_BUF_COLS + ATT_O_COL) + 16 * qq, o[qq]);
-        tmem_ld_wait();
-        sum = s_sum[(t & 3) * 128 + tl];
-      }
-      tc_fence_before_sync();
-      mbar_arrive(&s_free[bf]);                             // O and the row sum are in registers: the O columns may be reused
-      if (live) {
-        // O rows -> this warp's smem staging (row pitch hd*2+16 B: conflict-free), then the warp writes its 32 rows with
-        // consecutive lanes on consecutive 16-byte chunks of a row
-        const float inv = 1.0f / sum;
-        uint8_t* stage = sOut + quarter * 32 * Cfg::OUT_PITCH;
-        uint8_t* srow = stage + lane * Cfg::OUT_PITCH;
-#pragma unroll
-        for (int qq = 0; qq < OCH; ++qq) {
-#pragma unroll
-          for (int v = 0; v < 2; ++v) {
-            uint4 w;
-            w.x = pack_bf16(__uint_as_float(o[qq][8 * v + 0]) * inv, __uint_as_float(o[qq][8 * v + 1]) * inv);
-            w.y = pack_bf16(__uint_as_float(o[qq][8 * v + 2]) * inv, __uint_as_float(o[qq][8 * v + 3]) * inv);
-            w.z = pack_bf16(__uint_as_float(o[qq][8 * v + 4]) * inv, __uint_as_float(o[qq][8 * v + 5]) * inv);
-            w.w = pack_bf16(__uint_as_float(o[qq][8 * v + 6]) * inv, __uint_as_float(o[qq][8 * v + 7]) * inv);
-            *reinterpret_cast<uint4*>(srow + 32 * qq + 16 * v) = w;
-          }
-        }
-        __syncwarp();
-        constexpr int CPR = HD / 8;                         // 16-byte chunks per row
-        const int token0 = token - lane;                    // token of this warp's row 0 (rows are consecutive tokens)
-        __nv_bfloat16* obase = p.out + (static_cast<size_t>(b) * ATT_T + token0) * p.dim + h * HD;
-#pragma unroll
-        for (int j = lane; j < 32 * CPR; j += 32) {
-          const int rr = j / CPR, ch = j % CPR;
-          const uint4 w = *reinterpret_cast<const uint4*>(stage + rr * Cfg::OUT_PITCH + ch * 16);
-          *reinterpret_cast<uint4*>(obase + static_cast<size_t>(rr) * p.dim + ch * 8) = w;
-        }
-        __syncwarp();                                       // staging is reused by this warp's next tile
-      }
-      if (p.dbg) w_busy += clock64() - c0;
-    }
-    if (p.dbg && threadIdx.x == 256) { p.dbg[blockIdx.x * 8 + 3] = w_wait; p.dbg[blockIdx.x * 8 + 4] = w_busy; }
+  if (threadIdx.x == 0) {
+    if (static_cast<int>(blockIdx.x) < items) load_item(blockIdx.x, 0);
+    if (static_cast<int>(blockIdx.x + gridDim.x) < items) load_item(blockIdx.x + gridDim.x, 1);
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 12) tmem_dealloc(tmem_base, ATT_TMEM_COLS);
-  if (p.dbg && threadIdx.x == 0) { p.dbg[blockIdx.x * 8 + 0] = clock64() - t_cta0; p.dbg[blockIdx.x * 8 + 7] = T; }
+  constexpr float kLog2e = 1.4426950408889634f;
+  int li = 0;
+  for (int item = blockIdx.x; item < items; item += gridDim.x, ++li) {
+    const int q = li & 1;
+    const long long w0 = p.dbg ? clock64() : 0;
+    mbar_wait(&full[q], (li >> 1) & 1);
+    if (p.dbg && threadIdx.x == 0) t_wait += clock64() - w0;
+    const uint32_t sQ = smem_u32(oper(q, 0)), sK = smem_u32(oper(q, 1)), sV = smem_u32(oper(q, 2));
+
+    // ---- S = Q K^T for this warpgroup's 64 rows
+    float s[ATT_T / 2];
+    wgmma_fence();
+    {
+      const uint64_t qd = wgmma_desc<Cfg::MAIN_ROW>(sQ + wg * 64 * Cfg::MAIN_ROW), kd = wgmma_desc<Cfg::MAIN_ROW>(sK);
+#pragma unroll
+      for (int k = 0; k < Cfg::MAIN / 16; ++k) wgmma_ss<ATT_T>(s, qd + 2 * k, kd + 2 * k, k != 0);   // +32 B per K = 16 step
+      if constexpr (Cfg::TAIL > 0)
+        wgmma_ss<ATT_T>(s, wgmma_desc<32>(sQ + Cfg::MAIN_BYTES + wg * 64 * 32), wgmma_desc<32>(sK + Cfg::MAIN_BYTES), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+
+    // ---- softmax: thread rows r_lo (h = 0: s[4j], s[4j+1]) and r_lo + 8 (h = 1: s[4j+2], s[4j+3]); a row lives in one quad
+    float sum[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < ATT_T / 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mscaled = mx * kLog2e;
+      // P is rounded to bf16 here, and the row sum is taken over the ROUNDED weights that O = P V actually uses: the
+      // normalised weights then sum to 1 up to fp32 round-off instead of carrying a per-row scale error of up to 2^-9
+      float sm = 0.0f;
+#pragma unroll
+      for (int j = 0; j < ATT_T / 8; ++j) {
+        const float a1 = fmaf(s[4 * j + 2 * h + 1], kLog2e, -mscaled);
+        const float e0 = __bfloat162float(__float2bfloat16_rn(ex2_approx(fmaf(s[4 * j + 2 * h], kLog2e, -mscaled))));
+        const float e1 = __bfloat162float(__float2bfloat16_rn((NPOLY > 0 && (j & 1) == 0) ? ex2_poly(a1) : ex2_approx(a1)));
+        sm += e0 + e1;
+        s[4 * j + 2 * h] = e0;
+        s[4 * j + 2 * h + 1] = e1;
+      }
+      sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+      sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+      sum[h] = sm;
+    }
+
+    // ---- O = P V: 12 steps of 16 keys; P as bf16 A fragments, V MN-major
+    float o[Cfg::MAIN / 2];
+    [[maybe_unused]] float ot[8];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < ATT_T / 16; ++kk) {
+      uint32_t a[4];
+      a[0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+      a[1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+      a[2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+      a[3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+      const uint64_t vd = wgmma_desc<Cfg::MAIN_ROW>(sV + kk * 16 * Cfg::MAIN_ROW);
+      if constexpr (Cfg::MAIN == 64) wgmma_rs_n64<1>(o, a, vd, kk != 0);
+      else wgmma_rs_n32<1>(o, a, vd, kk != 0);
+      if constexpr (Cfg::TAIL > 0) wgmma_rs_n16<1>(ot, a, wgmma_desc<32>(sV + Cfg::MAIN_BYTES + kk * 16 * 32), kk != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if constexpr (Cfg::TAIL > 0) wgmma_fence_regs(ot);
+
+    // ---- every warpgroup is done with this stage's operands: thread 0 refills it with the item after next
+    __syncthreads();
+    if (threadIdx.x == 0 && item + 2 * static_cast<int>(gridDim.x) < items) load_item(item + 2 * gridDim.x, q);
+
+    // ---- O / rowsum -> bf16 -> attn_out
+    const int b = item / p.heads, h = item % p.heads;
+    const int r_lo = wg * 64 + wq * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const float inv = 1.0f / sum[hh];
+      __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * ATT_T + r_lo + 8 * hh) * p.dim + h * HD;
+#pragma unroll
+      for (int j = 0; j < Cfg::MAIN / 8; ++j)
+        *reinterpret_cast<uint32_t*>(orow + 8 * j + cq) = pack_bf16(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+      if constexpr (Cfg::TAIL > 0) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          *reinterpret_cast<uint32_t*>(orow + Cfg::MAIN + 8 * j + cq) = pack_bf16(ot[4 * j + 2 * hh] * inv, ot[4 * j + 2 * hh + 1] * inv);
+      }
+    }
+  }
+  if (p.dbg && threadIdx.x == 0) { p.dbg[blockIdx.x * 8 + 0] = clock64() - t_cta0; p.dbg[blockIdx.x * 8 + 1] = t_wait; p.dbg[blockIdx.x * 8 + 7] = li; }
 }
 
 }  // namespace vpb

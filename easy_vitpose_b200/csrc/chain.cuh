@@ -2,14 +2,14 @@
 //
 //     [proj (+= x)] -> LN -> [fc1 + GELU] -> [fc2 (+= x)] -> LN -> [qkv of the next block]        (backbone/vit.py:202-205,164-180)
 //
-// Round 1 ran these as 4 GEMM launches + 2 LayerNorm launches.  Each tensor-core launch paid ~2 us of head (barrier init,
-// TMEM alloc, first TMA round trip) and ~3 us of tail (last tile's epilogue, idle SMs in the last wave) that programmatic
-// dependent launch cannot hide (a 227 KB CTA leaves no room for the next grid), and every LayerNorm was a separate pass of
-// the fp32 stream through all SMs with nothing else running.  Here the tiles of all phases form ONE list, handed out
-// statically (tile g -> cluster g mod #clusters, phase-major, n fastest), and what used to be a kernel boundary is a counter:
+// Run as 4 GEMM launches + 2 LayerNorm launches, every launch pays a head (barrier init, first TMA round trip) and a tail (last
+// tile's epilogue, idle SMs in the last wave) that programmatic dependent launch cannot hide (a CTA near the 227 KB shared
+// memory limit leaves no room for the next grid), and every LayerNorm is a separate pass of the fp32 stream through all SMs
+// with nothing else running.  Here the tiles of all phases form ONE list, handed out statically (tile g -> CTA g mod grid,
+// phase-major, n fastest), and what used to be a kernel boundary is a counter:
 //
-//   * every 128-row block `mt` of an activation has a counter that the producing epilogue warps bump once their TMA stores /
-//     reduce-adds of a tile have COMPLETED (cp.async.bulk.wait_group 0, cross-proxy fence, release);
+//   * every 128-row block `mt` of an activation has a counter that the producing consumer warpgroups bump once their TMA
+//     stores / reduce-adds of a tile have COMPLETED (cp.async.bulk.wait_group 0, cross-proxy fence, release);
 //   * the TMA-producer warp of a consuming tile spins (acquire) on the counter of its A rows before its first load;
 //   * LayerNorm runs on four dedicated warps of every CTA, concurrently with that CTA's tensor-core tiles: 16-row jobs handed
 //     out statically (job j -> CTA j mod grid), each waiting for its row block's residual adds to complete; they read the fp32
@@ -18,15 +18,16 @@
 //     control warp (ln_ctl, default) so that the LayerNorm warps only load, normalise and store.
 //
 // Dependencies only point to tiles that come earlier in the list (and LN jobs only to tiles), all CTAs are resident (one per
-// SM, grid <= #SMs), every role walks its own list in order (see "Tile list" in the kernel for the order): the smallest unfinished tile can always run, so the waits cannot
-// deadlock; a counter that never arrives traps (VPB_HANG_TRAP_SPINS) instead of hanging the GPU.
+// SM, grid <= #SMs), every role walks its own list in order (see "Tile list" in the kernel for the order): the smallest
+// unfinished tile can always run, so the waits cannot deadlock; a counter that never arrives traps (VPB_HANG_TRAP_SPINS)
+// instead of hanging the GPU.
 // The arithmetic of every phase is that of gemm.cuh's kernels and of layernorm_f32_to_bf16, in the same order: results are
 // bit-identical to the unchained path (tests/test_gpu_engine.py::test_chain_is_bit_identical).
 //
-//   warps 0..7   epilogue (tcgen05.ld -> bias / GELU -> swizzled smem staging -> TMA store or TMA reduce-add)
-//   warp  8      TMEM allocator            warp 10  TMA producer (+ dependency waits)      warp 11  tcgen05.mma issuer (leader CTA)
-//   warp  9      LayerNorm control (ln_ctl): polls the residual counters / publishes the jobs for warps 12..15
-//   warps 12..15 LayerNorm jobs
+//   warps 0..7   consumers: two warpgroups, wgmma into registers, then the TMA epilogue of gemm.cuh
+//   warp  8      TMA producer (+ dependency waits)
+//   warp  9      LayerNorm control (ln_ctl): polls the residual counters / publishes the jobs for warps 10..13
+//   warps 10..13 LayerNorm jobs
 #pragma once
 #include "gemm.cuh"
 
@@ -34,7 +35,7 @@ namespace vpb {
 
 constexpr int CHAIN_MAX_PHASES = 4;
 constexpr int CHAIN_MAX_LN = 2;
-constexpr int CHAIN_THREADS = 512;
+constexpr int CHAIN_THREADS = 448;       // 8 consumer warps, producer, LayerNorm control, 4 LayerNorm warps
 constexpr int CHAIN_LN_WARPS = 4;
 constexpr int CHAIN_LN_JOB_ROWS = 16;      // default rows per LayerNorm job (ChainParams::ln_job_rows: 8 or 16): 4 per warp
 
@@ -61,15 +62,15 @@ struct ChainParams {
   const float* x;           // fp32 stream [M, D]
   __nv_bfloat16* xn;        // LayerNorm output [M, D]
   float eps;
-  int wave_lag[2];          // tile order: lag (in 256-row pairs) of the second phase behind the first inside wavefronts {0,1} and {2,3}
+  int wave_lag[2];          // tile order: lag (in 128-row blocks) of the second phase behind the first inside wavefronts {0,1} and {2,3}
   int ln_job_rows;          // rows per LayerNorm job: 16 (two 2-row iterations per warp) or 8 (one)
-  int ln_ctl;               // 1 = the counter polls / publishes of the LayerNorm jobs run on a control warp (warp 9), 0 = on warp 12
+  int ln_ctl;               // 1 = the counter polls / publishes of the LayerNorm jobs run on a control warp (warp 9), 0 = on warp 10
   int rmw;                  // fp32 residual phases: 1 = load + add + store in the generic proxy (gemm.cuh: epilogue_f32_rmw), 0 = TMA reduce-add
   int dbg_nowait;           // measurement only (results may be wrong): publish tiles without waiting for their stores to complete
-  long long* dbg;           // measurement: per cluster [CHAIN_MAX_PHASES][12] cycle counters (leader CTA) or nullptr (8..10: LayerNorm
-                            //   stage s under phase 2s, warp 12: wait for the residual rows, busy, jobs):
-                            //   0 mma busy+wait total, 1 mma wait full (operands), 2 mma wait acc_empty (epilogue), 3 producer dependency wait,
-                            //   4 producer wait empty (ring), 5 epilogue(warp 0) busy, 6 epilogue wait acc_full, 7 tiles
+  long long* dbg;           // measurement: per CTA [CHAIN_MAX_PHASES][12] cycle counters or nullptr (8..10: LayerNorm stage s under
+                            //   phase 2s, warp 10: wait for the residual rows, busy, jobs):
+                            //   1 consumer wait for operands, 3 producer dependency wait, 4 producer wait for ring slots, 5 epilogue
+                            //   (thread 0), 7 tiles, 11 dependency wait of the CTA's first tile of the phase
   ChainPhase ph[CHAIN_MAX_PHASES];
   ChainLn ln[CHAIN_MAX_LN];
 };
@@ -78,19 +79,7 @@ struct alignas(64) ChainMaps {
 };
 
 template <int BN>
-struct ChainCfg {
-  static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-  static constexpr int B_SLICE = BN * GEMM_BK * 2 / GEMM_CL;
-  static constexpr int STAGE_BYTES = A_BYTES + B_SLICE;
-  static constexpr int STAGING = GEMM_EPI_WARPS * GEMM_STAGE_TILE;
-  static constexpr int STAGES_RAW = (227 * 1024 - 2048 - STAGING) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int ACC_STRIDE = BN <= 128 ? 128 : 256;
-  static constexpr int TMEM_COLS = 2 * ACC_STRIDE;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int HALF = BN / 2;
-  static_assert(BN == 256 || BN == 128, "chain tiles");
-};
+using ChainCfg = TileCfg<BN, true>;
 
 // ---------------------------------------------------------------- counters in global memory
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
@@ -110,8 +99,7 @@ __device__ __forceinline__ int ld_relaxed_gpu(const int* p) {
 }
 // Whole warp spins (one coalesced load per probe) until *p >= target.  The probes are RELAXED loads and one acquire fence
 // follows the successful one: an acquire load at gpu scope is compiled to LDG + CCTL.IVALL, i.e. every probe of every waiting
-// warp invalidated the SM's L1 under the epilogue warps' bias loads (ncu source view of the first version: 8 % of all
-// stall samples on that CCTL, and the GELU epilogue three times over its pipe-bound time).
+// warp would invalidate the SM's L1 under the consumer warps' bias loads.
 __device__ __forceinline__ void wait_counter(const int* p, int target) {
   uint32_t spins = 0;
   while (ld_relaxed_gpu(p) < target) {
@@ -192,67 +180,9 @@ __device__ __forceinline__ void chain_ln_rows(const ChainParams& p, const ChainL
   }
 }
 
-// ---------------------------------------------------------------- one tile's epilogue (the TMA epilogues of gemm.cuh)
-template <int BN, int EPI>
-__device__ __forceinline__ void chain_epilogue_tile(uint32_t t_row, int half, int n0, int row0, const float* __restrict__ bias,
-                                                    uint8_t* stile, int lane, const CUtensorMap* tmap_out) {
-  constexpr int HALF = BN / 2;
-  constexpr int COLS = (EPI == EPI_F32_ADD) ? 32 : 64;       // one 128-byte staging row per round
-  const int sw = lane & 7;
-#pragma unroll 1
-  for (int c = 0; c < HALF; c += COLS) {
-    const int col = half * HALF + c;
-    const int n = n0 + col;
-    if (elect_one()) tma_store_wait_read<0>();                // previous store has finished reading the staging tile
-    __syncwarp();
-#pragma unroll
-    for (int sub = 0; sub < COLS; sub += 32) {
-      uint32_t r[32];
-      tmem_ld32(t_row + col + sub, r);
-      tmem_ld_wait();
-      float v[32];
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + n + sub + j));
-        v[j] = __uint_as_float(r[j]) + b4.x; v[j + 1] = __uint_as_float(r[j + 1]) + b4.y;
-        v[j + 2] = __uint_as_float(r[j + 2]) + b4.z; v[j + 3] = __uint_as_float(r[j + 3]) + b4.w;
-      }
-      if constexpr (EPI == EPI_BF16_GELU) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_fast(v[j]);
-      }
-      if constexpr (EPI == EPI_BF16_GELU_ERF) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = gelu_erf_as(v[j]);
-      }
-      uint8_t* srow = stile + lane * 128;                     // staging row = lane, 16-byte chunk index XOR (lane % 8): SWIZZLE_128B
-      if constexpr (EPI == EPI_F32_ADD) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(srow + ((q ^ sw) << 4)) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-      } else {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 w;
-          w.x = pack_bf16(v[8 * q], v[8 * q + 1]); w.y = pack_bf16(v[8 * q + 2], v[8 * q + 3]);
-          w.z = pack_bf16(v[8 * q + 4], v[8 * q + 5]); w.w = pack_bf16(v[8 * q + 6], v[8 * q + 7]);
-          *reinterpret_cast<uint4*>(srow + ((((sub >> 3) + q) ^ sw) << 4)) = w;
-        }
-      }
-    }
-    fence_proxy_async_smem();                                 // staging writes -> visible to the TMA engine
-    __syncwarp();
-    if (elect_one()) {
-      if constexpr (EPI == EPI_F32_ADD) tma_reduce_add_2d(tmap_out, stile, n, row0);
-      else tma_store_2d(tmap_out, stile, n, row0);            // rows past M are clipped by the tensor map
-      tma_store_commit();
-    }
-  }
-}
-
 template <int BN>
-__global__ void __cluster_dims__(GEMM_CL, 1, 1) __launch_bounds__(CHAIN_THREADS, 1)
-gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant__ ChainParams p) {
+__global__ void __launch_bounds__(CHAIN_THREADS, 1)
+gemm_chain_wgmma(const __grid_constant__ ChainMaps maps, const __grid_constant__ ChainParams p) {
   using Cfg = ChainCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -260,48 +190,39 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
   uint8_t* staging = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* acc_full = empty_bar + Cfg::STAGES;     // [2]
-  uint64_t* acc_empty = acc_full + 2;               // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  uint64_t* ln_done = reinterpret_cast<uint64_t*>(tmem_slot + 2);    // [2] LayerNorm warps -> control warp: the job's rows are written
+  uint64_t* ln_done = empty_bar + Cfg::STAGES;      // [2] LayerNorm warps -> control warp: the job's rows are written
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
-  const int cta_rank = static_cast<int>(cluster_ctarank());
-  const int cluster = static_cast<int>(cluster_id_x());
-  const int num_clusters = static_cast<int>(cluster_count_x());
   const int num_m = (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int num_mp = (num_m + GEMM_CL - 1) / GEMM_CL;
-  // Tile list.  Default (lag >= #pairs): PHASE-MAJOR, inside a phase tile = mp * num_n + nb (n fastest).  The general form pairs the
-  // phases into two wavefronts, {0, 1} then {2, 3}: slot s holds the tiles of the first phase for row-block pair s and those of the
-  // second phase for pair s - lag, so that a cluster alternates between a reduce-add phase (proj, fc2: epilogues bound by the
-  // L2's fp32 adds) and its consumer.  Dependencies only point backwards for any lag (tests/test_chain_order.py), but every lag
-  // tried was SLOWER than phase-major (engine.cu: VPB_CHAIN_LAG0/1), so this is kept as a measured experiment only.
+  // Tile list.  Default (lag >= #row blocks): PHASE-MAJOR, inside a phase tile = mt * num_n + nb (n fastest).  The general form pairs
+  // the phases into two wavefronts, {0, 1} then {2, 3}: slot s holds the tiles of the first phase for row block s and those of the
+  // second phase for row block s - lag, so that a CTA alternates between a reduce-add phase (proj, fc2) and its consumer.
+  // Dependencies only point backwards for any lag (tests/test_chain_order.py); kept as an experiment (engine.cu: VPB_CHAIN_LAG0/1).
   int n_of[CHAIN_MAX_PHASES];
 #pragma unroll
   for (int i = 0; i < CHAIN_MAX_PHASES; ++i) n_of[i] = i < p.num_phases ? p.ph[i].N / BN : 0;
-  const int lag0 = p.wave_lag[0] < num_mp ? p.wave_lag[0] : num_mp, lag1 = p.wave_lag[1] < num_mp ? p.wave_lag[1] : num_mp;
-  const int wave0_tiles = num_mp * (n_of[0] + n_of[1]);
-  const int total_tiles = wave0_tiles + num_mp * (n_of[2] + n_of[3]);
-  auto locate = [&](int g, int& ph, int& mp, int& nb) {
+  const int lag0 = p.wave_lag[0] < num_m ? p.wave_lag[0] : num_m, lag1 = p.wave_lag[1] < num_m ? p.wave_lag[1] : num_m;
+  const int wave0_tiles = num_m * (n_of[0] + n_of[1]);
+  const int total_tiles = wave0_tiles + num_m * (n_of[2] + n_of[3]);
+  auto locate = [&](int g, int& ph, int& mt, int& nb) {
     const bool w1 = g >= wave0_tiles;
     const int gg = w1 ? g - wave0_tiles : g;
     const int na = w1 ? n_of[2] : n_of[0], nbb = w1 ? n_of[3] : n_of[1];
-    const int lag = nbb == 0 ? num_mp : (w1 ? lag1 : lag0);
+    const int lag = nbb == 0 ? num_m : (w1 ? lag1 : lag0);
     const int pa = w1 ? 2 : 0;
     const int head = na * lag;                               // slots [0, lag): first phase only
-    const int mid = (num_mp - lag) * (na + nbb);             // slots [lag, num_mp): both
-    if (gg < head) { ph = pa; mp = gg / na; nb = gg % na; }
+    const int mid = (num_m - lag) * (na + nbb);              // slots [lag, num_m): both
+    if (gg < head) { ph = pa; mt = gg / na; nb = gg % na; }
     else if (gg < head + mid) {
       const int q = gg - head, s = lag + q / (na + nbb), r = q % (na + nbb);
-      if (r < na) { ph = pa; mp = s; nb = r; }
-      else { ph = pa + 1; mp = s - lag; nb = r - na; }
+      if (r < na) { ph = pa; mt = s; nb = r; }
+      else { ph = pa + 1; mt = s - lag; nb = r - na; }
     } else {
-      const int q = gg - head - mid;                         // slots [num_mp, num_mp + lag): second phase only
-      ph = pa + 1; mp = num_mp - lag + q / nbb; nb = q % nbb;
+      const int q = gg - head - mid;                         // slots [num_m, num_m + lag): second phase only
+      ph = pa + 1; mt = num_m - lag + q / nbb; nb = q % nbb;
     }
   };
-  constexpr uint16_t kAllCtas = (1u << GEMM_CL) - 1;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.num_phases; ++i) {
@@ -311,164 +232,96 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
     }
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], GEMM_CONSUMER_WARPS);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], GEMM_CL * GEMM_EPI_WARPS);
-      mbar_init(&ln_done[s], CHAIN_LN_WARPS);
-    }
+    for (int s = 0; s < 2; ++s) mbar_init(&ln_done[s], CHAIN_LN_WARPS);
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc_pair(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before_sync();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = uniform_u32(*tmem_slot);
+  __syncthreads();
   pdl_launch_dependents();
   pdl_wait();                                       // the previous kernel's outputs (first phase's A operand, x) are complete
 
-  if (warp == 10) {
+  if (warp == 8) {
     // ------------------------------------------------------------ TMA producer (+ the waits that replace kernel boundaries)
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos rp;
     int prev_ph = -1;
-    for (int g = cluster; g < total_tiles; g += num_clusters) {
-      int ph, mp, nb;
-      locate(g, ph, mp, nb);
+    for (int g = blockIdx.x; g < total_tiles; g += gridDim.x) {
+      int ph, mt, nb;
+      locate(g, ph, mt, nb);
       const ChainPhase& P = p.ph[ph];
-      const int mt = mp * GEMM_CL + cta_rank;
       const int m0 = mt * GEMM_BM, n0 = nb * BN;
       const bool first_of_phase = ph != prev_ph;
       prev_ph = ph;
       const int num_kb = P.K / GEMM_BK;
       long long c0 = p.dbg ? clock64() : 0, w_dep = 0, w_ring = 0;
-      if (P.a_ready != nullptr && mt < num_m) {
+      if (P.a_ready != nullptr) {
         wait_counter(P.a_ready + mt, P.a_target > 0 ? P.a_target : chain_ln_jobs_in_block(p.M, mt, p.ln_job_rows));
         fence_proxy_async_all();                    // the rows were written through the generic / async proxy of other SMs
       }
       if (p.dbg) w_dep = clock64() - c0;
       for (int kb = 0; kb < num_kb; ++kb) {
         if (p.dbg) c0 = clock64();
-        mbar_wait(&empty_bar[stage], phase ^ 1);
+        ring_wait_slot(empty_bar, rp);
         if (p.dbg) w_ring += clock64() - c0;
-        uint8_t* sa = ring + stage * Cfg::STAGE_BYTES;
+        uint8_t* sa = ring + rp.stage * Cfg::STAGE_BYTES;
         if (elect_one()) {
-          if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], GEMM_CL * Cfg::STAGE_BYTES);
-          tma_load_2d_pair(sa, &maps.a[ph], &full_bar[stage], kb * GEMM_BK, m0);
-          tma_load_2d_pair(sa + Cfg::A_BYTES, &maps.w[ph], &full_bar[stage], kb * GEMM_BK, n0 + cta_rank * (BN / GEMM_CL));
+          mbar_expect_tx(&full_bar[rp.stage], Cfg::STAGE_BYTES);
+          tma_load_2d(sa, &maps.a[ph], &full_bar[rp.stage], kb * GEMM_BK, m0);
+          tma_load_2d(sa + Cfg::A_BYTES, &maps.w[ph], &full_bar[rp.stage], kb * GEMM_BK, n0);
         }
         __syncwarp();
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (p.dbg && cta_rank == 0 && lane == 0) {
-        p.dbg[(cluster * CHAIN_MAX_PHASES + ph) * 12 + 3] += w_dep;
-        if (first_of_phase) p.dbg[(cluster * CHAIN_MAX_PHASES + ph) * 12 + 11] += w_dep;      // of which: this cluster's first tile of the phase
-        p.dbg[(cluster * CHAIN_MAX_PHASES + ph) * 12 + 4] += w_ring;
-      }
-    }
-  } else if (warp == 11 && cta_rank == 0) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA of the pair only)
-    constexpr uint32_t idesc = umma_idesc_bf16(GEMM_CL * GEMM_BM, BN);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int g = cluster; g < total_tiles; g += num_clusters, ++it) {
-      int ph, mp, nb;
-      locate(g, ph, mp, nb);
-      const int num_kb = p.ph[ph].K / GEMM_BK;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const long long t0 = p.dbg ? clock64() : 0;
-      long long w_full = 0, c0 = 0;
-      mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-      const long long w_acc = p.dbg ? clock64() - t0 : 0;
-      tc_fence_after_sync();
-      const uint32_t d_tmem = tmem_base + acc * Cfg::ACC_STRIDE;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        if (p.dbg) c0 = clock64();
-        mbar_wait(&full_bar[stage], phase);
-        if (p.dbg) w_full += clock64() - c0;
-        tc_fence_after_sync();
-        const uint32_t sa = smem_u32(ring + stage * Cfg::STAGE_BYTES);
-        const uint64_t adesc = umma_desc_sw128(sa, 1024);
-        const uint64_t bdesc = umma_desc_sw128(sa + Cfg::A_BYTES, 1024);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) umma_bf16_pair(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-          umma_commit_pair(&empty_bar[stage], kAllCtas);
-          if (kb == num_kb - 1) umma_commit_pair(&acc_full[acc], kAllCtas);
-        }
-        __syncwarp();
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+        rp.next(Cfg::STAGES);
       }
       if (p.dbg && lane == 0) {
-        long long* d = p.dbg + (cluster * CHAIN_MAX_PHASES + ph) * 12;
-        d[0] += clock64() - t0; d[1] += w_full; d[2] += w_acc; d[7] += 1;
+        long long* d = p.dbg + (blockIdx.x * CHAIN_MAX_PHASES + ph) * 12;
+        d[3] += w_dep;
+        if (first_of_phase) d[11] += w_dep;
+        d[4] += w_ring;
       }
     }
-  } else if (warp < GEMM_EPI_WARPS) {
-    // ------------------------------------------------------------ epilogue
-    const int quarter = warp & 3;
-    const int half = warp >> 2;
-    uint8_t* stile = staging + warp * GEMM_STAGE_TILE;
-    int it = 0;
-    for (int g = cluster; g < total_tiles; g += num_clusters, ++it) {
-      int ph, mp, nb;
-      locate(g, ph, mp, nb);
+  } else if (warp < GEMM_CONSUMER_WARPS) {
+    // ------------------------------------------------------------ consumers: MMA + epilogue
+    const int wg = warp >> 2;
+    const int tid = threadIdx.x & 127;
+    uint8_t* stiles = staging + wg * 2 * GEMM_STAGE_TILE;
+    RingPos rp;
+    float acc[BN / 2];
+    for (int g = blockIdx.x; g < total_tiles; g += gridDim.x) {
+      int ph, mt, nb;
+      locate(g, ph, mt, nb);
       const ChainPhase& P = p.ph[ph];
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int mt = mp * GEMM_CL + cta_rank;
-      const int row0 = mt * GEMM_BM + quarter * 32;
+      const int n0 = nb * BN, row0 = mt * GEMM_BM + 64 * wg;
+      long long w_full = 0;
+      tile_mainloop<BN>(acc, ring, Cfg::STAGE_BYTES, full_bar, empty_bar, P.K / GEMM_BK, Cfg::STAGES, rp, wg, lane,
+                        (p.dbg && threadIdx.x == 0) ? &w_full : nullptr);
       const long long e0 = p.dbg ? clock64() : 0;
-      // load + add + store form of the residual phases: the warp's first 32 x 32 box of x.  Rows last written by an earlier launch
-      // (no residual phase before this one in the launch) are requested before the accumulator is ready.
-      const bool rmw = p.rmw != 0 && P.epi == EPI_F32_ADD;
-      const int x_col0 = nb * BN + half * Cfg::HALF;
-      bool x_early = rmw;
-      for (int j = 0; j < ph; ++j) x_early = x_early && p.ph[j].epi != EPI_F32_ADD;
-      float4 xr[8];
-      if (x_early) rmw_load_box(xr, p.x, p.D, row0, lane, p.M, x_col0);
-      mbar_wait(&acc_full[acc], acc_phase);
-      const long long e1 = p.dbg ? clock64() : 0;
-      tc_fence_after_sync();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * Cfg::ACC_STRIDE;
-      if (rmw) {
-        if (!x_early) rmw_load_box(xr, p.x, p.D, row0, lane, p.M, x_col0);
-        epilogue_f32_rmw<Cfg::HALF / 32>(t_row + half * Cfg::HALF, x_col0, row0, p.M, P.bias, const_cast<float*>(p.x), p.D, xr, stile, lane);
-      } else if (P.epi == EPI_F32_ADD) chain_epilogue_tile<BN, EPI_F32_ADD>(t_row, half, nb * BN, row0, P.bias, stile, lane, &maps.out[ph]);
-      else if (P.epi == EPI_BF16_GELU) chain_epilogue_tile<BN, EPI_BF16_GELU>(t_row, half, nb * BN, row0, P.bias, stile, lane, &maps.out[ph]);
-      else if (P.epi == EPI_BF16_GELU_ERF) chain_epilogue_tile<BN, EPI_BF16_GELU_ERF>(t_row, half, nb * BN, row0, P.bias, stile, lane, &maps.out[ph]);
-      else chain_epilogue_tile<BN, EPI_BF16>(t_row, half, nb * BN, row0, P.bias, stile, lane, &maps.out[ph]);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&acc_empty[acc], 0);   // TMEM is free for the MMA thread; the stores may still be in flight
+      if (P.epi == EPI_F32_ADD && p.rmw) epilogue_f32_rmw<BN>(acc, n0, row0, p.M, P.bias, const_cast<float*>(p.x), p.D, tid);
+      else if (P.epi == EPI_F32_ADD) epilogue_tma<BN, EPI_F32_ADD>(acc, n0, row0, P.N, P.bias, stiles, wg, tid, &maps.out[ph]);
+      else if (P.epi == EPI_BF16_GELU) epilogue_tma<BN, EPI_BF16_GELU>(acc, n0, row0, P.N, P.bias, stiles, wg, tid, &maps.out[ph]);
+      else if (P.epi == EPI_BF16_GELU_ERF) epilogue_tma<BN, EPI_BF16_GELU_ERF>(acc, n0, row0, P.N, P.bias, stiles, wg, tid, &maps.out[ph]);
+      else epilogue_tma<BN, EPI_BF16>(acc, n0, row0, P.N, P.bias, stiles, wg, tid, &maps.out[ph]);
       if (P.out_done != nullptr) {
-        // publish the tile ONCE per CTA: every epilogue warp waits until its own stores / reduce-adds have been PERFORMED (not
-        // just read out of smem) and fences them across the proxies; the eight warps meet on a named barrier; one thread
-        // does the gpu-scope release on the row block's counter.  (First version: fence + release per warp = eight
-        // MEMBAR.GPU / ERRBAR / CCTL.IVALL sequences per tile -- 15 % of the kernel's stall samples.)
-        if (elect_one()) {
+        // publish the tile ONCE per CTA: each warpgroup's issuing thread waits until its stores / reduce-adds have been
+        // PERFORMED (not just read out of smem) and fences them across the proxies (the load + add + store form's plain stores
+        // are ordered by the release below); the two warpgroups meet on a named barrier; one thread does the gpu-scope release
+        if (tid == 0) {
           if (!p.dbg_nowait) tma_store_wait_all<0>();
           fence_proxy_async_all();
         }
-        __syncwarp();
-        asm volatile("bar.sync 3, 256;" ::: "memory");
-        if (warp == 0 && mt < num_m && elect_one()) red_release_gpu_add(P.out_done + mt, 1);
+        named_bar_sync(GEMM_BAR_EPI, 256);
+        if (threadIdx.x == 0) red_release_gpu_add(P.out_done + mt, 1);
       }
-      if (p.dbg && warp == 0 && lane == 0 && cta_rank == 0) {
-        long long* d = p.dbg + (cluster * CHAIN_MAX_PHASES + ph) * 12;
-        d[5] += clock64() - e1; d[6] += e1 - e0;
+      if (p.dbg && threadIdx.x == 0) {
+        long long* d = p.dbg + (blockIdx.x * CHAIN_MAX_PHASES + ph) * 12;
+        d[1] += w_full; d[5] += clock64() - e0; d[7] += 1;
       }
     }
-    if (elect_one()) tma_store_wait_all<0>();
+    if (tid == 0) tma_store_wait_all<0>();
   } else if (warp == 9 && p.ln_ctl != 0) {
     // ------------------------------------------------------------ LayerNorm control warp
     // The gpu-scope fences around a job -- the acquire after the poll of the residual phase's counter, fence.proxy.async +
-    // red.release to publish the normalised rows -- cost the LayerNorm warps ~3 k of the ~10.5 k cycles a job takes them
-    // (tools/chain_diag.py), and the LayerNorm stages are what the consumer phases wait for (fc1 / qkv dependency waits: a quarter
-    // of a chained launch).  This warp takes both over: it walks the CTA's job list (job j -> CTA j mod grid, stage-major), polls
+    // red.release to publish the normalised rows -- are latency the LayerNorm warps would otherwise sit in, and the LayerNorm
+    // stages are what the consumer phases wait for.  This warp takes both over: it walks the CTA's job list (job j -> CTA j mod grid, stage-major), polls
     // job i + 1 while the LayerNorm warps work on job i and publishes job i when they have arrived on ln_done.  Two slots each
     // way (slot = job sequence number & 1; "ready": named barriers 4 / 5, "done": mbarriers); "ready" for job i + 2 is only
     // signalled after "done" of job i was seen, so neither barrier can run a phase ahead.  Neither probe blocks: the first job of stage 1 waits for fc2 tiles that may
@@ -488,9 +341,8 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
           asm volatile("fence.acq_rel.gpu;" ::: "memory");
           __syncwarp();
           // "ready" is a NAMED barrier (ids 4 / 5 by slot, 4 LayerNorm warps + this one): the LayerNorm warps sleep in
-          // bar.sync without taking issue slots.  First version: an mbarrier they polled with try_wait -- four more spinning
-          // warps per SM, the epilogue warps sharing their schedulers lost 15 % (fc1 epilogue 8.8 k -> 10.3 k cycles per tile)
-          // and the MMA thread's accumulator waits rose from 5 % to 19 % of the fc1 phase, which ate the gain.
+          // bar.sync without taking issue slots (polling an mbarrier with try_wait would add four spinning warps per SM
+          // that share schedulers with the consumer warps).
           if (a_seq & 1) asm volatile("bar.arrive 5, 160;" ::: "memory");
           else asm volatile("bar.arrive 4, 160;" ::: "memory");
           ++a_seq;
@@ -516,9 +368,9 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
         if (++idle > (VPB_HANG_TRAP_SPINS >> 3)) __trap();
       }
     }
-  } else if (warp >= 12) {
+  } else if (warp >= 10) {
     // ------------------------------------------------------------ LayerNorm jobs
-    const int lw = warp - 12;
+    const int lw = warp - 10;
     const int jobs = (p.M + p.ln_job_rows - 1) / p.ln_job_rows;
     const int ROWS_PER_WARP = p.ln_job_rows / CHAIN_LN_WARPS;
     const bool ctl = p.ln_ctl != 0;                  // polls / publishes on the control warp (warp 9)
@@ -546,8 +398,8 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
           case 1024: chain_ln_rows<8>(p, L, r0, r1, lane); break;
           default: chain_ln_rows<10>(p, L, r0, r1, lane); break;     // 1280
         }
-        // one gpu-scope release per job and CTA (a MEMBAR.GPU on an SM with TMA traffic in flight costs thousands of cycles):
-        // the four warps meet on a named barrier (orders their row stores before the releasing thread), warp 12 publishes
+        // one gpu-scope release per job and CTA (a gpu-scope fence on an SM with TMA traffic in flight is expensive):
+        // the four warps meet on a named barrier (orders their row stores before the releasing thread), warp 10 publishes
         const long long l2 = p.dbg ? clock64() : 0;
         if (ctl) {
           __syncwarp();                                                // every lane's row stores precede the arrive
@@ -560,8 +412,8 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
           fence_proxy_async_all();                                     // consumed by TMA loads (async proxy) of other SMs
           red_release_gpu_add(L.ready + mt, 1);
         }
-        if (p.dbg && lw == 0 && lane == 0 && cta_rank == 0) {
-          long long* d = p.dbg + (cluster * CHAIN_MAX_PHASES + 2 * s) * 12;
+        if (p.dbg && lw == 0 && lane == 0) {
+          long long* d = p.dbg + (blockIdx.x * CHAIN_MAX_PHASES + 2 * s) * 12;
           const long long l4 = clock64();
           d[8] += l1 - l0; d[9] += l4 - l1; d[10] += 1;
           long long* e = d + 12;                                       // breakdown of the busy part, stored under the next phase's slots 8..10
@@ -571,9 +423,6 @@ gemm_chain_tcgen05(const __grid_constant__ ChainMaps maps, const __grid_constant
     }
   }
 
-  tc_fence_before_sync();
-  cluster_sync_all();
-  if (warp == 8) tmem_dealloc_pair(tmem_base, Cfg::TMEM_COLS);
 }
 
 }  // namespace vpb

@@ -102,8 +102,8 @@ __device__ __forceinline__ void transform_cs(float xr, float yr, int n_i, const 
   }
 }
 
-// warps (= maps) per CTA: 4 gives 272 CTAs for 64 x 17 maps (two per SM, 8 warps with 24 16-byte loads each in flight) where 8
-// left 12 of the 148 SMs idle and one CTA per SM
+// warps (= maps) per CTA: 4 gives 272 CTAs for 64 x 17 maps, i.e. about two per SM with 8 warps of 16-byte loads in flight;
+// wider CTAs would leave SMs idle at this size
 // GENERIC = false: the 11x11 kernel every reference config uses, taps and trip counts compiled in (the engine's hot path);
 // GENERIC = true: radius and taps from p.taps.
 constexpr int DECODE_WARPS = 4;
@@ -122,8 +122,7 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_heatmaps(const Decod
 
   // ---- first-index argmax over 3072 values.  The scan is branch-free so that the loads can run ahead of it (ptxas keeps a
   // rolling window of seven 16-byte loads per lane in flight): the first version's early-return comparison compiled to
-  // divergent branches between the loads, which left ONE load in flight per lane (ncu source view: 24 serial DRAM round
-  // trips = 19 of the kernel's 23 us).  A lane sees its elements in increasing index order, so "first index wins"
+  // divergent branches between the loads, which left ONE load in flight per lane.  A lane sees its elements in increasing index order, so "first index wins"
   // is "replace only when strictly better"; a NaN replaces a number and is never replaced (np.argmax: the first NaN).
   float bv;
   int bi;

@@ -19,7 +19,6 @@
 
 #include "../../include/vitpose_b200.h"
 #include "attention.cuh"
-#include "attention_pack.cuh"
 #include "chain.cuh"
 #include "decode.cuh"
 #include "gemm.cuh"
@@ -107,7 +106,7 @@ static long long* g_dbg_buf = nullptr;
 // reduce-add.  Bit-identical; process default from VPB_RESID_RMW, per engine through option "resid_rmw"; the debug flags 32 / 64
 // of vpb_debug_gemm force one form for every following launch (kernel-level tests).
 constexpr int kResidRmwDefault = 0;
-constexpr int kLnCtlDefault = 1;      // measured on B200 (ViT-B, 64 crops): 2.308 -> 2.245 ms per step, bit-identical
+constexpr int kLnCtlDefault = 1;      // bit-identical either way (tests/test_gpu_engine.py)
 static int resid_rmw_default() {
   static const int v = [] { const char* s = getenv("VPB_RESID_RMW"); return s ? (s[0] != '0') : kResidRmwDefault; }();
   return v;
@@ -148,13 +147,12 @@ static int num_sms() { return cur_dev()->sms; }
 
 // ------------------------------------------------------------------------------------------------ GEMM dispatch
 
-// `tout` is the output tensor map of the TMA epilogues (EPI_BF16, EPI_BF16_GELU: bf16 box 64x32; EPI_F32_ADD: f32 box
-// 32x32); direct epilogues ignore it (pass any valid map).  W maps carry boxes of BN/2 rows: each CTA of the pair
-// fetches half of the W tile and multicasts it.
+// `tout` is the output tensor map of the TMA epilogues (EPI_BF16, EPI_BF16_GELU: bf16 box 64 columns x 64 rows; EPI_F32_ADD:
+// f32 box 32 x 64); direct epilogues ignore it (pass any valid map).  W maps carry boxes of BN rows.
 template <int BN, int EPI>
 static int gemm_launch_t(const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tout, const GemmParams& p, cudaStream_t st) {
   using Cfg = GemmCfg<BN, EPI>;
-  auto kern = gemm_bf16_tcgen05<BN, EPI>;
+  auto kern = gemm_bf16_wgmma<BN, EPI>;
   DeviceState* ds = cur_dev();
   if (ds->sms == 0) return fail(VPB_ERR_STATE, "gemm: device not initialised (device_check)");
   constexpr unsigned slot = 1u << ((EPI == EPI_BF16_GELU_ERF ? 3 : EPI) * 4 + (BN == 256 ? 0 : BN == 128 ? 1 : BN == 144 ? 2 : 3));
@@ -164,9 +162,8 @@ static int gemm_launch_t(const CUtensorMap& ta, const CUtensorMap& tw, const CUt
   }
   const bool deconv = (EPI == EPI_BF16_RELU_UP);
   const int num_m = deconv ? p.M / (p.up_tr * p.up_tw) : (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int pairs = ((num_m + GEMM_CL - 1) / GEMM_CL) * (deconv ? 4 : (p.N + BN - 1) / BN);
-  const int max_clusters = ds->sms / GEMM_CL;
-  const int grid = GEMM_CL * (pairs < max_clusters ? pairs : max_clusters);
+  const int tiles = num_m * (deconv ? 4 : (p.N + BN - 1) / BN);
+  const int grid = tiles < ds->sms ? tiles : ds->sms;
   CU_TRY(launch_k(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, ta, tw, tout, p));
   return VPB_OK;
 }
@@ -194,18 +191,14 @@ static int device_check(int device) {
   if (ds->sms > 0 && ds->attn_attr) return VPB_OK;
   cudaDeviceProp prop;
   CU_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(VPB_ERR_ARG, "device %d is sm_%d%d; this library only runs on sm_100 (B200), no fallback", device,
+  if (prop.major != 9 || prop.minor != 0) return fail(VPB_ERR_ARG, "device %d is sm_%d%d; this library only runs on sm_90 (H100), no fallback", device,
                                     prop.major, prop.minor);
-  CU_TRY(cudaFuncSetAttribute(attention_tcgen05<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<32>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_tcgen05<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<64>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_tcgen05<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<80>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_tcgen05<32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<32>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_tcgen05<64, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<64>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_tcgen05<80, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<80>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_pack_tcgen05<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttPackCfg<32>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_pack_tcgen05<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttPackCfg<64>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_pack_tcgen05<32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttPackCfg<32>::SMEM));
-  CU_TRY(cudaFuncSetAttribute(attention_pack_tcgen05<64, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttPackCfg<64>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(attention_wgmma<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<32>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(attention_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<64>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(attention_wgmma<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<80>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(attention_wgmma<32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<32>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(attention_wgmma<64, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<64>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(attention_wgmma<80, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<80>::SMEM));
   ds->attn_attr = true;
   ds->sms = prop.multiProcessorCount;
   return VPB_OK;
@@ -215,7 +208,7 @@ static int device_check(int device) {
 template <int BN>
 static int chain_launch_t(const ChainMaps& maps, const ChainParams& p, cudaStream_t st) {
   using Cfg = ChainCfg<BN>;
-  auto kern = gemm_chain_tcgen05<BN>;
+  auto kern = gemm_chain_wgmma<BN>;
   DeviceState* ds = cur_dev();
   if (ds->sms == 0) return fail(VPB_ERR_STATE, "chain: device not initialised (device_check)");
   constexpr unsigned slot = BN == 256 ? (1u << 30) : (1u << 31);
@@ -223,54 +216,46 @@ static int chain_launch_t(const ChainMaps& maps, const ChainParams& p, cudaStrea
     CU_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     ds->gemm_attr |= slot;
   }
-  const int num_m = (p.M + GEMM_BM - 1) / GEMM_BM, num_mp = (num_m + GEMM_CL - 1) / GEMM_CL;
+  const int num_m = (p.M + GEMM_BM - 1) / GEMM_BM;
   int tiles = 0;
   for (int i = 0; i < p.num_phases; ++i) {
     if (p.ph[i].N % BN != 0 || p.ph[i].K % GEMM_BK != 0 || p.ph[i].bias == nullptr)
       return fail(VPB_ERR_ARG, "chain: phase %d N=%d K=%d does not tile by %d x 64", i, p.ph[i].N, p.ph[i].K, BN);
-    tiles += num_mp * (p.ph[i].N / BN);
+    tiles += num_m * (p.ph[i].N / BN);
   }
-  // every cluster of the grid must be resident at once: the in-kernel waits rely on it.  Ask the runtime how many 2-CTA
-  // clusters of this kernel the device can hold (74 on a whole B200) instead of assuming #SMs / 2.
+  // every CTA of the grid must be resident at once: the in-kernel waits rely on it.  Ask the runtime how many CTAs of this
+  // kernel an SM can hold instead of assuming one.
   static int max_active[kMaxDevices] = {0};
   int dev_id = 0;
   CU_TRY(cudaGetDevice(&dev_id));
   if (max_active[dev_id] == 0) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(ds->sms); cfg.blockDim = dim3(CHAIN_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n < 1) { cudaGetLastError(); n = ds->sms / GEMM_CL; }
-    max_active[dev_id] = n < ds->sms / GEMM_CL ? n : ds->sms / GEMM_CL;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, CHAIN_THREADS, Cfg::SMEM_BYTES) != cudaSuccess || n < 1) { cudaGetLastError(); n = 1; }
+    max_active[dev_id] = n * ds->sms;
   }
-  const int max_clusters = max_active[dev_id];
-  const int grid = GEMM_CL * (tiles < max_clusters ? tiles : max_clusters);
+  const int grid = tiles < max_active[dev_id] ? tiles : max_active[dev_id];
   CU_TRY(launch_k(kern, dim3(grid), dim3(CHAIN_THREADS), Cfg::SMEM_BYTES, st, maps, p));
   return VPB_OK;
 }
 static int chain_launch(int bn, const ChainMaps& maps, const ChainParams& p, cudaStream_t st) {
   if (p.num_phases < 1 || p.num_phases > CHAIN_MAX_PHASES || p.num_ln < 0 || p.num_ln > CHAIN_MAX_LN) return fail(VPB_ERR_ARG, "chain: bad phase count");
   if (p.D != 384 && p.D != 768 && p.D != 1024 && p.D != 1280) return fail(VPB_ERR_ARG, "chain: LayerNorm width %d not instantiated", p.D);
-  return bn == 256 ? chain_launch_t<256>(maps, p, st) : chain_launch_t<128>(maps, p, st);
+  if (bn != 128) return fail(VPB_ERR_ARG, "chain: tile width %d not built (128)", bn);
+  return chain_launch_t<128>(maps, p, st);
 }
 
 // ------------------------------------------------------------------------------------------------ attention dispatch
-// Attention variants (process-wide switches; environment at load time, or vpb_debug_attention() for A/B runs in one process):
-//   pack  attention_pack.cuh: the 64-row half tiles of two heads share one 128-lane pass (head_dim 32 / 64, an even number of
-//         items).  Default ON (VPB_ATT_PACK=0 switches it off): bit-identical to attention.cuh with the same exponentials.
+// Attention variant (process-wide switch; environment at load time, or vpb_debug_attention() for A/B runs in one process):
 //   poly  every 4th softmax exponential on the FMA pipe (ex2_poly, 7.5e-5 relative error, far below P's bf16 rounding) instead
-//         of the MUFU.  Default: ON in the packed kernel, where both softmax groups are always live and the MUFU bounds the
-//         exponential phase (ViT-B, 64 crops: 22.3 -> 17.8 us per launch), OFF in attention.cuh (no gain inside the step);
-//         VPB_ATT_POLY=0/1 forces it for both.
-static int g_att_poly = [] { const char* e = getenv("VPB_ATT_POLY"); return !e ? -1 : (e[0] == '1' ? 1 : 0); }();    // -1 = per kernel default
-static int g_att_pack = [] { const char* e = getenv("VPB_ATT_PACK"); return (e && e[0] == '0') ? 0 : 1; }();
-static const int g_att_poly_env = g_att_poly, g_att_pack_env = g_att_pack;
-static int g_att_grid_cap = 0;      // tests: launch the attention kernels with at most this many CTAs (0 = one per SM)
-// flags < 0: back to the defaults (environment); else bit 0 = poly, bit 1 = pack, bits 8.. = grid cap (how a device with fewer
-// SMs would split the steps: other range boundaries inside the pairs of the packed kernel)
+//         of the MUFU.  Default OFF; VPB_ATT_POLY=1 switches it on.
+static int g_att_poly = [] { const char* e = getenv("VPB_ATT_POLY"); return (e && e[0] == '1') ? 1 : 0; }();
+static const int g_att_poly_env = g_att_poly;
+static int g_att_grid_cap = 0;      // tests: launch the attention kernel with at most this many CTAs (0 = one per SM)
+// flags < 0: back to the defaults (environment); else bit 0 = poly, bits 8.. = grid cap (how a device with fewer SMs would split
+// the items)
 extern "C" int vpb_debug_attention(int32_t flags) {
-  if (flags < 0) { g_att_poly = g_att_poly_env; g_att_pack = g_att_pack_env; g_att_grid_cap = 0; }
-  else { g_att_poly = (flags & 1) ? 1 : 0; g_att_pack = (flags & 2) ? 1 : 0; g_att_grid_cap = flags >> 8; }
+  if (flags < 0) { g_att_poly = g_att_poly_env; g_att_grid_cap = 0; }
+  else { g_att_poly = (flags & 1) ? 1 : 0; g_att_grid_cap = flags >> 8; }
   return VPB_OK;
 }
 
@@ -285,27 +270,20 @@ static int make_attn_maps(CUtensorMap* main, CUtensorMap* tail, const void* qkv,
 static int attention_launch(int hd, const CUtensorMap& main, const CUtensorMap& tail, const AttnParams& ap, cudaStream_t st) {
   const int items = ap.batch * ap.heads;
   const int sms = (g_att_grid_cap > 0 && g_att_grid_cap < num_sms()) ? g_att_grid_cap : num_sms();
-  const dim3 grid(items < sms ? items : sms);      // one CTA per SM (512 TMEM columns each)
+  const dim3 grid(items < sms ? items : sms);      // one CTA per SM (two stages of Q, K, V fill the shared memory)
   cudaError_t err;
-  const bool pack = g_att_pack && hd <= 64 && items % 2 == 0;
-  const bool poly = g_att_poly < 0 ? pack : g_att_poly != 0;
-  if (pack) {
-    if (hd == 64) err = poly ? launch_k(attention_pack_tcgen05<64, 8>, grid, dim3(ATT_THREADS), AttPackCfg<64>::SMEM, st, main, ap)
-                                   : launch_k(attention_pack_tcgen05<64>, grid, dim3(ATT_THREADS), AttPackCfg<64>::SMEM, st, main, ap);
-    else err = poly ? launch_k(attention_pack_tcgen05<32, 8>, grid, dim3(ATT_THREADS), AttPackCfg<32>::SMEM, st, main, ap)
-                          : launch_k(attention_pack_tcgen05<32>, grid, dim3(ATT_THREADS), AttPackCfg<32>::SMEM, st, main, ap);
-  } else if (poly) {
+  if (g_att_poly) {
     switch (hd) {
-      case 32: err = launch_k(attention_tcgen05<32, 8>, grid, dim3(ATT_THREADS), AttCfg<32>::SMEM, st, main, tail, ap); break;
-      case 64: err = launch_k(attention_tcgen05<64, 8>, grid, dim3(ATT_THREADS), AttCfg<64>::SMEM, st, main, tail, ap); break;
-      case 80: err = launch_k(attention_tcgen05<80, 8>, grid, dim3(ATT_THREADS), AttCfg<80>::SMEM, st, main, tail, ap); break;
+      case 32: err = launch_k(attention_wgmma<32, 8>, grid, dim3(ATT_THREADS), AttCfg<32>::SMEM, st, main, tail, ap); break;
+      case 64: err = launch_k(attention_wgmma<64, 8>, grid, dim3(ATT_THREADS), AttCfg<64>::SMEM, st, main, tail, ap); break;
+      case 80: err = launch_k(attention_wgmma<80, 8>, grid, dim3(ATT_THREADS), AttCfg<80>::SMEM, st, main, tail, ap); break;
       default: return fail(VPB_ERR_ARG, "attention: head_dim %d not built (32, 64, 80)", hd);
     }
   } else {
     switch (hd) {
-      case 32: err = launch_k(attention_tcgen05<32>, grid, dim3(ATT_THREADS), AttCfg<32>::SMEM, st, main, tail, ap); break;
-      case 64: err = launch_k(attention_tcgen05<64>, grid, dim3(ATT_THREADS), AttCfg<64>::SMEM, st, main, tail, ap); break;
-      case 80: err = launch_k(attention_tcgen05<80>, grid, dim3(ATT_THREADS), AttCfg<80>::SMEM, st, main, tail, ap); break;
+      case 32: err = launch_k(attention_wgmma<32>, grid, dim3(ATT_THREADS), AttCfg<32>::SMEM, st, main, tail, ap); break;
+      case 64: err = launch_k(attention_wgmma<64>, grid, dim3(ATT_THREADS), AttCfg<64>::SMEM, st, main, tail, ap); break;
+      case 80: err = launch_k(attention_wgmma<80>, grid, dim3(ATT_THREADS), AttCfg<80>::SMEM, st, main, tail, ap); break;
       default: return fail(VPB_ERR_ARG, "attention: head_dim %d not built (32, 64, 80)", hd);
     }
   }
@@ -344,9 +322,9 @@ struct LinearW {
   __nv_bfloat16* w = nullptr;   // [N,K] bf16
   float* b = nullptr;           // [N padded]
   int n = 0, k = 0, bn = 0;
-  CUtensorMap map;              // W boxes of bn / 2 rows (the standalone GEMM's tile width for this N)
-  CUtensorMap map_c;            // W boxes of chain_bn / 2 rows (every phase of a chained launch uses one tile width)
-  CUtensorMap map128;           // W boxes of 64 rows: 128-wide tiles for small batches (pick_bn); valid when n_pad % 128 == 0
+  CUtensorMap map;              // W boxes of bn rows (the standalone GEMM's tile width for this N)
+  CUtensorMap map_c;            // W boxes of chain_bn rows (every phase of a chained launch uses one tile width)
+  CUtensorMap map128;           // W boxes of 128 rows: 128-wide tiles for small batches (pick_tile); valid when n_pad % 128 == 0
   bool has128 = false;
 };
 struct BlockW {
@@ -367,8 +345,9 @@ struct vpb_engine {
   std::vector<GraphEntry> graphs;
   bool use_graph = true;
   // L2 residency: the fp32 token stream x (37.7 MB at B=64) is read-modify-written by every residual GEMM and read by every
-  // LayerNorm, but the per-layer working set (~220 MB) would evict it from the 126 MB L2 in between; an access-policy window
-  // marks it persisting on every stream the engine launches on.
+  // LayerNorm, but the per-layer working set (~220 MB) would evict it from the 50 MB L2 in between; an access-policy window
+  // (clipped to what the device allows to persist) marks it persisting on every stream the engine launches on.  Measured on an
+  // H100 80GB HBM3 (700 W power limit), ViT-B, 64 crops: 9.39 ms per call with the window, 10.52 without (tools/defaults_ab.py).
   bool l2_persist = true;
   size_t l2_window_bytes = 0;
   std::vector<cudaStream_t> l2_streams;
@@ -392,29 +371,29 @@ struct vpb_engine {
   __nv_bfloat16 *patch_rows, *xn, *qkv, *attn, *hid, *d1, *d2;
   float *x, *heat;
   int* ln_counters = nullptr;      // one per 128-row block of x (fused LayerNorm tail of the residual GEMMs)
-  // Opt-in experiment ("ln_fused"): correct and bit-identical, but measured SLOWER (3.18 vs 2.69 ms/step at B=64): the CTA
-  // that finishes a row block normalises its 128 rows alone, latency-bound, and the last blocks' LayerNorm sits on the
-  // kernel's critical path; a standalone LayerNorm launch spreads the same rows over all SMs.
+  // Opt-in experiment ("ln_fused"): correct and bit-identical, off by default: the CTA that finishes a row block normalises
+  // its 128 rows alone, latency-bound, and the last blocks' LayerNorm sits on the kernel's critical path; a standalone
+  // LayerNorm launch spreads the same rows over all SMs.
   bool ln_fused = false;
   // Chained launches (chain.cuh): patch -> LN -> qkv0, then per block proj -> LN -> fc1 -> fc2 -> LN -> qkv(next) as ONE persistent
   // kernel each; the counters that replace the kernel boundaries live in chain_counters (5 arrays of one int per 128-row
   // block per chained launch), zeroed by one memset at the start of every forward.
   // Small batches (below chain_min_batch): LayerNorm + its consumer GEMM (qkv / fc1) as ONE two-stage chained launch -- the
   // LayerNorm jobs start at once (their rows are complete), the GEMM tiles wait for their rows -- instead of a LayerNorm
-  // launch followed by a GEMM launch (option "ln_in_gemm").  Bit-identical, but measured SLOWER than the two launches at every
-  // small batch (1 crop: 0.864 vs 0.711 ms per call; 9 crops: 0.884 vs 0.819; a LayerNorm job on the chain's spare warps takes
-  // ~5 us against 8.6 us for the whole LayerNorm launch, and the chained kernel cannot use the narrow tiles): off by default.
+  // launch followed by a GEMM launch (option "ln_in_gemm").  Bit-identical, off by default: the LayerNorm jobs then run on
+  // the chain's few spare warps instead of a whole launch, and the chained kernel uses one tile width.
   bool ln_in_gemm = false;
   bool gelu_erf = false;           // option "gelu_erf": fc1 epilogue with the A&S-7.1.26 erf instead of the fitted tanh form (A/B)
-  bool use_chain = true;
-  // Batches below this take the one-kernel-per-GEMM path (option "chain_min_batch" / VPB_CHAIN_MIN_BATCH): measured on B200
-  // (tools/latency_small_batches.py, ViT-B) the chained launches lose 3-8 % up to 32 crops per call (few row blocks: the
-  // dependent phases cannot overlap and every CTA spins) and win from 48 crops on.
-  int chain_min_batch = 48;
+  bool use_chain = false;
+  // Chained launches are off by default (option "chain" / VPB_CHAIN=1 turns them on, for batches of at least "chain_min_batch" /
+  // VPB_CHAIN_MIN_BATCH crops): on an H100 80GB HBM3 (700 W power limit) ViT-B ran slower chained than with one 128-wide-tile
+  // kernel per GEMM at every batch size measured, 1 to 64 crops (64 crops: 9.39 vs 6.26 ms per call; 1 crop: 1.00 vs 0.77;
+  // tools/defaults_ab.py).  Bit-identical either way.
+  int chain_min_batch = 1;
   int resid_rmw = 0;               // residual epilogues as load + add + store instead of TMA reduce-add (see resid_rmw_default)
   int ln_job_rows = CHAIN_LN_JOB_ROWS;   // rows per LayerNorm job of the chained launches (8 or 16); option "ln_job_rows", VPB_LN_JOB_ROWS
   int ln_ctl = 0;                  // chained launches: LayerNorm polls / publishes on a control warp (chain.cuh); option "ln_ctl", VPB_LN_CTL
-  int chain_bn = 256;
+  int chain_bn = 128;
   int* chain_counters = nullptr;
   size_t chain_blocks = 0;         // 128-row blocks at max_batch
   // host-facing path: two staging slots (crops, org_wh in; kpts, idx out) so that slot i+1's H2D overlaps slot i's compute
@@ -488,10 +467,10 @@ extern "C" int vpb_create(const vpb_config* cfg, vpb_engine** out) {
   e->cfg = *cfg;
   e->D = cfg->embed_dim; e->depth = cfg->depth; e->heads = cfg->num_heads; e->K = cfg->num_keypoints; e->maxB = cfg->max_batch;
   e->n_final = e->K <= 32 ? 32 : 144;
-  e->chain_bn = (e->D % 256 == 0) ? 256 : 128;               // D, 3D and 4D are then all multiples of the chain's tile width
+  e->chain_bn = 128;     // D, 3D and 4D are multiples of it for every ViT; 128 accumulator columns leave the LayerNorm warps room
   {
     const char* env = getenv("VPB_CHAIN");
-    if (env && env[0] == '0') e->use_chain = false;
+    if (env) e->use_chain = env[0] != '0';
     const char* ge = getenv("VPB_GELU_ERF");
     if (ge && ge[0] == '1') e->gelu_erf = true;
     const char* mb = getenv("VPB_CHAIN_MIN_BATCH");
@@ -565,11 +544,11 @@ static int pack_linear(vpb_engine* e, LinearW& L, const std::string& wkey, const
   if (!bkey.empty()) pack_bias<<<cdiv(n_pad, 256), 256>>>(e->staged[bkey].first, L.b, n, n_pad, scaled_rows, scale);
   else CU_TRY(cudaMemset(L.b, 0, n_pad * sizeof(float)));
   CU_TRY(cudaGetLastError());
-  VPB_TRY(make_map(&L.map, L.w, n_pad, k, k, bn / GEMM_CL));
-  if (n_pad % e->chain_bn == 0) VPB_TRY(make_map(&L.map_c, L.w, n_pad, k, k, e->chain_bn / GEMM_CL));
+  VPB_TRY(make_map(&L.map, L.w, n_pad, k, k, bn));
+  if (n_pad % e->chain_bn == 0) VPB_TRY(make_map(&L.map_c, L.w, n_pad, k, k, e->chain_bn));
   else L.map_c = L.map;                                        // never chained (final 1x1 conv)
   L.has128 = (n_pad % 128 == 0);
-  if (L.has128) VPB_TRY(make_map(&L.map128, L.w, n_pad, k, k, 128 / GEMM_CL));
+  if (L.has128) VPB_TRY(make_map(&L.map128, L.w, n_pad, k, k, 128));
   return VPB_OK;
 }
 
@@ -621,7 +600,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
                                          cin, 256, 1e-5f);
     CU_TRY(cudaGetLastError());
     dc.n = 256; dc.k = 4 * cin; dc.bn = 256;
-    VPB_TRY(make_map(&dc.map, dc.w, 4 * 256, 4 * cin, 4 * cin, 256 / GEMM_CL));
+    VPB_TRY(make_map(&dc.map, dc.w, 4 * 256, 4 * cin, 4 * cin, 256));
     cin = 256;
   }
   {  // final 1x1 conv: [K,256] zero-padded to the N tile
@@ -669,12 +648,12 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(make_map(&e->m_attn, e->attn, M, D, D, 128));
   VPB_TRY(make_map(&e->m_hid, e->hid, M, 4 * D, 4 * D, 128));
   VPB_TRY(make_map_nhwc(&e->m_feat_nhwc, e->xn, B, 16, 12, D, 8, 12));   // 8 x 12 = 96 positions per M tile (12 is not a multiple of 8)
-  VPB_TRY(make_map_nhwc(&e->m_d1_nhwc, e->d1, B, 32, 24, 256, 16, 8));  // 16 x 8 = 128 positions per M tile: full UMMA tiles
+  VPB_TRY(make_map_nhwc(&e->m_d1_nhwc, e->d1, B, 32, 24, 256, 16, 8));  // 16 x 8 = 128 positions per M tile: full tiles
   VPB_TRY(make_map(&e->m_d2, e->d2, B * 3072, 256, 256, 128));
   VPB_TRY(make_attn_maps(&e->m_qkv_att, &e->m_qkv_att_tail, e->qkv, M, D, D / e->heads));
-  VPB_TRY(make_map(&e->o_qkv, e->qkv, M, 3 * D, 3 * D, 32));
-  VPB_TRY(make_map(&e->o_hid, e->hid, M, 4 * D, 4 * D, 32));
-  VPB_TRY(make_map(&e->o_x, e->x, M, D, D, 32, /*f32=*/true));
+  VPB_TRY(make_map(&e->o_qkv, e->qkv, M, 3 * D, 3 * D, 64));
+  VPB_TRY(make_map(&e->o_hid, e->hid, M, 4 * D, 4 * D, 64));
+  VPB_TRY(make_map(&e->o_x, e->x, M, D, D, 64, /*f32=*/true));
   {
     const char* env = getenv("VPB_L2_PERSIST");
     if (env && env[0] == '0') e->l2_persist = false;
@@ -779,15 +758,14 @@ static int backbone_chained(vpb_engine* e, int B, cudaStream_t st) {
     p.dbg_nowait = nowait;
     p.rmw = resid_rmw(e->resid_rmw);
     p.ln_ctl = e->ln_ctl; p.ln_job_rows = e->ln_job_rows;
-    // tile order inside a chained launch: phase-major by default (lag >= number of row-block pairs).  Interleaving the
-    // reduce-add phases with their consumers (VPB_CHAIN_LAG0/1 = lag in 256-row pairs) was measured slower at every lag tried
-    // (B = 64: 27.4 k crops/s phase-major, 25.2 k at 24/32, 23.4 k at 16/22, 20.1 k at 8/12): a consumer tile needs the
-    // producer's tile + epilogue + LayerNorm job (~30 k cycles) behind it, and clusters stalled on that delay the very
-    // producer tiles the next consumers wait for.
+    // tile order inside a chained launch: phase-major by default (lag >= number of row blocks).  Interleaving the reduce-add
+    // phases with their consumers (VPB_CHAIN_LAG0/1 = lag in 128-row blocks) is an experiment: a consumer tile needs the
+    // producer's tile, its epilogue and a LayerNorm job behind it, and CTAs stalled on that delay the very producer tiles the
+    // next consumers wait for.
     static const int lag0 = [] { const char* v = getenv("VPB_CHAIN_LAG0"); return v ? atoi(v) : (1 << 20); }();
     static const int lag1 = [] { const char* v = getenv("VPB_CHAIN_LAG1"); return v ? atoi(v) : (1 << 20); }();
     p.wave_lag[0] = lag0; p.wave_lag[1] = lag1;
-    p.dbg = g_dbg_buf;                      // vpb_debug_gemm(0, counters): [74 clusters][4 phases][8] int64, accumulated over launches
+    p.dbg = g_dbg_buf;                      // vpb_debug_gemm(0, counters): [grid CTAs][4 phases][12] int64, accumulated over launches
   };
   const int nD = D / bn, n4D = 4 * D / bn;                    // column tiles of the D-wide and 4D-wide phases
   {
@@ -836,16 +814,14 @@ static int backbone_chained(vpb_engine* e, int B, cudaStream_t st) {
   return VPB_OK;
 }
 
-// Tile width of a standalone GEMM launch.  A 256-wide tile is the efficient one (128 flop per byte of operand traffic), but a small
-// batch has few of them: 9 crops -> 7 row-block pairs -> proj / fc2 have 21 tiles for 74 SM pairs and the launch lasts one full
-// K loop of a single tile.  Halving the width doubles the tiles and halves every tile's K-loop time; taken while the 128-wide
-// tiles still fit one wave.  The accumulation order of an output element does not depend on the tile shape: bit-identical.
-static const CUtensorMap& pick_tile(const LinearW& L, int M, int* bn) {
+// Tile width of a standalone GEMM launch: 128 wherever N allows.  A 256-wide tile moves fewer operand bytes per flop, but its 128
+// accumulators per consumer thread do not fit the register budget of a 384-thread CTA (ptxas spills), and on an H100 80GB HBM3
+// (700 W power limit) ViT-B ran faster with 128-wide tiles at every batch size from 4 crops up (64 crops: 6.26 vs 9.04 ms per
+// call; 1 crop: 0.77 vs 0.76 ms; tools/defaults_ab.py).  The 256-wide tiles stay reachable with debug flag 16.  The accumulation
+// order of an output element does not depend on the tile shape: bit-identical.
+static const CUtensorMap& pick_tile(const LinearW& L, int* bn) {
+  if (L.has128 && !(g_dbg_flags & 16)) { *bn = 128; return L.map128; }
   *bn = L.bn;
-  if (L.bn == 256 && L.has128 && !(g_dbg_flags & 16)) {      // debug flag 16: never narrow
-    const int pairs256 = cdiv(cdiv(M, GEMM_BM), GEMM_CL) * (L.n / 256);
-    if (2 * pairs256 <= num_sms() / GEMM_CL) { *bn = 128; return L.map128; }
-  }
   return L.map;
 }
 
@@ -892,7 +868,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     fuse_ln(p, e->blocks[0].ln1_g, e->blocks[0].ln1_b);
     e->prof.begin(KC_GEMM_PATCH, st);
     int bn;
-    const CUtensorMap& wm = pick_tile(e->patch, M, &bn);
+    const CUtensorMap& wm = pick_tile(e->patch, &bn);
     p.rmw = resid_rmw(e->resid_rmw);
     VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_patch_rows, wm, e->o_x, p, st));
     e->prof.end(st);
@@ -908,7 +884,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     e->prof.begin(KC_GEMM_QKV, st);
     {
       int bn;
-      const CUtensorMap& wm = pick_tile(b.qkv, M, &bn);
+      const CUtensorMap& wm = pick_tile(b.qkv, &bn);
       VPB_TRY(gemm_launch(bn, EPI_BF16, e->m_xn, wm, e->o_qkv, gp(M, 3 * D, D, b.qkv.b, e->qkv, 3 * D), st));
     }
     e->prof.end(st);
@@ -927,7 +903,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
       fuse_ln(p, b.ln2_g, b.ln2_b);
       e->prof.begin(KC_GEMM_PROJ, st);
       int bn;
-      const CUtensorMap& wm = pick_tile(b.proj, M, &bn);
+      const CUtensorMap& wm = pick_tile(b.proj, &bn);
       p.rmw = resid_rmw(e->resid_rmw);
       VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_attn, wm, e->o_x, p, st));
       e->prof.end(st);
@@ -940,7 +916,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     e->prof.begin(KC_GEMM_FC1, st);
     {
       int bn;
-      const CUtensorMap& wm = pick_tile(b.fc1, M, &bn);
+      const CUtensorMap& wm = pick_tile(b.fc1, &bn);
       VPB_TRY(gemm_launch(bn, e->gelu_erf ? EPI_BF16_GELU_ERF : EPI_BF16_GELU, e->m_xn, wm, e->o_hid, gp(M, 4 * D, D, b.fc1.b, e->hid, 4 * D), st));
     }
     e->prof.end(st);
@@ -952,7 +928,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
       else fuse_ln(p, e->lnf_g, e->lnf_b);
       e->prof.begin(KC_GEMM_FC2, st);
       int bn;
-      const CUtensorMap& wm = pick_tile(b.fc2, M, &bn);
+      const CUtensorMap& wm = pick_tile(b.fc2, &bn);
       p.rmw = resid_rmw(e->resid_rmw);
       VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_hid, wm, e->o_x, p, st));
       e->prof.end(st);
@@ -1552,14 +1528,14 @@ extern "C" int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, v
     if ((tile_w * aux2 != 96 && tile_w * aux2 != 128) || cin * 4 != k || aux0 % aux2 != 0 || aux1 % tile_w != 0 || m % (aux0 * aux1) != 0)
       return fail(VPB_ERR_ARG, "vpb_gemm: bad deconv geometry");
     VPB_TRY(make_map_nhwc(&ta, d_a, m / (aux0 * aux1), aux0, aux1, cin, aux2, tile_w));
-    VPB_TRY(make_map(&tw, d_w, 4 * n, k, k, bn / GEMM_CL));
+    VPB_TRY(make_map(&tw, d_w, 4 * n, k, k, bn));
   } else {
     VPB_TRY(make_map(&ta, d_a, m, k, k, 128));
-    VPB_TRY(make_map(&tw, d_w, n, k, k, bn / GEMM_CL));
+    VPB_TRY(make_map(&tw, d_w, n, k, k, bn));
   }
-  VPB_TRY(make_map(&tout, d_w, n, k, k, bn / GEMM_CL));   // placeholder for direct epilogues
-  if (epilogue == EPI_BF16 || epilogue == EPI_BF16_GELU || epilogue == EPI_BF16_GELU_ERF) VPB_TRY(make_map(&tout, d_out, m, n, n, 32));
-  if (epilogue == EPI_F32_ADD) VPB_TRY(make_map(&tout, d_out, m, n, n, 32, /*f32=*/true));
+  VPB_TRY(make_map(&tout, d_w, n, k, k, bn));   // placeholder for direct epilogues
+  if (epilogue == EPI_BF16 || epilogue == EPI_BF16_GELU || epilogue == EPI_BF16_GELU_ERF) VPB_TRY(make_map(&tout, d_out, m, n, n, 64));
+  if (epilogue == EPI_F32_ADD) VPB_TRY(make_map(&tout, d_out, m, n, n, 64, /*f32=*/true));
   GemmParams p = gp(m, n, k, d_bias, d_out, n);
   (void)d_resid; (void)resid_mod;
   if (epilogue == EPI_F32_NCHW) { p.n_valid = aux0; p.pix = aux1; }

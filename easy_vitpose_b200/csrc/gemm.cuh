@@ -1,27 +1,20 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  C[M,N] = A[M,K] * W[N,K]^T  (+ fused epilogue)
+// Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = A[M,K] * W[N,K]^T  (+ fused epilogue)
 //
-//   warps 0..7         epilogue: tcgen05.ld -> registers -> bias / GELU / ReLU -> swizzled smem staging ->
-//                      TMA store (bf16) or TMA reduce-add (fp32 residual, the add happens in L2)
-//   warp 8             TMEM allocator
-//   warp 10 (1 thread) TMA producer: A / W tiles -> 128B-swizzled smem ring, mbarrier full/empty
-//   warp 11 (1 thread) tcgen05.mma issuer (leader CTA): 256 x BN x 16 pair-UMMAs, fp32 accumulators in TMEM (2 stages)
-// (the warp scheduler favours high warp ids: the two single-thread roles must never queue behind epilogue math)
+//   warpgroups 0, 1    consumers: rows 0..63 / 64..127 of the 128 x BN tile, wgmma m64nBNk16 with fp32 accumulators in
+//                      registers, then the epilogue straight from those registers: bias / GELU / ReLU -> swizzled smem
+//                      staging -> TMA store (bf16) or TMA reduce-add (fp32 residual, the add happens in L2)
+//   warp 8             TMA producer: A / W tiles -> 128B-swizzled smem ring, mbarrier full / empty
 //
-// Both operands are K-major (nn.Linear keeps W as [N,K]), so no transposes anywhere.
-//
-// CTAs run as pairs (cluster of 2 along M, tcgen05 cta_group::2): the pair owns a 256 x BN output tile, each CTA
-// fetches its own 128 x 64 A tile and HALF of the BN x 64 W tile per k-block (32 KB instead of 48 KB at BN = 256:
-// 128 flop per L2 byte instead of 85, and 6 ring stages instead of 4 -- the ring depth is what hides the ~2000-cycle
-// TMA round trip, measured with the cycle counters in GemmParams::dbg).  The leader CTA's single MMA thread issues
-// M = 256 UMMAs that read both CTAs' smem and write both CTAs' TMEM; every TMA load of the pair completes on the
-// leader's full barrier; tcgen05.commit multicasts "slot free" / "accumulator ready" to both CTAs.
-// Pairs are handed tiles statically (tile = clusterid + i * nclusters, n fastest: the ~74 pairs running together cover
-// a few A row-blocks x all W column-blocks, which keeps the big streaming operand A hot in L2; measured +5-8 % over
-// m-fastest).  The accumulator double buffer lets the epilogue of tile i overlap the main loop of tile i+1.
+// Both operands are K-major (nn.Linear keeps W as [N,K]), so no transposes anywhere.  Tiles are handed out statically
+// (tile = blockIdx.x + i * gridDim.x, n fastest: the CTAs running together cover a few A row-blocks x all W column-blocks,
+// which keeps the big streaming operand A hot in L2).  The producer runs ahead of the consumers by the ring depth, across
+// tile boundaries, so the next tile's operands arrive while the consumers run the epilogue of the current one.
+// The accumulation order of an output element is the k order, whatever the tile width: every BN gives the same bits.
 #pragma once
 #include <cuda.h>
 
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace vpb {
 
@@ -54,43 +47,40 @@ struct GemmParams {
   __nv_bfloat16* ln_out;  // [M, N] or nullptr
   int* ln_counters;       // [ceil(M/128)] zero before the first launch; the last arriver resets its entry
   float ln_eps;
-  int rmw;                // EPI_F32_ADD: 1 = load + add + store in the generic proxy (epilogue_f32_rmw; needs out = the fp32 stream), 0 = TMA reduce-add
+  int rmw;                // EPI_F32_ADD: 1 = load + add + store in the generic proxy (needs out = the fp32 stream), 0 = TMA reduce-add
   int stages_limit;       // debug: use at most this many ring stages (0 = all)
-  int dbg_flags;          // debug (results become wrong!): 1 = every pair loads the SAME A rows, 2 = the same W rows
+  int dbg_flags;          // debug (results become wrong!): 1 = every CTA loads the SAME A rows, 2 = the same W rows
                           //        (probes whether L2 reads or SM-side delivery bound the loop); 4 = m-fastest tile order
-  long long* dbg;         // debug: per-CTA cycle counters [8] (nullptr = off): 0 mma total, 1 mma wait full, 2 mma wait acc,
-                          //        3 producer total, 4 producer wait empty, 5 epilogue(warp 4) total, 6 epilogue wait acc_full
+  long long* dbg;         // debug: per-CTA cycle counters [8] (nullptr = off): 0 consumer (thread 0) total, 1 its wait for
+                          //        operands, 3 producer total, 4 producer wait for free ring slots, 7 CTA lifetime
 };
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
 constexpr int GEMM_THREADS = 384;
-constexpr int GEMM_EPI_WARPS = 8;
-constexpr int GEMM_CL = 2;                 // CTAs per cluster (along M)
-constexpr int GEMM_STAGE_TILE = 4096;      // one epilogue warp's staging tile: 32 rows x 128 B
+constexpr int GEMM_CONSUMER_WARPS = 8;     // two warpgroups of 64 rows
+constexpr int GEMM_STAGE_TILE = 8192;      // one staging buffer: 64 rows x 128 B (two per consumer warpgroup)
+constexpr int GEMM_BAR_EPI = 1;            // named barrier of the 256 consumer threads (2, 3: the warpgroups' staging barriers)
 
 __host__ __device__ constexpr bool epi_uses_tma(int epi) { return epi == EPI_BF16 || epi == EPI_BF16_GELU || epi == EPI_F32_ADD || epi == EPI_BF16_GELU_ERF; }
 
-template <int BN, int EPI>
-struct GemmCfg {
+// Ring and staging layout of a 128 x BN tile, shared by the standalone GEMM and the chained launches (chain.cuh).
+template <int BN, bool STAGED>
+struct TileCfg {
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
-  static constexpr int B_SLICE = B_BYTES / GEMM_CL;                // the half of the W tile this CTA holds
-  static constexpr int STAGE_BYTES = A_BYTES + B_SLICE;
-  static constexpr int STAGING = epi_uses_tma(EPI) ? GEMM_EPI_WARPS * GEMM_STAGE_TILE : 0;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGING = STAGED ? 4 * GEMM_STAGE_TILE : 0;
   static constexpr int STAGES_RAW = (227 * 1024 - 2048 - STAGING) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int ACC_STRIDE = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
-  static constexpr int TMEM_COLS = 2 * ACC_STRIDE;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int HALF = BN / 2;                              // columns per epilogue warp-group
-  static constexpr int CH = (HALF % 32 == 0) ? 32 : (HALF % 16 == 0) ? 16 : 8;
-  static_assert(B_SLICE % 1024 == 0, "W slices must keep 1024-byte alignment of the ring");
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "UMMA N");
-  static_assert(HALF % CH == 0, "epilogue chunking");
-  static_assert(!epi_uses_tma(EPI) || HALF % 64 == 0, "TMA epilogues stage 64 bf16 / 32 f32 columns at a time");
+  static_assert(B_BYTES % 1024 == 0, "W tiles must keep 1024-byte alignment of the ring");
+  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "wgmma N");
+  static_assert(!STAGED || BN % 64 == 0, "TMA epilogues stage 64 bf16 / 32 f32 columns at a time");
   static_assert(STAGES >= 3, "ring too shallow");
 };
+template <int BN, int EPI>
+using GemmCfg = TileCfg<BN, epi_uses_tma(EPI)>;
 
 __device__ __forceinline__ float gelu_erf_as(float x) { return 0.5f * x * (1.0f + erf_as(x * 0.70710678118654752440f)); }
 #ifdef VPB_GELU_ERF
@@ -99,68 +89,121 @@ __device__ __forceinline__ float gelu_fast(float x) { return gelu_erf_as(x); }
 __device__ __forceinline__ float gelu_fast(float x) { return gelu_tanh_fit(x); }
 #endif
 
-// ---------------------------------------------------------------- fp32 residual epilogue as LOAD + ADD + STORE
-// x[tile] += acc + bias without the L2 reduction path and without TMA on the way out (option "resid_rmw", OFF by default:
-// bit-identical, measured slower -- kept as the A/B switch and as the record of what does not bound these epilogues).
-// A residual epilogue round of one warp (4 KB) takes ~3.4 k cycles as a TMA reduce-add against ~2.6 k for a bf16 TMA store
-// (tools/chain_diag.py: proj 13.7 k, fc2 14.2 k cycles per tile for four rounds, qkv 5.3 k for two); a K = 768 residual phase
-// (patch embed, proj) is epilogue-bound and its last epilogues head the chain proj -> LayerNorm -> first fc1 tile that every
-// cluster waits on.  Every element of the stream has exactly ONE writer per phase (no split-K), so that writer can do the add
-// itself: the warp reads its 32 x 32 fp32 box of x out of L2 with coalesced 16-byte loads (ld.global.cg; eight lanes per
-// 128-byte row segment, four rows per instruction), transposes acc + bias from the accumulator's row-per-lane layout into
-// that same layout through its staging buffer (plain st.shared / ld.shared, free again after a __syncwarp), adds -- fl(x +
-// fl(acc + bias)), the very two roundings of the reduce-add form, hence bit-identical -- and stores the box with coalesced
-// 16-byte st.global.cg.  The loads of box c + 1 are issued as soon as box c is stored; box 0 may be requested before the
-// accumulator is ready whenever the rows were last written by an EARLIER launch (proj, patch embed); inside a chained launch
-// the rows of a later residual phase (fc2) are complete once the tile's A operand is (proj -> LayerNorm -> fc1 -> this tile),
-// so they are requested after acc_full.
-// Measured on B200 (ViT-B, 64 crops, profiles/r2_ab_resid_rmw.txt), per proj tile / per step against 13.7 k cycles / 2.30-2.37 ms
-// for the reduce-add: (1) one lane per row for the loads + TMA store: 35.6 k / 2.72 ms (256 partial-sector requests per box);
-// (2) coalesced loads parked in the staging buffer, add in place, TMA store: 19.3 k / 2.44 ms; (3) this form, no TMA at all:
-// 20.5 k / 2.37-2.40 ms.  Neither the reduction unit nor the staging buffer's hand-back explains the round time.
-//
-// xr[i]: lane l holds the 16-byte chunk (l & 7) of row 4 i + (l >> 3) of the box whose first row is row0, first column n.
-__device__ __forceinline__ void rmw_load_box(float4 (&xr)[8], const float* __restrict__ x, int ldx, int row0, int lane, int M, int n) {
-  const float* src = x + static_cast<size_t>(row0 + (lane >> 3)) * ldx + n + 4 * (lane & 7);
+// ---------------------------------------------------------------- ring: producer and consumer sides
+// The ring position (stage, phase) runs on across tiles; both sides walk the same sequence of k-blocks.
+struct RingPos {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void next(int stages) { if (++stage == stages) { stage = 0; phase ^= 1; } }
+};
+
+// Producer side: wait until the consumers have released the slot at `rp` (a fresh barrier passes on parity 1).  Whole warp.
+__device__ __forceinline__ void ring_wait_slot(uint64_t* empty_bar, const RingPos& rp) { mbar_wait(&empty_bar[rp.stage], rp.phase ^ 1); }
+
+// Consumer warpgroup `wg`: acc = A[64 wg .. 64 wg + 63, :] * W[0 .. BN-1, :]^T over num_kb k-blocks of the ring.  Every
+// consumer warp releases a slot once the MMAs that read it have retired (empty barriers count GEMM_CONSUMER_WARPS arrivals).
+template <int BN>
+__device__ __forceinline__ void tile_mainloop(float (&acc)[BN / 2], uint8_t* ring, int stage_bytes, uint64_t* full_bar, uint64_t* empty_bar,
+                                              int num_kb, int stages, RingPos& rp, int wg, int lane, long long* t_wait) {
+  constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
+  int prev = -1;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const long long w0 = t_wait ? clock64() : 0;
+    mbar_wait(&full_bar[rp.stage], rp.phase);
+    if (t_wait) *t_wait += clock64() - w0;
+    const uint32_t sa = smem_u32(ring + rp.stage * stage_bytes) + wg * 64 * 128;
+    const uint32_t sb = smem_u32(ring + rp.stage * stage_bytes + A_BYTES);
+    const uint64_t ad = wgmma_desc<128>(sa), bd = wgmma_desc<128>(sb);
+    wgmma_fence();
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    // boxes are 32 columns wide and ldx % 32 == 0: a box lies inside or outside [0, ldx) as a whole
-    if (row0 + 4 * i + (lane >> 3) < M && n < ldx) xr[i] = __ldcg(reinterpret_cast<const float4*>(src + static_cast<size_t>(4 * i) * ldx));
-    else xr[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, ad + 2 * k, bd + 2 * k, (kb | k) != 0);   // +32 B per K = 16 step
+    wgmma_commit();
+    wgmma_wait<1>();                                  // k-block kb-1 has retired: its slot may be refilled
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = rp.stage;
+    rp.next(stages);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+}
+
+// ---------------------------------------------------------------- epilogues from the accumulator registers
+// Thread (warp w of the warpgroup, lane l) holds rows 16 w + l / 4 and + 8 of the warpgroup's 64, columns 8 j + 2 (l % 4) + {0, 1}.
+template <int EPI>
+__device__ __forceinline__ float epi_act(float v) {
+  if constexpr (EPI == EPI_BF16_GELU) return gelu_fast(v);
+  else if constexpr (EPI == EPI_BF16_GELU_ERF) return gelu_erf_as(v);
+  else if constexpr (EPI == EPI_BF16_RELU_UP) return fmaxf(v, 0.0f);
+  else return v;
+}
+
+// TMA epilogues: 64 bf16 / 32 f32 columns (one 128-byte staging row) per round, two staging buffers per warpgroup in turn.
+// `stiles` = this warpgroup's two buffers; `tid` = thread index inside the warpgroup (thread 0 issues and owns the bulk groups).
+template <int BN, int EPI>
+__device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], int n0, int row0, int N, const float* __restrict__ bias, uint8_t* stiles,
+                                             int wg, int tid, const CUtensorMap* tmap_out) {
+  constexpr int COLS = (EPI == EPI_F32_ADD) ? 32 : 64;
+  constexpr int JPC = COLS / 8;                       // accumulator column groups per round
+  const int lane = tid & 31, wq = tid >> 5;
+  const int r_lo = 16 * wq + (lane >> 2);             // staging rows r_lo and r_lo + 8 (same swizzle phase: (r + 8) % 8 = r % 8)
+  const int sw = r_lo & 7;
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int c = 0; c < BN / COLS; ++c) {
+    uint8_t* st = stiles + (c & 1) * GEMM_STAGE_TILE;
+    if (tid == 0) tma_store_wait_read<1>();           // the store that used this buffer two rounds ago has read it
+    named_bar_sync(GEMM_BAR_EPI + 1 + wg, 128);
+#pragma unroll
+    for (int jl = 0; jl < JPC; ++jl) {
+      const int j = c * JPC + jl;
+      const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * j + cq));
+      const float v0 = epi_act<EPI>(acc[4 * j] + b2.x), v1 = epi_act<EPI>(acc[4 * j + 1] + b2.y);
+      const float v2 = epi_act<EPI>(acc[4 * j + 2] + b2.x), v3 = epi_act<EPI>(acc[4 * j + 3] + b2.y);
+      if constexpr (EPI == EPI_F32_ADD) {
+        const int off = (((2 * jl + ((lane & 3) >> 1)) ^ sw) << 4) + (lane & 1) * 8;
+        *reinterpret_cast<float2*>(st + r_lo * 128 + off) = make_float2(v0, v1);
+        *reinterpret_cast<float2*>(st + (r_lo + 8) * 128 + off) = make_float2(v2, v3);
+      } else {
+        const int off = ((jl ^ sw) << 4) + (lane & 3) * 4;
+        *reinterpret_cast<uint32_t*>(st + r_lo * 128 + off) = pack_bf16(v0, v1);
+        *reinterpret_cast<uint32_t*>(st + (r_lo + 8) * 128 + off) = pack_bf16(v2, v3);
+      }
+    }
+    fence_proxy_async_smem();                         // staging writes -> visible to the TMA engine
+    named_bar_sync(GEMM_BAR_EPI + 1 + wg, 128);
+    const int n = n0 + c * COLS;
+    if (tid == 0 && n < N) {
+      if constexpr (EPI == EPI_F32_ADD) tma_reduce_add_2d(tmap_out, st, n, row0);
+      else tma_store_2d(tmap_out, st, n, row0);       // rows past M are clipped by the tensor map
+    }
+    if (tid == 0) tma_store_commit();
   }
 }
-// NCH boxes of 32 columns from column n_first / TMEM address t_col0 on; xr holds box 0.
-template <int NCH>
-__device__ __forceinline__ void epilogue_f32_rmw(uint32_t t_col0, int n_first, int row0, int M, const float* __restrict__ bias,
-                                                 float* __restrict__ x, int ldx, float4 (&xr)[8], uint8_t* stile, int lane) {
-  const int sw = lane & 7;
-  uint8_t* srow = stile + lane * 128;               // row = lane, 16-byte chunk index XOR (row % 8): conflict-free both ways
-  if (elect_one()) tma_store_wait_read<0>();        // a TMA store of an earlier (bf16) tile may still be reading the buffer
-#pragma unroll 1
-  for (int c = 0; c < NCH; ++c) {
-    const int n = n_first + 32 * c;
-    uint32_t r[32];
-    tmem_ld32(t_col0 + 32 * c, r);
-    tmem_ld_wait();
-    __syncwarp();                                   // the previous round's reads of the staging buffer are done
+
+// fp32 residual epilogue as LOAD + ADD + STORE (option "resid_rmw"): every element of the stream has exactly ONE writer per
+// launch (no split-K), so that writer can do the add itself: fl(x + fl(acc + bias)), the very two roundings of the reduce-add
+// form, hence bit-identical to it.
+template <int BN>
+__device__ __forceinline__ void epilogue_f32_rmw(const float (&acc)[BN / 2], int n0, int row0, int M, const float* __restrict__ bias,
+                                                 float* __restrict__ x, int ldx, int tid) {
+  const int lane = tid & 31, wq = tid >> 5;
+  const int r_lo = row0 + 16 * wq + (lane >> 2);
+  const int cq = 2 * (lane & 3);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + n + 4 * q));
-      *reinterpret_cast<float4*>(srow + ((q ^ sw) << 4)) =
-          make_float4(__uint_as_float(r[4 * q]) + b4.x, __uint_as_float(r[4 * q + 1]) + b4.y, __uint_as_float(r[4 * q + 2]) + b4.z,
-                      __uint_as_float(r[4 * q + 3]) + b4.w);
-    }
-    __syncwarp();
-    float* dst = x + static_cast<size_t>(row0 + (lane >> 3)) * ldx + n + 4 * (lane & 7);
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n0 + 8 * j + cq;
+    if (n >= ldx) continue;
+    const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int row = 4 * i + (lane >> 3);
-      const float4 t = *reinterpret_cast<const float4*>(stile + row * 128 + (((lane & 7) ^ (row & 7)) << 4));
-      if (row0 + row < M && n < ldx)
-        __stcg(reinterpret_cast<float4*>(dst + static_cast<size_t>(4 * i) * ldx),
-               make_float4(xr[i].x + t.x, xr[i].y + t.y, xr[i].z + t.z, xr[i].w + t.w));
+    for (int h = 0; h < 2; ++h) {
+      const int r = r_lo + 8 * h;
+      if (r < M) {
+        float2* px = reinterpret_cast<float2*>(x + static_cast<size_t>(r) * ldx + n);
+        const float2 xv = __ldcg(px);
+        __stcg(px, make_float2(xv.x + (acc[4 * j + 2 * h] + b2.x), xv.y + (acc[4 * j + 2 * h + 1] + b2.y)));
+      }
     }
-    if (c + 1 < NCH) rmw_load_box(xr, x, ldx, row0, lane, M, n + 32);           // in flight under the next round's TMEM read
   }
 }
 
@@ -202,9 +245,9 @@ __device__ __forceinline__ void ln_row_l2(const float* __restrict__ xrow, const 
 }
 
 template <int BN, int EPI>
-__global__ void __cluster_dims__(GEMM_CL, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
-                  const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+                const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
   using Cfg = GemmCfg<BN, EPI>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -212,294 +255,145 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   uint8_t* staging = smem + Cfg::STAGES * Cfg::STAGE_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* acc_full = empty_bar + Cfg::STAGES;     // [2]
-  uint64_t* acc_empty = acc_full + 2;               // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  volatile int* ln_flag = reinterpret_cast<volatile int*>(tmem_slot + 1);   // "this CTA finishes the row block" broadcast
+  volatile int* ln_flag = reinterpret_cast<volatile int*>(empty_bar + Cfg::STAGES);   // "this CTA finishes the row block" broadcast
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);     // warp-uniform for the compiler (see elect_one in ptx.cuh)
   const int lane = threadIdx.x & 31;
-  const int cta_rank = static_cast<int>(cluster_ctarank());
-  const int cluster = static_cast<int>(cluster_id_x());
-  const int num_clusters = static_cast<int>(cluster_count_x());
   constexpr bool kDeconv = (EPI == EPI_BF16_RELU_UP);
   // deconv: an M tile is a up_tr x up_tw patch (96 or 128 positions) of one crop, p.M counts positions; the 4 phases play the n-blocks
   const int up_pos = kDeconv ? p.up_tr * p.up_tw : GEMM_BM;
   const int num_m = kDeconv ? p.M / up_pos : (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int num_mp = (num_m + GEMM_CL - 1) / GEMM_CL;               // m-block pairs
   const int num_n = kDeconv ? 4 : (p.N + BN - 1) / BN;
-  const int num_pairs = num_mp * num_n;
+  const int num_tiles = num_m * num_n;
   const int num_kb = p.K / GEMM_BK;
   const int num_stages = (p.stages_limit > 0 && p.stages_limit < Cfg::STAGES) ? p.stages_limit : Cfg::STAGES;
-  constexpr uint16_t kAllCtas = (1u << GEMM_CL) - 1;
+  auto tile_mn = [&](int tile, int& mt, int& nb) {
+    if (p.dbg_flags & 4) { mt = tile % num_m; nb = tile / num_m; }
+    else { mt = tile / num_n; nb = tile % num_n; }
+  };
 
-  long long t_cta0 = 0, t_ns0 = 0;
-  if (p.dbg && threadIdx.x == 0) {
-    t_cta0 = clock64();
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_ns0));
-  }
+  const long long t_cta0 = (p.dbg && threadIdx.x == 0) ? clock64() : 0;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w);
     if constexpr (epi_uses_tma(EPI)) tma_prefetch_desc(&tmap_out);
     for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);                   // used in the leader only: its producer arms it for BOTH CTAs' bytes
-      mbar_init(&empty_bar[s], 1);                  // one multicast tcgen05.commit per use
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], GEMM_CL * GEMM_EPI_WARPS);   // leader only: the epilogue warps of both CTAs arrive
+      mbar_init(&full_bar[s], 1);                     // the producer's expect_tx arrival
+      mbar_init(&empty_bar[s], GEMM_CONSUMER_WARPS);  // every consumer warp releases the slot
     }
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc_pair(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before_sync();
-  cluster_sync_all();                               // barriers + TMEM of BOTH CTAs are live before any remote arrive / pair MMA
-  tc_fence_after_sync();
-  const uint32_t tmem_base = uniform_u32(*tmem_slot);
+  __syncthreads();
   pdl_launch_dependents();                          // the next kernel may start its prologue as SMs free up
   pdl_wait();                                       // previous kernel's outputs (our A operand / residual) are complete
 
-  if (warp == 10) {
+  if (warp == GEMM_CONSUMER_WARPS) {
     // ------------------------------------------------------------ TMA producer: the whole warp runs the (uniform) loop, one
-    // elected lane issues -- inside an `if (lane == 0)` branch every UTMALDG / UTCHMMA gets an ELECT + R2UR + BRA.U.ANY loop
-    int stage = 0;
-    uint32_t phase = 0;
+    // elected lane issues
+    RingPos rp;
     long long t_wait = 0;
     const long long t_begin = p.dbg ? clock64() : 0;
-    for (int pair = cluster; pair < num_pairs; pair += num_clusters) {
-      const int mp_i = (p.dbg_flags & 4) ? pair % num_mp : pair / num_n;
-      const int mt = mp_i * GEMM_CL + cta_rank;                          // this CTA's M tile
-      const int nb = (p.dbg_flags & 4) ? pair / num_mp : pair % num_n;   // n-block (deconv: sub-pixel phase)
-      const int m0 = (p.dbg_flags & 1) ? cta_rank * GEMM_BM : mt * GEMM_BM;   // may lie past M: TMA zero-fills
+    const int tiles_x = kDeconv ? p.up_w / p.up_tw : 1;
+    const int tiles_per_img = kDeconv ? (p.up_h / p.up_tr) * tiles_x : 1;
+    const int kb_per_tap = kDeconv ? p.up_c / GEMM_BK : 1;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int mt, nb;
+      tile_mn(tile, mt, nb);
+      const int m0 = (p.dbg_flags & 1) ? 0 : mt * GEMM_BM;   // may lie past M: TMA zero-fills
       const int n0 = (p.dbg_flags & 2) ? 0 : nb * BN;
-      const int tiles_x = kDeconv ? p.up_w / p.up_tw : 1;
-      const int tiles_per_img = kDeconv ? (p.up_h / p.up_tr) * tiles_x : 1;
-      const int kb_per_tap = kDeconv ? p.up_c / GEMM_BK : 1;
       for (int kb = 0; kb < num_kb; ++kb) {
         const long long w0 = p.dbg ? clock64() : 0;
-        mbar_wait(&empty_bar[stage], phase ^ 1);
+        ring_wait_slot(empty_bar, rp);
         if (p.dbg) t_wait += clock64() - w0;
-        uint8_t* sa = ring + stage * Cfg::STAGE_BYTES;
+        uint8_t* sa = ring + rp.stage * Cfg::STAGE_BYTES;
         if (elect_one()) {
-        if constexpr (kDeconv) {
-          // A tile = a up_tr x up_tw patch of the input map shifted by the tap's (dy, dx); the 4-D box is zero filled
-          // outside the map (= the transposed conv's border).  With 96-position tiles rows 96..127 of the smem tile are
-          // never written: they only feed accumulator rows nobody stores.
-          const int tap = kb / kb_per_tap, c0 = (kb % kb_per_tap) * GEMM_BK;
-          const int py = nb >> 1, px = nb & 1, iy = tap >> 1, ix = tap & 1;
-          const int dy = py ? (iy ? 0 : 1) : (iy ? -1 : 0);
-          const int dx = px ? (ix ? 0 : 1) : (ix ? -1 : 0);
-          if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], GEMM_CL * (up_pos * 128 + Cfg::B_SLICE));
-          const int ti = mt % tiles_per_img;
-          tma_load_4d_pair(sa, &tmap_a, &full_bar[stage], c0, (ti % tiles_x) * p.up_tw + dx, (ti / tiles_x) * p.up_tr + dy,
-                           mt / tiles_per_img);
-        } else {
-          if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], GEMM_CL * Cfg::STAGE_BYTES);   // bytes of both CTAs land here
-          tma_load_2d_pair(sa, &tmap_a, &full_bar[stage], kb * GEMM_BK, m0);
-        }
-        tma_load_2d_pair(sa + Cfg::A_BYTES, &tmap_w, &full_bar[stage], kb * GEMM_BK, n0 + cta_rank * (BN / GEMM_CL));
+          if constexpr (kDeconv) {
+            // A tile = a up_tr x up_tw patch of the input map shifted by the tap's (dy, dx); the 4-D box is zero filled
+            // outside the map (= the transposed conv's border).  With 96-position tiles rows 96..127 of the smem tile are
+            // never written: they only feed accumulator rows nobody stores.
+            const int tap = kb / kb_per_tap, c0 = (kb % kb_per_tap) * GEMM_BK;
+            const int py = nb >> 1, px = nb & 1, iy = tap >> 1, ix = tap & 1;
+            const int dy = py ? (iy ? 0 : 1) : (iy ? -1 : 0);
+            const int dx = px ? (ix ? 0 : 1) : (ix ? -1 : 0);
+            mbar_expect_tx(&full_bar[rp.stage], up_pos * 128 + Cfg::B_BYTES);
+            const int ti = mt % tiles_per_img;
+            tma_load_4d(sa, &tmap_a, &full_bar[rp.stage], c0, (ti % tiles_x) * p.up_tw + dx, (ti / tiles_x) * p.up_tr + dy, mt / tiles_per_img);
+          } else {
+            mbar_expect_tx(&full_bar[rp.stage], Cfg::STAGE_BYTES);
+            tma_load_2d(sa, &tmap_a, &full_bar[rp.stage], kb * GEMM_BK, m0);
+          }
+          tma_load_2d(sa + Cfg::A_BYTES, &tmap_w, &full_bar[rp.stage], kb * GEMM_BK, n0);
         }
         __syncwarp();
-        if (++stage == num_stages) { stage = 0; phase ^= 1; }
+        rp.next(num_stages);
       }
     }
     if (p.dbg && lane == 0) { p.dbg[blockIdx.x * 8 + 3] = clock64() - t_begin; p.dbg[blockIdx.x * 8 + 4] = t_wait; }
-  } else if (warp == 11 && cta_rank == 0) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA of the pair only)
-    constexpr uint32_t idesc = umma_idesc_bf16(GEMM_CL * GEMM_BM, BN);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    long long t_wfull = 0, t_wacc = 0;
+  } else if (warp < GEMM_CONSUMER_WARPS) {
+    // ------------------------------------------------------------ consumers: MMA + epilogue, warpgroup wg owns rows 64 wg ..
+    const int wg = warp >> 2;
+    const int tid = threadIdx.x & 127;
+    const int wq = warp & 3;
+    uint8_t* stiles = staging + wg * 2 * GEMM_STAGE_TILE;
+    RingPos rp;
+    long long t_full = 0;
     const long long t_begin = p.dbg ? clock64() : 0;
-    for (int pair = cluster; pair < num_pairs; pair += num_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      long long w0 = p.dbg ? clock64() : 0;
-      mbar_wait(&acc_empty[acc], acc_phase ^ 1);      // epilogue has drained this accumulator
-      if (p.dbg) t_wacc += clock64() - w0;
-      tc_fence_after_sync();
-      const uint32_t d_tmem = tmem_base + acc * Cfg::ACC_STRIDE;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        if (p.dbg) w0 = clock64();
-        mbar_wait(&full_bar[stage], phase);
-        if (p.dbg) t_wfull += clock64() - w0;
-        tc_fence_after_sync();
-        const uint32_t sa = smem_u32(ring + stage * Cfg::STAGE_BYTES);
-        const uint64_t adesc = umma_desc_sw128(sa, 1024);
-        const uint64_t bdesc = umma_desc_sw128(sa + Cfg::A_BYTES, 1024);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            // +32 B per K=16 step inside the 128-byte swizzle atom (start-address field is >>4)
-            umma_bf16_pair(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-          }
-          umma_commit_pair(&empty_bar[stage], kAllCtas);    // slot reusable in both CTAs once these MMAs retire
-          if (kb == num_kb - 1) umma_commit_pair(&acc_full[acc], kAllCtas);   // accumulators complete in both CTAs -> epilogues
-        }
-        __syncwarp();
-        if (++stage == num_stages) { stage = 0; phase ^= 1; }
-      }
-    }
-    if (p.dbg && lane == 0) { p.dbg[blockIdx.x * 8 + 0] = clock64() - t_begin; p.dbg[blockIdx.x * 8 + 1] = t_wfull; p.dbg[blockIdx.x * 8 + 2] = t_wacc; }
-  } else if (warp < GEMM_EPI_WARPS) {
-    // ------------------------------------------------------------ epilogue
-    const int ew = warp;
-    const int quarter = warp & 3;                     // TMEM lane quarter this warp may access
-    const int half = ew >> 2;                         // which half of the BN columns
-    uint8_t* stile = staging + ew * GEMM_STAGE_TILE;  // this warp's 32 x 128 B staging tile (TMA epilogues)
-    const int sw = lane & 7;
-    int it = 0;
-    long long t_wfull = 0;
-    const long long t_begin = clock64();
-    for (int pair = cluster; pair < num_pairs; pair += num_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int mp_i = (p.dbg_flags & 4) ? pair % num_mp : pair / num_n;
-      const int mt = mp_i * GEMM_CL + cta_rank;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int mt, nb;
+      tile_mn(tile, mt, nb);
       const int m0 = mt * GEMM_BM;
-      const int nb = (p.dbg_flags & 4) ? pair / num_mp : pair % num_n;
       const int n0 = kDeconv ? 0 : nb * BN;
-      const int row = m0 + quarter * 32 + lane;
-      const bool row_ok = kDeconv ? (quarter * 32 + lane < up_pos && mt < num_m) : (row < p.M);
-      const long long w0 = clock64();
-      // load + add + store form of the residual epilogue: the rows were completed by an earlier launch, so the warp's first
-      // 32 x 32 box of x is requested before the accumulator is ready
-      [[maybe_unused]] float4 xr[8];
-      [[maybe_unused]] bool rmw = false;
-      if constexpr (EPI == EPI_F32_ADD) {
-        rmw = p.rmw != 0;
-        if (rmw) rmw_load_box(xr, reinterpret_cast<const float*>(p.out), p.ldc, m0 + quarter * 32, lane, p.M, n0 + half * Cfg::HALF);
-      }
-      mbar_wait(&acc_full[acc], acc_phase);
-      t_wfull += clock64() - w0;
-      tc_fence_after_sync();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * Cfg::ACC_STRIDE;
+      tile_mainloop<BN>(acc, ring, Cfg::STAGE_BYTES, full_bar, empty_bar, num_kb, num_stages, rp, wg, lane,
+                        (p.dbg && threadIdx.x == 0) ? &t_full : nullptr);
+      const int row0 = m0 + 64 * wg;                  // first row of this warpgroup
 
-      if constexpr (EPI == EPI_F32_ADD) {
-        if (rmw)
-          epilogue_f32_rmw<Cfg::HALF / 32>(t_row + half * Cfg::HALF, n0 + half * Cfg::HALF, m0 + quarter * 32, p.M, p.bias,
-                                           reinterpret_cast<float*>(p.out), p.ldc, xr, stile, lane);
-      }
       if constexpr (epi_uses_tma(EPI)) {
-        if (!rmw) {
-        // 64 bf16 or 32 f32 output columns (= one 128-byte staging row) per round
-        constexpr int COLS = (EPI == EPI_F32_ADD) ? 32 : 64;
-#pragma unroll 1
-        for (int c = 0; c < Cfg::HALF; c += COLS) {
-          const int col = half * Cfg::HALF + c;
-          const int n = n0 + col;
-          if (elect_one()) tma_store_wait_read<0>();  // previous store has finished reading the staging tile (elect.sync is
-                                                      // deterministic for a full mask: the same lane commits and waits)
-          __syncwarp();
-#pragma unroll
-          for (int sub = 0; sub < COLS; sub += 32) {
-            uint32_t r[32];
-            tmem_ld32(t_row + col + sub, r);
-            tmem_ld_wait();
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n + sub + j));
-              v[j] = __uint_as_float(r[j]) + b4.x; v[j + 1] = __uint_as_float(r[j + 1]) + b4.y;
-              v[j + 2] = __uint_as_float(r[j + 2]) + b4.z; v[j + 3] = __uint_as_float(r[j + 3]) + b4.w;
-            }
-            if constexpr (EPI == EPI_BF16_GELU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = gelu_fast(v[j]);
-            }
-            if constexpr (EPI == EPI_BF16_GELU_ERF) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = gelu_erf_as(v[j]);
-            }
-            // staging row = lane, 16-byte chunk index XOR (lane % 8): what a SWIZZLE_128B tensor map expects
-            uint8_t* srow = stile + lane * 128;
-            if constexpr (EPI == EPI_F32_ADD) {
-#pragma unroll
-              for (int q = 0; q < 8; ++q)
-                *reinterpret_cast<float4*>(srow + ((q ^ sw) << 4)) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            } else {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint4 w;
-                w.x = pack_bf16(v[8 * q], v[8 * q + 1]); w.y = pack_bf16(v[8 * q + 2], v[8 * q + 3]);
-                w.z = pack_bf16(v[8 * q + 4], v[8 * q + 5]); w.w = pack_bf16(v[8 * q + 6], v[8 * q + 7]);
-                *reinterpret_cast<uint4*>(srow + ((((sub >> 3) + q) ^ sw) << 4)) = w;
-              }
-            }
-          }
-          fence_proxy_async_smem();                   // staging writes -> visible to the TMA engine
-          __syncwarp();
-          if (n < p.N && elect_one()) {
-            if constexpr (EPI == EPI_F32_ADD) tma_reduce_add_2d(&tmap_out, stile, n, m0 + quarter * 32);
-            else tma_store_2d(&tmap_out, stile, n, m0 + quarter * 32);   // rows past M are clipped by the tensor map
-            tma_store_commit();
-          }
-        }
-        }
+        if (EPI == EPI_F32_ADD && p.rmw) epilogue_f32_rmw<BN>(acc, n0, row0, p.M, p.bias, reinterpret_cast<float*>(p.out), p.ldc, tid);
+        else epilogue_tma<BN, EPI>(acc, n0, row0, p.N, p.bias, stiles, wg, tid, &tmap_out);
       } else {
         // ---- direct epilogues (scattered / transposed outputs)
-        size_t out_row = static_cast<size_t>(row);
-        if constexpr (EPI == EPI_BF16_RELU_UP) {
-          const int tiles_x = p.up_w / p.up_tw;
-          const int tiles_per_img = (p.up_h / p.up_tr) * tiles_x;
-          const int r = quarter * 32 + lane;                              // position inside the tile (valid < up_pos)
-          const int b = mt / tiles_per_img, ti = mt % tiles_per_img;
-          const int y = (ti / tiles_x) * p.up_tr + r / p.up_tw, x = (ti % tiles_x) * p.up_tw + r % p.up_tw;
-          out_row = (static_cast<size_t>(b) * (2 * p.up_h) + (2 * y + (nb >> 1))) * (2 * p.up_w) + (2 * x + (nb & 1));
-        }
-#pragma unroll 1
-        for (int c = 0; c < Cfg::HALF; c += Cfg::CH) {
-          const int col = half * Cfg::HALF + c;       // column inside the tile
-          const int n = n0 + col;                     // global column
-          uint32_t r[Cfg::CH];
-          tmem_ld<Cfg::CH>(t_row + col, r);
-          tmem_ld_wait();
-          float v[Cfg::CH];
+        const int cq = 2 * (lane & 3);
 #pragma unroll
-          for (int j = 0; j < Cfg::CH; ++j) v[j] = __uint_as_float(r[j]);
-          if (p.bias != nullptr) {
-#pragma unroll
-            for (int j = 0; j < Cfg::CH; j += 4) {
-              const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n + j));
-              v[j] += b4.x; v[j + 1] += b4.y; v[j + 2] += b4.z; v[j + 3] += b4.w;
-            }
-          }
+        for (int h = 0; h < 2; ++h) {
+          const int r = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;     // row inside the tile
           if constexpr (EPI == EPI_BF16_RELU_UP) {
+            if (r >= up_pos || mt >= num_m) continue;
+            const int tiles_x = p.up_w / p.up_tw;
+            const int tiles_per_img = (p.up_h / p.up_tr) * tiles_x;
+            const int b = mt / tiles_per_img, ti = mt % tiles_per_img;
+            const int y = (ti / tiles_x) * p.up_tr + r / p.up_tw, x = (ti % tiles_x) * p.up_tw + r % p.up_tw;
+            const size_t out_row = (static_cast<size_t>(b) * (2 * p.up_h) + (2 * y + (nb >> 1))) * (2 * p.up_w) + (2 * x + (nb & 1));
+            uint32_t* o = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + out_row * p.ldc);
 #pragma unroll
-            for (int j = 0; j < Cfg::CH; ++j) v[j] = fmaxf(v[j], 0.0f);
-            if (row_ok && n < p.N) {
-              __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + out_row * p.ldc + n;
-#pragma unroll
-              for (int j = 0; j < Cfg::CH; j += 8) {
-                uint4 q;
-                q.x = pack_bf16(v[j], v[j + 1]); q.y = pack_bf16(v[j + 2], v[j + 3]);
-                q.z = pack_bf16(v[j + 4], v[j + 5]); q.w = pack_bf16(v[j + 6], v[j + 7]);
-                *reinterpret_cast<uint4*>(o + j) = q;
-              }
+            for (int j = 0; j < BN / 8; ++j) {
+              const int n = 8 * j + cq;
+              if (n >= p.N) continue;
+              const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+              o[n >> 1] = pack_bf16(fmaxf(acc[4 * j + 2 * h] + b2.x, 0.0f), fmaxf(acc[4 * j + 2 * h + 1] + b2.y, 0.0f));
             }
-          } else {  // EPI_F32_NCHW: a warp's 32 lanes are 32 consecutive pixels -> coalesced per channel
-            if (row_ok) {
-              const int b = row / p.pix, pix = row % p.pix;
-              float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(b) * p.n_valid) * p.pix + pix;
+          } else {  // EPI_F32_NCHW
+            const int row = m0 + r;
+            if (row >= p.M) continue;
+            const int b = row / p.pix, pix = row % p.pix;
+            float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(b) * p.n_valid) * p.pix + pix;
 #pragma unroll
-              for (int j = 0; j < Cfg::CH; ++j) {
-                if (n + j < p.n_valid) o[static_cast<size_t>(n + j) * p.pix] = v[j];
-              }
+            for (int j = 0; j < BN / 8; ++j) {
+              const int n = n0 + 8 * j + cq;
+              float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+              if (p.bias != nullptr) { v0 += p.bias[n]; v1 += p.bias[n + 1]; }
+              if (n < p.n_valid) o[static_cast<size_t>(n) * p.pix] = v0;
+              if (n + 1 < p.n_valid) o[static_cast<size_t>(n + 1) * p.pix] = v1;
             }
           }
         }
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&acc_empty[acc], 0);   // the leader's MMA thread waits for both CTAs' epilogues
 
       if constexpr (EPI == EPI_F32_ADD) {
         if (p.ln_out != nullptr && mt < num_m) {
           // ---- fused LayerNorm tail
-          if (elect_one()) tma_store_wait_all<0>();         // this warp's reduce-adds have been performed in L2
-          asm volatile("bar.sync 2, 256;" ::: "memory");    // all 8 epilogue warps of this CTA are done with the tile
+          if (tid == 0) tma_store_wait_all<0>();            // this warpgroup's reduce-adds have been performed in L2
+          named_bar_sync(GEMM_BAR_EPI, 256);                // both consumer warpgroups are done with the tile
           if (threadIdx.x == 0) {
             __threadfence();
             const int old = atomicAdd(p.ln_counters + mt, 1);
@@ -507,13 +401,13 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             if (last) p.ln_counters[mt] = 0;                // every column tile has arrived: reset for the next launch
             *ln_flag = last;
           }
-          asm volatile("bar.sync 2, 256;" ::: "memory");
+          named_bar_sync(GEMM_BAR_EPI, 256);
           if (*ln_flag) {
             __threadfence();                                // acquire side of the counter hand-off
             const int r_end = min(GEMM_BM, p.M - m0);
             const float* xb = reinterpret_cast<const float*>(p.out) + static_cast<size_t>(m0) * p.N;
             __nv_bfloat16* yb = p.ln_out + static_cast<size_t>(m0) * p.N;
-            for (int r = ew; r < r_end; r += GEMM_EPI_WARPS) {
+            for (int r = warp; r < r_end; r += GEMM_CONSUMER_WARPS) {
               const float* xr = xb + static_cast<size_t>(r) * p.N;
               __nv_bfloat16* yr = yb + static_cast<size_t>(r) * p.N;
               switch (p.N) {
@@ -524,26 +418,16 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               }
             }
           }
-          asm volatile("bar.sync 2, 256;" ::: "memory");    // ln_flag is rewritten at the next tile
+          named_bar_sync(GEMM_BAR_EPI, 256);                // ln_flag is rewritten at the next tile
         }
       }
     }
     if constexpr (epi_uses_tma(EPI)) {
-      if (elect_one()) tma_store_wait_read<0>();      // staging must stay alive until the TMA engine has read it; the
-                                                      // writes themselves complete before the grid does
+      if (tid == 0) tma_store_wait_all<0>();        // staging must stay alive until the TMA engine is done with it
     }
-    if (p.dbg && warp == 0 && lane == 0) { p.dbg[blockIdx.x * 8 + 5] = clock64() - t_begin; p.dbg[blockIdx.x * 8 + 6] = t_wfull; }
+    if (p.dbg && threadIdx.x == 0) { p.dbg[blockIdx.x * 8 + 0] = clock64() - t_begin; p.dbg[blockIdx.x * 8 + 1] = t_full; }
   }
-
-  tc_fence_before_sync();
-  cluster_sync_all();                                 // the peer may still read this CTA's smem / arrive on its barriers
-  if (warp == 8) tmem_dealloc_pair(tmem_base, Cfg::TMEM_COLS);
-  if (p.dbg && threadIdx.x == 0) {                    // CTA lifetime in SM cycles, and (odd CTAs, slot 0) in nanoseconds
-    long long t_ns1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_ns1));
-    p.dbg[blockIdx.x * 8 + 7] = clock64() - t_cta0;
-    if (cta_rank == 1) p.dbg[blockIdx.x * 8 + 0] = t_ns1 - t_ns0;
-  }
+  if (p.dbg && threadIdx.x == 0) p.dbg[blockIdx.x * 8 + 7] = clock64() - t_cta0;
 }
 
 }  // namespace vpb

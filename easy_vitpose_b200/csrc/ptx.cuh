@@ -1,5 +1,5 @@
-// Inline-PTX building blocks for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA +
-// TMEM) and the shared-memory / instruction descriptors the tensor core consumes.
+// Inline-PTX building blocks for sm_90a: mbarrier, TMA (cp.async.bulk.tensor) and the shared-memory descriptors wgmma
+// consumes (the wgmma instructions themselves are in wgmma.cuh).
 // Everything here is a thin wrapper over one PTX instruction; the kernels own the protocol.
 #pragma once
 #include <cuda_bf16.h>
@@ -60,15 +60,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---------------------------------------------------------------- proxies / fences
-// generic-proxy smem writes -> visible to the async proxy (TMA / tensor core reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA stores, wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -82,38 +76,12 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-
-// Same load, multicast to every CTA of the cluster whose bit is set in `mask`: the box lands at the same
-// CTA-relative smem offset in each destination and completes tx bytes on the mbarrier at the same offset there.
-__device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// CTA-pair load (cta_group::2): the box lands in THIS CTA's smem, the tx bytes complete on the mbarrier at the same
-// offset in the pair's leader CTA (even rank: peer bit 24 of the shared::cluster address cleared).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
 // 4-D variant (NHWC feature maps: channel, x, y, image); coordinates may lie outside the tensor (zero fill = conv padding).
-__device__ __forceinline__ void tma_load_4d_pair(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, int c3) {
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
-}
-// arrive on the barrier at this offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(smem_u32(bar)), "r"(cta) : "memory");
 }
 // smem tile -> global through the tensor map (rows / columns outside the tensor are clipped).
 __device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int c0, int c1) {
@@ -133,153 +101,33 @@ __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bu
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // Kernels are chained on one stream with cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's CTAs
-// may be scheduled (and run their prologue: barrier init, TMEM alloc, descriptor prefetch) while the previous grid is
-// still draining.  pdl_wait() blocks until the previous grid has completed and its writes are visible; nothing that
-// reads or writes global memory may precede it.  Without the launch attribute both are no-ops.
+// may be scheduled (and run their prologue: barrier init, descriptor prefetch) while the previous grid is still draining.
+// pdl_wait() blocks until the previous grid has completed and its writes are visible; nothing that reads or writes global
+// memory may precede it.  Without the launch attribute both are no-ops.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// ---------------------------------------------------------------- clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_count_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+// named barrier over `count` threads (a multiple of 32) of the CTA
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// ---------------------------------------------------------------- TMEM
-// Whole-warp (.sync.aligned) instructions: call from one full warp.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// CTA-pair variants: issued by the same warp of BOTH CTAs of the pair with the same smem offset.
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 bit, N consecutive columns: thread i of the warp receives lane (base_lane + i),
-// columns col .. col+N-1.  A warp may only touch the lane quarter (warp_id % 4).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t (&r)[N]) {
-  static_assert(N == 8 || N == 16 || N == 32, "chunk width");
-  if constexpr (N == 32) tmem_ld32(taddr, r);
-  else if constexpr (N == 16) tmem_ld16(taddr, r);
-  else tmem_ld8(taddr, r);
-}
-
-// ---------------------------------------------------------------- UMMA (tcgen05.mma)
-// Shared-memory matrix descriptor (64 bit):
-//   [0,14) start address >> 4      [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version = 1 (sm_100)   [49,52) base offset                [61,64) layout: 0 none, 2 SW128, 4 SW64, 6 SW32
-// K-major operand, 128-byte swizzle: a row is 64 bf16 = 128 B, the 16-byte chunks of row r are
-// XOR-ed with (r % 8), 8-row groups are 1024 B apart (SBO); LBO is unused.  Tile base 1024-aligned.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout_type) {
+// ---------------------------------------------------------------- wgmma shared-memory operand descriptor (sm_90)
+//   [0,14) start address >> 4     [16,30) leading byte offset >> 4     [32,46) stride byte offset >> 4
+//   [49,52) base offset (0: tiles 1024-byte aligned)                     [62,64) layout: 0 none, 1 SW128, 2 SW64, 3 SW32
+// Operand tiles whose rows are W bytes wide (W = 128 / 64 / 32 = the swizzle span TMA wrote them with): 8-row groups are
+// 8*W bytes apart (SBO); LBO is unused for these single-atom-wide tiles.  K-major: a K = 16 step is +32 bytes of the start
+// address inside the swizzle atom.  MN-major (B = V of attention): a K = 16 step is 16 whole rows further.
+template <int ROW_BYTES>
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
+  static_assert(ROW_BYTES == 128 || ROW_BYTES == 64 || ROW_BYTES == 32, "swizzle span");
+  constexpr uint64_t layout = ROW_BYTES == 128 ? 1 : ROW_BYTES == 64 ? 2 : 3;
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout_type) << 61;
+  d |= static_cast<uint64_t>((8 * ROW_BYTES) >> 4) << 32;
+  d |= layout << 62;
   return d;
-}
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) { return umma_desc(smem_addr, sbo_bytes, 2); }
-// Operand tiles whose rows are W bytes wide (W = 128 / 64 / 32 = the swizzle span): 8-row groups are 8*W bytes apart.
-// Works for both majors: K-major reads 16 elements (32 B) of each row per MMA, MN-major reads 16 whole rows.
-template <int ROW_BYTES>
-__device__ __forceinline__ uint64_t umma_desc_rows(uint32_t smem_addr) {
-  static_assert(ROW_BYTES == 128 || ROW_BYTES == 64 || ROW_BYTES == 32, "swizzle span");
-  return umma_desc(smem_addr, 8 * ROW_BYTES, ROW_BYTES == 128 ? 2 : ROW_BYTES == 64 ? 4 : 6);
-}
-// Instruction descriptor, kind::f16, bf16 x bf16 -> f32:
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)      [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n, bool b_mn_major = false) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (b_mn_major ? (1u << 16) : 0u) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread for the whole CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(static_cast<uint32_t>(accumulate))
-      : "memory");
-}
-// CTA-pair MMA (cta_group::2, M = 256): issued by ONE thread of the leader CTA; A rows 0..127 / W rows 0..N/2-1 come from
-// the leader's smem, A rows 128..255 / W rows N/2..N-1 from the peer's smem at the same offsets; each CTA's TMEM receives
-// its own 128 accumulator rows.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(static_cast<uint32_t>(accumulate))
-      : "memory");
-}
-// arrive on the barrier at this offset in every CTA of `mask` once all pair-MMAs issued so far have completed
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// Arrive on `bar` once every tcgen05.mma issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// Same, arriving on the barrier at this offset in every CTA of the cluster selected by `mask`.
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
 }
 
 // ---------------------------------------------------------------- small math / packing
@@ -317,9 +165,9 @@ __device__ __forceinline__ float gelu_tanh_fit(float x) {
   return fmaf(hx, t, hx);
 }
 // One lane of a fully converged warp.  Issue loops run WARP-UNIFORM (all 32 lanes execute the control flow, descriptors and
-// addresses are the same in every lane) and only the tcgen05 / TMA instruction itself is predicated on this: inside an
-// `if (lane == 0)` branch the compiler cannot prove the operands uniform and wraps every UTCHMMA / UTMALDG in an
-// ELECT + R2UR.BROADCAST + BRA.U.ANY "waterfall" loop, which costs the issuing thread ~100 cycles per instruction.
+// addresses are the same in every lane) and only the TMA instruction itself is predicated on this: inside an
+// `if (lane == 0)` branch the compiler cannot prove the operands uniform and may wrap every UTMALDG in an
+// ELECT + R2UR.BROADCAST + BRA.U.ANY "waterfall" loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(

@@ -1,4 +1,4 @@
-"""Drop-in boundary for easy_ViTPose/inference.py: the torch engine backend re-bound to the B200 engine.
+"""Drop-in boundary for easy_ViTPose/inference.py: the torch engine backend re-bound to the H100 engine.
 
 The reference picks its engine in VitInference.__init__ by assigning `self._vit_pose` and
 `self._inference = self._inference_torch` (easy_ViTPose/inference.py:156-172); the per-person loop then
@@ -38,7 +38,7 @@ def pre_img(img: np.ndarray, target_size=(192, 256)):
 
 
 class B200PoseBackend:
-    """Owns a B200 `ViTPose` engine and exposes the three methods VitInference's torch backend consists of:
+    """Owns an H100 `ViTPose` engine and exposes the three methods VitInference's torch backend consists of:
     pre_img (:314-318), _inference (:320-328), postprocess (:187-205)."""
 
     def __init__(self, model: ViTPose, device: "int | str | None" = None):
@@ -148,7 +148,7 @@ def frame_inference(self, img: np.ndarray) -> dict:
 
 
 def install(vit_inference, max_batch: int = 64, device=None, batched: bool = False) -> B200PoseBackend:
-    """Re-bind a constructed reference `VitInference` (torch .pth backend) to the B200 engine: takes the
+    """Re-bind a constructed reference `VitInference` (torch .pth backend) to the H100 engine: takes the
     weights out of its `_vit_pose` module, then replaces `_vit_pose` and `_inference` exactly where
     easy_ViTPose/inference.py:156-172 set them.  With `batched=True` the object's `inference` method is re-bound to
     `frame_inference` as well (one engine call per frame instead of one per person).  Returns the backend (also stored

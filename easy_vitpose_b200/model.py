@@ -1,5 +1,5 @@
 """ViTPose(cfg): the reference's model object (easy_ViTPose/vit_models/model.py:10-24) backed by the
-sm_100a engine.  Same constructor argument, same state_dict key contract, same forward signature;
+sm_90a engine.  Same constructor argument, same state_dict key contract, same forward signature;
 the arithmetic runs in libvitpose_b200.so (bf16 tensor-core GEMMs, fp32 residual stream/softmax/LN).
 
 torch is used for what it is good at here: owning device memory and the current stream.
@@ -123,13 +123,13 @@ class ViTPose:
 
     def train(self, mode: bool = True):
         if mode:
-            raise RuntimeError("the B200 engine is inference-only (eval mode); training stays with the reference")
+            raise RuntimeError("the engine is inference-only (eval mode); training stays with the reference")
         return self
 
     def to(self, device):
         dev = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
         if dev.type != "cuda":
-            raise RuntimeError(f"ViTPose(B200) has no {dev.type} path: it needs a CUDA sm_100 device")
+            raise RuntimeError(f"ViTPose has no {dev.type} path: it needs a CUDA sm_90 (H100) device")
         index = dev.index if dev.index is not None else torch.cuda.current_device()
         if self._device is not None and self._device != index and self._handle:
             raise RuntimeError("engine already lives on another device")

@@ -1,12 +1,12 @@
-/* vitpose_b200.h -- C ABI of the B200-native ViTPose crop engine (libvitpose_b200.so).
+/* vitpose_b200.h -- C ABI of the H100-native ViTPose crop engine (libvitpose_b200.so).
  *
- * One data-parallel hot path of JunkyByte/easy_ViTPose, rebuilt for sm_100a:
+ * One data-parallel hot path of JunkyByte/easy_ViTPose, rebuilt for sm_90a:
  *     crops f32 [B,3,256,192] -> ViT backbone -> TopdownHeatmapSimpleHead -> heatmaps f32 [B,K,64,48]
  *     -> argmax + DARK/UDP refine -> keypoints f32 [B,K,3] rows (y, x, score)
  * Plain pointers and sizes only; no torch types.  Device pointers are CUDA device addresses on the
  * engine's device, `stream` is a cudaStream_t passed as void* (NULL = default stream).  All calls are
  * asynchronous on `stream` unless stated; none of them frees or keeps caller memory.
- * There is no CPU fallback: every entry point fails (non-zero + vpb_last_error()) without an sm_100 GPU.
+ * There is no CPU fallback: every entry point fails (non-zero + vpb_last_error()) without an sm_90 (H100) GPU.
  *
  * Concurrency contract.  An engine owns ONE activation workspace, two host-staging slots and its CUDA graphs:
  *   - calls on one engine must come from one host thread at a time (the handle holds no lock);
@@ -18,9 +18,9 @@
  *     submit(0) is ordered after them;
  *   - if `stream` is being captured by the caller, the engine launches its kernels eagerly into that capture (no nested
  *     graph) and leaves its cross-stream ordering to the caller;
- *   - several engines may share one GPU.  Calls that launch the chained persistent GEMM kernels (batch >= the "chain_min_batch"
- *     option, 48 by default) are serialised per device across engines and streams (a device-side event wait plus a host mutex
- *     around the enqueue): such a kernel needs all of its thread-block clusters resident at once and must not share the SMs
+ *   - several engines may share one GPU.  Calls that launch the chained persistent GEMM kernels (option "chain" on, batch >= the
+ *     "chain_min_batch" option) are serialised per device across engines and streams (a device-side event wait plus a host mutex
+ *     around the enqueue): such a kernel needs all of its CTAs resident at once and must not share the SMs
  *     with a second one.  Another PROCESS running chained launches on the same GPU (MPS) is outside that gate: give chained
  *     engines the GPU to themselves or set option "chain" = 0;
  *   - engines on different devices may live in one process: each entry point makes its engine's device current for the
@@ -172,11 +172,11 @@ int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* Options (all keep the results bit-identical unless noted): "stop_after", "profile", "pdl", "graph", "ln_fused",
- * "chain" (chained persistent launches, default 1), "chain_min_batch" (smallest batch that takes them, default 48),
+ * "chain" (chained persistent launches, default 0: measured slower on H100), "chain_min_batch" (smallest batch that takes them, default 1),
  * "ln_in_gemm" (LayerNorm + its consumer GEMM as one launch on the unchained path, default 0), "gelu_erf" (fc1 epilogue with
  * erf instead of the fitted tanh form: rounding-level differences), "ln_ctl" (chained launches: counter polls / publishes of
  * the LayerNorm jobs on a control warp, default 1; VPB_LN_CTL), "ln_job_rows" (8 | 16 rows per LayerNorm job, default 16),
- * "resid_rmw" (residual epilogues as load + add + store instead of TMA reduce-add: measured slower, default 0; VPB_RESID_RMW). */
+ * "resid_rmw" (residual epilogues as load + add + store instead of TMA reduce-add, default 0; VPB_RESID_RMW). */
 int vpb_set_option(vpb_engine* e, const char* name, int32_t value);
 /* With option "profile"=1 every launch is bracketed by a CUDA-event pair on its stream; collect() synchronises,
  * sums elapsed ms and launch counts per kernel class (arrays of vpb_profile_classes() entries) and resets. */
@@ -195,10 +195,10 @@ int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, void* d_out,
 /* Debug: limit the GEMM smem ring depth and/or collect per-CTA cycle counters (int64 [grid*8]) for following GEMM launches. */
 int vpb_debug_gemm(int32_t stages_limit, void* d_counters);
 int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream);
-/* Debug / measurement switch (process-wide) for the attention variants.  flags < 0: the defaults (packed half tiles for
- * head_dim 32 / 64 with every 4th softmax exponential evaluated by a polynomial on the FMA pipe; VPB_ATT_PACK / VPB_ATT_POLY = 0 / 1
- * in the environment change them); otherwise bit 0 = polynomial exponentials, bit 1 = packed half tiles, bits 8.. = cap on the
- * number of CTAs (0 = one per SM; tests use it to move the boundaries of the per-CTA step ranges). */
+/* Debug / measurement switch (process-wide) for the attention kernel.  flags < 0: the defaults (every softmax exponential on
+ * the MUFU; VPB_ATT_POLY = 1 in the environment evaluates every 4th one by a polynomial on the FMA pipe instead); otherwise
+ * bit 0 = polynomial exponentials, bits 8.. = cap on the number of CTAs (0 = one per SM; tests use it to give every CTA
+ * several items). */
 int vpb_debug_attention(int32_t flags);
 int vpb_layernorm(const float* d_x, const float* d_gamma, const float* d_beta, void* d_y, int32_t rows, int32_t dim,
                   float eps, void* stream);

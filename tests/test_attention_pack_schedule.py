@@ -1,78 +1,56 @@
-"""CPU: the step / item-stage schedule of the packed attention kernel (attention_pack.cuh), restated in Python.
+"""CPU: the item / operand-stage schedule of the attention kernel (attention.cuh), restated in Python.
 
-A launch has 3 steps per pair of heads (kind 0: rows 0..127 of item A, kind 1: rows 0..127 of item B, kind 2: rows 128..191 of
-both).  The steps are split into contiguous ranges over the CTAs; a CTA keeps Q,K and V of the items it needs in THREE stages
-(local item li -> stage li % 3) and refills the Q,K halves / the V halves of a pair's two stages after that pair's packed step.
-Invariants checked here for every CTA of many (batch, heads, grid) shapes -- they are what makes the kernel's waits terminate and
-its operands valid:
+A launch has batch * heads items (crop, head); CTA c of a grid of G takes items c, c + G, c + 2G, ... in order.  Q, K and V of an
+item live in one of TWO stages (local item li -> stage li % 2, its (li // 2)-th use: barrier phase (li // 2) & 1).  Thread 0
+loads local items 0 and 1 before the loop; after item li has been computed by all three warpgroups (a CTA barrier) it refills
+that item's stage with local item li + 2.  (The file keeps its name from the project's earlier packed-pair kernel; the
+properties it pins are the same ones.)  Invariants checked here for every CTA of many (batch, heads, grid) shapes -- they are
+what makes the kernel's waits terminate and its operands valid:
   * every row of every item is produced exactly once over the launch;
-  * every step finds the items it reads resident, in the stage and barrier phase the kernel computes for them;
-  * no load overwrites a stage whose current item is still needed by a later step of the CTA;
-  * every load a CTA issues is consumed by one of its steps (a CTA must not exit with a TMA load in flight).
+  * every item finds its operands resident, in the stage and barrier phase the kernel computes for it;
+  * no load overwrites a stage whose current item is still needed;
+  * every load a CTA issues is consumed by that CTA (a CTA must not exit with a TMA load in flight).
 Keep `cta_schedule` in step with the index arithmetic of the kernel.
 """
 import pytest
 
 
 def cta_schedule(items: int, grid: int, cta: int):
-    """Mirror of attention_pack_tcgen05's per-CTA bookkeeping: (steps, item0, n_items) with steps = [(kind, liA, liB)]."""
-    steps_all = 3 * (items // 2)
-    u0, u1 = steps_all * cta // grid, steps_all * (cta + 1) // grid
-    T = u1 - u0
-    item0 = 2 * (u0 // 3) + (1 if (u0 % 3 == 1 and T == 1) else 0)
-    last_u = u1 - 1
-    n_items = (2 * (last_u // 3) + (0 if last_u % 3 == 0 else 1) - item0 + 1) if T > 0 else 0
-    steps = []
-    for t in range(T):
-        u = u0 + t
-        liA = 2 * (u // 3) - item0
-        steps.append((u % 3, liA, liA + 1))
-    return u0, steps, item0, n_items
+    """Mirror of attention_wgmma's per-CTA bookkeeping: the global items of this CTA, in the order it computes them."""
+    return list(range(cta, items, grid))
 
 
 def simulate(items: int, grid: int, cta: int):
-    """Runs the QK-side (== the V-side: same rules) load / use protocol of one CTA; returns the rows it produces."""
-    u0, steps, item0, n_items = cta_schedule(items, grid, cta)
-    stage = [None, None, None]                              # local item resident in each stage
-    loads = []                                              # order of loads per stage: the li-th item is its (li // 3)-th use
+    """Runs the load / use protocol of one CTA; returns the rows it produces."""
+    mine = cta_schedule(items, grid, cta)
+    stage = [None, None]                                    # local item resident in each stage
+    loads = []
     used = set()
+    done = set()
 
     def load(li):
-        assert 0 <= li < n_items
-        s = li % 3
-        if stage[s] is not None:                            # the item being replaced must not be needed by any later step
-            assert all(stage[s] not in needs(k, a, b) for k, a, b in steps[t_now:]), (items, grid, cta, li, stage[s])
-        assert sum(1 for x in loads if x % 3 == s) == li // 3   # barrier phase (li // 3) & 1 = number of earlier loads of this stage
+        assert 0 <= li < len(mine)
+        s = li % 2
+        if stage[s] is not None:                            # the item being replaced must already be computed
+            assert stage[s] in done, (items, grid, cta, li, stage[s])
+        assert sum(1 for x in loads if x % 2 == s) == li // 2   # barrier phase (li // 2) & 1 = number of earlier loads of this stage
         stage[s] = li
         loads.append(li)
 
-    def needs(kind, liA, liB):
-        return {0: {liA}, 1: {liB}, 2: {liA, liB}}[kind]
-
-    t_now = 0
-    for li in range(min(3, n_items)):
-        load(li)
+    # prologue (thread 0): item blockIdx.x and item blockIdx.x + gridDim.x, when they exist
+    if cta < items:
+        load(0)
+    if cta + grid < items:
+        load(1)
     produced = []
-    for t, (kind, liA, liB) in enumerate(steps):
-        t_now = t
-        for li in needs(kind, liA, liB):
-            assert 0 <= li < n_items and stage[li % 3] == li, (items, grid, cta, t, kind, li, stage)
-            used.add(li)
-        if kind == 0:
-            produced += [(item0 + liA, r) for r in range(128)]
-        elif kind == 1:
-            produced += [(item0 + liB, r) for r in range(128)]
-        else:
-            produced += [(item0 + liA, r) for r in range(128, 192)] + [(item0 + liB, r) for r in range(128, 192)]
-        # the kernel refills after a packed step: Q,K in the NEXT iteration of the issue loop (once the packed step's MMAs have
-        # retired), V right after the packed step's last P V retired -- in both cases before the following step needs them
-        if kind == 2:
-            t_now = t + 1
-            if liA + 3 < n_items:
-                load(liA + 3)
-            if liA + 4 < n_items:
-                load(liA + 4)
-    assert set(loads) == used == set(range(n_items)), (items, grid, cta, loads, used)    # every load consumed, nothing missing
+    for li, item in enumerate(mine):
+        assert stage[li % 2] == li, (items, grid, cta, li, stage)
+        used.add(li)
+        produced += [(item, r) for r in range(192)]          # three warpgroups x 64 query rows
+        done.add(li)
+        if item + 2 * grid < items:                         # the refill after the CTA barrier
+            load(li + 2)
+    assert set(loads) == used == set(range(len(mine))), (items, grid, cta, loads, used)    # every load consumed, nothing missing
     return produced
 
 
@@ -80,7 +58,6 @@ def simulate(items: int, grid: int, cta: int):
 @pytest.mark.parametrize("sms", [148, 132, 8, 1])
 def test_every_row_once_and_operands_resident(batch, heads, sms):
     items = batch * heads
-    assert items % 2 == 0
     grid = min(items, sms)                                  # engine.cu: attention_launch
     rows = []
     for cta in range(grid):
@@ -89,19 +66,17 @@ def test_every_row_once_and_operands_resident(batch, heads, sms):
 
 
 def test_single_step_ranges_start_at_the_item_they_need():
-    """CTAs that own exactly one step: a lone kind-1 step must not load (and leave unconsumed) item A of its pair; a lone packed
-    step loads both items.  Swept over grids that produce all three cases."""
-    kinds = set()
+    """CTAs that own exactly one item load that item and nothing else (the prologue's second load must be skipped, or it would
+    stay unconsumed); CTAs with two items load both up front and refill nothing.  Swept over grids that produce both cases."""
+    counts = set()
     for items, grid in [(12, 12), (8, 7), (10, 9), (14, 13), (16, 11), (6, 5), (20, 19), (22, 17)]:
         for cta in range(grid):
-            u0, steps, item0, n_items = cta_schedule(items, grid, cta)
-            if len(steps) == 1:
-                kind, liA, liB = steps[0]
-                kinds.add(kind)
-                assert n_items == (2 if kind == 2 else 1)
-                if kind == 1:
-                    assert item0 % 2 == 1 and liB == 0
-                else:
-                    assert item0 % 2 == 0 and liA == 0
+            mine = cta_schedule(items, grid, cta)
+            counts.add(len(mine))
+            assert mine[0] == cta
+            if len(mine) == 1:
+                assert cta + grid >= items
+            if len(mine) == 2:
+                assert mine[1] + 2 * grid >= items            # hence no refill
             simulate(items, grid, cta)
-    assert kinds == {0, 1, 2}
+    assert {1, 2} <= counts

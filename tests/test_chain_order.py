@@ -7,7 +7,7 @@ import pytest
 
 
 def locate(g, num_mp, n_of, lag0, lag1):
-    """Mirror of the lambda in gemm_chain_tcgen05 (keep the two in step)."""
+    """Mirror of the lambda in gemm_chain_wgmma (keep the two in step); num_mp counts 128-row blocks."""
     lag0, lag1 = min(lag0, num_mp), min(lag1, num_mp)
     wave0 = num_mp * (n_of[0] + n_of[1])
     w1 = g >= wave0

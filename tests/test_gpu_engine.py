@@ -309,8 +309,7 @@ def test_shard_pipeline_single_rank_matches_infer_crops(golden_dir):
 
 
 def test_narrow_tiles_for_small_batches_are_bit_identical(golden_dir):
-    """Below ~16 crops the proj / fc2 / patch (and for <= 5 crops also qkv / fc1) GEMMs run 128-wide tiles instead of 256-wide ones
-    (engine.cu pick_tile: twice the tiles, half the K-loop time each).  The accumulation order of an output element does not depend
+    """The standalone GEMMs run 128-wide tiles instead of 256-wide ones where N allows (engine.cu pick_tile).  The accumulation order of an output element does not depend
     on the tile shape, so heatmaps, keypoints and argmax must not change by a bit (debug flag 16 forces the wide tiles)."""
     import ctypes as C
 
@@ -342,6 +341,8 @@ def test_two_engines_share_one_gpu_on_two_streams(golden_dir):
     B = 48
     a, _ = _engine(g, max_batch=B)
     b, _ = _engine(g, max_batch=B)
+    for e in (a, b):
+        e.set_option("chain", 1)                                      # chained launches are opt-in
     assert a.kernel_launches(B) == b.kernel_launches(B) == 1 + (1 + int(g["meta"][1])) + int(g["meta"][1]) + 4   # the chained count
     xs = [torch.from_numpy(O.make_crops(B, 900 + i)).cuda() for i in range(3)]
     org = torch.tensor([[190, 260]] * B, dtype=torch.int32).cuda()

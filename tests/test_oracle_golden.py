@@ -5,7 +5,7 @@ import os
 import numpy as np
 import pytest
 
-from oracle import ref_import, vitpose_oracle as O
+from oracle import vitpose_oracle as O
 
 FWD = ["s_coco", "b_coco", "l_coco_25", "h_wholebody"]
 
@@ -53,12 +53,13 @@ def test_decode_edge_cases(golden_dir, name, wrap):
     assert np.all(err[~well] <= 1e-3 + 1e-3 * np.abs(ref[~well]))
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree only exists in the build container")
-def test_live_reference_decode_matches_oracle():
-    ns = ref_import.load()
+def test_live_reference_decode_matches_oracle(golden_dir):
+    """The oracle's decode against the unmodified reference's postprocess of the same maps (stored by
+    oracle/make_golden_reference_checks.py)."""
+    ref_all = _load(golden_dir, "reference_checks")["decode_kpts"]
     maps = O.make_decode_maps(2, 17, 999)
     for i in range(2):
-        ref = ref_import.postprocess(ns, maps[i:i + 1], 200 + i, 300 + i)
+        ref = ref_all[i:i + 1]
         kp, _ = O.decode_maps(maps[i:i + 1], np.array([[200 + i, 300 + i]]), wrap="crop")
         assert np.array_equal(kp[..., 2], ref[..., 2])
         assert np.abs(kp - ref).max() < 1e-3 + 1e-3 * np.abs(ref).max()

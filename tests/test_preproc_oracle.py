@@ -1,11 +1,11 @@
 """CPU: oracle/preproc_oracle.py (SURVEY.md section 8 row f1) against the fixtures the UNMODIFIED reference produced
-(oracle/make_golden_frames.py), against cv2 where it is installed, and against the reference tree where it is mounted."""
+(oracle/make_golden_frames.py, oracle/make_golden_reference_checks.py) and against cv2 where it is installed."""
 import os
 
 import numpy as np
 import pytest
 
-from oracle import preproc_oracle as P, ref_import
+from oracle import preproc_oracle as P
 
 
 def _case(golden_dir, name):
@@ -67,21 +67,21 @@ def test_to_frame_coords_is_one_rounding():
     assert np.array_equal(out[..., 2], kp[..., 2])
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not mounted (GPU box)")
-def test_against_reference_pad_image_and_pre_img():
-    cv2 = pytest.importorskip("cv2")
-    inf = ref_import.load_vitinference()
-    rs = np.random.RandomState(2)
+def test_against_reference_pad_image_and_pre_img(golden_dir):
+    """The oracle's canvas and pre_img against the unmodified reference's pad_image / pre_img on seeded boxes (stored by
+    oracle/make_golden_reference_checks.py: whole canvases; pre_img's whole output for the first boxes, a seeded sample of it
+    for the others)."""
+    from oracle.make_golden_reference_checks import PRE_FULL, pre_boxes, pre_sample_index, unpack_exact
+    g = np.load(os.path.join(golden_dir, "reference_checks.npz"))
     frame = P.make_frame(200, 260, 5)
-    stub = type("S", (), {"target_size": (192, 256)})()
-    for _ in range(12):
-        x0, y0 = rs.randint(-20, 240), rs.randint(-20, 180)
-        box = np.array([x0, y0, x0 + rs.randint(1, 150), y0 + rs.randint(1, 150)])
-        bx0, by0, bx1, by1 = P.padded_box(box, 200, 260)
-        if bx1 <= bx0 or by1 <= by0:
-            continue
-        padded, (left, top) = inf.pad_image(frame[by0:by1, bx0:bx1], 3 / 4)
+    cases = pre_boxes()
+    assert np.array_equal(np.array([b for b, _ in cases]), g["pre_boxes"])
+    for i, (box, (bx0, by0, _, _)) in enumerate(cases):
+        left, top = (int(v) for v in g["pre_left_top"][i])
         canvas, off = P.crop_canvas(frame, box)
-        assert np.array_equal(canvas, padded) and off == (by0 - top, bx0 - left)
-        x, org_h, org_w = inf.VitInference.pre_img(stub, padded)
-        assert np.array_equal(P.pre_img(canvas), x) and (org_h, org_w) == canvas.shape[:2]
+        assert np.array_equal(canvas, g[f"canvas_{i}"]) and off == (by0 - top, bx0 - left)
+        x = P.pre_img(canvas)
+        assert np.array_equal(np.asarray(x, np.float32).reshape(-1)[pre_sample_index(i)], g["pre_x_sample"][i])
+        if i < PRE_FULL:
+            assert np.array_equal(np.asarray(x, np.float32), unpack_exact(g[f"pre_x_table_{i}"], g[f"pre_x_index_{i}"]))
+        assert tuple(canvas.shape[:2]) == tuple(int(v) for v in g["pre_org_hw"][i])

@@ -28,7 +28,7 @@ for (heads, hd, B), flags in itertools.product(((12, 64, 64), (16, 64, 64), (16,
         _lib.check(L.vpb_attention(C.c_void_p(qkv.data_ptr()), B, heads, hd, C.c_void_p(out.data_ptr()), None))
     e1.record(); torch.cuda.synchronize()
     us = e0.elapsed_time(e1) * 100
-    n = min(B * heads, 148)
+    n = min(B * heads, torch.cuda.get_device_properties(0).multi_processor_count)
     dbg = torch.zeros(n * 8, dtype=torch.int64, device=dev)
     L.vpb_debug_gemm(0, C.c_void_p(dbg.data_ptr()))
     attention(qkv, B, heads, hd)
@@ -38,7 +38,5 @@ for (heads, hd, B), flags in itertools.product(((12, 64, 64), (16, 64, 64), (16,
     steps = m[7]
     flops = 4 * B * heads * 192 * 192 * hd
     print(f"hd={hd} B={B} heads={heads}: {us:.1f} us/launch = {flops / us / 1e6:.0f} TFLOP/s; per CTA: lifetime {m[0]:.0f} cyc (max {d[:,0].max():.0f}), "
-          f"{steps:.2f} tile steps (max {d[:,7].max():.0f}) -> {m[0]/steps:.0f} cyc/step")
-    print(f"   softmax group A warp 0 (per step of the CTA): wait S {m[1]/steps:.0f} busy {m[2]/steps:.0f} | group B warp 4: wait S {m[5]/steps:.0f} busy {m[6]/steps:.0f} "
-          f"| epilogue warp 8: wait {m[3]/steps:.0f} busy {m[4]/steps:.0f}")
+          f"{steps:.2f} items (max {d[:,7].max():.0f}) -> {m[0]/max(steps, 1):.0f} cyc/item, of which waiting for operands {m[1]/max(steps, 1):.0f}")
 L.vpb_debug_attention(-1)

@@ -19,22 +19,22 @@ with torch.cuda.stream(side):
     for _ in range(3):
         m.forward_features(x)
     torch.cuda.synchronize()
-    dbg = torch.zeros(74 * 4 * 12, dtype=torch.int64, device="cuda")
+    SMS = torch.cuda.get_device_properties(0).multi_processor_count   # the chained grid is at most one CTA per SM
+    dbg = torch.zeros(SMS * 4 * 12, dtype=torch.int64, device="cuda")
     _lib.lib().vpb_debug_gemm(0, C.c_void_p(dbg.data_ptr()))
     m.forward_features(x)                  # backbone only: the head's GEMMs share the debug pointer
     torch.cuda.synchronize()
     _lib.lib().vpb_debug_gemm(0, None)
-d = dbg.cpu().numpy().reshape(74, 4, 12).astype(np.float64)
+d = dbg.cpu().numpy().reshape(SMS, 4, 12).astype(np.float64)
 # launch 0 (patch -> qkv) lands in phases 0,1 too: 13 launches accumulate; block launches dominate (12 of 13)
 names = ["proj(+patch)", "fc1(+qkv0)", "fc2", "qkv"]
-tot = d[:, :, 0].sum(1).mean()
-print(f"B={B}: MMA-thread cycles per cluster over one forward (13 chained launches): {tot:.0f}")
+print(f"B={B}: cycles per CTA over one forward (13 chained launches)")
 for ph in range(4):
-    t, wf, wa, dep, ring, eb, ew, n = d[:, ph, :8].mean(0)
-    print(f"  {names[ph]:13s} tiles/cluster {n:5.1f}  mma {t:9.0f} cyc ({t / tot:5.1%}) = {t / max(n, 1):7.0f}/tile | wait operands {wf / max(t, 1):5.1%}  wait epilogue {wa / max(t, 1):5.1%} "
-          f"| producer: dependency wait {dep / max(n, 1):6.0f}/tile ({d[:, ph, 11].mean() / max(dep, 1):.0%} of it on the cluster's first tile of the phase), ring wait {ring / max(n, 1):6.0f}/tile | epilogue warp 0: busy {eb / max(n, 1):6.0f}/tile, wait {ew / max(n, 1):6.0f}/tile")
+    _, wf, _, dep, ring, eb, _, n = d[:, ph, :8].mean(0)
+    print(f"  {names[ph]:13s} tiles/CTA {n:5.1f} | consumer wait for operands {wf / max(n, 1):6.0f}/tile, epilogue {eb / max(n, 1):6.0f}/tile "
+          f"| producer: dependency wait {dep / max(n, 1):6.0f}/tile ({d[:, ph, 11].mean() / max(dep, 1):.0%} of it on the CTA's first tile of the phase), ring wait {ring / max(n, 1):6.0f}/tile")
 for st, ph in ((0, 0), (1, 2)):
     w, b, n = d[:, ph, 8:11].mean(0)
     rows, other, pub = d[:, ph + 1, 8:11].mean(0)
-    print(f"  LayerNorm stage {st} (warp 12 of the leader CTAs): jobs/CTA {n:5.1f}, busy {b / max(n, 1):7.0f} cyc/job (own rows {rows / max(n, 1):.0f}, waiting for the other "
+    print(f"  LayerNorm stage {st} (first LayerNorm warp): jobs/CTA {n:5.1f}, busy {b / max(n, 1):7.0f} cyc/job (own rows {rows / max(n, 1):.0f}, waiting for the other "
           f"three warps {other / max(n, 1):.0f}, fence + release {pub / max(n, 1):.0f}), wait for the residual rows {w / max(n, 1):7.0f} cyc/job")

@@ -30,14 +30,14 @@ for name, (K, N, epi) in shapes.items():
         e1.record(); torch.cuda.synchronize()
         us = e0.elapsed_time(e1) * 100
         print(f"{name:5s} flags={stages >> 8} {us:8.1f} us  {2*M*N*K/us/1e6:8.1f} TFLOP/s")
-    dbg = torch.zeros(148 * 8, dtype=torch.int64, device=dev)
+    SMS = torch.cuda.get_device_properties(0).multi_processor_count    # the GEMM grid is at most one CTA per SM
+    dbg = torch.zeros(SMS * 8, dtype=torch.int64, device=dev)
     L.vpb_debug_gemm(0, C.c_void_p(dbg.data_ptr()))
     gemm(a, w, bias, out, epi)
-    d = dbg.cpu().reshape(148, 8).double()
+    d = dbg.cpu().reshape(SMS, 8).double()
     m = d.mean(0)
-    m[:3] = d[0::2, :3].mean(0)        # the MMA thread only exists in the leader (even) CTA of each pair
-    print(f"      cycles/CTA: mma total {m[0]:.0f} wait_full {m[1]:.0f} ({m[1]/m[0]:.0%}) wait_acc_empty {m[2]:.0f} ({m[2]/m[0]:.0%}) | "
-          f"producer total {m[3]:.0f} wait_empty {m[4]:.0f} ({m[4]/max(m[3],1):.0%}) | epilogue total {m[5]:.0f} wait_acc_full {m[6]:.0f} ({m[6]/max(m[5],1):.0%})")
+    print(f"      cycles/CTA: consumer total {m[0]:.0f} wait for operands {m[1]:.0f} ({m[1]/max(m[0],1):.0%}) | "
+          f"producer total {m[3]:.0f} wait_empty {m[4]:.0f} ({m[4]/max(m[3],1):.0%}) | CTA lifetime {m[7]:.0f}")
     life_cyc = d[:, 7].mean(); life_ns = d[1::2, 0].mean()
     print(f"      CTA lifetime {life_cyc:.0f} cycles = {life_ns/1e3:.1f} us -> SM clock {life_cyc/life_ns:.2f} GHz")
     L.vpb_debug_gemm(0, None)
