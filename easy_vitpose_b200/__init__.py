@@ -7,7 +7,7 @@ csrc/ holds the hand-written CUDA (wgmma GEMM + attention, LayerNorm, gathers, d
 model.ViTPose, top_down_eval.keypoints_from_heatmaps, inference.install / B200PoseBackend.
 """
 from . import distributed  # noqa: F401
-from .configs import data_cfg, dyn_model_import, model_cfg  # noqa: F401
+from .configs import COCO_FLIP_PAIRS, data_cfg, dyn_model_import, flip_pairs_for, model_cfg  # noqa: F401
 from .inference import B200PoseBackend, install  # noqa: F401
 from .model import ViTPose  # noqa: F401
 from .top_down_eval import decode_heatmaps, decode_topdown, keypoints_from_heatmaps  # noqa: F401

@@ -48,6 +48,7 @@ EXPORTS = {
     "vpb_host_free": (None, [C.c_void_p]),
     "vpb_kernel_launches": (C.c_int, [C.c_void_p, C.c_int32]),
     "vpb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int32]),
+    "vpb_set_flip_test": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]),
     "vpb_profile_classes": (C.c_int, []),
     "vpb_profile_class_name": (C.c_char_p, [C.c_int32]),
     "vpb_profile_collect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

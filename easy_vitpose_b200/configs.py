@@ -16,6 +16,21 @@ DATASET_KEYPOINTS = {"coco": 17, "coco_25": 25, "wholebody": 133, "mpii": 16, "a
 
 data_cfg = dict(image_size=[192, 256], heatmap_size=[48, 64])   # ViTPose_common.py:29-31
 
+# left/right keypoint pairs for the flip test: eye, ear, shoulder, elbow, wrist, hip, knee, ankle (datasets/COCO.py:114).
+# The reference defines pairs for COCO only.
+COCO_FLIP_PAIRS = ((1, 2), (3, 4), (5, 6), (7, 8), (9, 10), (11, 12), (13, 14), (15, 16))
+
+
+def flip_pairs_for(dataset: str, flip_pairs=None) -> "list[tuple[int, int]]":
+    """The flip pairs of a dataset: explicit `flip_pairs` win, 'coco' gets COCO_FLIP_PAIRS, any other dataset raises
+    ValueError -- the reference gives no pairs for them, and a keypoint count alone does not determine them (ap10k also has
+    17 keypoints, with other pairs)."""
+    if flip_pairs is not None:
+        return [(int(a), int(b)) for a, b in flip_pairs]
+    if dataset == "coco":
+        return list(COCO_FLIP_PAIRS)
+    raise ValueError(f"no flip pairs known for dataset {dataset!r}: pass flip_pairs explicitly")
+
 
 def model_cfg(size: str, num_keypoints: int) -> dict:
     name = MODEL_ABBR.get(size, size)

@@ -359,6 +359,11 @@ struct vpb_engine {
   uint8_t* frame_stage[2] = {nullptr, nullptr};
   size_t frame_cap[2] = {0, 0};
   int32_t* bbox_stage[2] = {nullptr, nullptr};
+  // flip test (vpb_set_flip_test): the keypoint entry points run each crop and its mirror image as one batch of 2n crops and
+  // decode the averaged maps; flip_perm = the keypoint permutation of the flip pairs, flip_shift = shift_heatmap
+  bool flip = false;
+  int flip_shift = 0;
+  int32_t* flip_perm = nullptr;
   std::map<std::string, std::pair<float*, int64_t>> staged;   // fp32 state_dict tensors on device until finalize
   std::vector<void*> allocs;
   // packed weights
@@ -641,6 +646,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(dev_alloc(e, &e->pp_status, 1));
   CU_TRY(cudaMemset(e->pp_status, 0, sizeof(int32_t)));
   for (int s = 0; s < 2; ++s) VPB_TRY(dev_alloc(e, &e->bbox_stage[s], B * 4));
+  VPB_TRY(dev_alloc(e, &e->flip_perm, e->K));
   CU_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
   CU_TRY(cudaStreamCreateWithFlags(&e->compute_stream, cudaStreamNonBlocking));
   VPB_TRY(make_map(&e->m_patch_rows, e->patch_rows, M, 768, 768, 128));
@@ -709,10 +715,11 @@ static GemmParams gp(int M, int N, int K, const float* bias, void* out, int ldc)
 
 // stop_after stages (debug): 1 patch rows, 2 patch embed, 3 first LN, 4 first qkv, 5 first attention, 6 first proj,
 // 7 first fc1, 8 first block, 9 all blocks, 10 last norm, 11 deconv1, 12 deconv2
-static int patch_gather(vpb_engine* e, const float* d_crops, int B, cudaStream_t st) {
+// B crops of patch rows from n_src source crops: n_src == B, or B == 2 n_src for the flip test (crops n_src.. mirrored)
+static int patch_gather(vpb_engine* e, const float* d_crops, int n_src, int B, cudaStream_t st) {
   e->prof.begin(KC_PATCH_IM2COL, st);
   CU_TRY(launch_k(patch_im2col, dim3(cdiv(static_cast<long long>(B) * 3 * 256 * 24, 256)), dim3(256), 0, st, d_crops, e->patch_rows, B,
-                  reinterpret_cast<const float4*>(e->pos_bias), reinterpret_cast<float4*>(e->x), e->D));
+                  n_src, reinterpret_cast<const float4*>(e->pos_bias), reinterpret_cast<float4*>(e->x), e->D));
   e->prof.end(st);
   return VPB_OK;
 }
@@ -724,18 +731,18 @@ struct Source {
   int fh = 0, fw = 0;
   const int32_t* bboxes = nullptr;
 };
-static int frame_gather(vpb_engine* e, const Source& src, int B, cudaStream_t st) {
+static int frame_gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
   FramePatchParams q;
   q.pp.frame = src.frame; q.pp.pitch = static_cast<long long>(src.fw) * 3; q.pp.fh = src.fh; q.pp.fw = src.fw; q.pp.bboxes = src.bboxes;
-  q.pp.n = B; q.pp.pad = 10; q.pp.crops = nullptr; q.pp.org_wh = e->pp_org; q.pp.offs_yx = e->pp_offs; q.pp.status = e->pp_status;
+  q.pp.n = n_src; q.pp.pad = 10; q.pp.crops = nullptr; q.pp.org_wh = e->pp_org; q.pp.offs_yx = e->pp_offs; q.pp.status = e->pp_status;
   q.rows = e->patch_rows; q.pos_bias = reinterpret_cast<const float4*>(e->pos_bias); q.stream = reinterpret_cast<float4*>(e->x); q.D = e->D;
   e->prof.begin(KC_PREPROCESS, st);
   CU_TRY(launch_k(frame_to_patch_rows, dim3(B, 16), dim3(384), 0, st, q));
   e->prof.end(st);
   return VPB_OK;
 }
-static int gather(vpb_engine* e, const Source& src, int B, cudaStream_t st) {
-  return src.crops ? patch_gather(e, src.crops, B, st) : frame_gather(e, src, B, st);
+static int gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
+  return src.crops ? patch_gather(e, src.crops, n_src, B, st) : frame_gather(e, src, n_src, B, st);
 }
 // Chained form of the backbone (chain.cuh): 1 + depth persistent GEMM launches + depth attention launches.
 //   launch 0:        patch embed (+= x) -> LN(norm1 of block 0) -> qkv of block 0
@@ -1056,6 +1063,13 @@ static int check_ready(vpb_engine* e, int batch) {
   if (batch < 1 || batch > e->maxB) return fail(VPB_ERR_ARG, "batch %d outside 1..max_batch=%d", batch, e->maxB);
   return VPB_OK;
 }
+// the keypoint entry points: with flip test on, the batch and its mirror images share the max_batch workspace
+static int check_ready_keypoints(vpb_engine* e, int batch) {
+  VPB_TRY(check_ready(e, batch));
+  if (e->flip && 2 * batch > e->maxB)
+    return fail(VPB_ERR_ARG, "batch %d: with flip test on a call takes at most max_batch / 2 = %d crops (max_batch=%d)", batch, e->maxB / 2, e->maxB);
+  return VPB_OK;
+}
 
 extern "C" int vpb_forward(vpb_engine* e, const float* d_crops, int32_t batch, float* d_heatmaps, void* stream) {
   VPB_TRY(check_ready(e, batch));
@@ -1065,7 +1079,7 @@ extern "C" int vpb_forward(vpb_engine* e, const float* d_crops, int32_t batch, f
   VPB_TRY(apply_l2_policy(e, st));
   WsScope ws(e, st);
   VPB_TRY(ws.begin(batch));
-  VPB_TRY(patch_gather(e, d_crops, batch, st));
+  VPB_TRY(patch_gather(e, d_crops, batch, batch, st));
   VPB_TRY(backbone(e, batch, st));
   if (!(e->stop_after && e->stop_after <= 10)) VPB_TRY(head(e, batch, d_heatmaps, st));
   return ws.end();
@@ -1078,7 +1092,7 @@ extern "C" int vpb_forward_features(vpb_engine* e, const float* d_crops, int32_t
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   WsScope ws(e, st);
   VPB_TRY(ws.begin(batch));
-  VPB_TRY(patch_gather(e, d_crops, batch, st));
+  VPB_TRY(patch_gather(e, d_crops, batch, batch, st));
   VPB_TRY(backbone(e, batch, st));
   const long long tot = static_cast<long long>(batch) * e->D * 192;
   tokens_to_nchw<<<cdiv(tot, 256), 256, 0, st>>>(e->xn, d_features, batch, e->D);
@@ -1193,14 +1207,30 @@ extern "C" int vpb_decode_frame(const float* d_heatmaps, int32_t n, int32_t k, c
   return decode_launch(d_heatmaps, n, k, d_org_wh, d_offs_yx, d_kpts, d_idx, wrap_batch, stream);
 }
 
+// Crops one keypoint call runs through the model: the batch, and with flip test on its mirror images as well.
+static int model_crops(const vpb_engine* e, int batch) { return e->flip ? 2 * batch : batch; }
+
+// Flip test: e->heat holds the 2 * batch raw maps of one forward; `out` (batch maps; may be e->heat) gets their flip-back average.
+static int flip_average(vpb_engine* e, int batch, float* out, cudaStream_t st) {
+  const long long tot = static_cast<long long>(batch) * e->K * 3072;
+  e->prof.begin(KC_DECODE, st);
+  CU_TRY(launch_k(flip_average_heatmaps, dim3(cdiv(tot, 256)), dim3(256), 0, st, static_cast<const float*>(e->heat), out,
+                  static_cast<const int*>(e->flip_perm), static_cast<int>(batch), e->K, e->flip_shift));
+  e->prof.end(st);
+  return VPB_OK;
+}
+
+// `heat` receives the batch maps the keypoints are decoded from; with flip test the raw 2 * batch maps go to e->heat first
 static int infer_enqueue(vpb_engine* e, const Source& src, const int32_t* d_org_wh, const int32_t* d_offs_yx, int32_t batch,
                          float* d_kpts, int32_t* d_idx, float* heat, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  VPB_TRY(gather(e, src, batch, st));
-  VPB_TRY(backbone(e, batch, st));
+  const int nb = model_crops(e, batch);
+  VPB_TRY(gather(e, src, batch, nb, st));
+  VPB_TRY(backbone(e, nb, st));
   if (e->stop_after && e->stop_after <= 10) return VPB_OK;
-  VPB_TRY(head(e, batch, heat, st));
+  VPB_TRY(head(e, nb, e->flip ? e->heat : heat, st));
   if (e->stop_after) return VPB_OK;
+  if (e->flip) VPB_TRY(flip_average(e, batch, heat, st));
   e->prof.begin(KC_DECODE, static_cast<cudaStream_t>(stream));
   VPB_TRY(decode_launch(heat, batch, e->K, d_org_wh, d_offs_yx, d_kpts, d_idx, 0, stream));
   e->prof.end(static_cast<cudaStream_t>(stream));
@@ -1215,7 +1245,7 @@ static int infer_core(vpb_engine* e, const Source& src, const int32_t* d_org_wh,
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   VPB_TRY(apply_l2_policy(e, st));
   WsScope ws(e, st);
-  VPB_TRY(ws.begin(batch));
+  VPB_TRY(ws.begin(model_crops(e, batch)));
   VPB_TRY(infer_core_locked(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, d_heatmaps, stream));
   return ws.end();
 }
@@ -1234,15 +1264,17 @@ static int infer_core_locked(vpb_engine* e, const Source& src, const int32_t* d_
     e->graphs.push_back({batch, 1, nullptr});
     return infer_enqueue(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, heat, stream);
   }
-  VPB_TRY(gather(e, src, batch, st));
+  const int nb = model_crops(e, batch);
+  VPB_TRY(gather(e, src, batch, nb, st));
   CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
   else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(batch) * 2 * sizeof(int32_t), st));
   if (!g->exec) {                                                         // second use: capture, instantiate
     cudaGraph_t graph = nullptr;
     CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = backbone(e, batch, st);
-    if (rc == VPB_OK) rc = head(e, batch, e->heat, st);
+    int rc = backbone(e, nb, st);
+    if (rc == VPB_OK) rc = head(e, nb, e->heat, st);
+    if (rc == VPB_OK && e->flip) rc = flip_average(e, batch, e->heat, st);      // in place: the first batch maps
     if (rc == VPB_OK) rc = decode_launch(e->heat, batch, e->K, e->g_org, e->g_offs, e->g_kpts, e->g_idx, 0, stream);
     const cudaError_t ce = cudaStreamEndCapture(st, &graph);
     if (rc != VPB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
@@ -1261,7 +1293,7 @@ static int infer_core_locked(vpb_engine* e, const Source& src, const int32_t* d_
 
 extern "C" int vpb_infer(vpb_engine* e, const float* d_crops, const int32_t* d_org_wh, int32_t batch, float* d_kpts, int32_t* d_idx,
                          float* d_heatmaps, void* stream) {
-  VPB_TRY(check_ready(e, batch));
+  VPB_TRY(check_ready_keypoints(e, batch));
   DeviceGuard dev_guard(e);
   if (!d_crops || !d_org_wh || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer: null pointer");
   Source src;
@@ -1296,7 +1328,7 @@ static int infer_frame_enqueue(vpb_engine* e, const uint8_t* d_frame, int32_t fr
 
 extern "C" int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int32_t frame_w, const int32_t* d_bboxes,
                                int32_t n, float* d_kpts, int32_t* d_idx, void* stream) {
-  VPB_TRY(check_ready(e, n));
+  VPB_TRY(check_ready_keypoints(e, n));
   DeviceGuard dev_guard(e);
   if (!d_frame || !d_bboxes || !d_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame: bad argument");
   return infer_frame_enqueue(e, d_frame, frame_h, frame_w, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
@@ -1337,7 +1369,7 @@ static int frame_stage_reserve(vpb_engine* e, int slot, size_t bytes) {
 
 extern "C" int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
                                     int32_t n, float* h_kpts, int32_t* h_idx, void* stream) {
-  VPB_TRY(check_ready(e, n));
+  VPB_TRY(check_ready_keypoints(e, n));
   DeviceGuard dev_guard(e);
   if (!h_frame || !h_bboxes || !h_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame_host: bad argument");
   VPB_TRY(check_boxes_host(h_bboxes, n, frame_h, frame_w));
@@ -1359,7 +1391,7 @@ extern "C" int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32
 // 16 B per box instead of 589 824 B per crop.
 extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
                                      int32_t n, float* h_kpts, int32_t* h_idx, int32_t slot) {
-  VPB_TRY(check_ready(e, n));
+  VPB_TRY(check_ready_keypoints(e, n));
   DeviceGuard dev_guard(e);
   if (!h_frame || !h_bboxes || !h_kpts || frame_h < 1 || frame_w < 1 || slot < 0 || slot > 1)
     return fail(VPB_ERR_ARG, "vpb_submit_frame_host: bad argument");
@@ -1380,7 +1412,7 @@ extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int3
 
 extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t* h_org_wh, int32_t batch, float* h_kpts,
                               int32_t* h_idx, void* stream) {
-  VPB_TRY(check_ready(e, batch));
+  VPB_TRY(check_ready_keypoints(e, batch));
   DeviceGuard dev_guard(e);
   if (!h_crops || !h_org_wh || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_host: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1400,7 +1432,7 @@ extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t
 // the H2D of batch i+1 runs under the compute of batch i.  Host buffers must stay valid (and should be pinned) until wait().
 extern "C" int vpb_submit_host(vpb_engine* e, const float* h_crops, const int32_t* h_org_wh, int32_t batch, float* h_kpts,
                                int32_t* h_idx, int32_t slot) {
-  VPB_TRY(check_ready(e, batch));
+  VPB_TRY(check_ready_keypoints(e, batch));
   DeviceGuard dev_guard(e);
   if (!h_crops || !h_org_wh || !h_kpts || slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "vpb_submit_host: bad argument");
   // the slot's previous use must have finished with its staging buffers before they are overwritten
@@ -1435,10 +1467,12 @@ extern "C" int vpb_kernel_launches(const vpb_engine* e, int32_t batch) {
   if (!e) return -1;
   // patch im2col + patch GEMM + depth*(qkv, attention, proj, fc1, fc2) + 2 deconv GEMMs + 1x1 GEMM + decode; the 2*depth+1
   // LayerNorms ride in the tails of the patch / proj / fc2 GEMMs unless ln_fused is switched off
-  if (e->use_chain && batch >= e->chain_min_batch && !e->ln_fused) return 1 + (1 + e->depth) + e->depth + 2 + 1 + 1;   // gather, chains, attention, deconvs, 1x1, decode
+  // flip test adds the flip-back average in front of the decode; the chains then see 2 * batch crops
+  if (e->use_chain && model_crops(e, batch) >= e->chain_min_batch && !e->ln_fused)
+    return 1 + (1 + e->depth) + e->depth + 2 + 1 + 1 + (e->flip ? 1 : 0);   // gather, chains, attention, deconvs, 1x1, decode
   // one kernel per GEMM: gather, patch GEMM, depth x (qkv, attention, proj, fc1, fc2), 2 deconvs, 1x1, decode; the LayerNorms are
   // launches of their own (2 * depth + 1), or ride in front of qkv / fc1 (ln_in_gemm: only last_norm is left), or in the tails
-  return 2 + e->depth * 5 + 2 + 1 + 1 + (e->ln_fused ? 0 : e->ln_in_gemm ? 1 : 2 * e->depth + 1);
+  return 2 + e->depth * 5 + 2 + 1 + 1 + (e->ln_fused ? 0 : e->ln_in_gemm ? 1 : 2 * e->depth + 1) + (e->flip ? 1 : 0);
 }
 
 extern "C" int vpb_set_option(vpb_engine* e, const char* name, int32_t value) {
@@ -1466,6 +1500,25 @@ extern "C" int vpb_set_option(vpb_engine* e, const char* name, int32_t value) {
     e->graphs.clear();
   }
   else return fail(VPB_ERR_ARG, "unknown option %s", name);
+  return VPB_OK;
+}
+
+extern "C" int vpb_set_flip_test(vpb_engine* e, const int32_t* h_perm, int32_t k, int32_t shift) {
+  if (!e) return fail(VPB_ERR_ARG, "vpb_set_flip_test: null engine");
+  if (!e->finalized) return fail(VPB_ERR_STATE, "not finalized");
+  if (h_perm) {
+    if (k != e->K) return fail(VPB_ERR_ARG, "vpb_set_flip_test: permutation of %d keypoints, the engine has %d", k, e->K);
+    for (int i = 0; i < k; ++i)
+      if (h_perm[i] < 0 || h_perm[i] >= k) return fail(VPB_ERR_ARG, "vpb_set_flip_test: perm[%d] = %d outside 0..%d", i, h_perm[i], k - 1);
+  }
+  DeviceGuard dev_guard(e);
+  // calls already enqueued (submit slots in flight included) read the old permutation: let them finish first
+  if (e->ws_used) CU_TRY(cudaEventSynchronize(e->ev_ws));
+  if (h_perm) CU_TRY(cudaMemcpy(e->flip_perm, h_perm, static_cast<size_t>(k) * sizeof(int32_t), cudaMemcpyHostToDevice));
+  e->flip = h_perm != nullptr;
+  e->flip_shift = shift ? 1 : 0;
+  for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);      // captured chains embed the batch and the average
+  e->graphs.clear();
   return VPB_OK;
 }
 

@@ -74,7 +74,10 @@ __global__ void __launch_bounds__(128) layernorm_f32_to_bf16(const float* __rest
 // row: reads 32 B of the image (8-byte aligned: columns start at -2), writes 16 B.
 // The same launch seeds the fp32 token stream with  pos_embed[1+t] + pos_embed[0] + conv bias  (vit.py:382), so that the
 // patch GEMM can add its product into it with the TMA reduce-add epilogue like every other residual GEMM.
-__global__ void __launch_bounds__(256) patch_im2col(const float* __restrict__ x, __nv_bfloat16* __restrict__ a, int batch,
+// Flip test: with n_src < batch (batch = 2 n_src) the rows of crop b >= n_src are the im2col of flip(x[b - n_src], dims=[3]):
+// image column xx reads source column 191 - xx, so the float2 pair (xx, xx + 1) is the source pair at 190 - xx (still
+// 8-byte aligned) with its halves swapped.  The mirrored crops are never written to memory.
+__global__ void __launch_bounds__(256) patch_im2col(const float* __restrict__ x, __nv_bfloat16* __restrict__ a, int batch, int n_src,
                                                     const float4* __restrict__ pos_bias, float4* __restrict__ stream, int D) {
   const int total = batch * 3 * 256 * 24;                  // (b, c, y', xchunk)
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -89,15 +92,21 @@ __global__ void __launch_bounds__(256) patch_im2col(const float* __restrict__ x,
   const int c = (i / (24 * 256)) % 3;
   const int b = i / (24 * 256 * 3);
   const int y = yp - 2, x0 = xc * 8 - 2;
+  const bool mirror = b >= n_src;
   float v[8];
   if (y >= 0) {                                            // y' < 256 -> y <= 253 < 256 always
-    const float* src = x + ((static_cast<size_t>(b) * 3 + c) * 256 + y) * 192;
+    const float* src = x + ((static_cast<size_t>(mirror ? b - n_src : b) * 3 + c) * 256 + y) * 192;
 #pragma unroll
     for (int j = 0; j < 8; j += 2) {
       const int xx = x0 + j;                               // even offset from -2: pairs never straddle the border
       if (xx >= 0 && xx < 192) {
-        const float2 f = *reinterpret_cast<const float2*>(src + xx);
-        v[j] = f.x; v[j + 1] = f.y;
+        if (mirror) {
+          const float2 f = *reinterpret_cast<const float2*>(src + 190 - xx);
+          v[j] = f.y; v[j + 1] = f.x;
+        } else {
+          const float2 f = *reinterpret_cast<const float2*>(src + xx);
+          v[j] = f.x; v[j + 1] = f.y;
+        }
       } else {
         v[j] = 0.f; v[j + 1] = 0.f;
       }
@@ -194,6 +203,23 @@ __global__ void flip_back_heatmaps(const float* __restrict__ in, float* __restri
   const int kk = static_cast<int>((i / 3072) % k), nn = static_cast<int>(i / (3072LL * k));
   const int xs = shift ? max(x - 1, 0) : x;
   out[i] = __ldg(in + ((static_cast<size_t>(nn) * k + perm[kk]) * 64 + y) * 48 + (47 - xs));
+}
+
+// Flip-test average over the 2n maps of one forward (maps i < n from the crops, maps n + i from their mirror images):
+//   out[i,k,y,x] = (heat[i,k,y,x] + heat[n+i, perm[k], y, 47 - x']) * 0.5f      (i < n, x' as in flip_back_heatmaps)
+// mmpose's (output + output_flipped) * 0.5 with output_flipped = flip_back_heatmaps of the second half, in the same fp32
+// operations, so bit-identical to that composition.  `out` may be `heat` itself: each output element reads its own position
+// of the first half and the second half, which is never written.
+__global__ void flip_average_heatmaps(const float* heat, float* out, const int* __restrict__ perm, int n, int k, int shift) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  pdl_launch_dependents();
+  pdl_wait();                                               // the 1x1-conv GEMM writes `heat`
+  if (i >= static_cast<long long>(n) * k * 3072) return;
+  const int x = static_cast<int>(i % 48), y = static_cast<int>((i / 48) % 64);
+  const int kk = static_cast<int>((i / 3072) % k), nn = static_cast<int>(i / (3072LL * k));
+  const int xs = shift ? max(x - 1, 0) : x;
+  const float m = heat[((static_cast<size_t>(n + nn) * k + perm[kk]) * 64 + y) * 48 + (47 - xs)];
+  out[i] = __fmul_rn(__fadd_rn(heat[i], m), 0.5f);
 }
 
 }  // namespace vpb

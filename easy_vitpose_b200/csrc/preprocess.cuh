@@ -127,8 +127,10 @@ __global__ void __launch_bounds__(PP_W) crop_resize_normalise(const PreprocParam
 // rows incl. the conv's 2-pixel zero border): the 16 x 192 x 3 pixels are gathered with lanes along the image row into a
 // shared bf16 tile, which is then written out as 16-byte chunks of the im2col rows.
 // Like patch_im2col, the launch also seeds the fp32 token stream with pos_embed + conv bias (vit.py:382).
+// Flip test: a grid of (2 pp.n, 16) CTAs; crop c >= pp.n is the mirror image of crop c - pp.n (box c - pp.n, pixel dx stored at
+// tile column 2 + (191 - dx)), i.e. the patch rows of flip(crop, dims=[3]).  Mirrored CTAs leave org_wh / offs_yx / status alone.
 struct FramePatchParams {
-  PreprocParams pp;             // crops / status unused
+  PreprocParams pp;             // crops unused; pp.n = number of boxes
   __nv_bfloat16* rows;          // [n*192, 768]
   const float4* pos_bias;       // [192*D/4]
   float4* stream;               // [n*192*D/4]
@@ -157,7 +159,9 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const FramePatchParam
     const float f = static_cast<float>(__ddiv_rn(__dsub_rn(__ddiv_rn(static_cast<double>(v), 255.0), mean), stdv));
     s_lut[c][v] = __bfloat16_as_ushort(__float2bfloat16_rn(f));
   }
-  const int* bb = p.bboxes + 4 * crop;
+  const bool mirror = crop >= p.n;
+  const int box = mirror ? crop - p.n : crop;
+  const int* bb = p.bboxes + 4 * box;
   const int x0 = min(max(bb[0] - p.pad, 0), p.fw), x1 = min(max(bb[2] + p.pad, 0), p.fw);
   const int y0 = min(max(bb[1] - p.pad, 0), p.fh), y1 = min(max(bb[3] + p.pad, 0), p.fh);
   int w = x1 - x0, h = y1 - y0;
@@ -168,7 +172,7 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const FramePatchParam
     if (4 * w < 3 * h) { cw = (3 * h) / 4; left = (cw - w) / 2; }
     else { ch = (4 * w) / 3; top = (ch - h) / 2; }
   }
-  if (tid == 0 && py == 0) {
+  if (tid == 0 && py == 0 && !mirror) {
     if (empty && p.status) atomicOr(p.status, 1);
     p.org_wh[2 * crop] = empty ? 0 : cw; p.org_wh[2 * crop + 1] = empty ? 0 : ch;
     p.offs_yx[2 * crop] = y0 - top; p.offs_yx[2 * crop + 1] = x0 - left;
@@ -207,8 +211,9 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const FramePatchParam
         v3[c] = s_lut[c][min(max(v, 0), 255)];
       }
     }
+    const int tx = 2 + (mirror ? PP_W - 1 - dx : dx);
 #pragma unroll
-    for (int c = 0; c < 3; ++c) s_tile[(c * 16 + ky) * FP_PITCH + 2 + dx] = v3[c];
+    for (int c = 0; c < 3; ++c) s_tile[(c * 16 + ky) * FP_PITCH + tx] = v3[c];
   }
   __syncthreads();
   // Phase 2: the im2col rows of this patch row, 16 bytes (8 kx) per store: element (px, c, ky, kx) = tile[c][ky][16 px + kx]

@@ -53,9 +53,10 @@ def infer_sharded(model, crops: torch.Tensor, org_wh: torch.Tensor, group=None):
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     n = crops.shape[0]
     lo, hi = shard_range(n, rank, world)
+    step = getattr(model, "batch_limit", model.max_batch)      # max_batch // 2 with flip test on
     outs_kp, outs_idx = [], []
-    for s in range(lo, hi, model.max_batch):
-        e = min(hi, s + model.max_batch)
+    for s in range(lo, hi, step):
+        e = min(hi, s + step)
         kp, idx = model.infer_crops(crops[s:e], org_wh[s:e])
         outs_kp.append(kp)
         outs_idx.append(idx)
@@ -78,8 +79,9 @@ def infer_frame_sharded(model, frame: torch.Tensor, bboxes: torch.Tensor, group=
     n = bboxes.shape[0]
     lo, hi = shard_range(n, rank, world)
     outs_kp, outs_idx = [], []
-    for s in range(lo, hi, model.max_batch):
-        kp, idx = model.infer_frame(frame, bboxes[s:min(hi, s + model.max_batch)])
+    step = getattr(model, "batch_limit", model.max_batch)
+    for s in range(lo, hi, step):
+        kp, idx = model.infer_frame(frame, bboxes[s:min(hi, s + step)])
         outs_kp.append(kp)
         outs_idx.append(idx)
     if outs_kp:

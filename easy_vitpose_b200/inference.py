@@ -17,7 +17,7 @@ import types
 import numpy as np
 import torch
 
-from .configs import data_cfg, model_cfg
+from .configs import data_cfg, flip_pairs_for, model_cfg
 from .model import ViTPose
 from .top_down_eval import decode_heatmaps
 
@@ -97,8 +97,9 @@ class B200PoseBackend:
         x = np.concatenate([p[0] for p in pre], 0)
         org = np.array([[p[2], p[1]] for p in pre], np.int32)
         out = []
-        for s in range(0, len(imgs), self.model.max_batch):
-            kp, _ = self.model.infer_host(x[s:s + self.model.max_batch], org[s:s + self.model.max_batch])
+        step = self.model.batch_limit
+        for s in range(0, len(imgs), step):
+            kp, _ = self.model.infer_host(x[s:s + step], org[s:s + step])
             out.append(kp)
         return np.concatenate(out, 0)
 
@@ -147,12 +148,16 @@ def frame_inference(self, img: np.ndarray) -> dict:
     return frame_keypoints
 
 
-def install(vit_inference, max_batch: int = 64, device=None, batched: bool = False) -> B200PoseBackend:
+def install(vit_inference, max_batch: int = 64, device=None, batched: bool = False, flip_test: bool = False,
+            flip_pairs=None) -> B200PoseBackend:
     """Re-bind a constructed reference `VitInference` (torch .pth backend) to the H100 engine: takes the
     weights out of its `_vit_pose` module, then replaces `_vit_pose` and `_inference` exactly where
     easy_ViTPose/inference.py:156-172 set them.  With `batched=True` the object's `inference` method is re-bound to
-    `frame_inference` as well (one engine call per frame instead of one per person).  Returns the backend (also stored
-    as `._b200`)."""
+    `frame_inference` as well (one engine call per frame instead of one per person).  With `flip_test=True` every
+    keypoint call runs the flip test of the reference configs (test_cfg flip_test=True, shift_heatmap=False), with the
+    pairs of `flip_pairs_for(vit_inference.dataset, flip_pairs)`; the engine is then built for 2 * max_batch crops, so
+    `max_batch` still counts people per call.  Returns the backend (also stored as `._b200`)."""
+    pairs = flip_pairs_for(getattr(vit_inference, "dataset", None), flip_pairs) if flip_test else None
     ref = vit_inference._vit_pose
     sd = {k: v.detach().cpu() for k, v in ref.state_dict().items()}
     D = sd["backbone.pos_embed"].shape[2]
@@ -161,9 +166,11 @@ def install(vit_inference, max_batch: int = 64, device=None, batched: bool = Fal
     K = sd["keypoint_head.final_layer.weight"].shape[0]
     cfg = model_cfg({384: "s", 768: "b", 1024: "l", 1280: "h"}[D], K)
     cfg["backbone"].update(embed_dim=D, depth=depth, num_heads=heads)
-    model = ViTPose(cfg, max_batch=max_batch)
+    model = ViTPose(cfg, max_batch=2 * max_batch if flip_test else max_batch)
     model.load_state_dict(sd)
     backend = B200PoseBackend(model, device if device is not None else "cuda")
+    if flip_test:
+        model.set_flip_test(pairs)
     vit_inference._vit_pose = model
     vit_inference._inference = backend._inference
     vit_inference.postprocess = types.MethodType(lambda self, hm, w, h: backend.postprocess(hm, w, h), vit_inference)

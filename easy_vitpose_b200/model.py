@@ -111,6 +111,7 @@ class ViTPose:
         self._state: "OrderedDict[str, torch.Tensor] | None" = None
         self._device = None
         self._side = None
+        self._flip = False
         self.backbone = _Backbone(self)              # model.backbone(x) / model.keypoint_head(f), as on the reference module
         self.keypoint_head = _Head(self)
         if device is not None:
@@ -202,13 +203,53 @@ class ViTPose:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self._device).cuda_stream)
 
-    def _check_input(self, x: torch.Tensor) -> torch.Tensor:
+    @property
+    def flip_test(self) -> bool:
+        """Whether the keypoint calls run the flip test (set_flip_test)."""
+        return self._flip
+
+    @property
+    def batch_limit(self) -> int:
+        """Most crops / boxes one keypoint call takes: max_batch, or max_batch // 2 with flip test on (each crop and its
+        mirror image share the workspace)."""
+        return self.max_batch // 2 if self._flip else self.max_batch
+
+    @staticmethod
+    def flip_permutation(num_keypoints: int, flip_pairs) -> "list[int]":
+        """The keypoint permutation the (left, right) pairs induce, built sequentially (a later pair overrides an earlier
+        one), like the loop of flip_back (post_processing/post_transforms.py:110-147)."""
+        perm = list(range(num_keypoints))
+        for left, right in flip_pairs:
+            perm[left], perm[right] = right, left
+        return perm
+
+    def set_flip_test(self, flip_pairs, shift_heatmap: bool = False) -> None:
+        """Flip test on every keypoint call (infer_crops, infer_host, submit_host, infer_frame, infer_frame_host,
+        submit_frame_host): heatmaps of each crop and of its mirror image (flipped back, pairs swapped, shifted by one pixel
+        when shift_heatmap) averaged before the decode -- the test_cfg flip_test=True of the reference configs
+        (configs/ViTPose_common.py:124).  Keypoints and returned heatmaps are then bit-identical to forward_flip_test
+        followed by decode_heatmaps.  A call then takes at most max_batch // 2 crops.  `None` turns it off.  Synchronises
+        the engine's pending work."""
+        self._ensure()
+        if flip_pairs is None:
+            _lib.check(_lib.lib().vpb_set_flip_test(self._handle, None, self.num_keypoints, 0))
+            self._flip = False
+            return
+        flip_pairs = [(int(a), int(b)) for a, b in flip_pairs]
+        if any(not (0 <= i < self.num_keypoints) for pair in flip_pairs for i in pair):
+            raise ValueError(f"flip pairs {flip_pairs} index outside 0..{self.num_keypoints - 1}")
+        perm = np.array(self.flip_permutation(self.num_keypoints, flip_pairs), np.int32)
+        _lib.check_value(_lib.lib().vpb_set_flip_test(self._handle, perm.ctypes.data_as(C.c_void_p), perm.size, 1 if shift_heatmap else 0))
+        self._flip = True
+
+    def _check_input(self, x: torch.Tensor, limit: "int | None" = None) -> torch.Tensor:
         if not isinstance(x, torch.Tensor):
             raise TypeError("expected a torch.Tensor [B,3,256,192]")
         if x.dim() != 4 or tuple(x.shape[1:]) != (3, IMG_H, IMG_W):
             raise ValueError(f"expected [B,3,256,192], got {tuple(x.shape)}")
-        if x.shape[0] < 1 or x.shape[0] > self.max_batch:
-            raise ValueError(f"batch {x.shape[0]} outside 1..max_batch={self.max_batch}")
+        limit = self.max_batch if limit is None else limit
+        if x.shape[0] < 1 or x.shape[0] > limit:
+            raise ValueError(f"batch {x.shape[0]} outside 1..{limit} (max_batch={self.max_batch}, flip test {'on' if self._flip else 'off'})")
         self._ensure()
         if not x.is_cuda:
             x = x.to(torch.device("cuda", self._device), non_blocking=True)
@@ -261,10 +302,7 @@ class ViTPose:
         if hm.dim() != 4 or tuple(hm.shape[2:]) != (HM_H, HM_W):
             raise ValueError(f"expected [N,K,64,48], got {tuple(hm.shape)}")
         K = hm.shape[1]
-        perm = list(range(K))
-        for left, right in flip_pairs:                       # sequential, like the reference's loop over (left, right)
-            perm[left], perm[right] = right, left
-        pt = torch.tensor(perm, dtype=torch.int32, device=hm.device)
+        pt = torch.tensor(self.flip_permutation(K, flip_pairs), dtype=torch.int32, device=hm.device)
         out = torch.empty_like(hm)
         with torch.cuda.device(hm.device):
             _lib.check(_lib.lib().vpb_flip_back(C.c_void_p(hm.data_ptr()), hm.shape[0], K, C.c_void_p(pt.data_ptr()), 1 if shift_heatmap else 0,
@@ -300,8 +338,9 @@ class ViTPose:
     @torch.no_grad()
     def infer_crops(self, x: torch.Tensor, org_wh: torch.Tensor, return_heatmaps: bool = False):
         """Batched crops -> keypoints [B,K,3] (y, x, score) in crop pixels + flat argmax [B,K].
-        org_wh int32 [B,2] = each crop's (width, height) before the resize to 192x256."""
-        x = self._check_input(x)
+        org_wh int32 [B,2] = each crop's (width, height) before the resize to 192x256.  With flip test on (set_flip_test)
+        the keypoints and the returned heatmaps are those of the flip-test average; B <= max_batch // 2."""
+        x = self._check_input(x, self.batch_limit)
         B = x.shape[0]
         org = torch.as_tensor(org_wh).to(device=x.device, dtype=torch.int32).contiguous()
         if tuple(org.shape) != (B, 2):
@@ -345,7 +384,7 @@ class ViTPose:
                                                   kpts_out.ctypes.data_as(C.c_void_p), idx_out.ctypes.data_as(C.c_void_p), int(slot)))
 
     # ---------------------------------------------------------------------------------------- frame-level calls (SURVEY 8 f1/f2)
-    def _check_frame(self, frame: torch.Tensor, bboxes) -> "tuple[torch.Tensor, torch.Tensor]":
+    def _check_frame(self, frame: torch.Tensor, bboxes, limit: "int | None" = None) -> "tuple[torch.Tensor, torch.Tensor]":
         self._ensure()
         if not isinstance(frame, torch.Tensor) or frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3:
             raise ValueError("frame must be a uint8 RGB tensor [H,W,3]")
@@ -358,8 +397,9 @@ class ViTPose:
         if bb.is_floating_point():
             bb = bb.round()                                  # easy_ViTPose/inference.py:253 (round half to even, like numpy)
         bb = bb.to(device=dev, dtype=torch.int32).reshape(-1, 4).contiguous()
-        if bb.shape[0] > self.max_batch:
-            raise ValueError(f"{bb.shape[0]} boxes exceed max_batch={self.max_batch}")
+        limit = self.max_batch if limit is None else limit
+        if bb.shape[0] > limit:
+            raise ValueError(f"{bb.shape[0]} boxes exceed {limit} (max_batch={self.max_batch}, flip test {'on' if self._flip else 'off'})")
         return frame.contiguous(), bb
 
     def preprocess(self, frame: torch.Tensor, bboxes, pad_bbox: int = 10):
@@ -395,8 +435,9 @@ class ViTPose:
         """uint8 RGB frame [H,W,3] (CUDA) + boxes [n,4] -> (kpts f32 [n,K,3] (y, x, score) in FRAME pixels, idx i32 [n,K]):
         the whole per-person loop of VitInference.inference (easy_ViTPose/inference.py:258-272) as one enqueue, no host sync.
         A box that is empty after clipping only sets the engine's status word (frame_status()); `check=True` synchronises
-        and raises ValueError like the reference does (pad_image / cv2.resize on an empty crop)."""
-        frame, bb = self._check_frame(frame, bboxes)
+        and raises ValueError like the reference does (pad_image / cv2.resize on an empty crop).  Honours the flip test
+        (set_flip_test): then n <= max_batch // 2."""
+        frame, bb = self._check_frame(frame, bboxes, self.batch_limit)
         n = bb.shape[0]
         kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=frame.device)
         idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=frame.device)
@@ -419,15 +460,15 @@ class ViTPose:
 
     def infer_frame_host(self, frame: np.ndarray, bboxes: np.ndarray):
         """HOST frame + boxes in, HOST keypoints out (vpb_infer_frame_host): H2D of the uint8 frame, the path, D2H, sync.
-        More than max_batch boxes are processed in chunks."""
+        More than batch_limit boxes (max_batch, or max_batch // 2 with flip test on) are processed in chunks."""
         self._ensure()
         frame, bb = self._host_frame_args(frame, bboxes)
         n = bb.shape[0]
         kp = np.empty((n, self.num_keypoints, 3), np.float32)
         idx = np.empty((n, self.num_keypoints), np.int32)
         with torch.cuda.device(self._device):
-            for s in range(0, n, self.max_batch):
-                m = min(self.max_batch, n - s)
+            for s in range(0, n, self.batch_limit):
+                m = min(self.batch_limit, n - s)
                 _lib.check_value(_lib.lib().vpb_infer_frame_host(
                     self._handle, frame.ctypes.data_as(C.c_void_p), frame.shape[0], frame.shape[1], bb[s:s + m].ctypes.data_as(C.c_void_p), m,
                     kp[s:s + m].ctypes.data_as(C.c_void_p), idx[s:s + m].ctypes.data_as(C.c_void_p), self._stream()))

@@ -178,6 +178,19 @@ int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels
  * the LayerNorm jobs on a control warp, default 1; VPB_LN_CTL), "ln_job_rows" (8 | 16 rows per LayerNorm job, default 16),
  * "resid_rmw" (residual epilogues as load + add + store instead of TMA reduce-add, default 0; VPB_RESID_RMW). */
 int vpb_set_option(vpb_engine* e, const char* name, int32_t value);
+/* Flip test, the test_cfg flip_test=True of every reference config (configs/ViTPose_common.py:91,124,157,190): mmpose's
+ * (output + output_flipped) * 0.5, where output_flipped is the model run on flip(crop, dims=[3]) and passed through flip_back
+ * (vit_utils/post_processing/post_transforms.py:110-147) and, with shift != 0, the one-pixel shift of
+ * TopdownHeatmapSimpleHead.inference_model (vit_models/head/topdown_heatmap_simple_head.py:195-218, shift at :210-212).
+ * h_perm i32 [k] (HOST) = the keypoint permutation the flip pairs induce (as for vpb_flip_back); k must equal the engine's K
+ * and every entry lie in [0,K), else VPB_ERR_ARG.  h_perm = NULL turns flip test off (the default).
+ * While it is on, vpb_infer, vpb_infer_host, vpb_submit_host, vpb_infer_frame, vpb_infer_frame_host and vpb_submit_frame_host
+ * run each crop and its mirror image as one batch of 2 * batch crops (the mirror images are gathered on the fly, never
+ * stored), average the maps and decode the averaged maps (wrap_batch = 0); d_heatmaps, when given, receives the averaged
+ * maps.  batch must then be <= max_batch / 2.  vpb_forward, vpb_forward_features, vpb_head, vpb_decode* and vpb_flip_back
+ * are unaffected.  SYNCHRONOUS: waits for the engine's pending work (which keeps the previous setting), and drops the
+ * engine's cached CUDA graphs. */
+int vpb_set_flip_test(vpb_engine* e, const int32_t* h_perm, int32_t k, int32_t shift);
 /* With option "profile"=1 every launch is bracketed by a CUDA-event pair on its stream; collect() synchronises,
  * sums elapsed ms and launch counts per kernel class (arrays of vpb_profile_classes() entries) and resets. */
 int vpb_profile_classes(void);
