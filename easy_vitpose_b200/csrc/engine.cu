@@ -147,6 +147,12 @@ static int num_sms() { return cur_dev()->sms; }
 
 // ------------------------------------------------------------------------------------------------ GEMM dispatch
 
+// Bit of DeviceState::gemm_attr for an instantiation: five tile widths per epilogue (EPI_BF16_GELU_ERF takes the unused index 3).
+constexpr int gemm_slot(int bn, int epi) {
+  return (epi == EPI_BF16_GELU_ERF ? 3 : epi) * 5 + (bn == 256 ? 0 : bn == 128 ? 1 : bn == 144 ? 2 : bn == 32 ? 3 : 4);
+}
+static_assert(gemm_slot(192, EPI_F32_ADD) < 32, "gemm_attr has 32 bits");
+
 // `tout` is the output tensor map of the TMA epilogues (EPI_BF16, EPI_BF16_GELU: bf16 box 64 columns x 64 rows; EPI_F32_ADD:
 // f32 box 32 x 64); direct epilogues ignore it (pass any valid map).  W maps carry boxes of BN rows.
 template <int BN, int EPI>
@@ -155,7 +161,7 @@ static int gemm_launch_t(const CUtensorMap& ta, const CUtensorMap& tw, const CUt
   auto kern = gemm_bf16_wgmma<BN, EPI>;
   DeviceState* ds = cur_dev();
   if (ds->sms == 0) return fail(VPB_ERR_STATE, "gemm: device not initialised (device_check)");
-  constexpr unsigned slot = 1u << ((EPI == EPI_BF16_GELU_ERF ? 3 : EPI) * 4 + (BN == 256 ? 0 : BN == 128 ? 1 : BN == 144 ? 2 : 3));
+  constexpr unsigned slot = 1u << gemm_slot(BN, EPI);
   if (!(ds->gemm_attr & slot)) {
     CU_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     ds->gemm_attr |= slot;
@@ -173,16 +179,15 @@ static int gemm_launch(int bn, int epi, const CUtensorMap& ta, const CUtensorMap
   if (epi_uses_tma(epi) && (p.N % 64 != 0 || p.bias == nullptr)) return fail(VPB_ERR_ARG, "gemm: TMA epilogue wants N %% 64 == 0 and a bias");
 #define VPB_CASE(BN_, EPI_) \
   if (bn == BN_ && epi == EPI_) return gemm_launch_t<BN_, EPI_>(ta, tw, tout, p, st);
-  VPB_CASE(256, EPI_BF16) VPB_CASE(128, EPI_BF16)
-  VPB_CASE(256, EPI_BF16_GELU) VPB_CASE(128, EPI_BF16_GELU)
-  VPB_CASE(256, EPI_BF16_GELU_ERF) VPB_CASE(128, EPI_BF16_GELU_ERF)
-  VPB_CASE(256, EPI_F32_ADD) VPB_CASE(128, EPI_F32_ADD)
+  VPB_CASE(256, EPI_BF16) VPB_CASE(192, EPI_BF16) VPB_CASE(128, EPI_BF16)
+  VPB_CASE(256, EPI_BF16_GELU) VPB_CASE(192, EPI_BF16_GELU) VPB_CASE(128, EPI_BF16_GELU)
+  VPB_CASE(256, EPI_BF16_GELU_ERF) VPB_CASE(192, EPI_BF16_GELU_ERF) VPB_CASE(128, EPI_BF16_GELU_ERF)
+  VPB_CASE(256, EPI_F32_ADD) VPB_CASE(192, EPI_F32_ADD) VPB_CASE(128, EPI_F32_ADD)
   VPB_CASE(256, EPI_BF16_RELU_UP)
   VPB_CASE(32, EPI_F32_NCHW) VPB_CASE(144, EPI_F32_NCHW)
 #undef VPB_CASE
   return fail(VPB_ERR_ARG, "gemm: no kernel for BN=%d epilogue=%d", bn, epi);
 }
-static int bn_for(int n) { return (n % 256 == 0 && !(g_dbg_flags & 8)) ? 256 : 128; }   // debug flag 8: force 128-wide tiles
 
 // `device` must be the current device (callers cudaSetDevice / cudaGetDevice first)
 static int device_check(int device) {
@@ -318,15 +323,28 @@ struct Profiler {
 };
 
 // ------------------------------------------------------------------------------------------------ engine
+constexpr int kTileWidths[3] = {128, 256, 192};   // tile widths of the standalone GEMM's TMA epilogues, in pick_tile's tie order
 struct LinearW {
   __nv_bfloat16* w = nullptr;   // [N,K] bf16
   float* b = nullptr;           // [N padded]
-  int n = 0, k = 0, bn = 0;
-  CUtensorMap map;              // W boxes of bn rows (the standalone GEMM's tile width for this N)
+  int n = 0, k = 0;
+  CUtensorMap tmap[3];          // W boxes of kTileWidths[i] rows, for each width that divides the padded N (has[i])
+  bool has[3] = {false, false, false};
   CUtensorMap map_c;            // W boxes of chain_bn rows (every phase of a chained launch uses one tile width)
-  CUtensorMap map128;           // W boxes of 128 rows: 128-wide tiles for small batches (pick_tile); valid when n_pad % 128 == 0
-  bool has128 = false;
+  const CUtensorMap* tile_map(int bn) const {
+    for (int i = 0; i < 3; ++i)
+      if (kTileWidths[i] == bn) return has[i] ? &tmap[i] : nullptr;
+    return nullptr;
+  }
 };
+// W maps of a [n_pad, k] weight for every tile width that divides n_pad
+static int make_tile_maps(LinearW& L, const void* w, int n_pad, int k) {
+  for (int i = 0; i < 3; ++i) {
+    L.has[i] = (n_pad % kTileWidths[i] == 0);
+    if (L.has[i]) VPB_TRY(make_map(&L.tmap[i], w, n_pad, k, k, kTileWidths[i]));
+  }
+  return VPB_OK;
+}
 struct BlockW {
   float *ln1_g, *ln1_b, *ln2_g, *ln2_b;
   LinearW qkv, proj, fc1, fc2;
@@ -414,6 +432,7 @@ struct vpb_engine {
   CUtensorMap m_patch_rows, m_xn, m_attn, m_hid, m_d2, m_qkv_att, m_qkv_att_tail;   // A operands / attention boxes
   CUtensorMap m_feat_nhwc, m_d1_nhwc;                                 // implicit-GEMM deconv inputs (4-D)
   CUtensorMap o_qkv, o_hid, o_x;                                                             // TMA-epilogue outputs
+  CUtensorMap m_fin_w;                          // final 1x1 conv W: boxes of n_final rows (one column tile)
 };
 
 template <typename T>
@@ -537,10 +556,11 @@ extern "C" int vpb_load_tensor(vpb_engine* e, const char* key, const float* data
 
 static inline int cdiv(long long a, long long b) { return static_cast<int>((a + b - 1) / b); }
 
-static int pack_linear(vpb_engine* e, LinearW& L, const std::string& wkey, const std::string& bkey, int n, int k, int bn,
+// W and bias zero-padded to a multiple of `pad` rows
+static int pack_linear(vpb_engine* e, LinearW& L, const std::string& wkey, const std::string& bkey, int n, int k, int pad,
                        int scaled_rows, float scale) {
-  L.n = n; L.k = k; L.bn = bn;
-  const int n_pad = cdiv(n, bn) * bn;
+  L.n = n; L.k = k;
+  const int n_pad = cdiv(n, pad) * pad;
   VPB_TRY(dev_alloc(e, &L.w, static_cast<size_t>(n_pad) * k));
   CU_TRY(cudaMemset(L.w, 0, static_cast<size_t>(n_pad) * k * 2));
   const long long ne = static_cast<long long>(n) * k;
@@ -549,11 +569,8 @@ static int pack_linear(vpb_engine* e, LinearW& L, const std::string& wkey, const
   if (!bkey.empty()) pack_bias<<<cdiv(n_pad, 256), 256>>>(e->staged[bkey].first, L.b, n, n_pad, scaled_rows, scale);
   else CU_TRY(cudaMemset(L.b, 0, n_pad * sizeof(float)));
   CU_TRY(cudaGetLastError());
-  VPB_TRY(make_map(&L.map, L.w, n_pad, k, k, bn));
-  if (n_pad % e->chain_bn == 0) VPB_TRY(make_map(&L.map_c, L.w, n_pad, k, k, e->chain_bn));
-  else L.map_c = L.map;                                        // never chained (final 1x1 conv)
-  L.has128 = (n_pad % 128 == 0);
-  if (L.has128) VPB_TRY(make_map(&L.map128, L.w, n_pad, k, k, 128));
+  VPB_TRY(make_tile_maps(L, L.w, n_pad, k));
+  if (n_pad % e->chain_bn == 0) VPB_TRY(make_map(&L.map_c, L.w, n_pad, k, k, e->chain_bn));   // else never chained (final 1x1 conv)
   return VPB_OK;
 }
 
@@ -573,7 +590,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   const int D = e->D;
   const float qscale = 1.0f / sqrtf(static_cast<float>(D / e->heads));
 
-  VPB_TRY(pack_linear(e, e->patch, "backbone.patch_embed.proj.weight", "", D, 768, bn_for(D), 0, 1.f));
+  VPB_TRY(pack_linear(e, e->patch, "backbone.patch_embed.proj.weight", "", D, 768, 128, 0, 1.f));
   VPB_TRY(dev_alloc(e, &e->pos_bias, 192 * D));
   pack_pos_bias<<<cdiv(192 * D, 256), 256>>>(e->staged["backbone.pos_embed"].first, e->staged["backbone.patch_embed.proj.bias"].first,
                                               e->pos_bias, 192, D);
@@ -584,10 +601,10 @@ extern "C" int vpb_finalize(vpb_engine* e) {
     VPB_TRY(copy_vec(e, &b.ln1_g, p + "norm1.weight")); VPB_TRY(copy_vec(e, &b.ln1_b, p + "norm1.bias"));
     VPB_TRY(copy_vec(e, &b.ln2_g, p + "norm2.weight")); VPB_TRY(copy_vec(e, &b.ln2_b, p + "norm2.bias"));
     // q rows (first D) carry head_dim^-0.5: vit.py:170 scales q before QK^T; fp32 multiply, then bf16 rounding
-    VPB_TRY(pack_linear(e, b.qkv, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, bn_for(3 * D), D, qscale));
-    VPB_TRY(pack_linear(e, b.proj, p + "attn.proj.weight", p + "attn.proj.bias", D, D, bn_for(D), 0, 1.f));
-    VPB_TRY(pack_linear(e, b.fc1, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, bn_for(4 * D), 0, 1.f));
-    VPB_TRY(pack_linear(e, b.fc2, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, bn_for(D), 0, 1.f));
+    VPB_TRY(pack_linear(e, b.qkv, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, 128, D, qscale));
+    VPB_TRY(pack_linear(e, b.proj, p + "attn.proj.weight", p + "attn.proj.bias", D, D, 128, 0, 1.f));
+    VPB_TRY(pack_linear(e, b.fc1, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, 128, 0, 1.f));
+    VPB_TRY(pack_linear(e, b.fc2, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 128, 0, 1.f));
   }
   VPB_TRY(copy_vec(e, &e->lnf_g, "backbone.last_norm.weight"));
   VPB_TRY(copy_vec(e, &e->lnf_b, "backbone.last_norm.bias"));
@@ -604,13 +621,14 @@ extern "C" int vpb_finalize(vpb_engine* e) {
                                          e->staged[bnp + "running_mean"].first, e->staged[bnp + "running_var"].first, dc.w, dc.b,
                                          cin, 256, 1e-5f);
     CU_TRY(cudaGetLastError());
-    dc.n = 256; dc.k = 4 * cin; dc.bn = 256;
-    VPB_TRY(make_map(&dc.map, dc.w, 4 * 256, 4 * cin, 4 * cin, 256));
+    dc.n = 256; dc.k = 4 * cin;
+    VPB_TRY(make_tile_maps(dc, dc.w, 4 * 256, 4 * cin));
     cin = 256;
   }
   {  // final 1x1 conv: [K,256] zero-padded to the N tile
     LinearW& L = e->fin;
     VPB_TRY(pack_linear(e, L, "keypoint_head.final_layer.weight", "keypoint_head.final_layer.bias", e->K, 256, e->n_final, 0, 1.f));
+    VPB_TRY(make_map(&e->m_fin_w, L.w, e->n_final, 256, 256, e->n_final));
   }
   // ---- workspace for max_batch crops
   const size_t B = e->maxB, M = B * 192;
@@ -821,15 +839,30 @@ static int backbone_chained(vpb_engine* e, int B, cudaStream_t st) {
   return VPB_OK;
 }
 
-// Tile width of a standalone GEMM launch: 128 wherever N allows.  A 256-wide tile moves fewer operand bytes per flop, but its 128
-// accumulators per consumer thread do not fit the register budget of a 384-thread CTA (ptxas spills), and on an H100 80GB HBM3
-// (700 W power limit) ViT-B ran faster with 128-wide tiles at every batch size from 4 crops up (64 crops: 6.26 vs 9.04 ms per
-// call; 1 crop: 0.77 vs 0.76 ms; tools/defaults_ab.py).  The 256-wide tiles stay reachable with debug flag 16.  The accumulation
-// order of an output element does not depend on the tile shape: bit-identical.
-static const CUtensorMap& pick_tile(const LinearW& L, int* bn) {
-  if (L.has128 && !(g_dbg_flags & 16)) { *bn = 128; return L.map128; }
-  *bn = L.bn;
-  return L.map;
+// Tile width of a standalone GEMM launch with a TMA epilogue, from the widths in kTileWidths that divide N.  A persistent launch
+// of T tiles on S SMs runs ceil(T / S) waves, and a tile costs about its width, so the rule takes the width with the least
+// ceil(num_m * N / BN / S) * BN.  At 1 crop (2 row blocks) that is 128: the narrow tile gives the most CTAs.  Ties go to the
+// later entry of kTileWidths: 192, then 256, then 128.  Measured on an H100 80GB HBM3 (700 W power limit), us per launch
+// (tools/gemm_width_ab.py), the three-way ties: ViT-B fc1 at 64 crops 101.1 / 100.4 / 104.0 (128 / 192 / 256), ViT-L qkv at
+// 64 crops 123.9 / 118.7 / 119.2; 128 against 256: ViT-B qkv at 8 crops 13.0 / 12.2, ViT-L fc2 at 64 crops 176.6 / 159.6,
+// ViT-H fc2 at 32 crops 147.9 / 125.3, ViT-H proj at 32 crops 52.1 / 52.0, ViT-L proj at 64 crops 69.3 / 75.7 (the one tie
+// the narrow tile wins).  Debug overrides (vpb_debug_gemm): flag 8 forces 128-wide tiles, flag 16 the widest width N allows,
+// and flags >> 8 = W forces width W.  The accumulation order of an output element does not depend on the tile width: every
+// choice is bit-identical.
+static int pick_tile(const LinearW& L, int M, int* bn, const CUtensorMap** wm) {
+  const int num_m = cdiv(M, GEMM_BM), sms = num_sms();
+  const int forced = (g_dbg_flags & 8) ? 128 : (g_dbg_flags >> 8);
+  *bn = 0;
+  long long best = 0;
+  for (int i = 0; i < 3; ++i) {
+    const int w = kTileWidths[i];
+    if (!L.has[i] || (forced && w != forced)) continue;
+    const long long cost = static_cast<long long>(cdiv(static_cast<long long>(num_m) * cdiv(L.n, w), sms)) * w;
+    if ((g_dbg_flags & 16) ? w > *bn : (*bn == 0 || cost <= best)) { *bn = w; best = cost; }
+  }
+  if (*bn == 0) return fail(VPB_ERR_ARG, "gemm: no tile width for N=%d (forced width %d)", L.n, forced);
+  *wm = L.tile_map(*bn);
+  return VPB_OK;
 }
 
 // everything after the patch gather, up to last_norm
@@ -875,9 +908,10 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     fuse_ln(p, e->blocks[0].ln1_g, e->blocks[0].ln1_b);
     e->prof.begin(KC_GEMM_PATCH, st);
     int bn;
-    const CUtensorMap& wm = pick_tile(e->patch, &bn);
+    const CUtensorMap* wm;
+    VPB_TRY(pick_tile(e->patch, M, &bn, &wm));
     p.rmw = resid_rmw(e->resid_rmw);
-    VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_patch_rows, wm, e->o_x, p, st));
+    VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_patch_rows, *wm, e->o_x, p, st));
     e->prof.end(st);
   }
   if (stop == 2) return VPB_OK;
@@ -891,8 +925,9 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     e->prof.begin(KC_GEMM_QKV, st);
     {
       int bn;
-      const CUtensorMap& wm = pick_tile(b.qkv, &bn);
-      VPB_TRY(gemm_launch(bn, EPI_BF16, e->m_xn, wm, e->o_qkv, gp(M, 3 * D, D, b.qkv.b, e->qkv, 3 * D), st));
+      const CUtensorMap* wm;
+      VPB_TRY(pick_tile(b.qkv, M, &bn, &wm));
+      VPB_TRY(gemm_launch(bn, EPI_BF16, e->m_xn, *wm, e->o_qkv, gp(M, 3 * D, D, b.qkv.b, e->qkv, 3 * D), st));
     }
     e->prof.end(st);
     }
@@ -910,9 +945,10 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
       fuse_ln(p, b.ln2_g, b.ln2_b);
       e->prof.begin(KC_GEMM_PROJ, st);
       int bn;
-      const CUtensorMap& wm = pick_tile(b.proj, &bn);
+      const CUtensorMap* wm;
+      VPB_TRY(pick_tile(b.proj, M, &bn, &wm));
       p.rmw = resid_rmw(e->resid_rmw);
-      VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_attn, wm, e->o_x, p, st));
+      VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_attn, *wm, e->o_x, p, st));
       e->prof.end(st);
     }
     if (stop == 6) return VPB_OK;
@@ -923,8 +959,9 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     e->prof.begin(KC_GEMM_FC1, st);
     {
       int bn;
-      const CUtensorMap& wm = pick_tile(b.fc1, &bn);
-      VPB_TRY(gemm_launch(bn, e->gelu_erf ? EPI_BF16_GELU_ERF : EPI_BF16_GELU, e->m_xn, wm, e->o_hid, gp(M, 4 * D, D, b.fc1.b, e->hid, 4 * D), st));
+      const CUtensorMap* wm;
+      VPB_TRY(pick_tile(b.fc1, M, &bn, &wm));
+      VPB_TRY(gemm_launch(bn, e->gelu_erf ? EPI_BF16_GELU_ERF : EPI_BF16_GELU, e->m_xn, *wm, e->o_hid, gp(M, 4 * D, D, b.fc1.b, e->hid, 4 * D), st));
     }
     e->prof.end(st);
     }
@@ -935,9 +972,10 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
       else fuse_ln(p, e->lnf_g, e->lnf_b);
       e->prof.begin(KC_GEMM_FC2, st);
       int bn;
-      const CUtensorMap& wm = pick_tile(b.fc2, &bn);
+      const CUtensorMap* wm;
+      VPB_TRY(pick_tile(b.fc2, M, &bn, &wm));
       p.rmw = resid_rmw(e->resid_rmw);
-      VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_hid, wm, e->o_x, p, st));
+      VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_hid, *wm, e->o_x, p, st));
       e->prof.end(st);
     }
     if (stop == 8) return VPB_OK;
@@ -953,7 +991,7 @@ static int head(vpb_engine* e, int B, float* d_heat, cudaStream_t st) {
     GemmParams p = gp(B * 192, 256, 4 * D, e->dc1.b, e->d1, 256);
     p.up_h = 16; p.up_w = 12; p.up_tr = 8; p.up_tw = 12; p.up_c = D;
     e->prof.begin(KC_GEMM_DECONV, st);
-    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, e->m_feat_nhwc, e->dc1.map, e->m_xn, p, st));
+    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, e->m_feat_nhwc, *e->dc1.tile_map(256), e->m_xn, p, st));
     e->prof.end(st);
   }
   if (stop == 11) return VPB_OK;
@@ -961,7 +999,7 @@ static int head(vpb_engine* e, int B, float* d_heat, cudaStream_t st) {
     GemmParams p = gp(B * 768, 256, 1024, e->dc2.b, e->d2, 256);
     p.up_h = 32; p.up_w = 24; p.up_tr = 16; p.up_tw = 8; p.up_c = 256;
     e->prof.begin(KC_GEMM_DECONV, st);
-    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, e->m_d1_nhwc, e->dc2.map, e->m_xn, p, st));
+    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, e->m_d1_nhwc, *e->dc2.tile_map(256), e->m_xn, p, st));
     e->prof.end(st);
   }
   if (stop == 12) return VPB_OK;
@@ -969,7 +1007,7 @@ static int head(vpb_engine* e, int B, float* d_heat, cudaStream_t st) {
     GemmParams p = gp(B * 3072, e->n_final, 256, e->fin.b, d_heat, 0);
     p.n_valid = e->K; p.pix = 3072;
     e->prof.begin(KC_GEMM_FINAL, st);
-    VPB_TRY(gemm_launch(e->n_final, EPI_F32_NCHW, e->m_d2, e->fin.map, e->m_d2, p, st));
+    VPB_TRY(gemm_launch(e->n_final, EPI_F32_NCHW, e->m_d2, e->m_fin_w, e->m_d2, p, st));
     e->prof.end(st);
   }
   return VPB_OK;
@@ -1568,12 +1606,18 @@ extern "C" int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, v
   VPB_TRY(device_check(dev));
   if (!d_a || !d_w || !d_out) return fail(VPB_ERR_ARG, "vpb_gemm: null pointer");
   int bn;
-  if (epilogue == EPI_F32_NCHW) bn = n <= 32 ? 32 : 144;
-  else if (epilogue == EPI_BF16_RELU_UP) bn = 256;
-  else bn = bn_for(n);
-  if (epilogue != EPI_F32_NCHW && n % bn != 0) return fail(VPB_ERR_ARG, "vpb_gemm: N=%d must be a multiple of %d", n, bn);
-  if (epilogue == EPI_F32_NCHW && n != bn) return fail(VPB_ERR_ARG, "vpb_gemm: NCHW epilogue wants W padded to %d rows", bn);
   CUtensorMap ta, tw, tout;
+  if (epi_uses_tma(epilogue)) {                  // the engine's width rule and debug overrides (pick_tile)
+    LinearW L;
+    L.n = n; L.k = k;
+    VPB_TRY(make_tile_maps(L, d_w, n, k));
+    const CUtensorMap* wm;
+    VPB_TRY(pick_tile(L, m, &bn, &wm));
+  } else {
+    bn = epilogue == EPI_F32_NCHW ? (n <= 32 ? 32 : 144) : 256;
+  }
+  if (epilogue == EPI_BF16_RELU_UP && n % bn != 0) return fail(VPB_ERR_ARG, "vpb_gemm: N=%d must be a multiple of %d", n, bn);
+  if (epilogue == EPI_F32_NCHW && n != bn) return fail(VPB_ERR_ARG, "vpb_gemm: NCHW epilogue wants W padded to %d rows", bn);
   if (epilogue == EPI_BF16_RELU_UP) {
     // d_a: NHWC input [m / (H*W), H, W, C] with H = aux0, W = aux1, tile = aux2 rows x (aux3 >> 16) columns (96 or 128
     // positions), C = aux3 & 0xffff = k / 4; d_w: the four phase matrices stacked [4*256, 4*C]

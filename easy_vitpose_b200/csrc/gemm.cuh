@@ -140,9 +140,11 @@ __device__ __forceinline__ float epi_act(float v) {
 
 // TMA epilogues: 64 bf16 / 32 f32 columns (one 128-byte staging row) per round, two staging buffers per warpgroup in turn.
 // `stiles` = this warpgroup's two buffers; `tid` = thread index inside the warpgroup (thread 0 issues and owns the bulk groups).
+// `first` = the buffer of round 0: with an odd number of rounds per tile (BN = 192, bf16) the caller alternates it from tile to
+// tile, so that round 0 never reuses the buffer of the previous tile's last round, whose store may still be reading it.
 template <int BN, int EPI>
 __device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], int n0, int row0, int N, const float* __restrict__ bias, uint8_t* stiles,
-                                             int wg, int tid, const CUtensorMap* tmap_out) {
+                                             int wg, int tid, const CUtensorMap* tmap_out, int first = 0) {
   constexpr int COLS = (EPI == EPI_F32_ADD) ? 32 : 64;
   constexpr int JPC = COLS / 8;                       // accumulator column groups per round
   const int lane = tid & 31, wq = tid >> 5;
@@ -151,7 +153,8 @@ __device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], int n0,
   const int cq = 2 * (lane & 3);
 #pragma unroll
   for (int c = 0; c < BN / COLS; ++c) {
-    uint8_t* st = stiles + (c & 1) * GEMM_STAGE_TILE;
+    uint8_t* st = stiles + ((c ^ first) & 1) * GEMM_STAGE_TILE;
+    const uint32_t sa = smem_u32(st);                 // st.shared with 32-bit addresses: generic 64-bit ones made ptxas spill BN = 256
     if (tid == 0) tma_store_wait_read<1>();           // the store that used this buffer two rounds ago has read it
     named_bar_sync(GEMM_BAR_EPI + 1 + wg, 128);
 #pragma unroll
@@ -162,12 +165,12 @@ __device__ __forceinline__ void epilogue_tma(const float (&acc)[BN / 2], int n0,
       const float v2 = epi_act<EPI>(acc[4 * j + 2] + b2.x), v3 = epi_act<EPI>(acc[4 * j + 3] + b2.y);
       if constexpr (EPI == EPI_F32_ADD) {
         const int off = (((2 * jl + ((lane & 3) >> 1)) ^ sw) << 4) + (lane & 1) * 8;
-        *reinterpret_cast<float2*>(st + r_lo * 128 + off) = make_float2(v0, v1);
-        *reinterpret_cast<float2*>(st + (r_lo + 8) * 128 + off) = make_float2(v2, v3);
+        sts_f32x2(sa + r_lo * 128 + off, v0, v1);
+        sts_f32x2(sa + (r_lo + 8) * 128 + off, v2, v3);
       } else {
         const int off = ((jl ^ sw) << 4) + (lane & 3) * 4;
-        *reinterpret_cast<uint32_t*>(st + r_lo * 128 + off) = pack_bf16(v0, v1);
-        *reinterpret_cast<uint32_t*>(st + (r_lo + 8) * 128 + off) = pack_bf16(v2, v3);
+        sts_u32(sa + r_lo * 128 + off, pack_bf16(v0, v1));
+        sts_u32(sa + (r_lo + 8) * 128 + off, pack_bf16(v2, v3));
       }
     }
     fence_proxy_async_smem();                         // staging writes -> visible to the TMA engine
@@ -287,7 +290,11 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
   pdl_launch_dependents();                          // the next kernel may start its prologue as SMs free up
   pdl_wait();                                       // previous kernel's outputs (our A operand / residual) are complete
 
-  if (warp == GEMM_CONSUMER_WARPS) {
+  // Register split: the producer warpgroup (warps 8..11; only warp 8 issues) needs few registers, the consumers' accumulators
+  // (BN / 2 per thread) and epilogue need many.  384 threads start at 168 each; 128 x 40 + 256 x 232 = 64512 <= 65536.
+  if (warp >= GEMM_CONSUMER_WARPS) {
+    setmaxnreg_dec<40>();
+    if (warp != GEMM_CONSUMER_WARPS) return;        // warps 9..11 only take part in the warpgroup-wide dec
     // ------------------------------------------------------------ TMA producer: the whole warp runs the (uniform) loop, one
     // elected lane issues
     RingPos rp;
@@ -329,13 +336,15 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
       }
     }
     if (p.dbg && lane == 0) { p.dbg[blockIdx.x * 8 + 3] = clock64() - t_begin; p.dbg[blockIdx.x * 8 + 4] = t_wait; }
-  } else if (warp < GEMM_CONSUMER_WARPS) {
+  } else {
+    setmaxnreg_inc<232>();
     // ------------------------------------------------------------ consumers: MMA + epilogue, warpgroup wg owns rows 64 wg ..
     const int wg = warp >> 2;
     const int tid = threadIdx.x & 127;
     const int wq = warp & 3;
     uint8_t* stiles = staging + wg * 2 * GEMM_STAGE_TILE;
     RingPos rp;
+    int sfirst = 0;                                   // staging buffer of the next tile's first epilogue round
     long long t_full = 0;
     const long long t_begin = p.dbg ? clock64() : 0;
     float acc[BN / 2];
@@ -350,7 +359,10 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
 
       if constexpr (epi_uses_tma(EPI)) {
         if (EPI == EPI_F32_ADD && p.rmw) epilogue_f32_rmw<BN>(acc, n0, row0, p.M, p.bias, reinterpret_cast<float*>(p.out), p.ldc, tid);
-        else epilogue_tma<BN, EPI>(acc, n0, row0, p.N, p.bias, stiles, wg, tid, &tmap_out);
+        else {
+          epilogue_tma<BN, EPI>(acc, n0, row0, p.N, p.bias, stiles, wg, tid, &tmap_out, sfirst);
+          sfirst ^= (BN / (EPI == EPI_F32_ADD ? 32 : 64)) & 1;
+        }
       } else {
         // ---- direct epilogues (scattered / transposed outputs)
         const int cq = 2 * (lane & 3);

@@ -112,6 +112,20 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// shared-memory stores through 32-bit shared addresses
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ void sts_f32x2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+
+// ---------------------------------------------------------------- per-warpgroup register budget
+// Warpgroup-wide (.sync.aligned): all four warps of the warpgroup execute it with the same N (a multiple of 8 in [24, 256]).
+// dec returns registers above N to the CTA's pool; inc blocks until the pool can raise every thread of the warpgroup to N.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- wgmma shared-memory operand descriptor (sm_90)
 //   [0,14) start address >> 4     [16,30) leading byte offset >> 4     [32,46) stride byte offset >> 4
 //   [49,52) base offset (0: tiles 1024-byte aligned)                     [62,64) layout: 0 none, 1 SW128, 2 SW64, 3 SW32

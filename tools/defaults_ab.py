@@ -2,8 +2,8 @@
 """A/B of the engine defaults that depend on the GPU (ViT-B COCO-17, seeded random weights and crops, CUDA-event timing of
 back-to-back calls, each arm measured twice in alternation):
   l2       the L2 persisting window over the fp32 token stream (default) against none (VPB_L2_PERSIST=0), at 64 crops
-  tiles    standalone GEMMs (unchained path) with 256-wide tiles where N allows (default) against 128-wide tiles everywhere
-           (vpb_debug_gemm flag 8 at weight packing)
+  tiles    standalone GEMMs (unchained path) with the tile-width rule of engine.cu pick_tile (default) against 128-wide tiles
+           everywhere (vpb_debug_gemm flag 8 around the narrow arm's calls)
   chain    chained launches against one kernel per GEMM, per batch size: where chain_min_batch belongs
 Prints the card and its power limit first: the numbers belong to them.
 
@@ -25,12 +25,10 @@ print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm"
 SD = {k: torch.from_numpy(np.asarray(v)) for k, v in random_state_dict("b", 17, seed=1).items()}
 
 
-def engine(l2=True, narrow=False):
+def engine(l2=True):
     os.environ["VPB_L2_PERSIST"] = "1" if l2 else "0"
-    _lib.lib().vpb_debug_gemm((8 << 8) if narrow else 0, None)
     m = ViTPose(model_cfg("b", 17), max_batch=64)
     m.load_state_dict(SD).to("cuda:0")
-    _lib.lib().vpb_debug_gemm(0, None)
     os.environ.pop("VPB_L2_PERSIST")
     return m
 
@@ -51,7 +49,7 @@ def ms_per_call(m, n, iters=30):
     return e0.elapsed_time(e1) / iters
 
 
-base, no_l2, narrow = engine(), engine(l2=False), engine(narrow=True)
+base, no_l2, narrow = engine(), engine(l2=False), engine()
 for m in (base, no_l2, narrow):
     m.set_option("chain_min_batch", 1)
 
@@ -65,8 +63,11 @@ for n in (1, 4, 9, 16, 32, 48, 64):
     for _ in range(2):
         for m in (base, narrow):
             m.set_option("chain", 0)
-        wide_t, narrow_t = ms_per_call(base, n), ms_per_call(narrow, n)
+        wide_t = ms_per_call(base, n)
+        _lib.lib().vpb_debug_gemm(8 << 8, None)
+        narrow_t = ms_per_call(narrow, n)
+        _lib.lib().vpb_debug_gemm(0, None)
         base.set_option("chain", 1)
         chain_t = ms_per_call(base, n)
         cells.append(f"{wide_t:.3f} / {narrow_t:.3f} / {chain_t:.3f}")
-    print(f"{n:2d} crops ms/call  unchained 256-wide / unchained 128-wide / chained:  " + "  |  ".join(cells), flush=True)
+    print(f"{n:2d} crops ms/call  unchained rule / unchained 128-wide / chained:  " + "  |  ".join(cells), flush=True)
