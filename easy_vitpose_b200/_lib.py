@@ -18,6 +18,15 @@ class VpbConfig(C.Structure):
                 ("num_keypoints", C.c_int32), ("max_batch", C.c_int32), ("device", C.c_int32)]
 
 
+MAX_FRAMES = 64                                       # VPB_MAX_FRAMES: frames with boxes per multi-frame call
+
+
+class VpbFrame(C.Structure):
+    """vpb_frame: one frame of a multi-frame call (vpb_infer_frames and its host forms)."""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("pitch_bytes", C.c_int64),
+                ("num_boxes", C.c_int32)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "vpb_last_error": (C.c_char_p, []),
@@ -44,6 +53,9 @@ EXPORTS = {
     "vpb_frame_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
     "vpb_infer_frame_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_submit_frame_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32]),
+    "vpb_infer_frames": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_frames_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_submit_frames_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
     "vpb_host_alloc": (C.c_void_p, [C.c_int64]),
     "vpb_host_free": (None, [C.c_void_p]),
     "vpb_kernel_launches": (C.c_int, [C.c_void_p, C.c_int32]),

@@ -741,19 +741,22 @@ static int patch_gather(vpb_engine* e, const float* d_crops, int n_src, int B, c
   e->prof.end(st);
   return VPB_OK;
 }
-// Where a batch of patch rows comes from: normalised f32 crops (patch_im2col) or a uint8 frame + boxes (frame_to_patch_rows:
-// crop pre-processing fused with the im2col; it also fills pp_org / pp_offs for the decode).
+// Where a batch of patch rows comes from: normalised f32 crops (patch_im2col) or a table of uint8 frames + boxes
+// (frame_to_patch_rows: crop pre-processing fused with the im2col; it also fills pp_org / pp_offs for the decode).
 struct Source {
   const float* crops = nullptr;
-  const uint8_t* frame = nullptr;
-  int fh = 0, fw = 0;
+  const FrameEntry* frames = nullptr;       // num_frames entries, only frames that have boxes
+  int num_frames = 0;
   const int32_t* bboxes = nullptr;
 };
 static int frame_gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
   FramePatchParams q;
-  q.pp.frame = src.frame; q.pp.pitch = static_cast<long long>(src.fw) * 3; q.pp.fh = src.fh; q.pp.fw = src.fw; q.pp.bboxes = src.bboxes;
+  memset(&q, 0, sizeof(q));
+  q.pp.bboxes = src.bboxes;
   q.pp.n = n_src; q.pp.pad = 10; q.pp.crops = nullptr; q.pp.org_wh = e->pp_org; q.pp.offs_yx = e->pp_offs; q.pp.status = e->pp_status;
   q.rows = e->patch_rows; q.pos_bias = reinterpret_cast<const float4*>(e->pos_bias); q.stream = reinterpret_cast<float4*>(e->x); q.D = e->D;
+  q.num_frames = src.num_frames;
+  memcpy(q.frames, src.frames, static_cast<size_t>(src.num_frames) * sizeof(FrameEntry));
   e->prof.begin(KC_PREPROCESS, st);
   CU_TRY(launch_k(frame_to_patch_rows, dim3(B, 16), dim3(384), 0, st, q));
   e->prof.end(st);
@@ -1356,12 +1359,53 @@ extern "C" int vpb_preprocess(const uint8_t* d_frame, int32_t frame_h, int32_t f
   return VPB_OK;
 }
 
-static int infer_frame_enqueue(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int32_t frame_w, const int32_t* d_bboxes,
-                               int32_t n, float* d_kpts, int32_t* d_idx, cudaStream_t st) {
+static_assert(VPB_MAX_FRAMES == FP_MAX_FRAMES, "the header's frame limit is the gather's table size");
+
+// `tab`: num_frames frames with boxes, first_box ascending; d_bboxes holds their n boxes in frame order
+static int infer_frames_enqueue(vpb_engine* e, const FrameEntry* tab, int num_frames, const int32_t* d_bboxes, int32_t n,
+                                float* d_kpts, int32_t* d_idx, cudaStream_t st) {
   Source src;                   // the crops are never materialised: frame_to_patch_rows writes the bf16 patch rows directly
-  src.frame = d_frame; src.fh = frame_h; src.fw = frame_w; src.bboxes = d_bboxes;
+  src.frames = tab; src.num_frames = num_frames; src.bboxes = d_bboxes;
   VPB_TRY(apply_l2_policy(e, st));
   return infer_core(e, src, e->pp_org, e->pp_offs, n, d_kpts, d_idx, nullptr, st);
+}
+
+// one packed frame that owns every box of the call
+static FrameEntry single_frame(const uint8_t* data, int32_t fh, int32_t fw) {
+  FrameEntry f;
+  memset(&f, 0, sizeof(f));
+  f.data = data; f.pitch = static_cast<long long>(fw) * 3; f.fh = fh; f.fw = fw; f.first_box = 0;
+  return f;
+}
+
+// The caller's frame array -> the gather's table.  Frames without boxes are left out (they do not count towards
+// VPB_MAX_FRAMES); pitch_bytes 0 means packed rows.  *n = the total number of boxes, checked against the batch limit.
+static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32_t num_frames, FrameEntry* tab, int* num_tab,
+                       int32_t* n) {
+  if (!e) return fail(VPB_ERR_ARG, "null engine");
+  if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
+  if (num_frames < 0 || (num_frames > 0 && !fr)) return fail(VPB_ERR_ARG, "%s: %d frames, frame array %p", fn, num_frames, fr);
+  long long boxes = 0;
+  int used = 0;
+  for (int j = 0; j < num_frames; ++j) {
+    const vpb_frame& f = fr[j];
+    if (f.num_boxes < 0) return fail(VPB_ERR_ARG, "%s: frame %d has num_boxes = %d", fn, j, f.num_boxes);
+    if (f.num_boxes == 0) continue;
+    const long long pitch = f.pitch_bytes ? f.pitch_bytes : 3LL * f.width;
+    if (!f.data || f.height < 1 || f.width < 1 || pitch < 3LL * f.width)
+      return fail(VPB_ERR_ARG, "%s: frame %d: data %p, %dx%d (w x h), pitch %lld bytes (0 or >= 3 * width expected)", fn, j,
+                  static_cast<const void*>(f.data), f.width, f.height, static_cast<long long>(f.pitch_bytes));
+    if (used == VPB_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than VPB_MAX_FRAMES = %d frames with boxes", fn, VPB_MAX_FRAMES);
+    if (boxes + f.num_boxes > e->maxB)
+      return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, e->maxB, j);
+    FrameEntry& t = tab[used++];
+    memset(&t, 0, sizeof(t));
+    t.data = f.data; t.pitch = pitch; t.fh = f.height; t.fw = f.width; t.first_box = static_cast<int>(boxes);
+    boxes += f.num_boxes;
+  }
+  *num_tab = used;
+  *n = static_cast<int32_t>(boxes);
+  return boxes ? check_ready_keypoints(e, *n) : VPB_OK;
 }
 
 extern "C" int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int32_t frame_w, const int32_t* d_bboxes,
@@ -1369,7 +1413,20 @@ extern "C" int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t fr
   VPB_TRY(check_ready_keypoints(e, n));
   DeviceGuard dev_guard(e);
   if (!d_frame || !d_bboxes || !d_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame: bad argument");
-  return infer_frame_enqueue(e, d_frame, frame_h, frame_w, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+  const FrameEntry f = single_frame(d_frame, frame_h, frame_w);
+  return infer_frames_enqueue(e, &f, 1, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_frames(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* d_bboxes,
+                                float* d_kpts, int32_t* d_idx, void* stream) {
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_frames", e, h_frames, num_frames, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames: null pointer");
+  return infer_frames_enqueue(e, tab, nt, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 
 // Status word of the device-side frame path (bit 0: a box was empty after padding + clipping; such a box is decoded from
@@ -1385,14 +1442,24 @@ extern "C" int vpb_frame_status(vpb_engine* e, int32_t* h_status) {
 }
 
 // host boxes are checked here, where the reference raises (ZeroDivisionError in pad_image / cv2.resize on an empty crop)
-static int check_boxes_host(const int32_t* bb, int32_t n, int32_t fh, int32_t fw) {
+// (frame >= 0: the multi-frame calls, whose message names the frame and the box's index within it)
+static int check_boxes_host(const int32_t* bb, int32_t n, int32_t fh, int32_t fw, int frame = -1) {
   for (int i = 0; i < n; ++i) {
     const int x0 = std::min(std::max(bb[4 * i] - 10, 0), fw), x1 = std::min(std::max(bb[4 * i + 2] + 10, 0), fw);
     const int y0 = std::min(std::max(bb[4 * i + 1] - 10, 0), fh), y1 = std::min(std::max(bb[4 * i + 3] + 10, 0), fh);
-    if (x1 - x0 <= 0 || y1 - y0 <= 0)
+    if (x1 - x0 <= 0 || y1 - y0 <= 0) {
+      if (frame >= 0)
+        return fail(VPB_ERR_ARG, "frame %d box %d (%d,%d,%d,%d) is empty after padding and clipping to the %dx%d frame", frame, i,
+                    bb[4 * i], bb[4 * i + 1], bb[4 * i + 2], bb[4 * i + 3], fw, fh);
       return fail(VPB_ERR_ARG, "box %d (%d,%d,%d,%d) is empty after padding and clipping to the %dx%d frame", i, bb[4 * i], bb[4 * i + 1],
                   bb[4 * i + 2], bb[4 * i + 3], fw, fh);
+    }
   }
+  return VPB_OK;
+}
+static int check_frames_boxes_host(const vpb_frame* fr, int32_t num_frames, const int32_t* bb) {
+  for (int j = 0, first = 0; j < num_frames; first += fr[j].num_boxes, ++j)
+    VPB_TRY(check_boxes_host(bb + 4 * static_cast<size_t>(first), fr[j].num_boxes, fr[j].height, fr[j].width, j));
   return VPB_OK;
 }
 static int frame_stage_reserve(vpb_engine* e, int slot, size_t bytes) {
@@ -1405,28 +1472,60 @@ static int frame_stage_reserve(vpb_engine* e, int slot, size_t bytes) {
   return VPB_OK;
 }
 
-extern "C" int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
-                                    int32_t n, float* h_kpts, int32_t* h_idx, void* stream) {
-  VPB_TRY(check_ready_keypoints(e, n));
-  DeviceGuard dev_guard(e);
-  if (!h_frame || !h_bboxes || !h_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame_host: bad argument");
-  VPB_TRY(check_boxes_host(h_bboxes, n, frame_h, frame_w));
-  const size_t fbytes = static_cast<size_t>(frame_h) * frame_w * 3;
-  VPB_TRY(frame_stage_reserve(e, 0, fbytes));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  CU_TRY(cudaStreamWaitEvent(st, e->ev_done[0], 0));      // slot 0 is shared with the pipelined path: its last user is done
-  CU_TRY(cudaMemcpyAsync(e->frame_stage[0], h_frame, fbytes, cudaMemcpyHostToDevice, st));
-  CU_TRY(cudaMemcpyAsync(e->bbox_stage[0], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-  VPB_TRY(infer_frame_enqueue(e, e->frame_stage[0], frame_h, frame_w, e->bbox_stage[0], n, e->kpts[0], e->idx[0], st));
+// Host frames -> staging slot `slot`, enqueued on `st` after the slot's last user: each frame packed (a 2D copy from its pitch),
+// then the boxes of all frames in one copy.  Repoints `tab` at the staged frames.
+static int stage_frames_host(vpb_engine* e, int slot, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, cudaStream_t st) {
+  size_t total = 0;
+  for (int j = 0; j < nt; ++j) total += static_cast<size_t>(tab[j].fh) * tab[j].fw * 3;
+  VPB_TRY(frame_stage_reserve(e, slot, total));
+  CU_TRY(cudaStreamWaitEvent(st, e->ev_done[slot], 0));   // slot 0 is shared with the pipelined path: its last user is done
+  size_t off = 0;
+  for (int j = 0; j < nt; ++j) {
+    const size_t row = static_cast<size_t>(tab[j].fw) * 3, bytes = row * tab[j].fh;
+    uint8_t* dst = e->frame_stage[slot] + off;
+    if (static_cast<size_t>(tab[j].pitch) == row) CU_TRY(cudaMemcpyAsync(dst, tab[j].data, bytes, cudaMemcpyHostToDevice, st));
+    else CU_TRY(cudaMemcpy2DAsync(dst, row, tab[j].data, static_cast<size_t>(tab[j].pitch), row, tab[j].fh, cudaMemcpyHostToDevice, st));
+    tab[j].data = dst; tab[j].pitch = static_cast<long long>(row);
+    off += bytes;
+  }
+  CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  return VPB_OK;
+}
+// synchronous host form on slot 0 and the caller's stream
+static int frames_host_sync(vpb_engine* e, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
+                            cudaStream_t st) {
+  VPB_TRY(stage_frames_host(e, 0, tab, nt, h_bboxes, n, st));
+  VPB_TRY(infer_frames_enqueue(e, tab, nt, e->bbox_stage[0], n, e->kpts[0], e->idx[0], st));
   CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
   if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CU_TRY(cudaEventRecord(e->ev_done[0], st));
   CU_TRY(cudaStreamSynchronize(st));
   return VPB_OK;
 }
-
-// Pipelined frames (video): same slots, events and vpb_wait_host as vpb_submit_host; the H2D per step is the uint8 frame and
+// Pipelined frames (video): same slots, events and vpb_wait_host as vpb_submit_host; the H2D per step is the uint8 frames and
 // 16 B per box instead of 589 824 B per crop.
+static int frames_host_submit(vpb_engine* e, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
+                              int slot) {
+  VPB_TRY(stage_frames_host(e, slot, tab, nt, h_bboxes, n, e->copy_stream));
+  CU_TRY(cudaEventRecord(e->ev_h2d[slot], e->copy_stream));
+  CU_TRY(cudaStreamWaitEvent(e->compute_stream, e->ev_h2d[slot], 0));
+  VPB_TRY(infer_frames_enqueue(e, tab, nt, e->bbox_stage[slot], n, e->kpts[slot], e->idx[slot], e->compute_stream));
+  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[slot], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->compute_stream));
+  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[slot], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, e->compute_stream));
+  CU_TRY(cudaEventRecord(e->ev_done[slot], e->compute_stream));
+  return VPB_OK;
+}
+
+extern "C" int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
+                                    int32_t n, float* h_kpts, int32_t* h_idx, void* stream) {
+  VPB_TRY(check_ready_keypoints(e, n));
+  DeviceGuard dev_guard(e);
+  if (!h_frame || !h_bboxes || !h_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame_host: bad argument");
+  VPB_TRY(check_boxes_host(h_bboxes, n, frame_h, frame_w));
+  FrameEntry f = single_frame(h_frame, frame_h, frame_w);
+  return frames_host_sync(e, &f, 1, h_bboxes, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
                                      int32_t n, float* h_kpts, int32_t* h_idx, int32_t slot) {
   VPB_TRY(check_ready_keypoints(e, n));
@@ -1434,18 +1533,35 @@ extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int3
   if (!h_frame || !h_bboxes || !h_kpts || frame_h < 1 || frame_w < 1 || slot < 0 || slot > 1)
     return fail(VPB_ERR_ARG, "vpb_submit_frame_host: bad argument");
   VPB_TRY(check_boxes_host(h_bboxes, n, frame_h, frame_w));
-  const size_t fbytes = static_cast<size_t>(frame_h) * frame_w * 3;
-  VPB_TRY(frame_stage_reserve(e, slot, fbytes));
-  CU_TRY(cudaStreamWaitEvent(e->copy_stream, e->ev_done[slot], 0));
-  CU_TRY(cudaMemcpyAsync(e->frame_stage[slot], h_frame, fbytes, cudaMemcpyHostToDevice, e->copy_stream));
-  CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, e->copy_stream));
-  CU_TRY(cudaEventRecord(e->ev_h2d[slot], e->copy_stream));
-  CU_TRY(cudaStreamWaitEvent(e->compute_stream, e->ev_h2d[slot], 0));
-  VPB_TRY(infer_frame_enqueue(e, e->frame_stage[slot], frame_h, frame_w, e->bbox_stage[slot], n, e->kpts[slot], e->idx[slot], e->compute_stream));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[slot], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->compute_stream));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[slot], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, e->compute_stream));
-  CU_TRY(cudaEventRecord(e->ev_done[slot], e->compute_stream));
-  return VPB_OK;
+  FrameEntry f = single_frame(h_frame, frame_h, frame_w);
+  return frames_host_submit(e, &f, 1, h_bboxes, n, h_kpts, h_idx, slot);
+}
+
+extern "C" int vpb_infer_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
+                                     float* h_kpts, int32_t* h_idx, void* stream) {
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_frames_host", e, h_frames, num_frames, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_host: null pointer");
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  return frames_host_sync(e, tab, nt, h_bboxes, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
+                                      float* h_kpts, int32_t* h_idx, int32_t slot) {
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_submit_frames_host", e, h_frames, num_frames, tab, &nt, &n));
+  if (slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "vpb_submit_frames_host: slot %d", slot);
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_submit_frames_host: null pointer");
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
 }
 
 extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t* h_org_wh, int32_t batch, float* h_kpts,

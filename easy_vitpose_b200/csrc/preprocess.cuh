@@ -129,15 +129,32 @@ __global__ void __launch_bounds__(PP_W) crop_resize_normalise(const PreprocParam
 // Like patch_im2col, the launch also seeds the fp32 token stream with pos_embed + conv bias (vit.py:382).
 // Flip test: a grid of (2 pp.n, 16) CTAs; crop c >= pp.n is the mirror image of crop c - pp.n (box c - pp.n, pixel dx stored at
 // tile column 2 + (191 - dx)), i.e. the patch rows of flip(crop, dims=[3]).  Mirrored CTAs leave org_wh / offs_yx / status alone.
+// Frames: the boxes may come from up to FP_MAX_FRAMES frames (vpb_infer_frames).  Frame j owns boxes first_box[j] ..
+// first_box[j+1]-1 (first_box strictly increasing, frames[0].first_box = 0); a single-frame call is a one-entry table.  The
+// table travels in the kernel's parameter block (64 x 32 B of the 4 KB): nothing to allocate or copy per call, and no shared
+// device buffer that two calls in flight could race on.  The entry is picked by a run-time index; __grid_constant__ guarantees
+// that this reads the parameter block in place, where a plain by-value parameter would allow the compiler to copy it to
+// local memory (ptxas reports no stack frame for the kernel either way with CUDA 12.9).
+constexpr int FP_MAX_FRAMES = 64;
+struct FrameEntry {
+  const uint8_t* data;          // [fh, fw, 3] RGB, row pitch `pitch` bytes
+  long long pitch;
+  int fh, fw;
+  int first_box;
+  int pad_;
+};
+static_assert(sizeof(FrameEntry) == 32, "frame table entry layout");
 struct FramePatchParams {
-  PreprocParams pp;             // crops unused; pp.n = number of boxes
+  PreprocParams pp;             // frame / pitch / fh / fw / crops unused (the table holds the frames); pp.n = number of boxes
   __nv_bfloat16* rows;          // [n*192, 768]
   const float4* pos_bias;       // [192*D/4]
   float4* stream;               // [n*192*D/4]
   int D;
+  int num_frames;               // 1..FP_MAX_FRAMES
+  FrameEntry frames[FP_MAX_FRAMES];
 };
 
-__global__ void __launch_bounds__(384) frame_to_patch_rows(const FramePatchParams q) {
+__global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant__ FramePatchParams q) {
   constexpr int FP_PITCH = 208;                               // 2 + 192 + 14 bf16 per tile row: 16-byte aligned rows
   __shared__ uint16_t s_lut[3][256];
   __shared__ PpAxis s_ay[16];
@@ -161,9 +178,18 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const FramePatchParam
   }
   const bool mirror = crop >= p.n;
   const int box = mirror ? crop - p.n : crop;
+  int lo = 0, hi = q.num_frames;                              // the last frame whose first_box <= box
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (q.frames[mid].first_box <= box) lo = mid; else hi = mid;
+  }
+  const FrameEntry& fr = q.frames[lo];
+  const uint8_t* frame = fr.data;
+  const long long pitch = fr.pitch;
+  const int fh = fr.fh, fw = fr.fw;
   const int* bb = p.bboxes + 4 * box;
-  const int x0 = min(max(bb[0] - p.pad, 0), p.fw), x1 = min(max(bb[2] + p.pad, 0), p.fw);
-  const int y0 = min(max(bb[1] - p.pad, 0), p.fh), y1 = min(max(bb[3] + p.pad, 0), p.fh);
+  const int x0 = min(max(bb[0] - p.pad, 0), fw), x1 = min(max(bb[2] + p.pad, 0), fw);
+  const int y0 = min(max(bb[1] - p.pad, 0), fh), y1 = min(max(bb[3] + p.pad, 0), fh);
   int w = x1 - x0, h = y1 - y0;
   const bool empty = w <= 0 || h <= 0;
   if (empty) { w = 0; h = 0; }
@@ -199,8 +225,8 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const FramePatchParam
       const PpAxis ax = s_ax[dx];
       const int cy0 = ay.i0 - top, cy1 = ay.i1 - top, cx0 = ax.i0 - left, cx1 = ax.i1 - left;
       const bool vy0 = cy0 >= 0 && cy0 < h, vy1 = cy1 >= 0 && cy1 < h, vx0 = cx0 >= 0 && cx0 < w, vx1 = cx1 >= 0 && cx1 < w;
-      const uint8_t* r0 = p.frame + static_cast<size_t>(vy0 ? y0 + cy0 : 0) * p.pitch;
-      const uint8_t* r1 = p.frame + static_cast<size_t>(vy1 ? y0 + cy1 : 0) * p.pitch;
+      const uint8_t* r0 = frame + static_cast<size_t>(vy0 ? y0 + cy0 : 0) * pitch;
+      const uint8_t* r1 = frame + static_cast<size_t>(vy1 ? y0 + cy1 : 0) * pitch;
       const int f0 = (vx0 ? x0 + cx0 : 0) * 3, f1 = (vx1 ? x0 + cx1 : 0) * 3;
 #pragma unroll
       for (int c = 0; c < 3; ++c) {

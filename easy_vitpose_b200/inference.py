@@ -89,6 +89,13 @@ class B200PoseBackend:
         return self.model.infer_frame_host(img, bboxes)[0]
 
     @torch.no_grad()
+    def inference_frames(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]") -> "list[np.ndarray]":
+        """Several uint8 RGB frames (cameras of a rig, frames of a video, several streams) + each frame's boxes -> one
+        float32 [n_i,K,3] (y, x, score) per frame, in that frame's pixels: inference_frame for all of them with the people of
+        all frames packed into as few engine calls as max_batch allows."""
+        return self.model.infer_frames_host(imgs, bboxes_list)[0]
+
+    @torch.no_grad()
     def inference_batch(self, imgs: "list[np.ndarray]") -> np.ndarray:
         """All person crops of a frame in one engine call -> float32 [n,K,3]."""
         if not imgs:

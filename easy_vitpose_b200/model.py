@@ -14,9 +14,45 @@ import torch
 
 from . import _lib
 
-__all__ = ["ViTPose"]
+__all__ = ["ViTPose", "plan_frame_chunks"]
 
 IMG_H, IMG_W, HM_H, HM_W = 256, 192, 64, 48
+
+
+def plan_frame_chunks(counts, limit: int, max_frames: int = _lib.MAX_FRAMES) -> "list[list[tuple[int, int, int]]]":
+    """Splits the boxes of several frames (counts[j] boxes in frame j) into engine calls of at most `limit` boxes from at most
+    `max_frames` frames.  Returns the calls in order; each is a list of (frame, first, stop): boxes first..stop-1 of that
+    frame.  Every box lands in exactly one call, in frame order; frames without boxes appear in none, and a frame's boxes
+    may continue in the next call."""
+    if limit < 1 or max_frames < 1:
+        raise ValueError(f"limit {limit} and max_frames {max_frames} must be >= 1")
+    chunks, cur, used = [], [], 0
+    for f, c in enumerate(counts):
+        c = int(c)
+        if c < 0:
+            raise ValueError(f"frame {f} has {c} boxes")
+        s = 0
+        while s < c:
+            if used == limit or len(cur) == max_frames:
+                chunks.append(cur)
+                cur, used = [], 0
+            take = min(c - s, limit - used)
+            cur.append((f, s, s + take))
+            used += take
+            s += take
+    if cur:
+        chunks.append(cur)
+    return chunks
+
+
+def _frame_array(frames, chunk):
+    """vpb_frame array for one planned call: entries 0..last frame of the call, so that the engine's messages name the
+    caller's frame index; frames outside the call get 0 boxes (skipped).  `frames` holds (data pointer, h, w, pitch)."""
+    arr = (_lib.VpbFrame * (chunk[-1][0] + 1))()
+    for f, s, e in chunk:
+        ptr, h, w, pitch = frames[f]
+        arr[f] = _lib.VpbFrame(ptr, h, w, pitch, e - s)
+    return arr
 
 
 def _expected_shapes(D: int, depth: int, K: int) -> "OrderedDict[str, tuple]":
@@ -225,7 +261,7 @@ class ViTPose:
 
     def set_flip_test(self, flip_pairs, shift_heatmap: bool = False) -> None:
         """Flip test on every keypoint call (infer_crops, infer_host, submit_host, infer_frame, infer_frame_host,
-        submit_frame_host): heatmaps of each crop and of its mirror image (flipped back, pairs swapped, shifted by one pixel
+        submit_frame_host, infer_frames, infer_frames_host, submit_frames_host): heatmaps of each crop and of its mirror image (flipped back, pairs swapped, shifted by one pixel
         when shift_heatmap) averaged before the decode -- the test_cfg flip_test=True of the reference configs
         (configs/ViTPose_common.py:124).  Keypoints and returned heatmaps are then bit-identical to forward_flip_test
         followed by decode_heatmaps.  A call then takes at most max_batch // 2 crops.  `None` turns it off.  Synchronises
@@ -488,6 +524,121 @@ class ViTPose:
             _lib.check_value(_lib.lib().vpb_submit_frame_host(
                 self._handle, frame.ctypes.data_as(C.c_void_p), frame.shape[0], frame.shape[1], bboxes.ctypes.data_as(C.c_void_p), n,
                 kpts_out.ctypes.data_as(C.c_void_p), idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+    # ---------------------------------------------------------------------------------------- multi-frame calls
+    def _device_frame(self, j: int, frame: torch.Tensor) -> torch.Tensor:
+        if not isinstance(frame, torch.Tensor) or frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[2] != 3:
+            raise ValueError(f"frame {j} must be a uint8 RGB tensor [H,W,3]")
+        if not frame.is_cuda:
+            frame = frame.to(torch.device("cuda", self._device), non_blocking=True)
+        if frame.device.index != self._device:
+            raise ValueError(f"frame {j} lives on {frame.device}, the engine on cuda:{self._device}")
+        if frame.stride(2) != 1 or frame.stride(1) != 3 or frame.stride(0) < 3 * frame.shape[1]:
+            frame = frame.contiguous()                       # rows of packed pixels at any pitch are read in place
+        return frame
+
+    @staticmethod
+    def _host_frame(j: int, frame: np.ndarray) -> np.ndarray:
+        if not isinstance(frame, np.ndarray) or frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
+            raise ValueError(f"frame {j} must be a uint8 RGB array [H,W,3]")
+        if frame.strides[2] != 1 or frame.strides[1] != 3 or frame.strides[0] < 3 * frame.shape[1]:
+            frame = np.ascontiguousarray(frame)
+        return frame
+
+    @staticmethod
+    def _round_boxes(bboxes) -> np.ndarray:
+        bb = np.asarray(bboxes)
+        if bb.dtype.kind == "f":
+            bb = bb.round()                                  # easy_ViTPose/inference.py:253 (round half to even)
+        return np.ascontiguousarray(bb.reshape(-1, 4), np.int32)
+
+    def infer_frames(self, frames, bboxes, check: bool = False):
+        """The people of several frames in as few engine calls as the limits allow: uint8 RGB frames [H_j,W_j,3] (CUDA) and
+        per-frame boxes [n_j,4] -> (list of kpts f32 [n_j,K,3] (y, x, score) in frame j's pixels, list of idx i32 [n_j,K]).
+        Bit-identical to one infer_frame per frame.  Calls hold at most batch_limit boxes from at most 64 frames with boxes; a
+        frame's boxes may be split over two calls.  A frame whose rows are packed pixels at a larger pitch (a column slice
+        of a wider image) is read in place.  Empty boxes set the status word; `check=True` synchronises and raises."""
+        self._ensure()
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        dev = torch.device("cuda", self._device)
+        boxes = []
+        for b in bboxes:                                     # rounded as _check_frame does; device boxes stay on the device
+            b = torch.as_tensor(b)
+            if b.is_floating_point():
+                b = b.round()
+            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
+        counts = [b.shape[0] for b in boxes]
+        bb = torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=dev)
+        n = bb.shape[0]
+        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
+        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
+        table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
+        s = 0                                                # first box of the current call
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            arr = _frame_array(table, chunk)
+            self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames(
+                self._handle, arr, len(arr), C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
+                C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 1:
+            raise ValueError("a box is empty after padding and clipping to its frame")
+        return list(kp.split(counts)) if counts else [], list(idx.split(counts)) if counts else []
+
+    def infer_frames_host(self, frames, bboxes):
+        """HOST form of infer_frames (vpb_infer_frames_host, synchronous): numpy frames [H_j,W_j,3] uint8 and per-frame boxes
+        -> (list of kpts [n_j,K,3], list of idx [n_j,K]) numpy arrays, chunked as infer_frames.  A box that is empty after
+        padding and clipping raises ValueError naming its frame."""
+        self._ensure()
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
+        boxes = [self._round_boxes(b) for b in bboxes]
+        counts = [len(b) for b in boxes]
+        bb = np.concatenate(boxes, 0) if boxes else np.zeros((0, 4), np.int32)
+        n = bb.shape[0]
+        kp = np.empty((n, self.num_keypoints, 3), np.float32)
+        idx = np.empty((n, self.num_keypoints), np.int32)
+        table = [(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames]
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, self.batch_limit):
+                arr = _frame_array(table, chunk)
+                _lib.check_value(_lib.lib().vpb_infer_frames_host(
+                    self._handle, arr, len(arr), bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
+                    idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        if not counts:
+            return [], []
+        split = np.cumsum(counts)[:-1]
+        return np.split(kp, split), np.split(idx, split)
+
+    def submit_frames_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int) -> None:
+        """Asynchronous vpb_submit_frames_host, ONE engine call (wait with wait_host(slot)): uint8 frames [H_j,W_j,3] whose
+        rows are packed pixels (any row pitch), per-frame int32 boxes [n_j,4] (already rounded), and the concatenated outputs
+        float32 kpts_out [n,K,3] / int32 idx_out [n,K], n = sum n_j <= batch_limit, at most 64 frames with boxes.  Frames and
+        outputs must stay alive and unmodified until the wait (pinned memory: real copy / compute overlap)."""
+        self._ensure()
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        for j, (f, b) in enumerate(zip(frames, bboxes)):
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
+                    or f.strides[2] != 1 or f.strides[1] != 3 or f.strides[0] < 3 * f.shape[1]:
+                raise ValueError(f"frame {j}: uint8 [H,W,3] with packed pixels in each row expected")
+            if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
+                raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
+        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
+        n = bb.shape[0]
+        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
+                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
+            raise ValueError("submit_frames_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
+        arr = (_lib.VpbFrame * len(frames))(*[_lib.VpbFrame(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0], len(b))
+                                             for f, b in zip(frames, bboxes)])
+        with torch.cuda.device(self._device):
+            _lib.check_value(_lib.lib().vpb_submit_frames_host(
+                self._handle, arr, len(arr), bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
+                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
 
     def wait_host(self, slot: int) -> None:
         _lib.check(_lib.lib().vpb_wait_host(self._handle, int(slot)))

@@ -169,6 +169,33 @@ int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h,
 int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
                           int32_t n, float* h_kpts, int32_t* h_idx, int32_t slot);
 
+/* ---- multi-frame entry points: the people of several frames (cameras, video frames, streams) as ONE engine call, so a
+ * call of many small frames runs the batch size of their sum.  h_frames is always a HOST array of num_frames entries; the
+ * boxes of all frames are concatenated in frame order (frame j owns the next h_frames[j].num_boxes rows), and the outputs
+ * [n,K,3] / [n,K] come back in the same order, n = the sum of num_boxes, each keypoint in its own frame's pixels.  The
+ * results are bit-identical to one vpb_infer_frame per frame (the forward is batch-invariant, the decode runs per crop).
+ * Frames with 0 boxes are skipped and do not count towards VPB_MAX_FRAMES; n = 0 returns VPB_OK and launches nothing.
+ * VPB_ERR_ARG: n above the batch limit (max_batch, max_batch / 2 with flip test on), more than VPB_MAX_FRAMES frames with
+ * boxes, a negative num_boxes, a frame with boxes whose data is NULL, height or width < 1, or pitch below 3 * width.
+ * Flip test (vpb_set_flip_test) applies as for the single-frame calls. */
+#define VPB_MAX_FRAMES 64
+typedef struct vpb_frame {
+  const uint8_t* data;    /* u8 [height, width, 3] RGB; device address (vpb_infer_frames) or host (the _host forms) */
+  int32_t height, width;
+  int64_t pitch_bytes;    /* row pitch; 0 = packed (3 * width) */
+  int32_t num_boxes;      /* this frame's boxes are the next num_boxes rows of the box array (0 allowed) */
+} vpb_frame;
+/* Device frames and boxes (d_bboxes i32 [n,4]); empty boxes set bit 0 of the status word, as vpb_infer_frame does. */
+int vpb_infer_frames(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* d_bboxes,
+                     float* d_kpts, int32_t* d_idx, void* stream);
+/* HOST frames (any pitch; each is staged packed) and boxes: every box is checked against its own frame and an empty one
+ * returns VPB_ERR_ARG naming the frame and the box.  Same staging slots, events, concurrency contract and vpb_wait_host as
+ * vpb_infer_frame_host / vpb_submit_frame_host; the slot's staging buffer grows to the sum of the frame sizes. */
+int vpb_infer_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
+                          float* h_kpts, int32_t* h_idx, void* stream);
+int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
+                           float* h_kpts, int32_t* h_idx, int32_t slot);     /* completes with vpb_wait_host(slot) */
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* Options (all keep the results bit-identical unless noted): "stop_after", "profile", "pdl", "graph", "ln_fused",
@@ -184,8 +211,8 @@ int vpb_set_option(vpb_engine* e, const char* name, int32_t value);
  * TopdownHeatmapSimpleHead.inference_model (vit_models/head/topdown_heatmap_simple_head.py:195-218, shift at :210-212).
  * h_perm i32 [k] (HOST) = the keypoint permutation the flip pairs induce (as for vpb_flip_back); k must equal the engine's K
  * and every entry lie in [0,K), else VPB_ERR_ARG.  h_perm = NULL turns flip test off (the default).
- * While it is on, vpb_infer, vpb_infer_host, vpb_submit_host, vpb_infer_frame, vpb_infer_frame_host and vpb_submit_frame_host
- * run each crop and its mirror image as one batch of 2 * batch crops (the mirror images are gathered on the fly, never
+ * While it is on, vpb_infer, vpb_infer_host, vpb_submit_host, vpb_infer_frame, vpb_infer_frame_host, vpb_submit_frame_host and
+ * the multi-frame calls (vpb_infer_frames, vpb_infer_frames_host, vpb_submit_frames_host) run each crop and its mirror image as one batch of 2 * batch crops (the mirror images are gathered on the fly, never
  * stored), average the maps and decode the averaged maps (wrap_batch = 0); d_heatmaps, when given, receives the averaged
  * maps.  batch must then be <= max_batch / 2.  vpb_forward, vpb_forward_features, vpb_head, vpb_decode* and vpb_flip_back
  * are unaffected.  SYNCHRONOUS: waits for the engine's pending work (which keeps the previous setting), and drops the
