@@ -11,3 +11,4 @@ from .configs import COCO_FLIP_PAIRS, data_cfg, dyn_model_import, flip_pairs_for
 from .inference import B200PoseBackend, install  # noqa: F401
 from .model import ViTPose  # noqa: F401
 from .top_down_eval import decode_heatmaps, decode_topdown, keypoints_from_heatmaps  # noqa: F401
+from .topdown import topdown_args  # noqa: F401

@@ -56,6 +56,11 @@ EXPORTS = {
     "vpb_infer_frames": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_infer_frames_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_submit_frames_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
+    "vpb_preprocess_affine": (C.c_int, [C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p]),
+    "vpb_infer_affine_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]),
     "vpb_host_alloc": (C.c_void_p, [C.c_int64]),
     "vpb_host_free": (None, [C.c_void_p]),
     "vpb_kernel_launches": (C.c_int, [C.c_void_p, C.c_int32]),

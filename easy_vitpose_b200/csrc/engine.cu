@@ -359,7 +359,8 @@ struct vpb_engine {
   // work per call, which is what bounds small ragged batches (video streams).  The graph only touches engine-owned
   // memory (the caller's crops are consumed by the eagerly launched patch_im2col; org_wh / keypoints / argmax / heatmaps
   // move by small device copies), so it is valid for any caller pointers.  Captured on a batch size's second use.
-  struct GraphEntry { int batch; int seen; cudaGraphExec_t exec; };
+  // affine = the graph decodes with centre / scale (vpb_infer_affine) instead of canvas sizes / offsets
+  struct GraphEntry { int batch; int seen; cudaGraphExec_t exec; bool affine; };
   std::vector<GraphEntry> graphs;
   bool use_graph = true;
   // L2 residency: the fp32 token stream x (37.7 MB at B=64) is read-modify-written by every residual GEMM and read by every
@@ -371,6 +372,10 @@ struct vpb_engine {
   std::vector<cudaStream_t> l2_streams;
   float* g_kpts = nullptr;      // graph-owned outputs / decode inputs: the captured chain only touches engine memory
   int32_t *g_idx = nullptr, *g_org = nullptr, *g_offs = nullptr;
+  float* g_cs = nullptr;        // [max_batch,4] centre / scale the affine graphs decode with
+  // affine host calls (vpb_infer_affine_host): matrices and centre / scale staged next to the slot-0 frames
+  double* mat_stage = nullptr;
+  float* cs_stage = nullptr;
   // frame-level entry points (crop pre-processing on the GPU): canvas sizes / frame offsets produced by frame_to_patch_rows,
   // the status word it flags empty boxes in, and per-slot frame + box staging for the host variants
   int32_t *pp_org = nullptr, *pp_offs = nullptr, *pp_status = nullptr;
@@ -659,6 +664,9 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(dev_alloc(e, &e->g_idx, B * e->K));
   VPB_TRY(dev_alloc(e, &e->g_org, B * 2));
   VPB_TRY(dev_alloc(e, &e->g_offs, B * 2));
+  VPB_TRY(dev_alloc(e, &e->g_cs, B * 4));
+  VPB_TRY(dev_alloc(e, &e->mat_stage, B * 6));
+  VPB_TRY(dev_alloc(e, &e->cs_stage, B * 4));
   VPB_TRY(dev_alloc(e, &e->pp_org, B * 2));
   VPB_TRY(dev_alloc(e, &e->pp_offs, B * 2));
   VPB_TRY(dev_alloc(e, &e->pp_status, 1));
@@ -743,12 +751,31 @@ static int patch_gather(vpb_engine* e, const float* d_crops, int n_src, int B, c
 }
 // Where a batch of patch rows comes from: normalised f32 crops (patch_im2col) or a table of uint8 frames + boxes
 // (frame_to_patch_rows: crop pre-processing fused with the im2col; it also fills pp_org / pp_offs for the decode).
+// Affine crops (frame_to_patch_rows_affine) take a matrix per box instead of a box, and their keypoints are decoded with
+// centre / scale (decode mode 4) instead of canvas sizes and offsets.
 struct Source {
   const float* crops = nullptr;
   const FrameEntry* frames = nullptr;       // num_frames entries, only frames that have boxes
   int num_frames = 0;
   const int32_t* bboxes = nullptr;
+  const double* mats = nullptr;             // [n,6] affine matrices (then bboxes is unused)
+  const float* cs = nullptr;                // [n,4] centre / scale of the affine decode
 };
+static AffineParams affine_params(const FrameEntry* frames, int num_frames, const double* mats, const float* cs, int n, int* status) {
+  AffineParams q;
+  memset(&q, 0, sizeof(q));
+  q.mats = mats; q.cs = cs; q.n = n; q.status = status; q.num_frames = num_frames;
+  memcpy(q.frames, frames, static_cast<size_t>(num_frames) * sizeof(FrameEntry));
+  return q;
+}
+static int affine_gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
+  AffineParams q = affine_params(src.frames, src.num_frames, src.mats, src.cs, n_src, e->pp_status);
+  q.rows = e->patch_rows; q.pos_bias = reinterpret_cast<const float4*>(e->pos_bias); q.stream = reinterpret_cast<float4*>(e->x); q.D = e->D;
+  e->prof.begin(KC_PREPROCESS, st);
+  CU_TRY(launch_k(frame_to_patch_rows_affine, dim3(B, 16), dim3(384), 0, st, q));
+  e->prof.end(st);
+  return VPB_OK;
+}
 static int frame_gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
   FramePatchParams q;
   memset(&q, 0, sizeof(q));
@@ -763,7 +790,8 @@ static int frame_gather(vpb_engine* e, const Source& src, int n_src, int B, cuda
   return VPB_OK;
 }
 static int gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
-  return src.crops ? patch_gather(e, src.crops, n_src, B, st) : frame_gather(e, src, n_src, B, st);
+  if (src.crops) return patch_gather(e, src.crops, n_src, B, st);
+  return src.mats ? affine_gather(e, src, n_src, B, st) : frame_gather(e, src, n_src, B, st);
 }
 // Chained form of the backbone (chain.cuh): 1 + depth persistent GEMM launches + depth attention launches.
 //   launch 0:        patch embed (+= x) -> LN(norm1 of block 0) -> qkv of block 0
@@ -1261,6 +1289,14 @@ static int flip_average(vpb_engine* e, int batch, float* out, cudaStream_t st) {
   return VPB_OK;
 }
 
+// The decode of a keypoint call: canvas sizes + frame offsets (VitInference.postprocess, one reference call per crop), or for
+// the affine calls centre / scale (mode 4, one reference call on the whole array, exactly as vpb_decode_modes).
+static int decode_keypoints(vpb_engine* e, const float* heat, int32_t batch, const int32_t* d_org_wh, const int32_t* d_offs_yx,
+                            const float* d_cs, float* d_kpts, int32_t* d_idx, cudaStream_t st) {
+  if (d_cs) return vpb_decode_modes(heat, batch, e->K, DECODE_DARK_UDP, d_cs, nullptr, d_kpts, d_idx, st);
+  return decode_launch(heat, batch, e->K, d_org_wh, d_offs_yx, d_kpts, d_idx, 0, st);
+}
+
 // `heat` receives the batch maps the keypoints are decoded from; with flip test the raw 2 * batch maps go to e->heat first
 static int infer_enqueue(vpb_engine* e, const Source& src, const int32_t* d_org_wh, const int32_t* d_offs_yx, int32_t batch,
                          float* d_kpts, int32_t* d_idx, float* heat, void* stream) {
@@ -1273,7 +1309,7 @@ static int infer_enqueue(vpb_engine* e, const Source& src, const int32_t* d_org_
   if (e->stop_after) return VPB_OK;
   if (e->flip) VPB_TRY(flip_average(e, batch, heat, st));
   e->prof.begin(KC_DECODE, static_cast<cudaStream_t>(stream));
-  VPB_TRY(decode_launch(heat, batch, e->K, d_org_wh, d_offs_yx, d_kpts, d_idx, 0, stream));
+  VPB_TRY(decode_keypoints(e, heat, batch, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, st));
   e->prof.end(static_cast<cudaStream_t>(stream));
   return VPB_OK;
 }
@@ -1298,25 +1334,30 @@ static int infer_core_locked(vpb_engine* e, const Source& src, const int32_t* d_
   // (a nested cudaStreamBeginCapture would fail): the engine's kernels then simply become nodes of the caller's graph
   if (!e->use_graph || e->prof.on || e->stop_after || st == nullptr || stream_is_capturing(st))
     return infer_enqueue(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, heat, stream);
+  const bool affine = src.cs != nullptr;
   vpb_engine::GraphEntry* g = nullptr;
   for (auto& c : e->graphs)
-    if (c.batch == batch) g = &c;
+    if (c.batch == batch && c.affine == affine) g = &c;
   if (!g) {                                                               // first use of this batch size: run eagerly
-    e->graphs.push_back({batch, 1, nullptr});
+    e->graphs.push_back({batch, 1, nullptr, affine});
     return infer_enqueue(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, heat, stream);
   }
   const int nb = model_crops(e, batch);
   VPB_TRY(gather(e, src, batch, nb, st));
-  CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(batch) * 2 * sizeof(int32_t), st));
+  if (affine) {
+    CU_TRY(cudaMemcpyAsync(e->g_cs, src.cs, static_cast<size_t>(batch) * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  } else {
+    CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(batch) * 2 * sizeof(int32_t), st));
+  }
   if (!g->exec) {                                                         // second use: capture, instantiate
     cudaGraph_t graph = nullptr;
     CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     int rc = backbone(e, nb, st);
     if (rc == VPB_OK) rc = head(e, nb, e->heat, st);
     if (rc == VPB_OK && e->flip) rc = flip_average(e, batch, e->heat, st);      // in place: the first batch maps
-    if (rc == VPB_OK) rc = decode_launch(e->heat, batch, e->K, e->g_org, e->g_offs, e->g_kpts, e->g_idx, 0, stream);
+    if (rc == VPB_OK) rc = decode_keypoints(e, e->heat, batch, e->g_org, e->g_offs, affine ? e->g_cs : nullptr, e->g_kpts, e->g_idx, st);
     const cudaError_t ce = cudaStreamEndCapture(st, &graph);
     if (rc != VPB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
     if (ce != cudaSuccess) return fail(VPB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
@@ -1380,10 +1421,9 @@ static FrameEntry single_frame(const uint8_t* data, int32_t fh, int32_t fw) {
 
 // The caller's frame array -> the gather's table.  Frames without boxes are left out (they do not count towards
 // VPB_MAX_FRAMES); pitch_bytes 0 means packed rows.  *n = the total number of boxes, checked against the batch limit.
-static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32_t num_frames, FrameEntry* tab, int* num_tab,
-                       int32_t* n) {
-  if (!e) return fail(VPB_ERR_ARG, "null engine");
-  if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
+// build_frame_table is the engine-free part (vpb_preprocess_affine): at most `limit` boxes.
+static int build_frame_table(const char* fn, const vpb_frame* fr, int32_t num_frames, int limit, FrameEntry* tab, int* num_tab,
+                             int32_t* n) {
   if (num_frames < 0 || (num_frames > 0 && !fr)) return fail(VPB_ERR_ARG, "%s: %d frames, frame array %p", fn, num_frames, fr);
   long long boxes = 0;
   int used = 0;
@@ -1396,8 +1436,8 @@ static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32
       return fail(VPB_ERR_ARG, "%s: frame %d: data %p, %dx%d (w x h), pitch %lld bytes (0 or >= 3 * width expected)", fn, j,
                   static_cast<const void*>(f.data), f.width, f.height, static_cast<long long>(f.pitch_bytes));
     if (used == VPB_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than VPB_MAX_FRAMES = %d frames with boxes", fn, VPB_MAX_FRAMES);
-    if (boxes + f.num_boxes > e->maxB)
-      return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, e->maxB, j);
+    if (boxes + f.num_boxes > limit)
+      return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, limit, j);
     FrameEntry& t = tab[used++];
     memset(&t, 0, sizeof(t));
     t.data = f.data; t.pitch = pitch; t.fh = f.height; t.fw = f.width; t.first_box = static_cast<int>(boxes);
@@ -1405,7 +1445,14 @@ static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32
   }
   *num_tab = used;
   *n = static_cast<int32_t>(boxes);
-  return boxes ? check_ready_keypoints(e, *n) : VPB_OK;
+  return VPB_OK;
+}
+static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32_t num_frames, FrameEntry* tab, int* num_tab,
+                       int32_t* n) {
+  if (!e) return fail(VPB_ERR_ARG, "null engine");
+  if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
+  VPB_TRY(build_frame_table(fn, fr, num_frames, e->maxB, tab, num_tab, n));
+  return *n ? check_ready_keypoints(e, *n) : VPB_OK;
 }
 
 extern "C" int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int32_t frame_w, const int32_t* d_bboxes,
@@ -1473,7 +1520,8 @@ static int frame_stage_reserve(vpb_engine* e, int slot, size_t bytes) {
 }
 
 // Host frames -> staging slot `slot`, enqueued on `st` after the slot's last user: each frame packed (a 2D copy from its pitch),
-// then the boxes of all frames in one copy.  Repoints `tab` at the staged frames.
+// then the boxes of all frames in one copy (none for h_bboxes = NULL: the affine calls stage matrices instead).  Repoints `tab`
+// at the staged frames.
 static int stage_frames_host(vpb_engine* e, int slot, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, cudaStream_t st) {
   size_t total = 0;
   for (int j = 0; j < nt; ++j) total += static_cast<size_t>(tab[j].fh) * tab[j].fw * 3;
@@ -1488,7 +1536,7 @@ static int stage_frames_host(vpb_engine* e, int slot, FrameEntry* tab, int nt, c
     tab[j].data = dst; tab[j].pitch = static_cast<long long>(row);
     off += bytes;
   }
-  CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (h_bboxes) CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   return VPB_OK;
 }
 // synchronous host form on slot 0 and the caller's stream
@@ -1562,6 +1610,76 @@ extern "C" int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, 
   if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_submit_frames_host: null pointer");
   VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
   return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
+}
+
+// ------------------------------------------------------------------------------------------------ affine top-down crops
+// host matrices / centre-scale: what the device forms can only flag in the status word is an argument error here
+static int check_affine_host(const double* mats, const float* cs, int32_t n) {
+  for (int i = 0; i < n; ++i) {
+    for (int j = 0; j < 6; ++j)
+      if (!std::isfinite(mats[6 * i + j])) return fail(VPB_ERR_ARG, "box %d: matrix entry %d is %g (finite expected)", i, j, mats[6 * i + j]);
+    if (!cs) continue;
+    const float* c = cs + 4 * i;
+    if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !(c[2] > 0.f) || !(c[3] > 0.f) || !std::isfinite(c[2]) || !std::isfinite(c[3]))
+      return fail(VPB_ERR_ARG, "box %d: centre (%g, %g), scale (%g, %g): finite centre and scale > 0 expected", i, c[0], c[1], c[2], c[3]);
+  }
+  return VPB_OK;
+}
+
+extern "C" int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, float* d_crops, void* stream) {
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(build_frame_table("vpb_preprocess_affine", h_frames, num_frames, 1 << 30, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  if (!d_mats || !d_crops) return fail(VPB_ERR_ARG, "vpb_preprocess_affine: null pointer");
+  AffineParams q = affine_params(tab, nt, d_mats, nullptr, n, nullptr);
+  q.crops = d_crops;
+  crop_warp_normalise<<<dim3(n, PP_H / PP_ROWS), PP_W, 0, static_cast<cudaStream_t>(stream)>>>(q);
+  CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+static int infer_affine_enqueue(vpb_engine* e, const FrameEntry* tab, int num_frames, const double* d_mats, const float* d_cs, int32_t n,
+                                float* d_kpts, int32_t* d_idx, cudaStream_t st) {
+  Source src;
+  src.frames = tab; src.num_frames = num_frames; src.mats = d_mats; src.cs = d_cs;
+  VPB_TRY(apply_l2_policy(e, st));
+  return infer_core(e, src, nullptr, nullptr, n, d_kpts, d_idx, nullptr, st);
+}
+
+extern "C" int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, const float* d_cs,
+                                float* d_kpts, int32_t* d_idx, void* stream) {
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_affine", e, h_frames, num_frames, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine: null pointer");
+  return infer_affine_enqueue(e, tab, nt, d_mats, d_cs, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* h_mats, const float* h_cs,
+                                     float* h_kpts, int32_t* h_idx, void* stream) {
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_affine_host", e, h_frames, num_frames, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_host: null pointer");
+  VPB_TRY(check_affine_host(h_mats, h_cs, n));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  VPB_TRY(stage_frames_host(e, 0, tab, nt, nullptr, n, st));         // waits for slot 0's last user
+  CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
+  VPB_TRY(infer_affine_enqueue(e, tab, nt, e->mat_stage, e->cs_stage, n, e->kpts[0], e->idx[0], st));
+  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU_TRY(cudaEventRecord(e->ev_done[0], st));
+  CU_TRY(cudaStreamSynchronize(st));
+  return VPB_OK;
 }
 
 extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t* h_org_wh, int32_t batch, float* h_kpts,

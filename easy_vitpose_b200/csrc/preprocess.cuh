@@ -250,4 +250,170 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Affine top-down crops (the mmpose / HRNet data path of the reference's datasets/COCO.py:288-302): per box a 2x3 matrix
+// M (what the caller hands to cv2.warpAffine), cv2.warpAffine(frame, M, (192, 256), INTER_LINEAR, constant 0 border), then
+// torchvision ToTensor + Normalize in float32.  cv2's uint8 path is fixed-point and restated exactly (oracle/affine_oracle.py
+// pins it against cv2 4.13):
+//   the inverse of M in double (D = M0 M4 - M1 M3, 1/D or 0 for a singular M), then with AB_BITS = 10, INTER_BITS = 5
+//   adelta[x] = cvRound(M0' x 1024), X0(y) = cvRound((M1' y + M2') 1024) + 16, X = (X0 + adelta) >> 5 (same for Y):
+//   integer tap X >> 5 (int16-saturated), fraction X & 31; int16 weights (32 - f | f)_y (32 - f | f)_x 32, which sum to 32768
+//   exactly; pixel (sum w p + 2^14) >> 15 with taps outside the frame reading 0.
+// The double arithmetic is spelled with __dmul_rn / __dadd_rn so that nothing contracts into an FMA (cv2 rounds each step).
+struct AffineInv { double m[6]; };     // the inverted matrix (M0', M1', M2', M3', M4', M5')
+__device__ __forceinline__ AffineInv affine_invert(const double* M) {
+  const double m0 = M[0], m1 = M[1], m2 = M[2], m3 = M[3], m4 = M[4], m5 = M[5];
+  double d = __dsub_rn(__dmul_rn(m0, m4), __dmul_rn(m1, m3));
+  d = d != 0.0 ? __ddiv_rn(1.0, d) : 0.0;
+  AffineInv r;
+  r.m[0] = __dmul_rn(m4, d);
+  r.m[1] = __dmul_rn(m1, -d);
+  r.m[3] = __dmul_rn(m3, -d);
+  r.m[4] = __dmul_rn(m0, d);
+  r.m[2] = __dsub_rn(__dmul_rn(-r.m[0], m2), __dmul_rn(r.m[1], m5));
+  r.m[5] = __dsub_rn(__dmul_rn(-r.m[3], m2), __dmul_rn(r.m[4], m5));
+  return r;
+}
+// adelta / bdelta of output column x
+__device__ __forceinline__ int2 affine_col(const AffineInv& a, int x) {
+  return make_int2(__double2int_rn(__dmul_rn(__dmul_rn(a.m[0], static_cast<double>(x)), 1024.0)),
+                   __double2int_rn(__dmul_rn(__dmul_rn(a.m[3], static_cast<double>(x)), 1024.0)));
+}
+// X0 / Y0 of output row y (the +16 = round_delta of INTER_BITS)
+__device__ __forceinline__ int2 affine_row(const AffineInv& a, int y) {
+  const double yd = static_cast<double>(y);
+  return make_int2(__double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.m[1], yd), a.m[2]), 1024.0)) + 16,
+                   __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.m[4], yd), a.m[5]), 1024.0)) + 16);
+}
+// one output pixel from its fixed-point source coordinates: the three warped bytes
+__device__ __forceinline__ void affine_pixel(const uint8_t* frame, long long pitch, int fh, int fw, int X, int Y, int v[3]) {
+  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767), fx = X & 31, fy = Y & 31;
+  const bool vx0 = sx >= 0 && sx < fw, vx1 = sx + 1 >= 0 && sx + 1 < fw, vy0 = sy >= 0 && sy < fh, vy1 = sy + 1 >= 0 && sy + 1 < fh;
+  const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
+  const uint8_t* r0 = frame + static_cast<size_t>(vy0 ? sy : 0) * pitch;     // only dereferenced when valid
+  const uint8_t* r1 = frame + static_cast<size_t>(vy1 ? sy + 1 : 0) * pitch;
+  const int c0 = (vx0 ? sx : 0) * 3, c1 = (vx1 ? sx + 1 : 0) * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int p00 = (vy0 && vx0) ? r0[c0 + c] : 0, p01 = (vy0 && vx1) ? r0[c1 + c] : 0;
+    const int p10 = (vy1 && vx0) ? r1[c0 + c] : 0, p11 = (vy1 && vx1) ? r1[c1 + c] : 0;
+    v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + (1 << 14)) >> 15;
+  }
+}
+// torchvision ToTensor + Normalize (COCO.py:120-123): float32 throughout, IEEE division
+__device__ __forceinline__ float affine_norm(int c, int v) {
+  const float mean = c == 0 ? 0.485f : (c == 1 ? 0.456f : 0.406f), stdv = c == 0 ? 0.229f : (c == 1 ? 0.224f : 0.225f);
+  return __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(v), 255.f), mean), stdv);
+}
+
+// Launch parameters of both affine kernels.  The frame table is frame_to_patch_rows' (same binary search on first_box).
+struct AffineParams {
+  const double* mats;           // [n,6] f64: the matrix given to cv2.warpAffine (image -> crop)
+  const float* cs;              // [n,4] (cx, cy, sx, sy) of the decode, checked for sx, sy > 0 (may be nullptr)
+  int n;
+  int* status;                  // bit 1 set if a matrix entry is not finite or a scale <= 0 (may be nullptr)
+  float* crops;                 // crop_warp_normalise: [n,3,256,192]
+  __nv_bfloat16* rows;          // frame_to_patch_rows_affine: [n*192, 768] (or [2n*192, 768] with the mirrors)
+  const float4* pos_bias;
+  float4* stream;
+  int D;
+  int num_frames;
+  FrameEntry frames[FP_MAX_FRAMES];
+};
+__device__ __forceinline__ const FrameEntry& affine_frame(const AffineParams& q, int box) {
+  int lo = 0, hi = q.num_frames;                              // the last frame whose first_box <= box
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (q.frames[mid].first_box <= box) lo = mid; else hi = mid;
+  }
+  return q.frames[lo];
+}
+// the device forms cannot return an error for a bad matrix without a sync: flag it (the arithmetic stays in bounds)
+__device__ __forceinline__ void affine_check(const AffineParams& q, int box) {
+  bool ok = true;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) ok = ok && isfinite(q.mats[6 * box + i]);
+  if (q.cs) ok = ok && q.cs[4 * box + 2] > 0.f && q.cs[4 * box + 3] > 0.f;
+  if (!ok && q.status) atomicOr(q.status, 2);
+}
+
+// f32 crops [n,3,256,192]: one CTA = one crop x 16 output rows, one thread per column
+__global__ void __launch_bounds__(PP_W) crop_warp_normalise(const __grid_constant__ AffineParams q) {
+  __shared__ int2 s_row[PP_ROWS];
+  const int crop = blockIdx.x, dx = threadIdx.x, dy0 = blockIdx.y * PP_ROWS;
+  const FrameEntry& fr = affine_frame(q, crop);
+  const AffineInv a = affine_invert(q.mats + 6 * crop);
+  if (dx < PP_ROWS) s_row[dx] = affine_row(a, dy0 + dx);
+  if (dx == 0 && blockIdx.y == 0) affine_check(q, crop);
+  const int2 col = affine_col(a, dx);
+  __syncthreads();
+  float* out = q.crops + static_cast<size_t>(crop) * 3 * PP_H * PP_W;
+  for (int r = 0; r < PP_ROWS; ++r) {
+    int v[3];
+    affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (s_row[r].x + col.x) >> 5, (s_row[r].y + col.y) >> 5, v);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[(c * PP_H + dy0 + r) * PP_W + dx] = affine_norm(c, v[c]);
+  }
+}
+
+// The same warp fused with the patch-embedding im2col: frame_to_patch_rows with a matrix per box instead of an int box.
+// Same grid ((n or 2n) x 16 CTAs, crop c >= n the mirror image of crop c - n), bf16 tile, im2col store and pos_embed + bias
+// seeding; each CTA inverts its matrix once and keeps adelta / bdelta of the 192 columns and X0 / Y0 of its 16 rows in shared
+// memory.  Rows 16 py - 2 < 0 are the conv's zero padding and are never warped.
+__global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_constant__ AffineParams q) {
+  constexpr int FP_PITCH = 208;                               // as frame_to_patch_rows
+  __shared__ uint16_t s_lut[3][256];
+  __shared__ int2 s_row[16];
+  __shared__ int2 s_col[PP_W];
+  __shared__ __align__(16) uint16_t s_tile[3 * 16 * FP_PITCH];
+  const int crop = blockIdx.x, py = blockIdx.y, tid = threadIdx.x;
+  pdl_launch_dependents();
+  pdl_wait();                                               // the previous step may still be reading patch rows / the stream
+  {
+    const int per_crop4 = 192 * q.D / 4, per_cta4 = per_crop4 / 16;
+    const float4* src = q.pos_bias + py * per_cta4;
+    float4* dst = q.stream + static_cast<size_t>(crop) * per_crop4 + py * per_cta4;
+    for (int j = tid; j < per_cta4; j += 384) dst[j] = __ldg(src + j);
+  }
+  for (int i = tid; i < 768; i += 384) s_lut[i >> 8][i & 255] = __bfloat16_as_ushort(__float2bfloat16_rn(affine_norm(i >> 8, i & 255)));
+  const bool mirror = crop >= q.n;
+  const int box = mirror ? crop - q.n : crop;
+  const FrameEntry& fr = affine_frame(q, box);
+  if (tid < PP_W + 16) {
+    const AffineInv a = affine_invert(q.mats + 6 * box);
+    if (tid < PP_W) s_col[tid] = affine_col(a, tid);
+    else {
+      const int dy = 16 * py - 2 + (tid - PP_W);
+      if (dy >= 0) s_row[tid - PP_W] = affine_row(a, dy);
+    }
+  }
+  if (tid == 0 && py == 0 && !mirror) affine_check(q, box);
+  for (int i = tid; i < 3 * 16 * 8; i += 384) {              // zero the padding columns once
+    const int row = i >> 3, e = i & 7;
+    s_tile[row * FP_PITCH + (e < 2 ? e : 192 + e)] = 0;
+  }
+  __syncthreads();
+  for (int i = tid; i < 16 * PP_W; i += 384) {
+    const int ky = i / PP_W, dx = i % PP_W;
+    const int dy = 16 * py - 2 + ky;
+    uint16_t v3[3] = {0, 0, 0};
+    if (dy >= 0) {
+      int v[3];
+      const int2 r = s_row[ky], c = s_col[dx];
+      affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) v3[ch] = s_lut[ch][v[ch]];
+    }
+    const int tx = 2 + (mirror ? PP_W - 1 - dx : dx);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s_tile[(c * 16 + ky) * FP_PITCH + tx] = v3[c];
+  }
+  __syncthreads();
+  for (int i = tid; i < 12 * 3 * 16 * 2; i += 384) {
+    const int hf = i & 1, ky = (i >> 1) & 15, c = (i >> 5) % 3, px = i / 96;
+    const uint4 v = *reinterpret_cast<const uint4*>(&s_tile[(c * 16 + ky) * FP_PITCH + 16 * px + 8 * hf]);
+    *reinterpret_cast<uint4*>(q.rows + ((static_cast<size_t>(crop) * 16 + py) * 12 + px) * 768 + c * 256 + ky * 16 + 8 * hf) = v;
+  }
+}
+
 }  // namespace vpb

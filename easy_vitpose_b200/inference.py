@@ -20,6 +20,7 @@ import torch
 from .configs import data_cfg, flip_pairs_for, model_cfg
 from .model import ViTPose
 from .top_down_eval import decode_heatmaps
+from .topdown import topdown_args
 
 __all__ = ["B200PoseBackend", "install", "frame_inference", "MEAN", "STD"]
 
@@ -94,6 +95,16 @@ class B200PoseBackend:
         float32 [n_i,K,3] (y, x, score) per frame, in that frame's pixels: inference_frame for all of them with the people of
         all frames packed into as few engine calls as max_batch allows."""
         return self.model.infer_frames_host(imgs, bboxes_list)[0]
+
+    @torch.no_grad()
+    def inference_topdown(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", padding: float = 1.25,
+                          use_udp: bool = True) -> "list[np.ndarray]":
+        """mmpose-style top-down inference: uint8 RGB frames + each frame's person boxes [n_i,4] (x, y, w, h) -> one float32
+        [n_i,K,3] (y, x, score) per frame in image pixels.  Each box becomes the reference's centre / scale and warp matrix
+        (topdown_args: datasets/COCO.py:318-337, the UDP get_warp_matrix of every config's test_cfg), the crop is
+        cv2.warpAffine's, and the keypoints are keypoints_from_heatmaps(c, s, use_udp=True)'s -- all on the device."""
+        args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
+        return self.model.infer_affine_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args])[0]
 
     @torch.no_grad()
     def inference_batch(self, imgs: "list[np.ndarray]") -> np.ndarray:

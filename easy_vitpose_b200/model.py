@@ -261,7 +261,7 @@ class ViTPose:
 
     def set_flip_test(self, flip_pairs, shift_heatmap: bool = False) -> None:
         """Flip test on every keypoint call (infer_crops, infer_host, submit_host, infer_frame, infer_frame_host,
-        submit_frame_host, infer_frames, infer_frames_host, submit_frames_host): heatmaps of each crop and of its mirror image (flipped back, pairs swapped, shifted by one pixel
+        submit_frame_host, infer_frames, infer_frames_host, submit_frames_host, infer_affine, infer_affine_host): heatmaps of each crop and of its mirror image (flipped back, pairs swapped, shifted by one pixel
         when shift_heatmap) averaged before the decode -- the test_cfg flip_test=True of the reference configs
         (configs/ViTPose_common.py:124).  Keypoints and returned heatmaps are then bit-identical to forward_flip_test
         followed by decode_heatmaps.  A call then takes at most max_batch // 2 crops.  `None` turns it off.  Synchronises
@@ -639,6 +639,116 @@ class ViTPose:
             _lib.check_value(_lib.lib().vpb_submit_frames_host(
                 self._handle, arr, len(arr), bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
                 idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+    # ---------------------------------------------------------------------------------------- affine top-down crops
+    @staticmethod
+    def _affine_args(mats, centers=None, scales=None, validate: bool = True):
+        """Per-frame matrices [n_j,2,3] | [n_j,6] and (optionally) centres / scales [n_j,2] -> (counts, mats f64 [n,6],
+        cs f32 [n,4] or None), concatenated in frame order on the device they came from.  With `validate`, host-side values
+        are checked here (a CUDA tensor is left to the engine's status word: checking it would synchronise)."""
+        if centers is not None and not (len(centers) == len(scales) == len(mats)):
+            raise ValueError(f"{len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        counts, ms, css = [], [], []
+        for j, m in enumerate(mats):
+            m = torch.as_tensor(m)
+            if not ((m.dim() == 3 and tuple(m.shape[1:]) == (2, 3)) or (m.dim() == 2 and m.shape[1] == 6)):
+                raise ValueError(f"matrices of frame {j}: [n,2,3] or [n,6] expected, got {tuple(m.shape)}")
+            m = m.reshape(-1, 6).to(torch.float64)
+            if validate and not m.is_cuda and not bool(torch.isfinite(m).all()):
+                raise ValueError(f"matrices of frame {j}: non-finite entries")
+            counts.append(m.shape[0])
+            ms.append(m)
+            if centers is None:
+                continue
+            c = torch.as_tensor(centers[j]).to(device=m.device, dtype=torch.float32).reshape(-1, 2)
+            s = torch.as_tensor(scales[j]).to(device=m.device, dtype=torch.float32).reshape(-1, 2)
+            if c.shape[0] != m.shape[0] or s.shape[0] != m.shape[0]:
+                raise ValueError(f"frame {j}: {m.shape[0]} matrices, {c.shape[0]} centres, {s.shape[0]} scales")
+            if validate and not m.is_cuda and not (bool(torch.isfinite(c).all()) and bool(torch.isfinite(s).all()) and bool((s > 0).all())):
+                raise ValueError(f"frame {j}: finite centres and scales > 0 expected")
+            css.append(torch.cat([c, s], 1))
+        if not ms:
+            return [], torch.zeros((0, 6), dtype=torch.float64), None if centers is None else torch.zeros((0, 4))
+        return counts, torch.cat(ms).contiguous(), None if centers is None else torch.cat(css).contiguous()
+
+    def preprocess_affine(self, frames, mats) -> torch.Tensor:
+        """Affine top-down crops: uint8 RGB frames [H_j,W_j,3] and per-frame matrices [n_j,2,3] (what cv2.warpAffine takes,
+        image -> 192x256 crop) -> crops f32 [n,3,256,192] on the device, boxes in frame order.  Bit-exact with
+        cv2.warpAffine(frame, M, (192, 256), INTER_LINEAR) + torchvision ToTensor / Normalize (datasets/COCO.py:289-302)."""
+        self._ensure()
+        if len(frames) != len(mats):
+            raise ValueError(f"{len(frames)} frames but {len(mats)} matrix arrays")
+        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        dev = torch.device("cuda", self._device)
+        counts, M, _ = self._affine_args(mats)
+        M = M.to(dev)
+        n = M.shape[0]
+        crops = torch.empty((n, 3, IMG_H, IMG_W), dtype=torch.float32, device=dev)
+        table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, max(n, 1)):       # only the 64-frame table limits a call
+                arr = _frame_array(table, chunk)
+                _lib.check(_lib.lib().vpb_preprocess_affine(arr, len(arr), C.c_void_p(M[s:].data_ptr()),
+                                                            C.c_void_p(crops[s:].data_ptr()), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        return crops
+
+    def infer_affine(self, frames, mats, centers, scales, check: bool = False):
+        """The top-down path of mmpose-style evaluation on the device: frames [H_j,W_j,3] uint8 (CUDA), per-frame matrices
+        [n_j,2,3], centres [n_j,2] and scales [n_j,2] in PIXELS (topdown_args gives all three) -> (list of kpts f32 [n_j,K,3]
+        (y, x, score), list of idx i32 [n_j,K]): the warp fused into the patch gather, the forward and
+        keypoints_from_heatmaps(c, s, use_udp=True), in the coordinates transform_preds gives (image pixels for unrotated
+        matrices).  Chunked like infer_frames; honours the flip test.  Host-side matrices / scales are checked here; CUDA
+        ones set bit 1 of the status word, which `check=True` turns into a ValueError."""
+        self._ensure()
+        if not (len(frames) == len(mats) == len(centers) == len(scales)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        dev = torch.device("cuda", self._device)
+        counts, M, CS = self._affine_args(mats, centers, scales)
+        M, CS = M.to(dev), CS.to(dev)
+        n = M.shape[0]
+        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
+        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
+        table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
+        s = 0
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            arr = _frame_array(table, chunk)
+            self._call_on_stream(frames + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine(
+                self._handle, arr, len(arr), C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 2:
+            raise ValueError("a matrix entry is not finite or a scale is <= 0")
+        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+
+    def infer_affine_host(self, frames, mats, centers, scales):
+        """HOST form of infer_affine (vpb_infer_affine_host, synchronous): numpy frames and per-frame matrices / centres /
+        scales -> (list of kpts [n_j,K,3], list of idx [n_j,K]) numpy arrays.  A non-finite matrix entry or a scale <= 0
+        raises ValueError naming the box."""
+        self._ensure()
+        if not (len(frames) == len(mats) == len(centers) == len(scales)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
+        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
+        M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
+        n = M.shape[0]
+        kp = np.empty((n, self.num_keypoints, 3), np.float32)
+        idx = np.empty((n, self.num_keypoints), np.int32)
+        table = [(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames]
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, self.batch_limit):
+                arr = _frame_array(table, chunk)
+                _lib.check_value(_lib.lib().vpb_infer_affine_host(
+                    self._handle, arr, len(arr), M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
+                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        if not counts:
+            return [], []
+        split = np.cumsum(counts)[:-1]
+        return np.split(kp, split), np.split(idx, split)
 
     def wait_host(self, slot: int) -> None:
         _lib.check(_lib.lib().vpb_wait_host(self._handle, int(slot)))

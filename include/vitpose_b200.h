@@ -159,8 +159,8 @@ int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int3
                     int32_t n, float* d_kpts, int32_t* d_idx, void* stream);
 /* Status of the device-side frame calls since the last query: bit 0 = some box was empty after padding and clipping
  * (the reference raises there: ZeroDivisionError in pad_image / cv2.resize, easy_ViTPose/inference.py:259-265; the
- * device path cannot raise without a sync and decodes such a box from a black crop).  Synchronises the device, clears
- * the word. */
+ * device path cannot raise without a sync and decodes such a box from a black crop); bit 1 = vpb_infer_affine got a
+ * non-finite matrix entry or a scale <= 0.  Synchronises the device, clears the word. */
 int vpb_frame_status(vpb_engine* e, int32_t* h_status);
 /* Same with HOST buffers (H2D of the packed uint8 frame + 16 B per box, D2H of the keypoints, stream sync); empty boxes
  * return VPB_ERR_ARG where the reference raises.  The pipelined form shares its slots and vpb_wait_host with vpb_submit_host. */
@@ -196,6 +196,33 @@ int vpb_infer_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_
 int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
                            float* h_kpts, int32_t* h_idx, int32_t slot);     /* completes with vpb_wait_host(slot) */
 
+/* ---- affine top-down crops: the mmpose / HRNet data path of easy_ViTPose/datasets/COCO.py:288-302 (the crop the published
+ * COCO AP numbers were measured with) for the people of up to VPB_MAX_FRAMES frames per call.  Frames and their boxes are given
+ * as for vpb_infer_frames (vpb_frame.num_boxes = how many of the next matrices belong to that frame).  Per box:
+ *   mats f64 [n,6] = the 2x3 matrix handed to cv2.warpAffine (image -> 192x256 crop), e.g. the UDP matrix
+ *   get_warp_matrix(rot, 2c, image_size - 1, s * 200) (vit_utils/post_processing/post_transforms.py:312-340) or the HRNet
+ *   get_affine_transform (vit_utils/transform.py:46-75);
+ *   cv2.warpAffine(frame, M, (192, 256), INTER_LINEAR) with the constant 0 border, then torchvision ToTensor + Normalize in
+ *   float32 (COCO.py:120-123, 300-302): bit-exact with cv2 4.13 and torchvision, singular matrices included.
+ * vpb_preprocess_affine (engine-free, like vpb_preprocess): d_crops f32 [n,3,256,192]. */
+int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, float* d_crops, void* stream);
+/* The fused gather (the crops are never stored), the engine's forward (cached CUDA graph per batch size) and
+ * keypoints_from_heatmaps(heatmaps, c, s * 200, use_udp=True) = vpb_decode_modes mode 4 with d_cs f32 [n,4] (cx, cy, sx, sy) in
+ * pixels, as keypoints_from_heatmaps takes them (top_down_eval.py:576-579, one reference call on the whole call's array).
+ * d_kpts f32 [n,K,3] (y, x, score), d_idx i32 [n,K] or NULL.  The keypoints are in the coordinates transform_preds gives:
+ * image pixels for an unrotated matrix.  The reference's decode has no rotation, and neither has this one: for a rotated
+ * matrix they are the reference's values, not the rotated-back positions.  Bit-identical to vpb_preprocess_affine ->
+ * vpb_forward -> vpb_decode_modes(mode 4); flip test (vpb_set_flip_test) applies as to the frame calls.
+ * VPB_ERR_ARG: n above the batch limit, more than VPB_MAX_FRAMES frames with boxes, a negative num_boxes, a frame with boxes
+ * whose data is NULL, height or width < 1 or pitch below 3 * width.  A non-finite matrix entry or a scale <= 0 cannot be
+ * returned by the device form without a synchronisation: it sets bit 1 of the status word (vpb_frame_status) instead. */
+int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, const float* d_cs,
+                     float* d_kpts, int32_t* d_idx, void* stream);
+/* HOST frames, matrices and centre / scale, staged on slot 0 like vpb_infer_frames_host (synchronous).  A non-finite
+ * matrix or centre entry or a scale <= 0 returns VPB_ERR_ARG naming the box. */
+int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* h_mats, const float* h_cs,
+                          float* h_kpts, int32_t* h_idx, void* stream);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* Options (all keep the results bit-identical unless noted): "stop_after", "profile", "pdl", "graph", "ln_fused",
@@ -212,7 +239,8 @@ int vpb_set_option(vpb_engine* e, const char* name, int32_t value);
  * h_perm i32 [k] (HOST) = the keypoint permutation the flip pairs induce (as for vpb_flip_back); k must equal the engine's K
  * and every entry lie in [0,K), else VPB_ERR_ARG.  h_perm = NULL turns flip test off (the default).
  * While it is on, vpb_infer, vpb_infer_host, vpb_submit_host, vpb_infer_frame, vpb_infer_frame_host, vpb_submit_frame_host and
- * the multi-frame calls (vpb_infer_frames, vpb_infer_frames_host, vpb_submit_frames_host) run each crop and its mirror image as one batch of 2 * batch crops (the mirror images are gathered on the fly, never
+ * the multi-frame calls (vpb_infer_frames, vpb_infer_frames_host, vpb_submit_frames_host) and the affine calls
+ * (vpb_infer_affine, vpb_infer_affine_host) run each crop and its mirror image as one batch of 2 * batch crops (the mirror images are gathered on the fly, never
  * stored), average the maps and decode the averaged maps (wrap_batch = 0); d_heatmaps, when given, receives the averaged
  * maps.  batch must then be <= max_batch / 2.  vpb_forward, vpb_forward_features, vpb_head, vpb_decode* and vpb_flip_back
  * are unaffected.  SYNCHRONOUS: waits for the engine's pending work (which keeps the previous setting), and drops the
