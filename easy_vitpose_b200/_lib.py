@@ -27,6 +27,15 @@ class VpbFrame(C.Structure):
                 ("num_boxes", C.c_int32)]
 
 
+MAX_HEADS = 8                                         # VPB_MAX_HEADS: keypoint heads of one engine
+MAX_SEGMENTS = 64                                     # VPB_MAX_SEGMENTS: runs of one head per multi-head call
+
+
+class VpbSegment(C.Structure):
+    """vpb_segment: `count` consecutive crops of head `head` (vpb_infer_heads)."""
+    _fields_ = [("head", C.c_int32), ("count", C.c_int32)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "vpb_last_error": (C.c_char_p, []),
@@ -61,9 +70,18 @@ EXPORTS = {
                                    C.c_void_p]),
     "vpb_infer_affine_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]),
+    "vpb_create_heads": (C.c_int, [C.POINTER(VpbConfig), C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+    "vpb_infer_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(VpbSegment), C.c_int32, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
+    "vpb_infer_frames_heads": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
+    "vpb_infer_frames_heads_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]),
     "vpb_host_alloc": (C.c_void_p, [C.c_int64]),
     "vpb_host_free": (None, [C.c_void_p]),
     "vpb_kernel_launches": (C.c_int, [C.c_void_p, C.c_int32]),
+    "vpb_cached_graphs": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "vpb_device_bytes": (C.c_int64, [C.c_void_p]),
     "vpb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int32]),
     "vpb_set_flip_test": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]),
     "vpb_profile_classes": (C.c_int, []),

@@ -14,6 +14,10 @@ _DROP_PATH = {"small": 0.1, "base": 0.3, "large": 0.5, "huge": 0.55}
 # dataset -> number of keypoints (configs/ViTPose_<dataset>.py: channel_cfg['num_output_channels'])
 DATASET_KEYPOINTS = {"coco": 17, "coco_25": 25, "wholebody": 133, "mpii": 16, "aic": 14, "ap10k": 17, "apt36k": 17, "custom": 18}
 
+# The heads of a ViTPose+ checkpoint in model_split.py's order (:71-74): keypoint_head is COCO, associate_keypoint_heads.{i}
+# the others; head j uses fc2 expert j.
+VITPOSE_PLUS_HEADS = (("coco", 17), ("aic", 14), ("mpii", 16), ("ap10k", 17), ("apt36k", 17), ("wholebody", 133))
+
 data_cfg = dict(image_size=[192, 256], heatmap_size=[48, 64])   # ViTPose_common.py:29-31
 
 # left/right keypoint pairs for the flip test: eye, ear, shoulder, elbow, wrist, hip, knee, ankle (datasets/COCO.py:114).

@@ -75,6 +75,9 @@ struct DecodeParams {
   const int* offs_yx;      // [N,2] integer (y, x) added to the keypoints: crop -> frame coordinates (inference.py:270); may be nullptr
   int n, k;
   int wrap_batch;          // sentinel quirk: 0 = previous map wraps inside the crop, 1 = inside the whole call
+  // maps / keypoint rows between consecutive crops in heatmaps, kpts and idx (0 = k): a multi-head call decodes each
+  // segment's K_head maps out of crops laid out K_max apart (wrap_batch 0 only)
+  int kstride = 0;
   // general transform_preds (post_transforms.py:150-194) for callers other than VitInference.postprocess: per crop
   // (centre_x, centre_y, scale_x, scale_y) either as float32 (numpy keeps the whole expression in float32) or as float64
   // (int64 / float64 arrays promote it to float64); both null = the VitInference form above (scale = org, centre = org // 2)
@@ -113,11 +116,12 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_heatmaps(const Decod
   const int R = GENERIC ? p.taps.radius : 5, KS = 2 * R + 1;
   auto tap = [&](int d) { return GENERIC ? p.taps.t[d] : c_gauss11[5 - d]; };
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = blockIdx.x * DECODE_WARPS + wib;            // map index n*K + k
+  const int g0 = blockIdx.x * DECODE_WARPS + wib;           // map index n*K + k
   const int total = p.n * p.k;
   pdl_launch_dependents();
   pdl_wait();
-  if (g >= total) return;
+  if (g0 >= total) return;
+  const int g = p.kstride ? (g0 / p.k) * p.kstride + g0 % p.k : g0;   // the map's slot in heatmaps / kpts / idx
   const float* hm = p.heatmaps + static_cast<size_t>(g) * HM_PIX;
 
   // ---- first-index argmax over 3072 values.  The scan is branch-free so that the loads can run ahead of it (ptxas keeps a
@@ -170,8 +174,8 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_heatmaps(const Decod
   } else {
     // (-1,-1): four reads land on this map's top-left pad corner (= l(0,0)); the three "minus" reads
     // underflow into the previous map's padded slab: l_prev(W-1,H-1) twice and l_prev(0,H-1).
-    const int n_i = g / p.k, k_i = g % p.k;
-    const int prev = p.wrap_batch ? (g + total - 1) % total : n_i * p.k + (k_i + p.k - 1) % p.k;
+    const int n_i = g0 / p.k, k_i = g0 % p.k;
+    const int prev = p.wrap_batch ? (g0 + total - 1) % total : n_i * (p.kstride ? p.kstride : p.k) + (k_i + p.k - 1) % p.k;
     const float* hp = p.heatmaps + static_cast<size_t>(prev) * HM_PIX;
 #pragma unroll
     for (int i = 0; i < 4; ++i) { pmap[i] = hm; ptx[i] = 0; pty[i] = 0; }
@@ -235,7 +239,7 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_heatmaps(const Decod
     const double offy = (a * static_cast<double>(dy) - b * static_cast<double>(dx)) / det;
     const float xr = static_cast<float>(static_cast<double>(x) - offx);
     const float yr = static_cast<float>(static_cast<double>(y) - offy);
-    const int n_i = g / p.k;
+    const int n_i = g0 / p.k;
     float X, Y;
     if (p.cs32 != nullptr || p.cs64 != nullptr) {
       transform_cs(xr, yr, n_i, p.cs32, p.cs64, true, X, Y);

@@ -21,6 +21,7 @@
 #include "attention.cuh"
 #include "chain.cuh"
 #include "decode.cuh"
+#include "expert_gemm.cuh"
 #include "gemm.cuh"
 #include "pointwise.cuh"
 #include "preprocess.cuh"
@@ -136,6 +137,7 @@ struct DeviceState {
   int sms = 0;                      // 0 = not checked yet
   bool attn_attr = false;
   unsigned gemm_attr = 0;           // bit per gemm instantiation (see gemm_slot)
+  unsigned expert_attr = 0;         // bit per expert GEMM tile width (expert_launch)
 };
 static DeviceState g_devs[kMaxDevices];
 static DeviceState* cur_dev() {
@@ -176,7 +178,9 @@ static int gemm_launch_t(const CUtensorMap& ta, const CUtensorMap& tw, const CUt
 static int gemm_launch(int bn, int epi, const CUtensorMap& ta, const CUtensorMap& tw, const CUtensorMap& tout, const GemmParams& p,
                        cudaStream_t st) {
   if (p.K % GEMM_BK != 0 || p.K <= 0) return fail(VPB_ERR_ARG, "gemm: K=%d must be a positive multiple of 64", p.K);
-  if (epi_uses_tma(epi) && (p.N % 64 != 0 || p.bias == nullptr)) return fail(VPB_ERR_ARG, "gemm: TMA epilogue wants N %% 64 == 0 and a bias");
+  // the fp32 epilogue stores 32 columns per TMA box (the shared columns of a ViTPose+ fc2 are D - P wide, P % 32 == 0)
+  if (epi_uses_tma(epi) && (p.N % (epi == EPI_F32_ADD ? 32 : 64) != 0 || p.bias == nullptr))
+    return fail(VPB_ERR_ARG, "gemm: TMA epilogue wants N %% 64 == 0 (N %% 32 == 0 for the fp32 one) and a bias");
 #define VPB_CASE(BN_, EPI_) \
   if (bn == BN_ && epi == EPI_) return gemm_launch_t<BN_, EPI_>(ta, tw, tout, p, st);
   VPB_CASE(256, EPI_BF16) VPB_CASE(192, EPI_BF16) VPB_CASE(128, EPI_BF16)
@@ -187,6 +191,42 @@ static int gemm_launch(int bn, int epi, const CUtensorMap& ta, const CUtensorMap
   VPB_CASE(32, EPI_F32_NCHW) VPB_CASE(144, EPI_F32_NCHW)
 #undef VPB_CASE
   return fail(VPB_ERR_ARG, "gemm: no kernel for BN=%d epilogue=%d", bn, epi);
+}
+
+// Grouped expert GEMM (expert_gemm.cuh).  Tile width: the widest of kExpertWidths that divides P, so no tile reads columns of
+// the next expert; `tw` carries W boxes of that many rows.
+constexpr int kExpertWidths[5] = {192, 128, 96, 64, 32};
+static int expert_width(int P) {
+  for (int w : kExpertWidths)
+    if (P % w == 0) return w;
+  return 0;
+}
+template <int BN>
+static int expert_launch_t(const CUtensorMap& ta, const CUtensorMap& tw, const ExpertParams& p, cudaStream_t st) {
+  using Cfg = TileCfg<BN, false>;
+  auto kern = gemm_expert_segments<BN>;
+  DeviceState* ds = cur_dev();
+  if (ds->sms == 0) return fail(VPB_ERR_STATE, "expert gemm: device not initialised (device_check)");
+  constexpr unsigned slot = 1u << (BN / 32);
+  if (!(ds->expert_attr & slot)) {
+    CU_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    ds->expert_attr |= slot;
+  }
+  const int grid = p.num_tiles < ds->sms ? p.num_tiles : ds->sms;
+  CU_TRY(launch_k(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, st, ta, tw, p));
+  return VPB_OK;
+}
+static int expert_launch(int bn, const CUtensorMap& ta, const CUtensorMap& tw, const ExpertParams& p, cudaStream_t st) {
+  if (p.K % GEMM_BK != 0 || p.K <= 0 || p.num_segs < 1 || p.num_segs > EXPERT_MAX_SEGMENTS || bn <= 0 || p.P % bn != 0)
+    return fail(VPB_ERR_ARG, "expert gemm: K=%d P=%d BN=%d segments=%d", p.K, p.P, bn, p.num_segs);
+  switch (bn) {
+    case 192: return expert_launch_t<192>(ta, tw, p, st);
+    case 128: return expert_launch_t<128>(ta, tw, p, st);
+    case 96: return expert_launch_t<96>(ta, tw, p, st);
+    case 64: return expert_launch_t<64>(ta, tw, p, st);
+    case 32: return expert_launch_t<32>(ta, tw, p, st);
+  }
+  return fail(VPB_ERR_ARG, "expert gemm: no kernel for BN=%d", bn);
 }
 
 // `device` must be the current device (callers cudaSetDevice / cudaGetDevice first)
@@ -347,11 +387,27 @@ static int make_tile_maps(LinearW& L, const void* w, int n_pad, int k) {
 }
 struct BlockW {
   float *ln1_g, *ln1_b, *ln2_g, *ln2_b;
-  LinearW qkv, proj, fc1, fc2;
+  // fc2 of an engine with experts (P > 0): W and bias are stacked [shared (D-P rows); expert 0 (P); ...; expert H-1], so the
+  // first D rows are head 0's whole fc2 and `fc2` is exactly the single-head linear.  fc2s = the shared rows alone (maps of
+  // D-P rows: TMA zero-fills the rest of a tile), m_exp = the whole stack in boxes of expert_bn rows.
+  LinearW qkv, proj, fc1, fc2, fc2s;
+  CUtensorMap m_exp;
 };
+// One keypoint head: TopdownHeatmapSimpleHead weights (keypoint_head.* for head 0, associate_keypoint_heads.{j-1}.* for head j)
+struct HeadW {
+  int K = 0, n_final = 0;           // n_final = padded channel count of the 1x1 conv GEMM
+  LinearW dc1, dc2, fin;            // dc*: the 4 phase matrices stacked [4*256, 4*Cin]
+  CUtensorMap m_fin_w;              // final 1x1 conv W: boxes of n_final rows (one column tile)
+};
+// A run of consecutive crops of one head in a multi-head call
+struct Segment { int head, count; };
+static bool operator==(const Segment& a, const Segment& b) { return a.head == b.head && a.count == b.count; }
 struct vpb_engine {
   vpb_config cfg;
-  int D, depth, heads, K, maxB, n_final;   // n_final = padded channel count of the 1x1 conv GEMM
+  int D, depth, heads, K, maxB;    // K = head 0's keypoints: what the single-head calls return per crop
+  // keypoint heads (vpb_create_heads; vpb_create: one head, P = 0) and the expert width P of each block's fc2
+  int num_kheads = 1, P = 0, Kmax = 0, expert_bn = 0;
+  std::vector<HeadW> hw;
   bool finalized = false;
   int stop_after = 0;
   Profiler prof;
@@ -362,6 +418,10 @@ struct vpb_engine {
   // affine = the graph decodes with centre / scale (vpb_infer_affine) instead of canvas sizes / offsets
   struct GraphEntry { int batch; int seen; cudaGraphExec_t exec; bool affine; };
   std::vector<GraphEntry> graphs;
+  // multi-head calls: one graph per segment list (heads and counts), at most kMaxMixedGraphs, least recently used out first
+  struct MixedGraph { std::vector<Segment> segs; cudaGraphExec_t exec; unsigned long long used; };
+  std::vector<MixedGraph> mixed_graphs;
+  unsigned long long mixed_clock = 0;
   bool use_graph = true;
   // L2 residency: the fp32 token stream x (37.7 MB at B=64) is read-modify-written by every residual GEMM and read by every
   // LayerNorm, but the per-layer working set (~220 MB) would evict it from the 50 MB L2 in between; an access-policy window
@@ -389,12 +449,12 @@ struct vpb_engine {
   int32_t* flip_perm = nullptr;
   std::map<std::string, std::pair<float*, int64_t>> staged;   // fp32 state_dict tensors on device until finalize
   std::vector<void*> allocs;
+  size_t alloc_bytes = 0;          // what `allocs` holds: packed weights + workspace (vpb_device_bytes)
   // packed weights
   LinearW patch;            // bias unused (folded into pos_bias)
   float* pos_bias = nullptr;   // [192, D]
   std::vector<BlockW> blocks;
   float *lnf_g = nullptr, *lnf_b = nullptr;
-  LinearW dc1, dc2, fin;            // dc*: the 4 phase matrices stacked [4*256, 4*Cin]
   // workspace
   __nv_bfloat16 *patch_rows, *xn, *qkv, *attn, *hid, *d1, *d2;
   float *x, *heat;
@@ -437,7 +497,7 @@ struct vpb_engine {
   CUtensorMap m_patch_rows, m_xn, m_attn, m_hid, m_d2, m_qkv_att, m_qkv_att_tail;   // A operands / attention boxes
   CUtensorMap m_feat_nhwc, m_d1_nhwc;                                 // implicit-GEMM deconv inputs (4-D)
   CUtensorMap o_qkv, o_hid, o_x;                                                             // TMA-epilogue outputs
-  CUtensorMap m_fin_w;                          // final 1x1 conv W: boxes of n_final rows (one column tile)
+  CUtensorMap o_xs;                             // x bounded to the shared columns [0, D-P) (multi-head fc2)
 };
 
 template <typename T>
@@ -445,12 +505,17 @@ static int dev_alloc(vpb_engine* e, T** p, size_t count) {
   void* q = nullptr;
   CU_TRY(cudaMalloc(&q, count * sizeof(T) + 256));
   e->allocs.push_back(q);
+  e->alloc_bytes += count * sizeof(T) + 256;
   *p = reinterpret_cast<T*>(q);
   return VPB_OK;
 }
 
+// ViTPose+ key names: head 0 is keypoint_head, head j >= 1 is associate_keypoint_heads.{j-1} (model_split.py:97-99)
+static std::string head_prefix(int j) {
+  return j == 0 ? std::string("keypoint_head.") : "associate_keypoint_heads." + std::to_string(j - 1) + ".";
+}
 static std::vector<std::pair<std::string, int64_t>> expected_keys(const vpb_engine* e) {
-  const int64_t D = e->D, K = e->K;
+  const int64_t D = e->D, P = e->P;
   std::vector<std::pair<std::string, int64_t>> v;
   v.push_back({"backbone.pos_embed", 193 * D});
   v.push_back({"backbone.patch_embed.proj.weight", D * 768});
@@ -462,18 +527,25 @@ static std::vector<std::pair<std::string, int64_t>> expected_keys(const vpb_engi
     v.push_back({p + "attn.proj.weight", D * D}); v.push_back({p + "attn.proj.bias", D});
     v.push_back({p + "norm2.weight", D}); v.push_back({p + "norm2.bias", D});
     v.push_back({p + "mlp.fc1.weight", 4 * D * D}); v.push_back({p + "mlp.fc1.bias", 4 * D});
-    v.push_back({p + "mlp.fc2.weight", 4 * D * D}); v.push_back({p + "mlp.fc2.bias", D});
+    v.push_back({p + "mlp.fc2.weight", 4 * D * (D - P)}); v.push_back({p + "mlp.fc2.bias", D - P});
+    for (int j = 0; P > 0 && j < e->num_kheads; ++j) {         // ViTPose+ experts: the last P output rows of head j's fc2
+      v.push_back({p + "mlp.experts." + std::to_string(j) + ".weight", 4 * D * P});
+      v.push_back({p + "mlp.experts." + std::to_string(j) + ".bias", P});
+    }
   }
   v.push_back({"backbone.last_norm.weight", D}); v.push_back({"backbone.last_norm.bias", D});
-  int64_t cin = D;
-  for (int li : {0, 3}) {
-    const std::string p = "keypoint_head.deconv_layers.";
-    v.push_back({p + std::to_string(li) + ".weight", cin * 256 * 16});
-    for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) v.push_back({p + std::to_string(li + 1) + s, 256});
-    cin = 256;
+  for (int j = 0; j < e->num_kheads; ++j) {
+    const std::string hp = head_prefix(j);
+    int64_t cin = D;
+    for (int li : {0, 3}) {
+      const std::string p = hp + "deconv_layers.";
+      v.push_back({p + std::to_string(li) + ".weight", cin * 256 * 16});
+      for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) v.push_back({p + std::to_string(li + 1) + s, 256});
+      cin = 256;
+    }
+    v.push_back({hp + "final_layer.weight", static_cast<int64_t>(e->hw[j].K) * 256});
+    v.push_back({hp + "final_layer.bias", e->hw[j].K});
   }
-  v.push_back({"keypoint_head.final_layer.weight", K * 256});
-  v.push_back({"keypoint_head.final_layer.bias", K});
   return v;
 }
 
@@ -495,7 +567,10 @@ extern "C" int vpb_create(const vpb_config* cfg, vpb_engine** out) {
   vpb_engine* e = new vpb_engine();
   e->cfg = *cfg;
   e->D = cfg->embed_dim; e->depth = cfg->depth; e->heads = cfg->num_heads; e->K = cfg->num_keypoints; e->maxB = cfg->max_batch;
-  e->n_final = e->K <= 32 ? 32 : 144;
+  e->Kmax = e->K;
+  e->hw.resize(1);
+  e->hw[0].K = e->K;
+  e->hw[0].n_final = e->K <= 32 ? 32 : 144;
   e->chain_bn = 128;     // D, 3D and 4D are multiples of it for every ViT; 128 accumulator columns leave the LayerNorm warps room
   {
     const char* env = getenv("VPB_CHAIN");
@@ -516,6 +591,30 @@ extern "C" int vpb_create(const vpb_config* cfg, vpb_engine** out) {
   return VPB_OK;
 }
 
+extern "C" int vpb_create_heads(const vpb_config* cfg, int32_t num_heads, const int32_t* h_keypoints, int32_t expert_rows, vpb_engine** out) {
+  if (!cfg || !h_keypoints || !out) return fail(VPB_ERR_ARG, "vpb_create_heads: null argument");
+  *out = nullptr;
+  if (num_heads < 1 || num_heads > VPB_MAX_HEADS) return fail(VPB_ERR_ARG, "vpb_create_heads: %d heads (1..%d)", num_heads, VPB_MAX_HEADS);
+  for (int j = 0; j < num_heads; ++j)
+    if (h_keypoints[j] < 1 || h_keypoints[j] > 144) return fail(VPB_ERR_ARG, "vpb_create_heads: head %d has %d keypoints (1..144)", j, h_keypoints[j]);
+  if (expert_rows != 0 && (expert_rows < 0 || expert_rows >= cfg->embed_dim || expert_rows % 32 != 0))
+    return fail(VPB_ERR_ARG, "vpb_create_heads: expert_rows=%d must be 0 or a multiple of 32 below embed_dim=%d", expert_rows, cfg->embed_dim);
+  vpb_config c = *cfg;
+  c.num_keypoints = h_keypoints[0];
+  VPB_TRY(vpb_create(&c, out));
+  vpb_engine* e = *out;
+  e->num_kheads = num_heads;
+  e->P = expert_rows;
+  e->expert_bn = expert_width(expert_rows);
+  e->hw.resize(num_heads);
+  for (int j = 0; j < num_heads; ++j) {
+    e->hw[j].K = h_keypoints[j];
+    e->hw[j].n_final = h_keypoints[j] <= 32 ? 32 : 144;
+    e->Kmax = std::max(e->Kmax, static_cast<int>(h_keypoints[j]));
+  }
+  return VPB_OK;
+}
+
 extern "C" void vpb_destroy(vpb_engine* e) {
   if (!e) return;
   int prev = -1;
@@ -526,6 +625,7 @@ extern "C" void vpb_destroy(vpb_engine* e) {
   for (auto& kv : e->staged) cudaFree(kv.second.first);
   for (void* p : e->allocs) cudaFree(p);
   for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+  for (auto& g : e->mixed_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (int s = 0; s < 2; ++s) {
     if (e->ev_h2d[s]) cudaEventDestroy(e->ev_h2d[s]);
     if (e->ev_done[s]) cudaEventDestroy(e->ev_done[s]);
@@ -579,6 +679,34 @@ static int pack_linear(vpb_engine* e, LinearW& L, const std::string& wkey, const
   return VPB_OK;
 }
 
+// ViTPose+ fc2 with experts: W / bias stacked [shared; expert 0; ...; expert H-1] (see BlockW).  The first D rows are the fc2
+// that model_split.py gives head 0 (torch.cat([fc2, experts.0]), :56), packed exactly as pack_linear packs it.
+static int pack_fc2_experts(vpb_engine* e, BlockW& b, const std::string& p) {
+  const int D = e->D, P = e->P, K = 4 * D, S = D - P, rows = S + e->num_kheads * P;
+  LinearW& L = b.fc2;
+  L.n = D; L.k = K;
+  VPB_TRY(dev_alloc(e, &L.w, static_cast<size_t>(rows) * K));
+  VPB_TRY(dev_alloc(e, &L.b, rows));
+  auto put = [&](const std::string& key, int row0, int n) -> int {
+    const long long ne = static_cast<long long>(n) * K;
+    pack_linear_bf16<<<cdiv(ne, 256), 256>>>(e->staged[key + ".weight"].first, L.w + static_cast<size_t>(row0) * K, ne, K, 0, 1.f);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpy(L.b + row0, e->staged[key + ".bias"].first, n * sizeof(float), cudaMemcpyDeviceToDevice));
+    return VPB_OK;
+  };
+  VPB_TRY(put(p + "mlp.fc2", 0, S));
+  for (int j = 0; j < e->num_kheads; ++j) VPB_TRY(put(p + "mlp.experts." + std::to_string(j), S + j * P, P));
+  VPB_TRY(make_tile_maps(L, L.w, D, K));
+  VPB_TRY(make_map(&L.map_c, L.w, D, K, K, e->chain_bn));
+  LinearW& Ls = b.fc2s;
+  Ls.w = L.w; Ls.b = L.b; Ls.n = S; Ls.k = K;
+  for (int i = 0; i < 3; ++i) {
+    Ls.has[i] = (cdiv(S, 128) * 128) % kTileWidths[i] == 0;
+    if (Ls.has[i]) VPB_TRY(make_map(&Ls.tmap[i], L.w, S, K, K, kTileWidths[i]));
+  }
+  return make_map(&b.m_exp, L.w, rows, K, K, e->expert_bn);
+}
+
 static int copy_vec(vpb_engine* e, float** dst, const std::string& key) {
   auto& s = e->staged[key];
   VPB_TRY(dev_alloc(e, dst, s.second));
@@ -609,31 +737,36 @@ extern "C" int vpb_finalize(vpb_engine* e) {
     VPB_TRY(pack_linear(e, b.qkv, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, 128, D, qscale));
     VPB_TRY(pack_linear(e, b.proj, p + "attn.proj.weight", p + "attn.proj.bias", D, D, 128, 0, 1.f));
     VPB_TRY(pack_linear(e, b.fc1, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, 128, 0, 1.f));
-    VPB_TRY(pack_linear(e, b.fc2, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 128, 0, 1.f));
+    if (e->P == 0) VPB_TRY(pack_linear(e, b.fc2, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 128, 0, 1.f));
+    else VPB_TRY(pack_fc2_experts(e, b, p));
   }
   VPB_TRY(copy_vec(e, &e->lnf_g, "backbone.last_norm.weight"));
   VPB_TRY(copy_vec(e, &e->lnf_b, "backbone.last_norm.bias"));
-  // deconv layers: 4 phase matrices [256, 4*Cin] each, BN folded (eps 1e-5 = nn.BatchNorm2d default)
-  int cin = D;
-  for (int layer = 0; layer < 2; ++layer) {
-    LinearW& dc = layer == 0 ? e->dc1 : e->dc2;
-    const std::string wk = "keypoint_head.deconv_layers." + std::to_string(layer * 3) + ".weight";
-    const std::string bnp = "keypoint_head.deconv_layers." + std::to_string(layer * 3 + 1) + ".";
-    VPB_TRY(dev_alloc(e, &dc.w, static_cast<size_t>(4) * 256 * 4 * cin));
-    VPB_TRY(dev_alloc(e, &dc.b, 256));
-    const long long tot = 4LL * 256 * 4 * cin;
-    pack_deconv<<<cdiv(tot, 256), 256>>>(e->staged[wk].first, e->staged[bnp + "weight"].first, e->staged[bnp + "bias"].first,
-                                         e->staged[bnp + "running_mean"].first, e->staged[bnp + "running_var"].first, dc.w, dc.b,
-                                         cin, 256, 1e-5f);
-    CU_TRY(cudaGetLastError());
-    dc.n = 256; dc.k = 4 * cin;
-    VPB_TRY(make_tile_maps(dc, dc.w, 4 * 256, 4 * cin));
-    cin = 256;
-  }
-  {  // final 1x1 conv: [K,256] zero-padded to the N tile
-    LinearW& L = e->fin;
-    VPB_TRY(pack_linear(e, L, "keypoint_head.final_layer.weight", "keypoint_head.final_layer.bias", e->K, 256, e->n_final, 0, 1.f));
-    VPB_TRY(make_map(&e->m_fin_w, L.w, e->n_final, 256, 256, e->n_final));
+  // per head: deconv layers (4 phase matrices [256, 4*Cin] each, BN folded: eps 1e-5 = nn.BatchNorm2d default), final 1x1 conv
+  for (int j = 0; j < e->num_kheads; ++j) {
+    HeadW& h = e->hw[j];
+    const std::string hp = head_prefix(j);
+    int cin = D;
+    for (int layer = 0; layer < 2; ++layer) {
+      LinearW& dc = layer == 0 ? h.dc1 : h.dc2;
+      const std::string wk = hp + "deconv_layers." + std::to_string(layer * 3) + ".weight";
+      const std::string bnp = hp + "deconv_layers." + std::to_string(layer * 3 + 1) + ".";
+      VPB_TRY(dev_alloc(e, &dc.w, static_cast<size_t>(4) * 256 * 4 * cin));
+      VPB_TRY(dev_alloc(e, &dc.b, 256));
+      const long long tot = 4LL * 256 * 4 * cin;
+      pack_deconv<<<cdiv(tot, 256), 256>>>(e->staged[wk].first, e->staged[bnp + "weight"].first, e->staged[bnp + "bias"].first,
+                                           e->staged[bnp + "running_mean"].first, e->staged[bnp + "running_var"].first, dc.w, dc.b,
+                                           cin, 256, 1e-5f);
+      CU_TRY(cudaGetLastError());
+      dc.n = 256; dc.k = 4 * cin;
+      VPB_TRY(make_tile_maps(dc, dc.w, 4 * 256, 4 * cin));
+      cin = 256;
+    }
+    {  // final 1x1 conv: [K,256] zero-padded to the N tile
+      LinearW& L = h.fin;
+      VPB_TRY(pack_linear(e, L, hp + "final_layer.weight", hp + "final_layer.bias", h.K, 256, h.n_final, 0, 1.f));
+      VPB_TRY(make_map(&h.m_fin_w, L.w, h.n_final, 256, 256, h.n_final));
+    }
   }
   // ---- workspace for max_batch crops
   const size_t B = e->maxB, M = B * 192;
@@ -645,10 +778,10 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(dev_alloc(e, &e->hid, M * 4 * D));
   VPB_TRY(dev_alloc(e, &e->d1, B * 768 * 256));
   VPB_TRY(dev_alloc(e, &e->d2, B * 3072 * 256));
-  VPB_TRY(dev_alloc(e, &e->heat, B * e->K * 3072));
+  VPB_TRY(dev_alloc(e, &e->heat, B * e->Kmax * 3072));
   for (int s = 0; s < 2; ++s) {
-    VPB_TRY(dev_alloc(e, &e->kpts[s], B * e->K * 3));
-    VPB_TRY(dev_alloc(e, &e->idx[s], B * e->K));
+    VPB_TRY(dev_alloc(e, &e->kpts[s], B * e->Kmax * 3));
+    VPB_TRY(dev_alloc(e, &e->idx[s], B * e->Kmax));
     VPB_TRY(dev_alloc(e, &e->org_wh[s], B * 2));
     VPB_TRY(dev_alloc(e, &e->crops_stage[s], B * 3 * 256 * 192));
     CU_TRY(cudaEventCreateWithFlags(&e->ev_h2d[s], cudaEventDisableTiming));
@@ -660,8 +793,8 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   CU_TRY(cudaMemset(e->chain_counters, 0, static_cast<size_t>(e->depth + 1) * 5 * e->chain_blocks * sizeof(int)));
   VPB_TRY(dev_alloc(e, &e->ln_counters, (M + 127) / 128 + 1));
   CU_TRY(cudaMemset(e->ln_counters, 0, ((M + 127) / 128 + 1) * sizeof(int)));
-  VPB_TRY(dev_alloc(e, &e->g_kpts, B * e->K * 3));
-  VPB_TRY(dev_alloc(e, &e->g_idx, B * e->K));
+  VPB_TRY(dev_alloc(e, &e->g_kpts, B * e->Kmax * 3));
+  VPB_TRY(dev_alloc(e, &e->g_idx, B * e->Kmax));
   VPB_TRY(dev_alloc(e, &e->g_org, B * 2));
   VPB_TRY(dev_alloc(e, &e->g_offs, B * 2));
   VPB_TRY(dev_alloc(e, &e->g_cs, B * 4));
@@ -686,6 +819,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(make_map(&e->o_qkv, e->qkv, M, 3 * D, 3 * D, 64));
   VPB_TRY(make_map(&e->o_hid, e->hid, M, 4 * D, 4 * D, 64));
   VPB_TRY(make_map(&e->o_x, e->x, M, D, D, 64, /*f32=*/true));
+  if (e->P > 0) VPB_TRY(make_map(&e->o_xs, e->x, M, D - e->P, D, 64, /*f32=*/true));
   {
     const char* env = getenv("VPB_L2_PERSIST");
     if (env && env[0] == '0') e->l2_persist = false;
@@ -896,19 +1030,54 @@ static int pick_tile(const LinearW& L, int M, int* bn, const CUtensorMap** wm) {
   return VPB_OK;
 }
 
-// everything after the patch gather, up to last_norm
-static int backbone(vpb_engine* e, int B, cudaStream_t st) {
+// fc2 of a multi-head call on an engine with experts: the shared columns [0, D-P) for all rows (the standalone GEMM, its
+// output map bounded to those columns), then the expert columns of every segment in one grouped launch (expert_gemm.cuh)
+static int fc2_experts(vpb_engine* e, const BlockW& b, int M, const std::vector<Segment>& segs, cudaStream_t st) {
+  const int D = e->D, P = e->P;
+  {
+    GemmParams p = gp(M, D - P, 4 * D, b.fc2s.b, e->x, D);
+    p.rmw = 0;                        // TMA reduce-add: the rmw epilogue bounds columns by ldc, not N (bit-identical either way)
+    int bn;
+    const CUtensorMap* wm;
+    VPB_TRY(pick_tile(b.fc2s, M, &bn, &wm));
+    e->prof.begin(KC_GEMM_FC2, st);
+    VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_hid, *wm, e->o_xs, p, st));
+    e->prof.end(st);
+  }
+  ExpertParams q;
+  memset(&q, 0, sizeof(q));
+  q.K = 4 * D; q.P = P; q.col0 = D - P; q.ldx = D; q.w_row0 = D - P; q.n_tiles = P / e->expert_bn;
+  q.bias = b.fc2.b; q.x = e->x;
+  int row = 0;
+  for (const Segment& sg : segs) {
+    ExpertSegment& t = q.seg[q.num_segs++];
+    t.row_begin = row; t.row_end = row + sg.count * 192; t.expert = sg.head; t.first_tile = q.num_tiles;
+    q.num_tiles += cdiv(sg.count * 192, GEMM_BM) * q.n_tiles;
+    row = t.row_end;
+  }
+  e->prof.begin(KC_GEMM_FC2, st);
+  VPB_TRY(expert_launch(e->expert_bn, e->m_hid, b.m_exp, q, st));
+  e->prof.end(st);
+  return VPB_OK;
+}
+
+// everything after the patch gather, up to last_norm.  `segs` (a multi-head call): the heads of the crops, in runs
+static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Segment>* segs = nullptr) {
   const int D = e->D, M = B * 192;
   const int stop = e->stop_after;
   if (stop == 1) return VPB_OK;
-  if (e->use_chain && B >= e->chain_min_batch && !stop && !e->ln_fused) return backbone_chained(e, B, st);
+  // multi-head calls run unchained (bit-identical to the chained form); with experts the LayerNorm after fc2 cannot ride in the
+  // fc2 tail (two launches write x) and runs standalone, bit-identical to the fused tail
+  const bool experts = segs != nullptr && e->P > 0;
+  const bool ln_fused = e->ln_fused;
+  if (e->use_chain && B >= e->chain_min_batch && !stop && !e->ln_fused && !segs) return backbone_chained(e, B, st);
   // LayerNorm i is produced either by its own kernel or (ln_fused) by the tail of the GEMM that completes x
   auto fuse_ln = [&](GemmParams& p, const float* g, const float* b) {
-    if (!e->ln_fused) return;
+    if (!ln_fused) return;
     p.ln_gamma = g; p.ln_beta = b; p.ln_out = e->xn; p.ln_counters = e->ln_counters; p.ln_eps = 1e-6f;
   };
   auto standalone_ln = [&](const float* g, const float* b) -> int {
-    if (e->ln_fused) return VPB_OK;
+    if (ln_fused) return VPB_OK;
     e->prof.begin(KC_LN, st);
     VPB_TRY(layernorm(e->x, g, b, e->xn, M, D, 1e-6f, st));
     e->prof.end(st);
@@ -916,7 +1085,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
   };
   // LayerNorm(x; g, b) -> xn followed by xn * W^T + bias (epilogue epi) as one chained launch: one LayerNorm stage whose source
   // rows are already complete (target 0) and one GEMM phase that waits for the normalised rows of its tile
-  const bool mini = e->ln_in_gemm && !e->ln_fused && !stop;
+  const bool mini = e->ln_in_gemm && !ln_fused && !stop;
   const size_t nblk = e->chain_blocks;
   if (mini) CU_TRY(cudaMemsetAsync(e->chain_counters, 0, static_cast<size_t>(e->depth + 1) * 5 * nblk * sizeof(int), st));
   auto ln_gemm = [&](const float* g, const float* b, const LinearW& L, const CUtensorMap& out, int epi, int slot, int kclass) -> int {
@@ -997,7 +1166,15 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
     e->prof.end(st);
     }
     if (stop == 7) return VPB_OK;
-    {
+    if (experts) {
+      VPB_TRY(fc2_experts(e, b, M, *segs, st));
+      if (ln_fused) {
+        const bool last = i + 1 == e->depth;
+        e->prof.begin(KC_LN, st);
+        VPB_TRY(layernorm(e->x, last ? e->lnf_g : e->blocks[i + 1].ln1_g, last ? e->lnf_b : e->blocks[i + 1].ln1_b, e->xn, M, D, 1e-6f, st));
+        e->prof.end(st);
+      }
+    } else {
       GemmParams p = gp(M, D, 4 * D, b.fc2.b, e->x, D);  // [+ norm1 of the next block, or last_norm]
       if (i + 1 < e->depth) fuse_ln(p, e->blocks[i + 1].ln1_g, e->blocks[i + 1].ln1_b);
       else fuse_ln(p, e->lnf_g, e->lnf_b);
@@ -1015,30 +1192,40 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st) {
   return standalone_ln(e->lnf_g, e->lnf_b);
 }
 
-static int head(vpb_engine* e, int B, float* d_heat, cudaStream_t st) {
+// Head j on crops c0 .. c0+B-1 of the workspace -> heatmaps of crop c at d_heat + c * ch_stride maps (ch_stride = the head's K
+// for the single-head calls, K_max for a multi-head call).  A deconv tile never straddles a crop, so a segment of crops is the
+// same launches on A maps and outputs that start at crop c0; the crop-0 maps are the engine's own.
+static int head(vpb_engine* e, int B, float* d_heat, cudaStream_t st, int j = 0, int c0 = 0, int ch_stride = 0) {
   const int D = e->D;
   const int stop = e->stop_after;
+  const HeadW& h = e->hw[j];
+  CUtensorMap feat = e->m_feat_nhwc, d1 = e->m_d1_nhwc, d2 = e->m_d2;
+  if (c0 > 0) {
+    VPB_TRY(make_map_nhwc(&feat, e->xn + static_cast<size_t>(c0) * 192 * D, B, 16, 12, D, 8, 12));
+    VPB_TRY(make_map_nhwc(&d1, e->d1 + static_cast<size_t>(c0) * 768 * 256, B, 32, 24, 256, 16, 8));
+    VPB_TRY(make_map(&d2, e->d2 + static_cast<size_t>(c0) * 3072 * 256, static_cast<uint64_t>(B) * 3072, 256, 256, 128));
+  }
   {  // deconv 1: tokens as NHWC 16x12xD -> d1 NHWC 32x24x256, all four sub-pixel phases in one implicit-GEMM launch
-    GemmParams p = gp(B * 192, 256, 4 * D, e->dc1.b, e->d1, 256);
+    GemmParams p = gp(B * 192, 256, 4 * D, h.dc1.b, e->d1 + static_cast<size_t>(c0) * 768 * 256, 256);
     p.up_h = 16; p.up_w = 12; p.up_tr = 8; p.up_tw = 12; p.up_c = D;
     e->prof.begin(KC_GEMM_DECONV, st);
-    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, e->m_feat_nhwc, *e->dc1.tile_map(256), e->m_xn, p, st));
+    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, feat, *h.dc1.tile_map(256), e->m_xn, p, st));
     e->prof.end(st);
   }
   if (stop == 11) return VPB_OK;
   {  // deconv 2: d1 -> d2 NHWC 64x48x256
-    GemmParams p = gp(B * 768, 256, 1024, e->dc2.b, e->d2, 256);
+    GemmParams p = gp(B * 768, 256, 1024, h.dc2.b, e->d2 + static_cast<size_t>(c0) * 3072 * 256, 256);
     p.up_h = 32; p.up_w = 24; p.up_tr = 16; p.up_tw = 8; p.up_c = 256;
     e->prof.begin(KC_GEMM_DECONV, st);
-    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, e->m_d1_nhwc, *e->dc2.tile_map(256), e->m_xn, p, st));
+    VPB_TRY(gemm_launch(256, EPI_BF16_RELU_UP, d1, *h.dc2.tile_map(256), e->m_xn, p, st));
     e->prof.end(st);
   }
   if (stop == 12) return VPB_OK;
   {
-    GemmParams p = gp(B * 3072, e->n_final, 256, e->fin.b, d_heat, 0);
-    p.n_valid = e->K; p.pix = 3072;
+    GemmParams p = gp(B * 3072, h.n_final, 256, h.fin.b, d_heat, 0);
+    p.n_valid = h.K; p.pix = 3072; p.ch_stride = ch_stride;
     e->prof.begin(KC_GEMM_FINAL, st);
-    VPB_TRY(gemm_launch(e->n_final, EPI_F32_NCHW, e->m_d2, e->m_fin_w, e->m_d2, p, st));
+    VPB_TRY(gemm_launch(h.n_final, EPI_F32_NCHW, d2, h.m_fin_w, d2, p, st));
     e->prof.end(st);
   }
   return VPB_OK;
@@ -1682,6 +1869,196 @@ extern "C" int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, i
   return VPB_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ multi-head calls
+static_assert(VPB_MAX_SEGMENTS == EXPERT_MAX_SEGMENTS, "the header's segment limit is the expert GEMM's table size");
+constexpr size_t kMaxMixedGraphs = 16;
+
+static void drop_graphs(vpb_engine* e) {
+  for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+  e->graphs.clear();
+  for (auto& g : e->mixed_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+  e->mixed_graphs.clear();
+}
+
+static int check_ready_heads(vpb_engine* e, const char* fn) {
+  if (!e) return fail(VPB_ERR_ARG, "%s: null engine", fn);
+  if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
+  if (e->flip) return fail(VPB_ERR_STATE, "%s: the multi-head calls do not run the flip test; switch it off first", fn);
+  return VPB_OK;
+}
+// appends `count` crops of `head` to the runs (runs of one head merge; empty ones vanish)
+static int add_segment(vpb_engine* e, const char* fn, std::vector<Segment>& segs, int item, int head, int count) {
+  if (head < 0 || head >= e->num_kheads) return fail(VPB_ERR_ARG, "%s: entry %d names head %d (the engine has %d)", fn, item, head, e->num_kheads);
+  if (count < 0) return fail(VPB_ERR_ARG, "%s: entry %d has count %d", fn, item, count);
+  if (count == 0) return VPB_OK;
+  if (!segs.empty() && segs.back().head == head) segs.back().count += count;
+  else segs.push_back({head, count});
+  return VPB_OK;
+}
+
+// Gather (unless done), backbone with the experts of `segs`, then per segment the head's deconvs + 1x1 conv into `heat`
+// (crop c at heat + c * K_max maps) and the per-crop decode of its K_head maps into kpts [n, K_max, 3] / idx [n, K_max].
+// A single segment of head 0 runs the single-head backbone launches.
+static int heads_enqueue(vpb_engine* e, const Source* src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
+                         const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* heat, cudaStream_t st) {
+  const int Km = e->Kmax;
+  if (src) VPB_TRY(gather(e, *src, n, n, st));
+  VPB_TRY(backbone(e, n, st, (segs.size() == 1 && segs[0].head == 0) ? nullptr : &segs));
+  if (e->stop_after && e->stop_after <= 10) return VPB_OK;
+  int c0 = 0;
+  for (const Segment& sg : segs) {
+    VPB_TRY(head(e, sg.count, heat + static_cast<size_t>(c0) * Km * 3072, st, sg.head, c0, Km));
+    c0 += sg.count;
+  }
+  if (e->stop_after) return VPB_OK;
+  c0 = 0;
+  for (const Segment& sg : segs) {
+    DecodeParams p;
+    p.heatmaps = heat + static_cast<size_t>(c0) * Km * 3072; p.org_wh = d_org_wh + 2 * c0; p.offs_yx = d_offs_yx ? d_offs_yx + 2 * c0 : nullptr;
+    p.kpts = d_kpts + static_cast<size_t>(c0) * Km * 3; p.idx = d_idx ? d_idx + static_cast<size_t>(c0) * Km : nullptr;
+    p.n = sg.count; p.k = e->hw[sg.head].K; p.kstride = Km; p.wrap_batch = 0;
+    e->prof.begin(KC_DECODE, st);
+    CU_TRY(launch_k(decode_heatmaps<false>, dim3(cdiv(static_cast<long long>(p.n) * p.k, DECODE_WARPS)), dim3(DECODE_WARPS * 32), 0, st, p));
+    e->prof.end(st);
+    c0 += sg.count;
+  }
+  return VPB_OK;
+}
+
+// rows 0 .. K_head-1 of every crop of every segment: [n, K_max, row] -> [n, K_max, row] (rows past K_head are left alone)
+static int copy_head_rows(const vpb_engine* e, const std::vector<Segment>& segs, void* dst, const void* src, size_t row_bytes, cudaMemcpyKind kind,
+                          cudaStream_t st) {
+  const size_t pitch = static_cast<size_t>(e->Kmax) * row_bytes;
+  size_t off = 0;
+  for (const Segment& sg : segs) {
+    CU_TRY(cudaMemcpy2DAsync(static_cast<char*>(dst) + off, pitch, static_cast<const char*>(src) + off, pitch, e->hw[sg.head].K * row_bytes,
+                             sg.count, kind, st));
+    off += sg.count * pitch;
+  }
+  return VPB_OK;
+}
+
+// Graph replay as infer_core_locked, keyed by the segment list: eager on a list's first use, captured on its second.
+static int heads_core_locked(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
+                             const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
+  float* heat = d_heatmaps ? d_heatmaps : e->heat;
+  if (!e->use_graph || e->prof.on || e->stop_after || st == nullptr || stream_is_capturing(st))
+    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, heat, st);
+  vpb_engine::MixedGraph* g = nullptr;
+  for (auto& c : e->mixed_graphs)
+    if (c.segs == segs) g = &c;
+  if (!g) {                                                               // first use of this list: run eagerly
+    if (e->mixed_graphs.size() == kMaxMixedGraphs) {
+      auto lru = std::min_element(e->mixed_graphs.begin(), e->mixed_graphs.end(),
+                                  [](const vpb_engine::MixedGraph& a, const vpb_engine::MixedGraph& b) { return a.used < b.used; });
+      if (lru->exec) cudaGraphExecDestroy(lru->exec);
+      e->mixed_graphs.erase(lru);
+    }
+    e->mixed_graphs.push_back({segs, nullptr, ++e->mixed_clock});
+    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, heat, st);
+  }
+  g->used = ++e->mixed_clock;
+  VPB_TRY(gather(e, src, n, n, st));
+  CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(n) * 2 * sizeof(int32_t), st));
+  if (!g->exec) {
+    cudaGraph_t graph = nullptr;
+    CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    const int rc = heads_enqueue(e, nullptr, segs, n, e->g_org, e->g_offs, e->g_kpts, e->g_idx, e->heat, st);
+    const cudaError_t ce = cudaStreamEndCapture(st, &graph);
+    if (rc != VPB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
+    if (ce != cudaSuccess) return fail(VPB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
+    const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (ie != cudaSuccess) { g->exec = nullptr; return fail(VPB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(ie)); }
+  }
+  CU_TRY(cudaGraphLaunch(g->exec, st));
+  VPB_TRY(copy_head_rows(e, segs, d_kpts, e->g_kpts, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (d_idx) VPB_TRY(copy_head_rows(e, segs, d_idx, e->g_idx, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  if (d_heatmaps) VPB_TRY(copy_head_rows(e, segs, d_heatmaps, e->heat, 3072 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return VPB_OK;
+}
+static int heads_core(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
+                      const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
+  VPB_TRY(apply_l2_policy(e, st));
+  WsScope ws(e, st);
+  VPB_TRY(ws.begin(n));
+  VPB_TRY(heads_core_locked(e, src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, d_heatmaps, st));
+  return ws.end();
+}
+
+extern "C" int vpb_infer_heads(vpb_engine* e, const float* d_crops, const int32_t* d_org_wh, const vpb_segment* h_segs, int32_t num_segs,
+                               float* d_kpts, int32_t* d_idx, float* d_heatmaps, void* stream) {
+  VPB_TRY(check_ready_heads(e, "vpb_infer_heads"));
+  if (num_segs < 0 || num_segs > VPB_MAX_SEGMENTS || (num_segs > 0 && !h_segs))
+    return fail(VPB_ERR_ARG, "vpb_infer_heads: %d segments (0..%d), segment array %p", num_segs, VPB_MAX_SEGMENTS, static_cast<const void*>(h_segs));
+  std::vector<Segment> segs;
+  long long n = 0;
+  for (int i = 0; i < num_segs; ++i) {
+    VPB_TRY(add_segment(e, "vpb_infer_heads", segs, i, h_segs[i].head, h_segs[i].count));
+    n += h_segs[i].count;
+  }
+  if (n > e->maxB) return fail(VPB_ERR_ARG, "vpb_infer_heads: %lld crops exceed max_batch = %d", n, e->maxB);
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_crops || !d_org_wh || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_heads: null pointer");
+  Source src;
+  src.crops = d_crops;
+  return heads_core(e, src, segs, static_cast<int>(n), d_org_wh, nullptr, d_kpts, d_idx, d_heatmaps, static_cast<cudaStream_t>(stream));
+}
+
+// the runs of equal head over the frames that have boxes (frame j's boxes all belong to head h_heads[j])
+static int frame_segments(vpb_engine* e, const char* fn, const vpb_frame* fr, int32_t num_frames, const int32_t* h_heads,
+                          std::vector<Segment>* segs) {
+  if (num_frames > 0 && !h_heads) return fail(VPB_ERR_ARG, "%s: null head array", fn);
+  for (int j = 0; j < num_frames; ++j)
+    if (fr[j].num_boxes > 0) VPB_TRY(add_segment(e, fn, *segs, j, h_heads[j], fr[j].num_boxes));
+  return VPB_OK;
+}
+
+extern "C" int vpb_infer_frames_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                      const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, "vpb_infer_frames_heads"));
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_frames_heads", e, h_frames, num_frames, tab, &nt, &n));
+  std::vector<Segment> segs;
+  VPB_TRY(frame_segments(e, "vpb_infer_frames_heads", h_frames, num_frames, h_heads, &segs));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_heads: null pointer");
+  Source src;
+  src.frames = tab; src.num_frames = nt; src.bboxes = d_bboxes;
+  return heads_core(e, src, segs, n, e->pp_org, e->pp_offs, d_kpts, d_idx, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                           const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, "vpb_infer_frames_heads_host"));
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_frames_heads_host", e, h_frames, num_frames, tab, &nt, &n));
+  std::vector<Segment> segs;
+  VPB_TRY(frame_segments(e, "vpb_infer_frames_heads_host", h_frames, num_frames, h_heads, &segs));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_heads_host: null pointer");
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  VPB_TRY(stage_frames_host(e, 0, tab, nt, h_bboxes, n, st));
+  Source src;
+  src.frames = tab; src.num_frames = nt; src.bboxes = e->bbox_stage[0];
+  VPB_TRY(heads_core(e, src, segs, n, e->pp_org, e->pp_offs, e->kpts[0], e->idx[0], nullptr, st));
+  VPB_TRY(copy_head_rows(e, segs, h_kpts, e->kpts[0], 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_idx) VPB_TRY(copy_head_rows(e, segs, h_idx, e->idx[0], sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU_TRY(cudaEventRecord(e->ev_done[0], st));
+  CU_TRY(cudaStreamSynchronize(st));
+  return VPB_OK;
+}
+
 extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t* h_org_wh, int32_t batch, float* h_kpts,
                               int32_t* h_idx, void* stream) {
   VPB_TRY(check_ready_keypoints(e, batch));
@@ -1735,6 +2112,23 @@ extern "C" void vpb_host_free(void* p) {
   if (p) cudaFreeHost(p);
 }
 
+extern "C" int vpb_cached_graphs(const vpb_engine* e, int32_t mixed, int32_t* entries, int32_t* captured) {
+  if (!e || !entries || !captured) return fail(VPB_ERR_ARG, "vpb_cached_graphs: null argument");
+  *entries = *captured = 0;
+  auto count = [&](const auto& list) {
+    for (const auto& g : list) { ++*entries; *captured += g.exec != nullptr; }
+  };
+  if (mixed) count(e->mixed_graphs);
+  else count(e->graphs);
+  return VPB_OK;
+}
+extern "C" int64_t vpb_device_bytes(const vpb_engine* e) {
+  if (!e) return -1;
+  size_t b = e->alloc_bytes;
+  for (int s = 0; s < 2; ++s) b += e->frame_cap[s] ? e->frame_cap[s] + 256 : 0;
+  return static_cast<int64_t>(b);
+}
+
 extern "C" int vpb_kernel_launches(const vpb_engine* e, int32_t batch) {
   if (!e) return -1;
   // patch im2col + patch GEMM + depth*(qkv, attention, proj, fc1, fc2) + 2 deconv GEMMs + 1x1 GEMM + decode; the 2*depth+1
@@ -1763,13 +2157,11 @@ extern "C" int vpb_set_option(vpb_engine* e, const char* name, int32_t value) {
     else if (!strcmp(name, "ln_in_gemm")) e->ln_in_gemm = value != 0;
     else if (!strcmp(name, "chain")) e->use_chain = value != 0;
     else e->chain_min_batch = value;
-    for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);      // captured chains embed the choice
-    e->graphs.clear();
+    drop_graphs(e);                   // captured chains embed the choice
   }
   else if (!strcmp(name, "ln_fused")) {
     e->ln_fused = value != 0;
-    for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);      // captured chains embed the choice
-    e->graphs.clear();
+    drop_graphs(e);                   // captured chains embed the choice
   }
   else return fail(VPB_ERR_ARG, "unknown option %s", name);
   return VPB_OK;
@@ -1778,6 +2170,7 @@ extern "C" int vpb_set_option(vpb_engine* e, const char* name, int32_t value) {
 extern "C" int vpb_set_flip_test(vpb_engine* e, const int32_t* h_perm, int32_t k, int32_t shift) {
   if (!e) return fail(VPB_ERR_ARG, "vpb_set_flip_test: null engine");
   if (!e->finalized) return fail(VPB_ERR_STATE, "not finalized");
+  if (e->num_kheads > 1) return fail(VPB_ERR_STATE, "vpb_set_flip_test: not supported on an engine with %d heads", e->num_kheads);
   if (h_perm) {
     if (k != e->K) return fail(VPB_ERR_ARG, "vpb_set_flip_test: permutation of %d keypoints, the engine has %d", k, e->K);
     for (int i = 0; i < k; ++i)
@@ -1789,8 +2182,7 @@ extern "C" int vpb_set_flip_test(vpb_engine* e, const int32_t* h_perm, int32_t k
   if (h_perm) CU_TRY(cudaMemcpy(e->flip_perm, h_perm, static_cast<size_t>(k) * sizeof(int32_t), cudaMemcpyHostToDevice));
   e->flip = h_perm != nullptr;
   e->flip_shift = shift ? 1 : 0;
-  for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);      // captured chains embed the batch and the average
-  e->graphs.clear();
+  drop_graphs(e);                     // captured chains embed the batch and the average
   return VPB_OK;
 }
 

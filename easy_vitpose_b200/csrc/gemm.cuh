@@ -36,6 +36,7 @@ struct GemmParams {
   int ldc;                // row pitch of out in elements (direct row-major epilogues)
   int n_valid;            // EPI_F32_NCHW: number of real output channels
   int pix;                // EPI_F32_NCHW: pixels per image (rows per batch item)
+  int ch_stride;          // EPI_F32_NCHW: channels between consecutive images of out (0 = n_valid; a multi-head call: K_max)
   int up_h, up_w;         // EPI_BF16_RELU_UP: input grid (H, W)
   int up_tr, up_tw;       // EPI_BF16_RELU_UP: an M tile is a up_tr x up_tw patch of positions (96 = 8x12 or 128 = 16x8)
   int up_c;               // EPI_BF16_RELU_UP: input channels (K = 4 taps * up_c)
@@ -388,7 +389,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
             const int row = m0 + r;
             if (row >= p.M) continue;
             const int b = row / p.pix, pix = row % p.pix;
-            float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(b) * p.n_valid) * p.pix + pix;
+            float* o = reinterpret_cast<float*>(p.out) + (static_cast<size_t>(b) * (p.ch_stride ? p.ch_stride : p.n_valid)) * p.pix + pix;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
               const int n = n0 + 8 * j + cq;

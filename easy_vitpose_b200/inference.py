@@ -97,6 +97,13 @@ class B200PoseBackend:
         return self.model.infer_frames_host(imgs, bboxes_list)[0]
 
     @torch.no_grad()
+    def inference_frames_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list) -> "list[np.ndarray]":
+        """inference_frames on a multi-head engine (ViTPose(..., heads=...)), with a head index per box (heads_list: per frame
+        an int array [n_i], e.g. 0 for people and 3 for animals of a ViTPose+ engine) -> one float32 [n_i,K_max,3] (y, x,
+        score) per frame; a box of head j fills rows 0..K_j-1."""
+        return self.model.infer_frames_heads_host(imgs, bboxes_list, heads_list)[0]
+
+    @torch.no_grad()
     def inference_topdown(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", padding: float = 1.25,
                           use_udp: bool = True) -> "list[np.ndarray]":
         """mmpose-style top-down inference: uint8 RGB frames + each frame's person boxes [n_i,4] (x, y, w, h) -> one float32

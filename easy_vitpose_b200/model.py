@@ -13,8 +13,9 @@ import numpy as np
 import torch
 
 from . import _lib
+from .configs import VITPOSE_PLUS_HEADS
 
-__all__ = ["ViTPose", "plan_frame_chunks"]
+__all__ = ["ViTPose", "plan_frame_chunks", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head"]
 
 IMG_H, IMG_W, HM_H, HM_W = 256, 192, 64, 48
 
@@ -55,8 +56,116 @@ def _frame_array(frames, chunk):
     return arr
 
 
-def _expected_shapes(D: int, depth: int, K: int) -> "OrderedDict[str, tuple]":
-    """state_dict contract of the reference ViTPose (SURVEY.md section 8b)."""
+def group_by_head(heads, num_heads: int) -> "tuple[np.ndarray, list[int]]":
+    """Per-box head indices -> (order, counts): `order` lists the boxes grouped by head, stable inside a head (box order[i]
+    goes to position i of the grouped call), counts[h] = boxes of head h.  Raises ValueError for an index outside
+    0..num_heads-1."""
+    h = np.asarray(heads).reshape(-1)
+    if h.size and (h.dtype.kind not in "iu" or h.min() < 0 or h.max() >= num_heads):
+        raise ValueError(f"head indices must be integers in 0..{num_heads - 1}")
+    h = h.astype(np.int64)
+    return np.argsort(h, kind="stable"), [int(c) for c in np.bincount(h, minlength=num_heads)]
+
+
+def _inverse(order: np.ndarray) -> np.ndarray:
+    inv = np.empty_like(order)
+    inv[order] = np.arange(order.size)
+    return inv
+
+
+# the head tensors model_split.py moves (:35-48), relative to the head's prefix
+_HEAD_PARTS = ("deconv_layers.0.weight", "deconv_layers.1.weight", "deconv_layers.1.bias", "deconv_layers.1.running_mean",
+               "deconv_layers.1.running_var", "deconv_layers.1.num_batches_tracked", "deconv_layers.3.weight",
+               "deconv_layers.4.weight", "deconv_layers.4.bias", "deconv_layers.4.running_mean", "deconv_layers.4.running_var",
+               "deconv_layers.4.num_batches_tracked", "final_layer.weight", "final_layer.bias")
+
+
+def _head_prefix(j: int) -> str:
+    return "keypoint_head." if j == 0 else f"associate_keypoint_heads.{j - 1}."
+
+
+def _unwrap(sd):
+    return sd["state_dict"] if "state_dict" in sd and not any(k.startswith("backbone.") for k in sd) else sd
+
+
+def split_vitpose_plus(sd, names=None, keypoints=None) -> "OrderedDict[str, OrderedDict[str, torch.Tensor]]":
+    """model_split.py in torch on the CPU: an unsplit ViTPose+ state_dict -> {dataset: single-dataset state_dict}.  Head i
+    (names[i], default the VITPOSE_PLUS_HEADS order) gets fc2 = cat([fc2, experts.i]) in every block (:53-57, :83-92) and,
+    for i >= 1, associate_keypoint_heads.{i-1} as keypoint_head with final_layer cut to keypoints[i] rows (:97-102); the
+    expert and associate tensors are dropped (:59-69, :104-114).  A checkpoint without experts (a frozen-backbone fine-tune
+    merged with P = 0) keeps its fc2 as is."""
+    sd = _unwrap(sd)
+    table = dict(VITPOSE_PLUS_HEADS)
+    names = [n for n, _ in VITPOSE_PLUS_HEADS] if names is None else list(names)
+    keypoints = [table[n] for n in names] if keypoints is None else [int(k) for k in keypoints]
+    if len(names) != len(keypoints):
+        raise ValueError(f"{len(names)} names but {len(keypoints)} keypoint counts")
+    experts = any(".mlp.experts." in k for k in sd)
+    out: "OrderedDict[str, OrderedDict[str, torch.Tensor]]" = OrderedDict()
+    for i, (name, K) in enumerate(zip(names, keypoints)):
+        d: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+        for k, v in sd.items():
+            if "expert" in k or k.startswith("associate_keypoint_heads."):
+                continue
+            if "mlp.fc2" in k and experts:
+                ek = k.replace("fc2.", f"experts.{i}.")
+                if ek not in sd:
+                    raise KeyError(f"{ek}: the checkpoint has no expert {i} for {name!r}")
+                v = torch.cat([torch.as_tensor(v), torch.as_tensor(sd[ek])], 0)
+            d[k] = v
+        if i > 0:
+            for part in _HEAD_PARTS:
+                src = _head_prefix(i) + part
+                if src in sd:
+                    d["keypoint_head." + part] = sd[src]
+                elif not part.endswith("num_batches_tracked"):
+                    raise KeyError(f"{src} missing")
+            for part in ("final_layer.weight", "final_layer.bias"):
+                d["keypoint_head." + part] = d["keypoint_head." + part][:K]
+        out[name] = d
+    return out
+
+
+def merge_split_state_dicts(sds, part_features: int) -> "OrderedDict[str, torch.Tensor]":
+    """The inverse of split_vitpose_plus: {dataset: state_dict} (split ViTPose+ checkpoints, or frozen-backbone fine-tunes with
+    part_features = 0) -> one state_dict under ViTPose+ keys for a multi-head ViTPose, heads in the dict's order: each
+    block's fc2 is split into the shared rows (mlp.fc2) and the last part_features rows of checkpoint j (mlp.experts.{j}),
+    checkpoint 0's head is keypoint_head and checkpoint j's is associate_keypoint_heads.{j-1}.  Every other backbone tensor,
+    and the shared rows of fc2, must be equal in all checkpoints: ValueError names the first key whose shared part differs."""
+    items = [(str(n), {k: torch.as_tensor(v) for k, v in _unwrap(sd).items()}) for n, sd in sds.items()]
+    if not items:
+        raise ValueError("no checkpoints to merge")
+    P = int(part_features)
+    base_name, base = items[0]
+    for name, sd in items[1:]:
+        for k in sd:
+            if not k.startswith("keypoint_head.") and k not in base:
+                raise ValueError(f"{k}: in {name!r} but not in {base_name!r}")
+    out: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    for k, v in base.items():
+        if k.startswith("keypoint_head."):
+            continue
+        split = P > 0 and "mlp.fc2" in k
+        shared = v[: v.shape[0] - P] if split else v
+        for name, sd in items[1:]:
+            w = sd.get(k)
+            ws = None if w is None else (w[: w.shape[0] - P] if split else w)
+            if ws is None or ws.shape != shared.shape or not torch.equal(ws, shared):
+                raise ValueError(f"{k}: the shared part of {name!r} differs from {base_name!r}")
+        out[k] = shared
+        if split:
+            for j, (_, sd) in enumerate(items):
+                out[k.replace("fc2.", f"experts.{j}.")] = sd[k][sd[k].shape[0] - P:]
+    for j, (_, sd) in enumerate(items):
+        for k, v in sd.items():
+            if k.startswith("keypoint_head."):
+                out[_head_prefix(j) + k[len("keypoint_head."):]] = v
+    return out
+
+
+def _expected_shapes(D: int, depth: int, K: int, head_keypoints=None, P: int = 0) -> "OrderedDict[str, tuple]":
+    """state_dict contract of the reference ViTPose (SURVEY.md section 8b); with head_keypoints / P the ViTPose+ key set of a
+    multi-head engine (vpb_create_heads)."""
     s: "OrderedDict[str, tuple]" = OrderedDict()
     s["backbone.pos_embed"] = (1, 193, D)
     s["backbone.patch_embed.proj.weight"] = (D, 3, 16, 16)
@@ -68,17 +177,21 @@ def _expected_shapes(D: int, depth: int, K: int) -> "OrderedDict[str, tuple]":
         s[p + "attn.proj.weight"] = (D, D); s[p + "attn.proj.bias"] = (D,)
         s[p + "norm2.weight"] = (D,); s[p + "norm2.bias"] = (D,)
         s[p + "mlp.fc1.weight"] = (4 * D, D); s[p + "mlp.fc1.bias"] = (4 * D,)
-        s[p + "mlp.fc2.weight"] = (D, 4 * D); s[p + "mlp.fc2.bias"] = (D,)
+        s[p + "mlp.fc2.weight"] = (D - P, 4 * D); s[p + "mlp.fc2.bias"] = (D - P,)
+        for j in range(len(head_keypoints) if P else 0):
+            s[p + f"mlp.experts.{j}.weight"] = (P, 4 * D); s[p + f"mlp.experts.{j}.bias"] = (P,)
     s["backbone.last_norm.weight"] = (D,); s["backbone.last_norm.bias"] = (D,)
-    cin = D
-    for li in (0, 3):
-        s[f"keypoint_head.deconv_layers.{li}.weight"] = (cin, 256, 4, 4)
-        for n in ("weight", "bias", "running_mean", "running_var"):
-            s[f"keypoint_head.deconv_layers.{li + 1}.{n}"] = (256,)
-        s[f"keypoint_head.deconv_layers.{li + 1}.num_batches_tracked"] = ()
-        cin = 256
-    s["keypoint_head.final_layer.weight"] = (K, 256, 1, 1)
-    s["keypoint_head.final_layer.bias"] = (K,)
+    for j, Kj in enumerate(head_keypoints or [K]):
+        hp = _head_prefix(j)
+        cin = D
+        for li in (0, 3):
+            s[f"{hp}deconv_layers.{li}.weight"] = (cin, 256, 4, 4)
+            for n in ("weight", "bias", "running_mean", "running_var"):
+                s[f"{hp}deconv_layers.{li + 1}.{n}"] = (256,)
+            s[f"{hp}deconv_layers.{li + 1}.num_batches_tracked"] = ()
+            cin = 256
+        s[hp + "final_layer.weight"] = (Kj, 256, 1, 1)
+        s[hp + "final_layer.bias"] = (Kj,)
     return s
 
 
@@ -125,7 +238,8 @@ class ViTPose:
     mlp_ratio 4, qkv_bias, two 4x4 deconvs of 256 filters and a 1x1 final conv.
     """
 
-    def __init__(self, cfg: dict, max_batch: int = 64, device: "int | str | torch.device | None" = None) -> None:
+    def __init__(self, cfg: dict, max_batch: int = 64, device: "int | str | torch.device | None" = None, *, heads=None,
+                 expert_rows: int = 0) -> None:
         bb = {k: v for k, v in cfg["backbone"].items() if k != "type"}
         hd = {k: v for k, v in cfg["keypoint_head"].items() if k != "type"}
         if tuple(bb.get("img_size", (256, 192))) != (256, 192) or bb.get("patch_size", 16) != 16 or bb.get("ratio", 1) != 1:
@@ -137,6 +251,28 @@ class ViTPose:
             raise ValueError("only the 2x deconv(256,4x4) + 1x1 conv head of the reference's configs is built")
         self.embed_dim = int(bb["embed_dim"]); self.depth = int(bb["depth"]); self.num_heads = int(bb["num_heads"])
         self.num_keypoints = int(hd["out_channels"])
+        # several keypoint heads on one backbone (ViTPose+ / frozen-backbone fine-tunes): `heads` = keypoint counts or
+        # (dataset, keypoints) pairs, head j using fc2 expert j of width expert_rows (0 = a fully shared backbone)
+        self.head_names = None
+        self.head_keypoints = [self.num_keypoints]
+        self.expert_rows = int(expert_rows)
+        self._multi = heads is not None
+        if self._multi:
+            heads = list(heads)
+            if not 1 <= len(heads) <= _lib.MAX_HEADS:
+                raise ValueError(f"{len(heads)} heads: 1..{_lib.MAX_HEADS} expected")
+            if all(isinstance(h, (tuple, list)) for h in heads):
+                self.head_names = [str(n) for n, _ in heads]
+                heads = [k for _, k in heads]
+            self.head_keypoints = [int(k) for k in heads]
+            if any(not 1 <= k <= 144 for k in self.head_keypoints):
+                raise ValueError(f"keypoint counts {self.head_keypoints}: 1..144 each")
+            if self.expert_rows and not (0 < self.expert_rows < self.embed_dim and self.expert_rows % 32 == 0):
+                raise ValueError(f"expert_rows={self.expert_rows}: 0 or a multiple of 32 below embed_dim={self.embed_dim}")
+            self.num_keypoints = self.head_keypoints[0]
+        elif self.expert_rows:
+            raise ValueError("expert_rows needs heads=")
+        self.num_keypoints_max = max(self.head_keypoints)
         if int(hd["in_channels"]) != self.embed_dim:
             raise ValueError("keypoint_head.in_channels must equal backbone.embed_dim")
         self.max_batch = int(max_batch)
@@ -188,7 +324,8 @@ class ViTPose:
         shape mismatches raise (easy_ViTPose/inference.py:162-166 calls it exactly like this)."""
         if "state_dict" in state_dict and not any(k.startswith("backbone.") for k in state_dict):
             state_dict = state_dict["state_dict"]
-        exp = _expected_shapes(self.embed_dim, self.depth, self.num_keypoints)
+        exp = _expected_shapes(self.embed_dim, self.depth, self.num_keypoints, self.head_keypoints if self._multi else None,
+                               self.expert_rows)
         missing = [k for k in exp if k not in state_dict and not k.endswith("num_batches_tracked")]
         unexpected = [k for k in state_dict if k not in exp]
         if strict and (missing or unexpected):
@@ -227,7 +364,11 @@ class ViTPose:
         L = _lib.lib()
         cfg = _lib.VpbConfig(self.embed_dim, self.depth, self.num_heads, self.num_keypoints, self.max_batch, self._device)
         with torch.cuda.device(self._device):
-            _lib.check(L.vpb_create(C.byref(cfg), C.byref(self._handle)))
+            if self._multi:
+                ks = (C.c_int32 * len(self.head_keypoints))(*self.head_keypoints)
+                _lib.check(L.vpb_create_heads(C.byref(cfg), len(ks), ks, self.expert_rows, C.byref(self._handle)))
+            else:
+                _lib.check(L.vpb_create(C.byref(cfg), C.byref(self._handle)))
             for k, v in self._state.items():
                 if k.endswith("num_batches_tracked"):
                     continue
@@ -750,12 +891,147 @@ class ViTPose:
         split = np.cumsum(counts)[:-1]
         return np.split(kp, split), np.split(idx, split)
 
+    # ---------------------------------------------------------------------------------------- several heads (datasets)
+    @staticmethod
+    def _segments(chunk):
+        return (_lib.VpbSegment * len(chunk))(*[_lib.VpbSegment(h, e - s) for h, s, e in chunk])
+
+    def _head_indices(self, j: "int | None", heads, n: int) -> np.ndarray:
+        h = np.asarray(heads.cpu() if isinstance(heads, torch.Tensor) else heads).reshape(-1)
+        if h.size != n:
+            raise ValueError(f"{n} boxes but {h.size} head indices" + ("" if j is None else f" in frame {j}"))
+        group_by_head(h, len(self.head_keypoints))           # range check
+        return h.astype(np.int64)
+
+    @torch.no_grad()
+    def infer_crops_heads(self, x: torch.Tensor, org_wh: torch.Tensor, heads, return_heatmaps: bool = False):
+        """infer_crops with a keypoint head per crop (heads [B] ints, 0..H-1): the crops are grouped by head (stable) and run
+        in as few vpb_infer_heads calls as batch_limit allows, each with one backbone pass.  Returns (kpts [B,K_max,3],
+        idx [B,K_max][, heatmaps [B,K_max,64,48]]) in the caller's crop order; crop c of head j fills rows 0..K_j-1, the rest
+        are zeros.  Bit-identical to infer_crops on single-head engines loaded with split_vitpose_plus's checkpoints."""
+        x = self._check_input(x, 1 << 30)                  # any batch: the calls are chunked below
+        n = x.shape[0]
+        h = self._head_indices(None, heads, n)
+        org = torch.as_tensor(org_wh).to(device=x.device, dtype=torch.int32).contiguous()
+        if tuple(org.shape) != (n, 2):
+            raise ValueError(f"org_wh must be [B,2], got {tuple(org.shape)}")
+        order, counts = group_by_head(h, len(self.head_keypoints))
+        perm = torch.as_tensor(order, device=x.device)
+        xs, org = x.index_select(0, perm).contiguous(), org.index_select(0, perm).contiguous()
+        Km = self.num_keypoints_max
+        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=x.device)
+        idx = torch.zeros((n, Km), dtype=torch.int32, device=x.device)
+        hm = torch.zeros((n, Km, HM_H, HM_W), dtype=torch.float32, device=x.device) if return_heatmaps else None
+        s = 0
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            segs = self._segments(chunk)
+            self._call_on_stream((xs, org, kp, idx, hm), lambda st: _lib.lib().vpb_infer_heads(
+                self._handle, C.c_void_p(xs[s:].data_ptr()), C.c_void_p(org[s:].data_ptr()), segs, len(segs),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), C.c_void_p(hm[s:].data_ptr()) if hm is not None else None, st))
+            s += sum(e - b for _, b, e in chunk)
+        inv = torch.as_tensor(_inverse(order), device=x.device)
+        out = (kp.index_select(0, inv), idx.index_select(0, inv))
+        return out + (hm.index_select(0, inv),) if return_heatmaps else out
+
+    def _head_entries(self, counts, heads):
+        """Per-frame head indices -> the call's table entries grouped by head (stable): [(frame, box indices, head)]."""
+        hs = [self._head_indices(j, h, c) for j, (c, h) in enumerate(zip(counts, heads))]
+        return [(j, np.nonzero(h == k)[0], k) for k in range(len(self.head_keypoints)) for j, h in enumerate(hs) if (h == k).any()]
+
+    def infer_frames_heads(self, frames, bboxes, heads, check: bool = False):
+        """infer_frames with a keypoint head per box (heads: per frame an int array [n_j]): the boxes are grouped by head
+        (stable; a frame appears once per head it uses) and run through vpb_infer_frames_heads in calls of at most batch_limit
+        boxes and 64 entries.  Returns per frame kpts f32 [n_j,K_max,3] (y, x, score) in that frame's pixels and idx i32
+        [n_j,K_max], rows K_j.. of a head-j box zero."""
+        self._ensure()
+        if not (len(frames) == len(bboxes) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        dev = torch.device("cuda", self._device)
+        boxes = []
+        for b in bboxes:
+            b = torch.as_tensor(b)
+            if b.is_floating_point():
+                b = b.round()
+            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
+        ents = self._head_entries([b.shape[0] for b in boxes], heads)
+        n = sum(len(sel) for _, sel, _ in ents)
+        bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
+        Km = self.num_keypoints_max
+        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
+        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
+        table = [(frames[j].data_ptr(), frames[j].shape[0], frames[j].shape[1], frames[j].stride(0)) for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        for chunk in plan_frame_chunks([len(sel) for _, sel, _ in ents], self.batch_limit):
+            arr = _frame_array(table, chunk)
+            ha = np.ascontiguousarray(hv[:len(arr)])
+            self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads(
+                self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), C.c_void_p(bb[s:].data_ptr()),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 1:
+            raise ValueError("a box is empty after padding and clipping to its frame")
+        return self._per_frame(ents, [b.shape[0] for b in boxes], kp, idx)
+
+    @staticmethod
+    def _per_frame(ents, counts, kp, idx):
+        outs_k = [kp.new_zeros((c,) + tuple(kp.shape[1:])) for c in counts]
+        outs_i = [idx.new_zeros((c,) + tuple(idx.shape[1:])) for c in counts]
+        s = 0
+        for j, sel, _ in ents:
+            outs_k[j][sel] = kp[s:s + len(sel)]
+            outs_i[j][sel] = idx[s:s + len(sel)]
+            s += len(sel)
+        return outs_k, outs_i
+
+    def infer_frames_heads_host(self, frames, bboxes, heads):
+        """HOST form of infer_frames_heads (vpb_infer_frames_heads_host, synchronous): numpy frames, per-frame boxes and
+        head indices -> (list of kpts [n_j,K_max,3], list of idx [n_j,K_max]) numpy arrays.  An empty box raises ValueError."""
+        self._ensure()
+        if not (len(frames) == len(bboxes) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
+        boxes = [self._round_boxes(b) for b in bboxes]
+        ents = self._head_entries([len(b) for b in boxes], heads)
+        n = sum(len(sel) for _, sel, _ in ents)
+        bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
+        Km = self.num_keypoints_max
+        kp = np.zeros((n, Km, 3), np.float32)
+        idx = np.zeros((n, Km), np.int32)
+        table = [(frames[j].ctypes.data, frames[j].shape[0], frames[j].shape[1], frames[j].strides[0]) for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks([len(sel) for _, sel, _ in ents], self.batch_limit):
+                arr = _frame_array(table, chunk)
+                ha = np.ascontiguousarray(hv[:len(arr)])
+                _lib.check_value(_lib.lib().vpb_infer_frames_heads_host(
+                    self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), bb[s:].ctypes.data_as(C.c_void_p),
+                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        k_t, i_t = self._per_frame(ents, [len(b) for b in boxes], torch.from_numpy(kp), torch.from_numpy(idx))
+        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+
     def wait_host(self, slot: int) -> None:
         _lib.check(_lib.lib().vpb_wait_host(self._handle, int(slot)))
 
     def kernel_launches(self, batch: int) -> int:
         self._ensure()
         return int(_lib.lib().vpb_kernel_launches(self._handle, batch))
+
+    def cached_graphs(self, mixed: bool = False) -> "tuple[int, int]":
+        """(layouts kept, of which captured) of the engine's CUDA-graph cache: the single-head calls', or with `mixed` the
+        multi-head calls' (vpb_cached_graphs)."""
+        self._ensure()
+        n, c = C.c_int32(0), C.c_int32(0)
+        _lib.check(_lib.lib().vpb_cached_graphs(self._handle, 1 if mixed else 0, C.byref(n), C.byref(c)))
+        return int(n.value), int(c.value)
+
+    def device_bytes(self) -> int:
+        """Device memory the engine holds: packed weights, workspace and staging buffers (vpb_device_bytes)."""
+        self._ensure()
+        return int(_lib.lib().vpb_device_bytes(self._handle))
 
     def set_option(self, name: str, value: int) -> None:
         self._ensure()

@@ -223,8 +223,54 @@ int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frame
 int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* h_mats, const float* h_cs,
                           float* h_kpts, int32_t* h_idx, void* stream);
 
+/* ---- several keypoint heads (datasets) on one backbone: ViTPose+ (model_split.py) and frozen-backbone fine-tunes
+ * (train.py --freeze-backbone).  vpb_create_heads makes an engine with num_heads heads of h_keypoints[j] keypoints each
+ * (1 <= num_heads <= VPB_MAX_HEADS, 1..144 keypoints; cfg->num_keypoints is ignored) and an expert width P = expert_rows:
+ *   P = 0              every head shares the whole backbone (frozen-backbone fine-tunes);
+ *   0 < P < D, P % 32  each block's fc2 is a shared part [D-P, 4D] writing columns [0, D-P) plus, per head j, an expert
+ *                      [P, 4D] writing columns [D-P, D) -- head j always uses expert j, the pairing model_split.py makes.
+ * Any other P returns VPB_ERR_ARG.  The weights load under ViTPose+ key names, so an unsplit ViTPose+ state_dict loads as is:
+ * backbone.blocks.{i}.mlp.fc2.{weight,bias} is the shared part, backbone.blocks.{i}.mlp.experts.{j}.{weight,bias} expert j,
+ * keypoint_head.* head 0 and associate_keypoint_heads.{j-1}.* head j >= 1; loading is strict as for vpb_create.  Crops of head j
+ * give bit-identical results to a single-head engine loaded with model_split.py's checkpoint j.  vpb_create is the
+ * num_heads = 1, P = 0 engine.  On a multi-head engine the single-head calls (vpb_infer, vpb_forward, vpb_infer_frames, ...)
+ * run every crop through head 0 and return K_0 keypoints per crop, with the single-head launches.  A multi-head call whose
+ * crops all use head 0 issues the single-head backbone launches too (head 0's fc2 is the first D rows of the stacked weight);
+ * any other call on an engine with P > 0, a single segment of head j != 0 included, runs each block's fc2 as two launches
+ * (shared columns, then the grouped expert GEMM), and with option "ln_fused" the LayerNorm after fc2 as a launch of its own; vpb_set_flip_test returns VPB_ERR_STATE (the reference
+ * defines flip pairs for COCO only), and the multi-head calls below return VPB_ERR_STATE while flip test is on. */
+#define VPB_MAX_HEADS 8
+#define VPB_MAX_SEGMENTS 64
+int vpb_create_heads(const vpb_config* cfg, int32_t num_heads, const int32_t* h_keypoints, int32_t expert_rows, vpb_engine** out);
+/* A run of `count` consecutive crops of head `head`. */
+typedef struct vpb_segment {
+  int32_t head, count;
+} vpb_segment;
+/* Mixed batch: the n crops (n = the sum of the counts, <= max_batch) are the segments h_segs[0 .. num_segs-1] in order (HOST
+ * array, num_segs <= VPB_MAX_SEGMENTS; counts of 0 are allowed).  d_crops f32 [n,3,256,192], d_org_wh i32 [n,2] as for vpb_infer;
+ * d_kpts f32 [n,K_max,3], d_idx i32 [n,K_max] or NULL, d_heatmaps f32 [n,K_max,64,48] or NULL, K_max = the largest head's K:
+ * crop c of head j fills rows / maps 0 .. K_j-1; rows and maps at or beyond K_j are not written.  One backbone pass for all
+ * crops (the fc2 expert columns of every segment in one grouped launch), then each segment's head and decode.  Cached CUDA
+ * graph per segment list (at most 16, least recently used out first; a list runs eagerly on its first use).
+ * VPB_ERR_ARG: a head index out of range, a negative count, more than VPB_MAX_SEGMENTS segments, n above max_batch. */
+int vpb_infer_heads(vpb_engine* e, const float* d_crops, const int32_t* d_org_wh, const vpb_segment* h_segs, int32_t num_segs,
+                    float* d_kpts, int32_t* d_idx, float* d_heatmaps, void* stream);
+/* vpb_infer_frames with a head per frame entry: h_heads i32 [num_frames] (HOST) is the head of every box of that entry (a
+ * frame may appear once per head); the segments are the runs of equal head over the entries that have boxes.  Outputs as
+ * vpb_infer_heads; the errors of vpb_infer_frames plus a head index out of range.  The _host form stages frames and boxes on
+ * slot 0 as vpb_infer_frames_host does and is synchronous. */
+int vpb_infer_frames_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads, const int32_t* d_bboxes,
+                           float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
+/* The engine's cached CUDA graphs: mixed = 0 the single-head calls' (one per batch size and decode kind), 1 the multi-head
+ * calls' (one per segment list, at most 16).  *entries = layouts seen and kept, *captured = those with a captured graph. */
+int vpb_cached_graphs(const vpb_engine* e, int32_t mixed, int32_t* entries, int32_t* captured);
+/* Device bytes the engine holds: packed weights, workspace, staging buffers. */
+int64_t vpb_device_bytes(const vpb_engine* e);
 /* Options (all keep the results bit-identical unless noted): "stop_after", "profile", "pdl", "graph", "ln_fused",
  * "chain" (chained persistent launches, default 0: measured slower on H100), "chain_min_batch" (smallest batch that takes them, default 1),
  * "ln_in_gemm" (LayerNorm + its consumer GEMM as one launch on the unchained path, default 0), "gelu_erf" (fc1 epilogue with
