@@ -9,6 +9,6 @@ model.ViTPose, top_down_eval.keypoints_from_heatmaps, inference.install / B200Po
 from . import distributed  # noqa: F401
 from .configs import COCO_FLIP_PAIRS, VITPOSE_PLUS_HEADS, data_cfg, dyn_model_import, flip_pairs_for, model_cfg  # noqa: F401
 from .inference import B200PoseBackend, install  # noqa: F401
-from .model import ViTPose, merge_split_state_dicts, split_vitpose_plus  # noqa: F401
+from .model import ViTPose, head_flip_permutations, merge_split_state_dicts, plan_head_calls, split_vitpose_plus  # noqa: F401
 from .top_down_eval import decode_heatmaps, decode_topdown, keypoints_from_heatmaps  # noqa: F401
 from .topdown import topdown_args  # noqa: F401

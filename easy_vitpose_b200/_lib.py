@@ -77,6 +77,10 @@ EXPORTS = {
                                          C.c_void_p]),
     "vpb_infer_frames_heads_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine_heads": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine_heads_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_host_alloc": (C.c_void_p, [C.c_int64]),
     "vpb_host_free": (None, [C.c_void_p]),
     "vpb_kernel_launches": (C.c_int, [C.c_void_p, C.c_int32]),
@@ -84,6 +88,7 @@ EXPORTS = {
     "vpb_device_bytes": (C.c_int64, [C.c_void_p]),
     "vpb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int32]),
     "vpb_set_flip_test": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]),
+    "vpb_set_flip_test_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]),
     "vpb_profile_classes": (C.c_int, []),
     "vpb_profile_class_name": (C.c_char_p, [C.c_int32]),
     "vpb_profile_collect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

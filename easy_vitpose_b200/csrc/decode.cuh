@@ -76,7 +76,8 @@ struct DecodeParams {
   int n, k;
   int wrap_batch;          // sentinel quirk: 0 = previous map wraps inside the crop, 1 = inside the whole call
   // maps / keypoint rows between consecutive crops in heatmaps, kpts and idx (0 = k): a multi-head call decodes each
-  // segment's K_head maps out of crops laid out K_max apart (wrap_batch 0 only)
+  // segment's K_head maps out of crops laid out K_max apart.  With wrap_batch = 1 the "previous map" is taken over the
+  // compact n * k maps of the call (one reference call on the segment's own [n, K_head] array), read at its strided slot.
   int kstride = 0;
   // general transform_preds (post_transforms.py:150-194) for callers other than VitInference.postprocess: per crop
   // (centre_x, centre_y, scale_x, scale_y) either as float32 (numpy keeps the whole expression in float32) or as float64
@@ -174,8 +175,9 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_heatmaps(const Decod
   } else {
     // (-1,-1): four reads land on this map's top-left pad corner (= l(0,0)); the three "minus" reads
     // underflow into the previous map's padded slab: l_prev(W-1,H-1) twice and l_prev(0,H-1).
-    const int n_i = g0 / p.k, k_i = g0 % p.k;
-    const int prev = p.wrap_batch ? (g0 + total - 1) % total : n_i * (p.kstride ? p.kstride : p.k) + (k_i + p.k - 1) % p.k;
+    const int n_i = g0 / p.k, k_i = g0 % p.k, ks = p.kstride ? p.kstride : p.k;
+    const int pc = (g0 + total - 1) % total;                // wrap_batch: the previous compact map of the whole call
+    const int prev = p.wrap_batch ? (pc / p.k) * ks + pc % p.k : n_i * ks + (k_i + p.k - 1) % p.k;
     const float* hp = p.heatmaps + static_cast<size_t>(prev) * HM_PIX;
 #pragma unroll
     for (int i = 0; i < 4; ++i) { pmap[i] = hm; ptx[i] = 0; pty[i] = 0; }

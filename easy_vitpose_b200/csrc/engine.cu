@@ -419,7 +419,8 @@ struct vpb_engine {
   struct GraphEntry { int batch; int seen; cudaGraphExec_t exec; bool affine; };
   std::vector<GraphEntry> graphs;
   // multi-head calls: one graph per segment list (heads and counts), at most kMaxMixedGraphs, least recently used out first
-  struct MixedGraph { std::vector<Segment> segs; cudaGraphExec_t exec; unsigned long long used; };
+  // affine = the graph decodes with centre / scale (vpb_infer_affine_heads)
+  struct MixedGraph { std::vector<Segment> segs; bool affine; cudaGraphExec_t exec; unsigned long long used; };
   std::vector<MixedGraph> mixed_graphs;
   unsigned long long mixed_clock = 0;
   bool use_graph = true;
@@ -443,8 +444,10 @@ struct vpb_engine {
   size_t frame_cap[2] = {0, 0};
   int32_t* bbox_stage[2] = {nullptr, nullptr};
   // flip test (vpb_set_flip_test): the keypoint entry points run each crop and its mirror image as one batch of 2n crops and
-  // decode the averaged maps; flip_perm = the keypoint permutation of the flip pairs, flip_shift = shift_heatmap
-  bool flip = false;
+  // decode the averaged maps; flip_perm = the keypoint permutation of the flip pairs, flip_shift = shift_heatmap.
+  // flip_heads: set by vpb_set_flip_test_heads, flip_perm then holds every head's permutation in head order (head j's at
+  // perm_offset(e, j)) and the multi-head calls run the flip test too
+  bool flip = false, flip_heads = false;
   int flip_shift = 0;
   int32_t* flip_perm = nullptr;
   std::map<std::string, std::pair<float*, int64_t>> staged;   // fp32 state_dict tensors on device until finalize
@@ -805,7 +808,11 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(dev_alloc(e, &e->pp_status, 1));
   CU_TRY(cudaMemset(e->pp_status, 0, sizeof(int32_t)));
   for (int s = 0; s < 2; ++s) VPB_TRY(dev_alloc(e, &e->bbox_stage[s], B * 4));
-  VPB_TRY(dev_alloc(e, &e->flip_perm, e->K));
+  {
+    int ksum = 0;
+    for (const HeadW& h : e->hw) ksum += h.K;
+    VPB_TRY(dev_alloc(e, &e->flip_perm, ksum));        // every head's permutation (vpb_set_flip_test_heads)
+  }
   CU_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
   CU_TRY(cudaStreamCreateWithFlags(&e->compute_stream, cudaStreamNonBlocking));
   VPB_TRY(make_map(&e->m_patch_rows, e->patch_rows, M, 768, 768, 128));
@@ -1466,14 +1473,20 @@ extern "C" int vpb_decode_frame(const float* d_heatmaps, int32_t n, int32_t k, c
 // Crops one keypoint call runs through the model: the batch, and with flip test on its mirror images as well.
 static int model_crops(const vpb_engine* e, int batch) { return e->flip ? 2 * batch : batch; }
 
-// Flip test: e->heat holds the 2 * batch raw maps of one forward; `out` (batch maps; may be e->heat) gets their flip-back average.
-static int flip_average(vpb_engine* e, int batch, float* out, cudaStream_t st) {
-  const long long tot = static_cast<long long>(batch) * e->K * 3072;
+// Flip test: `raw` holds the raw maps of one forward, crop c at raw + c * kstride maps (kstride 0 = k) and its mirror image
+// `mirror` crops later; `out` (same layout; may be `raw`) gets the flip-back average of the first `batch` crops, with head
+// permutation `perm` of k keypoints.
+static int flip_average(vpb_engine* e, const float* raw, int batch, int k, const int* perm, int kstride, int mirror, float* out,
+                        cudaStream_t st) {
+  const long long tot = static_cast<long long>(batch) * k * 3072;
   e->prof.begin(KC_DECODE, st);
-  CU_TRY(launch_k(flip_average_heatmaps, dim3(cdiv(tot, 256)), dim3(256), 0, st, static_cast<const float*>(e->heat), out,
-                  static_cast<const int*>(e->flip_perm), static_cast<int>(batch), e->K, e->flip_shift));
+  CU_TRY(launch_k(flip_average_heatmaps, dim3(cdiv(tot, 256)), dim3(256), 0, st, raw, out, perm, batch, k, e->flip_shift, kstride, mirror));
   e->prof.end(st);
   return VPB_OK;
+}
+// the single-head calls: e->heat holds the 2 * batch raw maps; `out` (batch maps; may be e->heat) gets their average
+static int flip_average(vpb_engine* e, int batch, float* out, cudaStream_t st) {
+  return flip_average(e, e->heat, batch, e->K, e->flip_perm, 0, batch, out, st);
 }
 
 // The decode of a keypoint call: canvas sizes + frame offsets (VitInference.postprocess, one reference call per crop), or for
@@ -1870,7 +1883,7 @@ extern "C" int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, i
 }
 
 // ------------------------------------------------------------------------------------------------ multi-head calls
-static_assert(VPB_MAX_SEGMENTS == EXPERT_MAX_SEGMENTS, "the header's segment limit is the expert GEMM's table size");
+static_assert(2 * VPB_MAX_SEGMENTS <= EXPERT_MAX_SEGMENTS, "a flip-test call's crops and mirror images fit the expert GEMM's table");
 constexpr size_t kMaxMixedGraphs = 16;
 
 static void drop_graphs(vpb_engine* e) {
@@ -1883,8 +1896,15 @@ static void drop_graphs(vpb_engine* e) {
 static int check_ready_heads(vpb_engine* e, const char* fn) {
   if (!e) return fail(VPB_ERR_ARG, "%s: null engine", fn);
   if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
-  if (e->flip) return fail(VPB_ERR_STATE, "%s: the multi-head calls do not run the flip test; switch it off first", fn);
+  if (e->flip && !e->flip_heads)
+    return fail(VPB_ERR_STATE, "%s: flip test was set by vpb_set_flip_test; the multi-head calls take vpb_set_flip_test_heads", fn);
   return VPB_OK;
+}
+// first entry of head j's permutation in flip_perm (the heads' permutations concatenated in head order)
+static int perm_offset(const vpb_engine* e, int j) {
+  int off = 0;
+  for (int i = 0; i < j; ++i) off += e->hw[i].K;
+  return off;
 }
 // appends `count` crops of `head` to the runs (runs of one head merge; empty ones vanish)
 static int add_segment(vpb_engine* e, const char* fn, std::vector<Segment>& segs, int item, int head, int count) {
@@ -1896,27 +1916,49 @@ static int add_segment(vpb_engine* e, const char* fn, std::vector<Segment>& segs
   return VPB_OK;
 }
 
-// Gather (unless done), backbone with the experts of `segs`, then per segment the head's deconvs + 1x1 conv into `heat`
-// (crop c at heat + c * K_max maps) and the per-crop decode of its K_head maps into kpts [n, K_max, 3] / idx [n, K_max].
-// A single segment of head 0 runs the single-head backbone launches.
-static int heads_enqueue(vpb_engine* e, const Source* src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
-                         const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* heat, cudaStream_t st) {
-  const int Km = e->Kmax;
-  if (src) VPB_TRY(gather(e, *src, n, n, st));
-  VPB_TRY(backbone(e, n, st, (segs.size() == 1 && segs[0].head == 0) ? nullptr : &segs));
-  if (e->stop_after && e->stop_after <= 10) return VPB_OK;
-  int c0 = 0;
+// The segments the model runs for a multi-head call: `segs`, and with flip test on `segs` again for the mirror images (the
+// gathers mirror crop b - n into model crop b >= n), runs of one head merged across the seam.
+static std::vector<Segment> model_segments(const vpb_engine* e, const std::vector<Segment>& segs) {
+  std::vector<Segment> out = segs;
+  if (!e->flip) return out;
   for (const Segment& sg : segs) {
-    VPB_TRY(head(e, sg.count, heat + static_cast<size_t>(c0) * Km * 3072, st, sg.head, c0, Km));
+    if (out.back().head == sg.head) out.back().count += sg.count;
+    else out.push_back(sg);
+  }
+  return out;
+}
+
+// Gather (unless done), backbone with the experts of the model segments, then per model segment the head's deconvs + 1x1
+// conv (crop c at c * K_max maps), and per segment the flip-back average (flip test: raw maps in e->heat, average into
+// `heat`) and the decode of its K_head maps into kpts [n, K_max, 3] / idx [n, K_max].  d_cs (affine calls): centre / scale,
+// decode mode 4 as one reference call per segment; else canvas sizes + offsets, one reference call per crop.  A call whose
+// model crops all use head 0 runs the single-head backbone launches.
+static int heads_enqueue(vpb_engine* e, const Source* src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
+                         const int32_t* d_offs_yx, const float* d_cs, float* d_kpts, int32_t* d_idx, float* heat, cudaStream_t st) {
+  const int Km = e->Kmax;
+  const std::vector<Segment> msegs = model_segments(e, segs);
+  const int nb = model_crops(e, n);
+  if (src) VPB_TRY(gather(e, *src, n, nb, st));
+  VPB_TRY(backbone(e, nb, st, (msegs.size() == 1 && msegs[0].head == 0) ? nullptr : &msegs));
+  if (e->stop_after && e->stop_after <= 10) return VPB_OK;
+  float* raw = e->flip ? e->heat : heat;
+  int c0 = 0;
+  for (const Segment& sg : msegs) {
+    VPB_TRY(head(e, sg.count, raw + static_cast<size_t>(c0) * Km * 3072, st, sg.head, c0, Km));
     c0 += sg.count;
   }
   if (e->stop_after) return VPB_OK;
   c0 = 0;
   for (const Segment& sg : segs) {
+    const size_t m0 = static_cast<size_t>(c0) * Km * 3072;
+    const int K = e->hw[sg.head].K;
+    if (e->flip) VPB_TRY(flip_average(e, raw + m0, sg.count, K, e->flip_perm + perm_offset(e, sg.head), Km, n, heat + m0, st));
     DecodeParams p;
-    p.heatmaps = heat + static_cast<size_t>(c0) * Km * 3072; p.org_wh = d_org_wh + 2 * c0; p.offs_yx = d_offs_yx ? d_offs_yx + 2 * c0 : nullptr;
+    p.heatmaps = heat + m0; p.org_wh = d_cs ? nullptr : d_org_wh + 2 * c0; p.offs_yx = (d_offs_yx && !d_cs) ? d_offs_yx + 2 * c0 : nullptr;
     p.kpts = d_kpts + static_cast<size_t>(c0) * Km * 3; p.idx = d_idx ? d_idx + static_cast<size_t>(c0) * Km : nullptr;
-    p.n = sg.count; p.k = e->hw[sg.head].K; p.kstride = Km; p.wrap_batch = 0;
+    p.n = sg.count; p.k = K; p.kstride = Km;
+    p.wrap_batch = d_cs ? 1 : 0;                            // mode 4: keypoints_from_heatmaps on the segment's array
+    p.cs32 = d_cs ? d_cs + 4 * c0 : nullptr;
     e->prof.begin(KC_DECODE, st);
     CU_TRY(launch_k(decode_heatmaps<false>, dim3(cdiv(static_cast<long long>(p.n) * p.k, DECODE_WARPS)), dim3(DECODE_WARPS * 32), 0, st, p));
     e->prof.end(st);
@@ -1938,34 +1980,40 @@ static int copy_head_rows(const vpb_engine* e, const std::vector<Segment>& segs,
   return VPB_OK;
 }
 
-// Graph replay as infer_core_locked, keyed by the segment list: eager on a list's first use, captured on its second.
+// Graph replay as infer_core_locked, keyed by the segment list and the decode kind: eager on a key's first use, captured on
+// its second.  The affine graphs decode with the centre / scale copied to e->g_cs.
 static int heads_core_locked(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
                              const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
   float* heat = d_heatmaps ? d_heatmaps : e->heat;
   if (!e->use_graph || e->prof.on || e->stop_after || st == nullptr || stream_is_capturing(st))
-    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, heat, st);
+    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, heat, st);
+  const bool affine = src.cs != nullptr;
   vpb_engine::MixedGraph* g = nullptr;
   for (auto& c : e->mixed_graphs)
-    if (c.segs == segs) g = &c;
-  if (!g) {                                                               // first use of this list: run eagerly
+    if (c.segs == segs && c.affine == affine) g = &c;
+  if (!g) {                                                               // first use of this key: run eagerly
     if (e->mixed_graphs.size() == kMaxMixedGraphs) {
       auto lru = std::min_element(e->mixed_graphs.begin(), e->mixed_graphs.end(),
                                   [](const vpb_engine::MixedGraph& a, const vpb_engine::MixedGraph& b) { return a.used < b.used; });
       if (lru->exec) cudaGraphExecDestroy(lru->exec);
       e->mixed_graphs.erase(lru);
     }
-    e->mixed_graphs.push_back({segs, nullptr, ++e->mixed_clock});
-    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, heat, st);
+    e->mixed_graphs.push_back({segs, affine, nullptr, ++e->mixed_clock});
+    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, heat, st);
   }
   g->used = ++e->mixed_clock;
-  VPB_TRY(gather(e, src, n, n, st));
-  CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(n) * 2 * sizeof(int32_t), st));
+  VPB_TRY(gather(e, src, n, model_crops(e, n), st));
+  if (affine) {
+    CU_TRY(cudaMemcpyAsync(e->g_cs, src.cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  } else {
+    CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(n) * 2 * sizeof(int32_t), st));
+  }
   if (!g->exec) {
     cudaGraph_t graph = nullptr;
     CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int rc = heads_enqueue(e, nullptr, segs, n, e->g_org, e->g_offs, e->g_kpts, e->g_idx, e->heat, st);
+    const int rc = heads_enqueue(e, nullptr, segs, n, e->g_org, e->g_offs, affine ? e->g_cs : nullptr, e->g_kpts, e->g_idx, e->heat, st);
     const cudaError_t ce = cudaStreamEndCapture(st, &graph);
     if (rc != VPB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
     if (ce != cudaSuccess) return fail(VPB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
@@ -1983,7 +2031,7 @@ static int heads_core(vpb_engine* e, const Source& src, const std::vector<Segmen
                       const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
   VPB_TRY(apply_l2_policy(e, st));
   WsScope ws(e, st);
-  VPB_TRY(ws.begin(n));
+  VPB_TRY(ws.begin(model_crops(e, n)));
   VPB_TRY(heads_core_locked(e, src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, d_heatmaps, st));
   return ws.end();
 }
@@ -2000,6 +2048,8 @@ extern "C" int vpb_infer_heads(vpb_engine* e, const float* d_crops, const int32_
     n += h_segs[i].count;
   }
   if (n > e->maxB) return fail(VPB_ERR_ARG, "vpb_infer_heads: %lld crops exceed max_batch = %d", n, e->maxB);
+  if (e->flip && 2 * n > e->maxB)
+    return fail(VPB_ERR_ARG, "vpb_infer_heads: %lld crops: with flip test on a call takes at most max_batch / 2 = %d", n, e->maxB / 2);
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!d_crops || !d_org_wh || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_heads: null pointer");
@@ -2052,6 +2102,50 @@ extern "C" int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_fra
   Source src;
   src.frames = tab; src.num_frames = nt; src.bboxes = e->bbox_stage[0];
   VPB_TRY(heads_core(e, src, segs, n, e->pp_org, e->pp_offs, e->kpts[0], e->idx[0], nullptr, st));
+  VPB_TRY(copy_head_rows(e, segs, h_kpts, e->kpts[0], 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_idx) VPB_TRY(copy_head_rows(e, segs, h_idx, e->idx[0], sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU_TRY(cudaEventRecord(e->ev_done[0], st));
+  CU_TRY(cudaStreamSynchronize(st));
+  return VPB_OK;
+}
+
+extern "C" int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                      const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, "vpb_infer_affine_heads"));
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_affine_heads", e, h_frames, num_frames, tab, &nt, &n));
+  std::vector<Segment> segs;
+  VPB_TRY(frame_segments(e, "vpb_infer_affine_heads", h_frames, num_frames, h_heads, &segs));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_heads: null pointer");
+  Source src;
+  src.frames = tab; src.num_frames = nt; src.mats = d_mats; src.cs = d_cs;
+  return heads_core(e, src, segs, n, nullptr, nullptr, d_kpts, d_idx, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                           const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, "vpb_infer_affine_heads_host"));
+  FrameEntry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table("vpb_infer_affine_heads_host", e, h_frames, num_frames, tab, &nt, &n));
+  std::vector<Segment> segs;
+  VPB_TRY(frame_segments(e, "vpb_infer_affine_heads_host", h_frames, num_frames, h_heads, &segs));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_heads_host: null pointer");
+  VPB_TRY(check_affine_host(h_mats, h_cs, n));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  VPB_TRY(stage_frames_host(e, 0, tab, nt, nullptr, n, st));         // waits for slot 0's last user
+  CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
+  Source src;
+  src.frames = tab; src.num_frames = nt; src.mats = e->mat_stage; src.cs = e->cs_stage;
+  VPB_TRY(heads_core(e, src, segs, n, nullptr, nullptr, e->kpts[0], e->idx[0], nullptr, st));
   VPB_TRY(copy_head_rows(e, segs, h_kpts, e->kpts[0], 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
   if (h_idx) VPB_TRY(copy_head_rows(e, segs, h_idx, e->idx[0], sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CU_TRY(cudaEventRecord(e->ev_done[0], st));
@@ -2181,8 +2275,31 @@ extern "C" int vpb_set_flip_test(vpb_engine* e, const int32_t* h_perm, int32_t k
   if (e->ws_used) CU_TRY(cudaEventSynchronize(e->ev_ws));
   if (h_perm) CU_TRY(cudaMemcpy(e->flip_perm, h_perm, static_cast<size_t>(k) * sizeof(int32_t), cudaMemcpyHostToDevice));
   e->flip = h_perm != nullptr;
+  e->flip_heads = false;
   e->flip_shift = shift ? 1 : 0;
   drop_graphs(e);                     // captured chains embed the batch and the average
+  return VPB_OK;
+}
+
+extern "C" int vpb_set_flip_test_heads(vpb_engine* e, const int32_t* h_perms, int32_t total, int32_t shift) {
+  if (!e) return fail(VPB_ERR_ARG, "vpb_set_flip_test_heads: null engine");
+  if (!e->finalized) return fail(VPB_ERR_STATE, "not finalized");
+  if (h_perms) {
+    const int want = perm_offset(e, e->num_kheads);
+    if (total != want) return fail(VPB_ERR_ARG, "vpb_set_flip_test_heads: %d permutation entries, the heads have %d keypoints in all", total, want);
+    for (int j = 0; j < e->num_kheads; ++j) {
+      const int32_t* p = h_perms + perm_offset(e, j);
+      for (int i = 0; i < e->hw[j].K; ++i)
+        if (p[i] < 0 || p[i] >= e->hw[j].K)
+          return fail(VPB_ERR_ARG, "vpb_set_flip_test_heads: head %d: perm[%d] = %d outside 0..%d", j, i, p[i], e->hw[j].K - 1);
+    }
+  }
+  DeviceGuard dev_guard(e);
+  if (e->ws_used) CU_TRY(cudaEventSynchronize(e->ev_ws));     // pending calls read the old permutations
+  if (h_perms) CU_TRY(cudaMemcpy(e->flip_perm, h_perms, static_cast<size_t>(total) * sizeof(int32_t), cudaMemcpyHostToDevice));
+  e->flip = e->flip_heads = h_perms != nullptr;
+  e->flip_shift = shift ? 1 : 0;
+  drop_graphs(e);
   return VPB_OK;
 }
 

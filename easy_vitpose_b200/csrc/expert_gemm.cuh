@@ -16,7 +16,9 @@
 
 namespace vpb {
 
-constexpr int EXPERT_MAX_SEGMENTS = 64;
+// 128: a flip-test call of VPB_MAX_SEGMENTS segments runs its crops, then their mirror images, as twice that many (2 KB of the
+// 4 KB parameter block)
+constexpr int EXPERT_MAX_SEGMENTS = 128;
 
 struct ExpertSegment {
   int row_begin, row_end;   // token rows of the segment (192 per crop)

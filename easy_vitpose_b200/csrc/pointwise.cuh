@@ -205,21 +205,27 @@ __global__ void flip_back_heatmaps(const float* __restrict__ in, float* __restri
   out[i] = __ldg(in + ((static_cast<size_t>(nn) * k + perm[kk]) * 64 + y) * 48 + (47 - xs));
 }
 
-// Flip-test average over the 2n maps of one forward (maps i < n from the crops, maps n + i from their mirror images):
-//   out[i,k,y,x] = (heat[i,k,y,x] + heat[n+i, perm[k], y, 47 - x']) * 0.5f      (i < n, x' as in flip_back_heatmaps)
-// mmpose's (output + output_flipped) * 0.5 with output_flipped = flip_back_heatmaps of the second half, in the same fp32
-// operations, so bit-identical to that composition.  `out` may be `heat` itself: each output element reads its own position
-// of the first half and the second half, which is never written.
-__global__ void flip_average_heatmaps(const float* heat, float* out, const int* __restrict__ perm, int n, int k, int shift) {
+// Flip-test average over the maps of one forward (maps of crop i < n from the crops, those of crop mirror + i from their mirror
+// images):
+//   out[i,k,y,x] = (heat[i,k,y,x] + heat[mirror+i, perm[k], y, 47 - x']) * 0.5f      (i < n, x' as in flip_back_heatmaps)
+// mmpose's (output + output_flipped) * 0.5 with output_flipped = flip_back_heatmaps of the mirror maps, in the same fp32
+// operations, so bit-identical to that composition.  kstride = maps between consecutive crops in heat and out (0 = k).  The
+// single-head calls pass mirror = n and kstride = 0; a multi-head call launches once per segment, with heat / out at the
+// segment's first crop, its head's k and permutation, kstride = K_max and mirror = the call's crop count.  `out` may be
+// `heat` itself: each output element reads its own position and a mirror position, which is never written.
+__global__ void flip_average_heatmaps(const float* heat, float* out, const int* __restrict__ perm, int n, int k, int shift, int kstride,
+                                      int mirror) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   pdl_launch_dependents();
   pdl_wait();                                               // the 1x1-conv GEMM writes `heat`
   if (i >= static_cast<long long>(n) * k * 3072) return;
   const int x = static_cast<int>(i % 48), y = static_cast<int>((i / 48) % 64);
   const int kk = static_cast<int>((i / 3072) % k), nn = static_cast<int>(i / (3072LL * k));
+  const int ks = kstride ? kstride : k;
   const int xs = shift ? max(x - 1, 0) : x;
-  const float m = heat[((static_cast<size_t>(n + nn) * k + perm[kk]) * 64 + y) * 48 + (47 - xs)];
-  out[i] = __fmul_rn(__fadd_rn(heat[i], m), 0.5f);
+  const size_t o = (static_cast<size_t>(nn) * ks + kk) * 3072 + y * 48 + x;
+  const float m = heat[((static_cast<size_t>(mirror + nn) * ks + perm[kk]) * 64 + y) * 48 + (47 - xs)];
+  out[o] = __fmul_rn(__fadd_rn(heat[o], m), 0.5f);
 }
 
 }  // namespace vpb

@@ -114,6 +114,15 @@ class B200PoseBackend:
         return self.model.infer_affine_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args])[0]
 
     @torch.no_grad()
+    def inference_topdown_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list, padding: float = 1.25,
+                                use_udp: bool = True) -> "list[np.ndarray]":
+        """inference_topdown on a multi-head engine, with a head index per box (heads_list: per frame an int array [n_i]) -> one
+        float32 [n_i,K_max,3] (y, x, score) per frame in image pixels; a box of head j fills rows 0..K_j-1.  Flip test, when set
+        with ViTPose.set_flip_test_heads, applies with each box's head's pairs."""
+        args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
+        return self.model.infer_affine_heads_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list)[0]
+
+    @torch.no_grad()
     def inference_batch(self, imgs: "list[np.ndarray]") -> np.ndarray:
         """All person crops of a frame in one engine call -> float32 [n,K,3]."""
         if not imgs:

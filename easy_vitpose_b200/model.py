@@ -15,7 +15,8 @@ import torch
 from . import _lib
 from .configs import VITPOSE_PLUS_HEADS
 
-__all__ = ["ViTPose", "plan_frame_chunks", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head"]
+__all__ = ["ViTPose", "plan_frame_chunks", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head", "head_flip_permutations",
+           "plan_head_calls"]
 
 IMG_H, IMG_W, HM_H, HM_W = 256, 192, 64, 48
 
@@ -65,6 +66,46 @@ def group_by_head(heads, num_heads: int) -> "tuple[np.ndarray, list[int]]":
         raise ValueError(f"head indices must be integers in 0..{num_heads - 1}")
     h = h.astype(np.int64)
     return np.argsort(h, kind="stable"), [int(c) for c in np.bincount(h, minlength=num_heads)]
+
+
+def head_flip_permutations(head_keypoints, flip_pairs_per_head) -> np.ndarray:
+    """The permutation of every head (ViTPose.flip_permutation of its pairs), concatenated in head order: what
+    vpb_set_flip_test_heads takes.  Raises ValueError when the pair lists do not match the heads or a pair index lies outside
+    its head's 0..K_j-1."""
+    ks = [int(k) for k in head_keypoints]
+    pairs = list(flip_pairs_per_head)
+    if len(pairs) != len(ks):
+        raise ValueError(f"{len(pairs)} flip pair lists for {len(ks)} heads")
+    out = []
+    for j, (K, pp) in enumerate(zip(ks, pairs)):
+        pp = [(int(a), int(b)) for a, b in pp]
+        if any(not 0 <= i < K for pair in pp for i in pair):
+            raise ValueError(f"head {j}: flip pairs {pp} index outside 0..{K - 1}")
+        out += ViTPose.flip_permutation(K, pp)
+    return np.array(out, np.int32)
+
+
+def plan_head_calls(counts, heads, num_heads: int, limit: int, max_frames: int = _lib.MAX_FRAMES):
+    """The boxes of several frames (counts[j] boxes in frame j, heads[j] = their head indices) grouped by head for the
+    multi-head frame / affine calls -> (entries, order, chunks):
+      entries  [(frame, box indices within the frame, head)], head-major, frame order inside a head: a frame appears once
+               per head it uses;
+      order    the flat index (frames concatenated) of each box in call order;
+      chunks   plan_frame_chunks over the entries: calls of at most `limit` boxes from at most `max_frames` entries.
+    The one planner of infer_frames_heads(_host) and infer_affine_heads(_host).  heads[j] may be a list, array or tensor."""
+    if len(counts) != len(heads):
+        raise ValueError(f"{len(counts)} frames but {len(heads)} head arrays")
+    hs = []
+    for j, (c, h) in enumerate(zip(counts, heads)):
+        h = np.asarray(h.cpu() if isinstance(h, torch.Tensor) else h).reshape(-1)
+        if h.size != int(c):
+            raise ValueError(f"{int(c)} boxes but {h.size} head indices in frame {j}")
+        group_by_head(h, num_heads)                         # range check
+        hs.append(h.astype(np.int64))
+    entries = [(j, np.nonzero(h == k)[0], k) for k in range(num_heads) for j, h in enumerate(hs) if (h == k).any()]
+    first = np.concatenate([[0], np.cumsum([int(c) for c in counts])]).astype(np.int64)
+    order = np.concatenate([first[j] + sel for j, sel, _ in entries]) if entries else np.zeros((0,), np.int64)
+    return entries, order, plan_frame_chunks([len(sel) for _, sel, _ in entries], limit, max_frames)
 
 
 def _inverse(order: np.ndarray) -> np.ndarray:
@@ -417,6 +458,24 @@ class ViTPose:
             raise ValueError(f"flip pairs {flip_pairs} index outside 0..{self.num_keypoints - 1}")
         perm = np.array(self.flip_permutation(self.num_keypoints, flip_pairs), np.int32)
         _lib.check_value(_lib.lib().vpb_set_flip_test(self._handle, perm.ctypes.data_as(C.c_void_p), perm.size, 1 if shift_heatmap else 0))
+        self._flip = True
+
+    def set_flip_test_heads(self, flip_pairs_per_head, shift_heatmap: bool = False) -> None:
+        """Flip test on every keypoint call of a multi-head engine (also valid with one head): flip_pairs_per_head holds the
+        (left, right) pairs of every head, in head order (the reference defines pairs for COCO only, so the caller names them
+        for the other datasets; an empty list for a head without pairs).  The multi-head calls (infer_crops_heads,
+        infer_frames_heads(_host), infer_affine_heads(_host)) then average each crop's maps with those of its mirror image
+        under its head's pairs; the single-head calls run head 0 with head 0's pairs.  One shift for all heads.  A call then
+        takes at most max_batch // 2 crops.  `None` turns it off.  Replaces a setting made by set_flip_test, and the other
+        way round.  Synchronises the engine's pending work."""
+        self._ensure()
+        L = _lib.lib()
+        if flip_pairs_per_head is None:
+            _lib.check(L.vpb_set_flip_test_heads(self._handle, None, 0, 0))
+            self._flip = False
+            return
+        perms = head_flip_permutations(self.head_keypoints, flip_pairs_per_head)
+        _lib.check_value(L.vpb_set_flip_test_heads(self._handle, perms.ctypes.data_as(C.c_void_p), perms.size, 1 if shift_heatmap else 0))
         self._flip = True
 
     def _check_input(self, x: torch.Tensor, limit: "int | None" = None) -> torch.Tensor:
@@ -933,11 +992,6 @@ class ViTPose:
         out = (kp.index_select(0, inv), idx.index_select(0, inv))
         return out + (hm.index_select(0, inv),) if return_heatmaps else out
 
-    def _head_entries(self, counts, heads):
-        """Per-frame head indices -> the call's table entries grouped by head (stable): [(frame, box indices, head)]."""
-        hs = [self._head_indices(j, h, c) for j, (c, h) in enumerate(zip(counts, heads))]
-        return [(j, np.nonzero(h == k)[0], k) for k in range(len(self.head_keypoints)) for j, h in enumerate(hs) if (h == k).any()]
-
     def infer_frames_heads(self, frames, bboxes, heads, check: bool = False):
         """infer_frames with a keypoint head per box (heads: per frame an int array [n_j]): the boxes are grouped by head
         (stable; a frame appears once per head it uses) and run through vpb_infer_frames_heads in calls of at most batch_limit
@@ -954,7 +1008,7 @@ class ViTPose:
             if b.is_floating_point():
                 b = b.round()
             boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
-        ents = self._head_entries([b.shape[0] for b in boxes], heads)
+        ents, _, chunks = plan_head_calls([b.shape[0] for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
         n = sum(len(sel) for _, sel, _ in ents)
         bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
         Km = self.num_keypoints_max
@@ -963,7 +1017,7 @@ class ViTPose:
         table = [(frames[j].data_ptr(), frames[j].shape[0], frames[j].shape[1], frames[j].stride(0)) for j, _, _ in ents]
         hv = np.array([k for _, _, k in ents], np.int32)
         s = 0
-        for chunk in plan_frame_chunks([len(sel) for _, sel, _ in ents], self.batch_limit):
+        for chunk in chunks:
             arr = _frame_array(table, chunk)
             ha = np.ascontiguousarray(hv[:len(arr)])
             self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads(
@@ -993,7 +1047,7 @@ class ViTPose:
             raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
         frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
         boxes = [self._round_boxes(b) for b in bboxes]
-        ents = self._head_entries([len(b) for b in boxes], heads)
+        ents, _, chunks = plan_head_calls([len(b) for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
         n = sum(len(sel) for _, sel, _ in ents)
         bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
         Km = self.num_keypoints_max
@@ -1003,7 +1057,7 @@ class ViTPose:
         hv = np.array([k for _, _, k in ents], np.int32)
         s = 0
         with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks([len(sel) for _, sel, _ in ents], self.batch_limit):
+            for chunk in chunks:
                 arr = _frame_array(table, chunk)
                 ha = np.ascontiguousarray(hv[:len(arr)])
                 _lib.check_value(_lib.lib().vpb_infer_frames_heads_host(
@@ -1011,6 +1065,72 @@ class ViTPose:
                     kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
                 s += sum(e - b for _, b, e in chunk)
         k_t, i_t = self._per_frame(ents, [len(b) for b in boxes], torch.from_numpy(kp), torch.from_numpy(idx))
+        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+
+    def infer_affine_heads(self, frames, mats, centers, scales, heads, check: bool = False):
+        """infer_affine with a keypoint head per box (heads: per frame an int array [n_j]): the boxes are grouped by head (stable;
+        a frame appears once per head it uses) and run through vpb_infer_affine_heads in calls of at most batch_limit boxes and
+        64 entries (plan_head_calls).  Each call decodes a segment (a run of one head) as one keypoints_from_heatmaps(c, s,
+        use_udp=True) call.  Returns per frame kpts f32 [n_j,K_max,3] (y, x, score) and idx i32 [n_j,K_max], rows K_j.. of a
+        head-j box zero.  Honours the flip test set by set_flip_test_heads."""
+        self._ensure()
+        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
+                             f"arrays, {len(heads)} head arrays")
+        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        dev = torch.device("cuda", self._device)
+        counts, M, CS = self._affine_args(mats, centers, scales)
+        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        o = torch.as_tensor(order, device=M.device)
+        M, CS = M.index_select(0, o).contiguous().to(dev), CS.index_select(0, o).contiguous().to(dev)
+        n = M.shape[0]
+        Km = self.num_keypoints_max
+        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
+        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
+        table = [(frames[j].data_ptr(), frames[j].shape[0], frames[j].shape[1], frames[j].stride(0)) for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        for chunk in chunks:
+            arr = _frame_array(table, chunk)
+            ha = np.ascontiguousarray(hv[:len(arr)])
+            self._call_on_stream(frames + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_heads(
+                self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 2:
+            raise ValueError("a matrix entry is not finite or a scale is <= 0")
+        return self._per_frame(ents, counts, kp, idx)
+
+    def infer_affine_heads_host(self, frames, mats, centers, scales, heads):
+        """HOST form of infer_affine_heads (vpb_infer_affine_heads_host, synchronous): numpy frames and per-frame matrices /
+        centres / scales / head indices -> (list of kpts [n_j,K_max,3], list of idx [n_j,K_max]) numpy arrays.  A non-finite
+        matrix entry or a scale <= 0 raises ValueError."""
+        self._ensure()
+        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
+                             f"arrays, {len(heads)} head arrays")
+        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
+        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
+        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        M = np.ascontiguousarray(M.cpu().numpy()[order])
+        CS = np.ascontiguousarray(CS.cpu().numpy()[order], np.float32)
+        n = M.shape[0]
+        Km = self.num_keypoints_max
+        kp = np.zeros((n, Km, 3), np.float32)
+        idx = np.zeros((n, Km), np.int32)
+        table = [(frames[j].ctypes.data, frames[j].shape[0], frames[j].shape[1], frames[j].strides[0]) for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in chunks:
+                arr = _frame_array(table, chunk)
+                ha = np.ascontiguousarray(hv[:len(arr)])
+                _lib.check_value(_lib.lib().vpb_infer_affine_heads_host(
+                    self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),
+                    CS[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p),
+                    self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        k_t, i_t = self._per_frame(ents, counts, torch.from_numpy(kp), torch.from_numpy(idx))
         return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
 
     def wait_host(self, slot: int) -> None:

@@ -238,7 +238,8 @@ int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_
  * crops all use head 0 issues the single-head backbone launches too (head 0's fc2 is the first D rows of the stacked weight);
  * any other call on an engine with P > 0, a single segment of head j != 0 included, runs each block's fc2 as two launches
  * (shared columns, then the grouped expert GEMM), and with option "ln_fused" the LayerNorm after fc2 as a launch of its own; vpb_set_flip_test returns VPB_ERR_STATE (the reference
- * defines flip pairs for COCO only), and the multi-head calls below return VPB_ERR_STATE while flip test is on. */
+ * defines flip pairs for COCO only), and the multi-head calls below return VPB_ERR_STATE while flip test set by vpb_set_flip_test is
+ * on.  Flip test on a multi-head engine is set with vpb_set_flip_test_heads, which takes a permutation per head. */
 #define VPB_MAX_HEADS 8
 #define VPB_MAX_SEGMENTS 64
 int vpb_create_heads(const vpb_config* cfg, int32_t num_heads, const int32_t* h_keypoints, int32_t expert_rows, vpb_engine** out);
@@ -263,6 +264,17 @@ int vpb_infer_frames_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num
                            float* d_kpts, int32_t* d_idx, void* stream);
 int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
                                 const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream);
+/* vpb_infer_affine with a head per frame entry (h_heads as for vpb_infer_frames_heads): frames, matrices d_mats f64 [n,6] and
+ * centre / scale d_cs f32 [n,4] as for vpb_infer_affine, in the order of the entries.  Outputs as vpb_infer_heads: d_kpts f32
+ * [n,K_max,3], d_idx i32 [n,K_max] or NULL, rows at or beyond K_j not written.  Each segment is decoded as ONE reference call,
+ * keypoints_from_heatmaps(c, s * 200, use_udp=True) on that segment's [count, K_j] array (the max <= 0 "previous map" included), so a
+ * segment's keypoints equal vpb_infer_affine of a single-head engine on that segment's boxes.  Errors and status bit 1 as for
+ * vpb_infer_affine, plus a head index out of range; graphs cached per (segment list, affine).  The _host form stages frames,
+ * matrices and centre / scale on slot 0 as vpb_infer_affine_host does, is synchronous and rejects what that call rejects. */
+int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads, const double* d_mats,
+                           const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream);
 
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
@@ -292,6 +304,16 @@ int vpb_set_option(vpb_engine* e, const char* name, int32_t value);
  * are unaffected.  SYNCHRONOUS: waits for the engine's pending work (which keeps the previous setting), and drops the
  * engine's cached CUDA graphs. */
 int vpb_set_flip_test(vpb_engine* e, const int32_t* h_perm, int32_t k, int32_t shift);
+/* Flip test for every head of an engine (vpb_create_heads; also valid with one head): h_perms i32 [total] (HOST) = the
+ * permutation of every head, concatenated in head order; total must equal the sum of the heads' K_j and every entry of head j
+ * lie in [0, K_j), else VPB_ERR_ARG.  h_perms = NULL turns flip test off.  One shift for all heads.  While it is on, the
+ * multi-head calls (vpb_infer_heads, vpb_infer_frames_heads, vpb_infer_frames_heads_host, vpb_infer_affine_heads,
+ * vpb_infer_affine_heads_host) run the n crops in segment order followed by their n mirror images (the fc2 expert segments of
+ * those 2n crops are the segment list twice, runs of one head merged), average each segment's maps with its head's permutation
+ * and decode them; the single-head calls run head 0 with head 0's permutation, bit-identical to a head-0 single-head engine with
+ * vpb_set_flip_test.  Every keypoint call then takes at most max_batch / 2 crops.  Synchronous like vpb_set_flip_test, and drops
+ * both graph caches; this call and vpb_set_flip_test each replace the other's setting. */
+int vpb_set_flip_test_heads(vpb_engine* e, const int32_t* h_perms, int32_t total, int32_t shift);
 /* With option "profile"=1 every launch is bracketed by a CUDA-event pair on its stream; collect() synchronises,
  * sums elapsed ms and launch counts per kernel class (arrays of vpb_profile_classes() entries) and resets. */
 int vpb_profile_classes(void);
