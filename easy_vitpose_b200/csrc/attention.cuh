@@ -44,13 +44,104 @@ struct AttnParams {
   long long* dbg;         // debug: per CTA [8] or nullptr: 0 lifetime (cycles), 1 wait for operands (thread 0), 7 items of this CTA
 };
 
+// One item's attention for warpgroup wg (query rows 64 wg .. 64 wg + 63), from Q, K, V in shared memory laid out as the TMA
+// boxes above (sQ, sK, sV: shared addresses of the three operands), into out[b*192 + t, head*hd + d] (row pitch dim).
+// `operands_done` runs once this warpgroup's last MMA on the operands (O = P V) has retired, before the store.  Shared by
+// attention_wgmma and qkv_attention_wgmma (qkv_attention.cuh).
+template <int HD, int NPOLY, typename OperandsDone>
+__device__ __forceinline__ void attend_item(uint32_t sQ, uint32_t sK, uint32_t sV, __nv_bfloat16* out, int dim, int b, int head, int wg,
+                                            int lane, int wq, OperandsDone&& operands_done) {
+  using Cfg = AttCfg<HD>;
+  static_assert(NPOLY == 0 || NPOLY == 8, "NPOLY");
+  constexpr float kLog2e = 1.4426950408889634f;
+  // ---- S = Q K^T for this warpgroup's 64 rows
+  float s[ATT_T / 2];
+  wgmma_fence();
+  {
+    const uint64_t qd = wgmma_desc<Cfg::MAIN_ROW>(sQ + wg * 64 * Cfg::MAIN_ROW), kd = wgmma_desc<Cfg::MAIN_ROW>(sK);
+#pragma unroll
+    for (int k = 0; k < Cfg::MAIN / 16; ++k) wgmma_ss<ATT_T>(s, qd + 2 * k, kd + 2 * k, k != 0);   // +32 B per K = 16 step
+    if constexpr (Cfg::TAIL > 0)
+      wgmma_ss<ATT_T>(s, wgmma_desc<32>(sQ + Cfg::MAIN_BYTES + wg * 64 * 32), wgmma_desc<32>(sK + Cfg::MAIN_BYTES), 1);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+
+  // ---- softmax: thread rows r_lo (h = 0: s[4j], s[4j+1]) and r_lo + 8 (h = 1: s[4j+2], s[4j+3]); a row lives in one quad
+  float sum[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < ATT_T / 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float mscaled = mx * kLog2e;
+    // P is rounded to bf16 here, and the row sum is taken over the ROUNDED weights that O = P V actually uses: the
+    // normalised weights then sum to 1 up to fp32 round-off instead of carrying a per-row scale error of up to 2^-9
+    float sm = 0.0f;
+#pragma unroll
+    for (int j = 0; j < ATT_T / 8; ++j) {
+      const float a1 = fmaf(s[4 * j + 2 * h + 1], kLog2e, -mscaled);
+      const float e0 = __bfloat162float(__float2bfloat16_rn(ex2_approx(fmaf(s[4 * j + 2 * h], kLog2e, -mscaled))));
+      const float e1 = __bfloat162float(__float2bfloat16_rn((NPOLY > 0 && (j & 1) == 0) ? ex2_poly(a1) : ex2_approx(a1)));
+      sm += e0 + e1;
+      s[4 * j + 2 * h] = e0;
+      s[4 * j + 2 * h + 1] = e1;
+    }
+    sm += __shfl_xor_sync(0xffffffffu, sm, 1);
+    sm += __shfl_xor_sync(0xffffffffu, sm, 2);
+    sum[h] = sm;
+  }
+
+  // ---- O = P V: 12 steps of 16 keys; P as bf16 A fragments, V MN-major
+  float o[Cfg::MAIN / 2];
+  [[maybe_unused]] float ot[8];
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < ATT_T / 16; ++kk) {
+    uint32_t a[4];
+    a[0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+    a[1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+    a[2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+    a[3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+    const uint64_t vd = wgmma_desc<Cfg::MAIN_ROW>(sV + kk * 16 * Cfg::MAIN_ROW);
+    if constexpr (Cfg::MAIN == 64) wgmma_rs_n64<1>(o, a, vd, kk != 0);
+    else wgmma_rs_n32<1>(o, a, vd, kk != 0);
+    if constexpr (Cfg::TAIL > 0) wgmma_rs_n16<1>(ot, a, wgmma_desc<32>(sV + Cfg::MAIN_BYTES + kk * 16 * 32), kk != 0);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+  if constexpr (Cfg::TAIL > 0) wgmma_fence_regs(ot);
+
+  operands_done();
+
+  // ---- O / rowsum -> bf16 -> attn_out
+  const int r_lo = wg * 64 + wq * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const float inv = 1.0f / sum[hh];
+    __nv_bfloat16* orow = out + (static_cast<size_t>(b) * ATT_T + r_lo + 8 * hh) * dim + head * HD;
+#pragma unroll
+    for (int j = 0; j < Cfg::MAIN / 8; ++j)
+      *reinterpret_cast<uint32_t*>(orow + 8 * j + cq) = pack_bf16(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+    if constexpr (Cfg::TAIL > 0) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        *reinterpret_cast<uint32_t*>(orow + Cfg::MAIN + 8 * j + cq) = pack_bf16(ot[4 * j + 2 * hh] * inv, ot[4 * j + 2 * hh + 1] * inv);
+    }
+  }
+}
+
 // tmap_main: box [192 rows x MAIN cols] (swizzle = MAIN*2 bytes); tmap_tail: box [192 x 16] (32B swizzle), hd 80 only.
 // NPOLY of every 32 exponentials go through ex2_poly (FMA pipe) instead of the MUFU: 0 (all MUFU) or 8 (every 4th)
 template <int HD, int NPOLY = 0>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_wgmma(const __grid_constant__ CUtensorMap tmap_main, const __grid_constant__ CUtensorMap tmap_tail, const AttnParams p) {
   using Cfg = AttCfg<HD>;
-  static_assert(NPOLY == 0 || NPOLY == 8, "NPOLY");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * Cfg::STAGE_BYTES);    // [2] Q, K, V of a stage landed
@@ -88,7 +179,6 @@ attention_wgmma(const __grid_constant__ CUtensorMap tmap_main, const __grid_cons
     if (static_cast<int>(blockIdx.x + gridDim.x) < items) load_item(blockIdx.x + gridDim.x, 1);
   }
 
-  constexpr float kLog2e = 1.4426950408889634f;
   int li = 0;
   for (int item = blockIdx.x; item < items; item += gridDim.x, ++li) {
     const int q = li & 1;
@@ -97,89 +187,11 @@ attention_wgmma(const __grid_constant__ CUtensorMap tmap_main, const __grid_cons
     if (p.dbg && threadIdx.x == 0) t_wait += clock64() - w0;
     const uint32_t sQ = smem_u32(oper(q, 0)), sK = smem_u32(oper(q, 1)), sV = smem_u32(oper(q, 2));
 
-    // ---- S = Q K^T for this warpgroup's 64 rows
-    float s[ATT_T / 2];
-    wgmma_fence();
-    {
-      const uint64_t qd = wgmma_desc<Cfg::MAIN_ROW>(sQ + wg * 64 * Cfg::MAIN_ROW), kd = wgmma_desc<Cfg::MAIN_ROW>(sK);
-#pragma unroll
-      for (int k = 0; k < Cfg::MAIN / 16; ++k) wgmma_ss<ATT_T>(s, qd + 2 * k, kd + 2 * k, k != 0);   // +32 B per K = 16 step
-      if constexpr (Cfg::TAIL > 0)
-        wgmma_ss<ATT_T>(s, wgmma_desc<32>(sQ + Cfg::MAIN_BYTES + wg * 64 * 32), wgmma_desc<32>(sK + Cfg::MAIN_BYTES), 1);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-
-    // ---- softmax: thread rows r_lo (h = 0: s[4j], s[4j+1]) and r_lo + 8 (h = 1: s[4j+2], s[4j+3]); a row lives in one quad
-    float sum[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < ATT_T / 8; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float mscaled = mx * kLog2e;
-      // P is rounded to bf16 here, and the row sum is taken over the ROUNDED weights that O = P V actually uses: the
-      // normalised weights then sum to 1 up to fp32 round-off instead of carrying a per-row scale error of up to 2^-9
-      float sm = 0.0f;
-#pragma unroll
-      for (int j = 0; j < ATT_T / 8; ++j) {
-        const float a1 = fmaf(s[4 * j + 2 * h + 1], kLog2e, -mscaled);
-        const float e0 = __bfloat162float(__float2bfloat16_rn(ex2_approx(fmaf(s[4 * j + 2 * h], kLog2e, -mscaled))));
-        const float e1 = __bfloat162float(__float2bfloat16_rn((NPOLY > 0 && (j & 1) == 0) ? ex2_poly(a1) : ex2_approx(a1)));
-        sm += e0 + e1;
-        s[4 * j + 2 * h] = e0;
-        s[4 * j + 2 * h + 1] = e1;
-      }
-      sm += __shfl_xor_sync(0xffffffffu, sm, 1);
-      sm += __shfl_xor_sync(0xffffffffu, sm, 2);
-      sum[h] = sm;
-    }
-
-    // ---- O = P V: 12 steps of 16 keys; P as bf16 A fragments, V MN-major
-    float o[Cfg::MAIN / 2];
-    [[maybe_unused]] float ot[8];
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < ATT_T / 16; ++kk) {
-      uint32_t a[4];
-      a[0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
-      a[1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
-      a[2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
-      a[3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
-      const uint64_t vd = wgmma_desc<Cfg::MAIN_ROW>(sV + kk * 16 * Cfg::MAIN_ROW);
-      if constexpr (Cfg::MAIN == 64) wgmma_rs_n64<1>(o, a, vd, kk != 0);
-      else wgmma_rs_n32<1>(o, a, vd, kk != 0);
-      if constexpr (Cfg::TAIL > 0) wgmma_rs_n16<1>(ot, a, wgmma_desc<32>(sV + Cfg::MAIN_BYTES + kk * 16 * 32), kk != 0);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(o);
-    if constexpr (Cfg::TAIL > 0) wgmma_fence_regs(ot);
-
-    // ---- every warpgroup is done with this stage's operands: thread 0 refills it with the item after next
-    __syncthreads();
-    if (threadIdx.x == 0 && item + 2 * static_cast<int>(gridDim.x) < items) load_item(item + 2 * gridDim.x, q);
-
-    // ---- O / rowsum -> bf16 -> attn_out
-    const int b = item / p.heads, h = item % p.heads;
-    const int r_lo = wg * 64 + wq * 16 + (lane >> 2);
-    const int cq = 2 * (lane & 3);
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const float inv = 1.0f / sum[hh];
-      __nv_bfloat16* orow = p.out + (static_cast<size_t>(b) * ATT_T + r_lo + 8 * hh) * p.dim + h * HD;
-#pragma unroll
-      for (int j = 0; j < Cfg::MAIN / 8; ++j)
-        *reinterpret_cast<uint32_t*>(orow + 8 * j + cq) = pack_bf16(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
-      if constexpr (Cfg::TAIL > 0) {
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-          *reinterpret_cast<uint32_t*>(orow + Cfg::MAIN + 8 * j + cq) = pack_bf16(ot[4 * j + 2 * hh] * inv, ot[4 * j + 2 * hh + 1] * inv);
-      }
-    }
+    attend_item<HD, NPOLY>(sQ, sK, sV, p.out, p.dim, item / p.heads, item % p.heads, wg, lane, wq, [&] {
+      // every warpgroup is done with this stage's operands: thread 0 refills it with the item after next
+      __syncthreads();
+      if (threadIdx.x == 0 && item + 2 * static_cast<int>(gridDim.x) < items) load_item(item + 2 * gridDim.x, q);
+    });
   }
   if (p.dbg && threadIdx.x == 0) { p.dbg[blockIdx.x * 8 + 0] = clock64() - t_cta0; p.dbg[blockIdx.x * 8 + 1] = t_wait; p.dbg[blockIdx.x * 8 + 7] = li; }
 }

@@ -25,6 +25,7 @@
 #include "gemm.cuh"
 #include "pointwise.cuh"
 #include "preprocess.cuh"
+#include "qkv_attention.cuh"
 
 using namespace vpb;
 
@@ -244,6 +245,12 @@ static int device_check(int device) {
   CU_TRY(cudaFuncSetAttribute(attention_wgmma<32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<32>::SMEM));
   CU_TRY(cudaFuncSetAttribute(attention_wgmma<64, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<64>::SMEM));
   CU_TRY(cudaFuncSetAttribute(attention_wgmma<80, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttCfg<80>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(qkv_attention_wgmma<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg<32>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(qkv_attention_wgmma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg<64>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(qkv_attention_wgmma<80>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg<80>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(qkv_attention_wgmma<32, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg<32>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(qkv_attention_wgmma<64, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg<64>::SMEM));
+  CU_TRY(cudaFuncSetAttribute(qkv_attention_wgmma<80, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvAttCfg<80>::SMEM));
   ds->attn_attr = true;
   ds->sms = prop.multiProcessorCount;
   return VPB_OK;
@@ -295,13 +302,18 @@ static int chain_launch(int bn, const ChainMaps& maps, const ChainParams& p, cud
 //         of the MUFU.  Default OFF; VPB_ATT_POLY=1 switches it on.
 static int g_att_poly = [] { const char* e = getenv("VPB_ATT_POLY"); return (e && e[0] == '1') ? 1 : 0; }();
 static const int g_att_poly_env = g_att_poly;
-static int g_att_grid_cap = 0;      // tests: launch the attention kernel with at most this many CTAs (0 = one per SM)
-// flags < 0: back to the defaults (environment); else bit 0 = poly, bits 8.. = grid cap (how a device with fewer SMs would split
-// the items)
+static int g_att_grid_cap = 0;      // tests: launch the attention kernels with at most this many CTAs (0 = one per SM)
+static int g_att_form = 0;          // tests / A/B: 0 = fuse qkv + attention by the rule (fuse_qkv_attention), 1 = always, 2 = never
+// flags < 0: back to the defaults (environment); else bit 0 = poly, bit 1 = force the fused qkv + attention launch, bit 2 = force
+// the qkv GEMM + attention pair, bits 8.. = grid cap (how a device with fewer SMs would split the items)
 extern "C" int vpb_debug_attention(int32_t flags) {
-  if (flags < 0) { g_att_poly = g_att_poly_env; g_att_grid_cap = 0; }
-  else { g_att_poly = (flags & 1) ? 1 : 0; g_att_grid_cap = flags >> 8; }
+  if (flags < 0) { g_att_poly = g_att_poly_env; g_att_grid_cap = 0; g_att_form = 0; }
+  else { g_att_poly = (flags & 1) ? 1 : 0; g_att_grid_cap = flags >> 8; g_att_form = (flags & 2) ? 1 : (flags & 4) ? 2 : 0; }
   return VPB_OK;
+}
+static int att_grid(int items) {
+  const int sms = (g_att_grid_cap > 0 && g_att_grid_cap < num_sms()) ? g_att_grid_cap : num_sms();
+  return items < sms ? items : sms;              // one CTA per SM (the operand stages fill the shared memory)
 }
 
 // qkv bf16 [rows, 3*D]: main operand boxes [192 x 64] (128B swizzle) or [192 x 32] (64B swizzle, head_dim 32), plus a
@@ -313,9 +325,7 @@ static int make_attn_maps(CUtensorMap* main, CUtensorMap* tail, const void* qkv,
   return VPB_OK;
 }
 static int attention_launch(int hd, const CUtensorMap& main, const CUtensorMap& tail, const AttnParams& ap, cudaStream_t st) {
-  const int items = ap.batch * ap.heads;
-  const int sms = (g_att_grid_cap > 0 && g_att_grid_cap < num_sms()) ? g_att_grid_cap : num_sms();
-  const dim3 grid(items < sms ? items : sms);      // one CTA per SM (two stages of Q, K, V fill the shared memory)
+  const dim3 grid(att_grid(ap.batch * ap.heads));
   cudaError_t err;
   if (g_att_poly) {
     switch (hd) {
@@ -333,6 +343,29 @@ static int attention_launch(int hd, const CUtensorMap& main, const CUtensorMap& 
     }
   }
   if (err != cudaSuccess) return fail(VPB_ERR_CUDA, "attention launch: %s", cudaGetErrorString(err));
+  return VPB_OK;
+}
+// qkv GEMM + attention as one launch (qkv_attention.cuh).  tx: xn in boxes of [192 x 64]; tw: the packed qkv weight in boxes of
+// [head_dim x 64]
+static int qkv_attention_launch(int hd, const CUtensorMap& tx, const CUtensorMap& tw, const QkvAttnParams& qp, cudaStream_t st) {
+  const dim3 grid(att_grid(qp.batch * qp.heads));
+  cudaError_t err;
+  if (g_att_poly) {
+    switch (hd) {
+      case 32: err = launch_k(qkv_attention_wgmma<32, 8>, grid, dim3(ATT_THREADS), QkvAttCfg<32>::SMEM, st, tx, tw, qp); break;
+      case 64: err = launch_k(qkv_attention_wgmma<64, 8>, grid, dim3(ATT_THREADS), QkvAttCfg<64>::SMEM, st, tx, tw, qp); break;
+      case 80: err = launch_k(qkv_attention_wgmma<80, 8>, grid, dim3(ATT_THREADS), QkvAttCfg<80>::SMEM, st, tx, tw, qp); break;
+      default: return fail(VPB_ERR_ARG, "qkv attention: head_dim %d not built (32, 64, 80)", hd);
+    }
+  } else {
+    switch (hd) {
+      case 32: err = launch_k(qkv_attention_wgmma<32>, grid, dim3(ATT_THREADS), QkvAttCfg<32>::SMEM, st, tx, tw, qp); break;
+      case 64: err = launch_k(qkv_attention_wgmma<64>, grid, dim3(ATT_THREADS), QkvAttCfg<64>::SMEM, st, tx, tw, qp); break;
+      case 80: err = launch_k(qkv_attention_wgmma<80>, grid, dim3(ATT_THREADS), QkvAttCfg<80>::SMEM, st, tx, tw, qp); break;
+      default: return fail(VPB_ERR_ARG, "qkv attention: head_dim %d not built (32, 64, 80)", hd);
+    }
+  }
+  if (err != cudaSuccess) return fail(VPB_ERR_CUDA, "qkv attention launch: %s", cudaGetErrorString(err));
   return VPB_OK;
 }
 
@@ -392,6 +425,7 @@ struct BlockW {
   // D-P rows: TMA zero-fills the rest of a tile), m_exp = the whole stack in boxes of expert_bn rows.
   LinearW qkv, proj, fc1, fc2, fc2s;
   CUtensorMap m_exp;
+  CUtensorMap m_qkv_head;       // qkv W in boxes of head_dim rows: the fused qkv + attention launch
 };
 // One keypoint head: TopdownHeatmapSimpleHead weights (keypoint_head.* for head 0, associate_keypoint_heads.{j-1}.* for head j)
 struct HeadW {
@@ -498,6 +532,7 @@ struct vpb_engine {
   cudaStream_t ws_last = nullptr;
   bool ws_used = false;
   CUtensorMap m_patch_rows, m_xn, m_attn, m_hid, m_d2, m_qkv_att, m_qkv_att_tail;   // A operands / attention boxes
+  CUtensorMap m_xn_att;                                                 // xn in boxes of one crop's 192 rows (fused qkv + attention)
   CUtensorMap m_feat_nhwc, m_d1_nhwc;                                 // implicit-GEMM deconv inputs (4-D)
   CUtensorMap o_qkv, o_hid, o_x;                                                             // TMA-epilogue outputs
   CUtensorMap o_xs;                             // x bounded to the shared columns [0, D-P) (multi-head fc2)
@@ -738,6 +773,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
     VPB_TRY(copy_vec(e, &b.ln2_g, p + "norm2.weight")); VPB_TRY(copy_vec(e, &b.ln2_b, p + "norm2.bias"));
     // q rows (first D) carry head_dim^-0.5: vit.py:170 scales q before QK^T; fp32 multiply, then bf16 rounding
     VPB_TRY(pack_linear(e, b.qkv, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, 128, D, qscale));
+    VPB_TRY(make_map(&b.m_qkv_head, b.qkv.w, 3 * D, D, D, D / e->heads));
     VPB_TRY(pack_linear(e, b.proj, p + "attn.proj.weight", p + "attn.proj.bias", D, D, 128, 0, 1.f));
     VPB_TRY(pack_linear(e, b.fc1, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, 128, 0, 1.f));
     if (e->P == 0) VPB_TRY(pack_linear(e, b.fc2, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 128, 0, 1.f));
@@ -817,6 +853,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   CU_TRY(cudaStreamCreateWithFlags(&e->compute_stream, cudaStreamNonBlocking));
   VPB_TRY(make_map(&e->m_patch_rows, e->patch_rows, M, 768, 768, 128));
   VPB_TRY(make_map(&e->m_xn, e->xn, M, D, D, 128));
+  VPB_TRY(make_map(&e->m_xn_att, e->xn, M, D, D, 192));
   VPB_TRY(make_map(&e->m_attn, e->attn, M, D, D, 128));
   VPB_TRY(make_map(&e->m_hid, e->hid, M, 4 * D, 4 * D, 128));
   VPB_TRY(make_map_nhwc(&e->m_feat_nhwc, e->xn, B, 16, 12, D, 8, 12));   // 8 x 12 = 96 positions per M tile (12 is not a multiple of 8)
@@ -1068,6 +1105,28 @@ static int fc2_experts(vpb_engine* e, const BlockW& b, int M, const std::vector<
   return VPB_OK;
 }
 
+// Whether the unchained backbone runs each block's qkv GEMM and attention as ONE launch (qkv_attention.cuh) at B model crops:
+// head_dim 64 (ViT-B, ViT-L) with at least two items (crop, head) per SM.  The fused launch has B * heads items, one CTA per SM
+// at most, where the standalone qkv GEMM spreads 128 x BN tiles over every SM, so small batches stay with the two launches.
+// Measured on an H100 80GB HBM3 (700 W power limit), ms per keypoint call with its CUDA graph, separate / fused
+// (tools/qkv_attention_ab.py, median of 3):
+//   ViT-B   1 crop 0.85 / 0.91, 2: 0.85 / 0.90, 4: 1.02 / 0.98, 8: 1.46 / 1.31, 11: 1.74 / 1.52, 16: 2.19 / 2.01, 32: 4.06 / 3.50,
+//           64: 6.09 / 5.76
+//   ViT-L   1 crop 1.77 / 1.95, 2: 1.85 / 2.01, 4: 2.39 / 2.22, 8: 3.46 / 2.99, 16: 5.58 / 5.20, 32: 10.11 / 9.65, 64: 18.21 / 17.31
+//   ViT-S   0.96 to 1.04 of the separate time from 1 to 64 crops, within the run-to-run spread: no gain, so head_dim 32 stays unfused
+//   ViT-H   slower fused at every batch (1 crop 2.78 / 3.67, 16: 9.80 / 9.85, 64: 36.2 / 37.7): at head_dim 80 the shared memory
+//           leaves two ring stages, too few to keep the MMAs fed, so head_dim 80 stays unfused
+// With the threshold at one item per SM (ViT-B 11 crops), bench.py --config ap10k-streams (16 calls of Poisson(10) ViT-B crops per
+// step) ran 18.16 ms per step against 17.92 with every call unfused (two runs each, alternating), although the calls timed alone
+// favour fusing from 4 crops up; at two items per SM (ViT-B 22 crops, ViT-L 17) those ragged calls keep the two launches and
+// b17x64 / l25x64 fuse.  The ln_in_gemm mini-chains and stop_after keep the two launches.  Bit-identical either way
+// (tests/test_gpu_qkv_attention.py); vpb_debug_attention can force either form.
+static bool fuse_qkv_attention(const vpb_engine* e, int B) {
+  if ((e->ln_in_gemm && !e->ln_fused) || e->stop_after) return false;
+  if (g_att_form) return g_att_form == 1;
+  return e->D / e->heads == 64 && B * e->heads >= 2 * num_sms();
+}
+
 // everything after the patch gather, up to last_norm.  `segs` (a multi-head call): the heads of the crops, in runs
 static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Segment>* segs = nullptr) {
   const int D = e->D, M = B * 192;
@@ -1093,6 +1152,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Seg
   // LayerNorm(x; g, b) -> xn followed by xn * W^T + bias (epilogue epi) as one chained launch: one LayerNorm stage whose source
   // rows are already complete (target 0) and one GEMM phase that waits for the normalised rows of its tile
   const bool mini = e->ln_in_gemm && !ln_fused && !stop;
+  const bool fused = fuse_qkv_attention(e, B);
   const size_t nblk = e->chain_blocks;
   if (mini) CU_TRY(cudaMemsetAsync(e->chain_counters, 0, static_cast<size_t>(e->depth + 1) * 5 * nblk * sizeof(int), st));
   auto ln_gemm = [&](const float* g, const float* b, const LinearW& L, const CUtensorMap& out, int epi, int slot, int kclass) -> int {
@@ -1130,7 +1190,11 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Seg
     VPB_TRY(standalone_ln(b.ln1_g, b.ln1_b));
     if (stop == 3) return VPB_OK;
     e->prof.begin(KC_GEMM_QKV, st);
-    {
+    if (fused) {                                        // qkv + attention: the profile's gemm_qkv then includes the attention
+      QkvAttnParams qp;
+      qp.batch = B; qp.heads = e->heads; qp.dim = D; qp.bias = b.qkv.b; qp.out = e->attn;
+      VPB_TRY(qkv_attention_launch(D / e->heads, e->m_xn_att, b.m_qkv_head, qp, st));
+    } else {
       int bn;
       const CUtensorMap* wm;
       VPB_TRY(pick_tile(b.qkv, M, &bn, &wm));
@@ -1139,7 +1203,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Seg
     e->prof.end(st);
     }
     if (stop == 4) return VPB_OK;
-    {
+    if (!fused) {
       AttnParams ap;
       ap.batch = B; ap.heads = e->heads; ap.dim = D; ap.out = e->attn; ap.dbg = nullptr;
       e->prof.begin(KC_ATTN, st);
@@ -2231,8 +2295,10 @@ extern "C" int vpb_kernel_launches(const vpb_engine* e, int32_t batch) {
   if (e->use_chain && model_crops(e, batch) >= e->chain_min_batch && !e->ln_fused)
     return 1 + (1 + e->depth) + e->depth + 2 + 1 + 1 + (e->flip ? 1 : 0);   // gather, chains, attention, deconvs, 1x1, decode
   // one kernel per GEMM: gather, patch GEMM, depth x (qkv, attention, proj, fc1, fc2), 2 deconvs, 1x1, decode; the LayerNorms are
-  // launches of their own (2 * depth + 1), or ride in front of qkv / fc1 (ln_in_gemm: only last_norm is left), or in the tails
-  return 2 + e->depth * 5 + 2 + 1 + 1 + (e->ln_fused ? 0 : e->ln_in_gemm ? 1 : 2 * e->depth + 1) + (e->flip ? 1 : 0);
+  // launches of their own (2 * depth + 1), or ride in front of qkv / fc1 (ln_in_gemm: only last_norm is left), or in the tails.
+  // qkv and attention are one launch per block where fuse_qkv_attention says so (large batches)
+  return 2 + e->depth * (fuse_qkv_attention(e, model_crops(e, batch)) ? 4 : 5) + 2 + 1 + 1 +
+         (e->ln_fused ? 0 : e->ln_in_gemm ? 1 : 2 * e->depth + 1) + (e->flip ? 1 : 0);
 }
 
 extern "C" int vpb_set_option(vpb_engine* e, const char* name, int32_t value) {

@@ -333,8 +333,9 @@ int vpb_debug_gemm(int32_t stages_limit, void* d_counters);
 int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream);
 /* Debug / measurement switch (process-wide) for the attention kernel.  flags < 0: the defaults (every softmax exponential on
  * the MUFU; VPB_ATT_POLY = 1 in the environment evaluates every 4th one by a polynomial on the FMA pipe instead); otherwise
- * bit 0 = polynomial exponentials, bits 8.. = cap on the number of CTAs (0 = one per SM; tests use it to give every CTA
- * several items). */
+ * bit 0 = polynomial exponentials, bit 1 = run every block's qkv GEMM and attention as one fused launch, bit 2 = as two launches
+ * (neither: the engine's rule; both forms are bit-identical), bits 8.. = cap on the number of CTAs of both attention kernels
+ * (0 = one per SM; tests use it to give every CTA several items).  Engines capture CUDA graphs with the setting in effect. */
 int vpb_debug_attention(int32_t flags);
 int vpb_layernorm(const float* d_x, const float* d_gamma, const float* d_beta, void* d_y, int32_t rows, int32_t dim,
                   float eps, void* stream);
