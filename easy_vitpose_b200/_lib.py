@@ -27,7 +27,16 @@ class VpbFrame(C.Structure):
                 ("num_boxes", C.c_int32)]
 
 
-MAX_HEADS = 8                                         # VPB_MAX_HEADS: keypoint heads of one engine
+YUV_MATRICES = {"bt601": 0, "bt709": 1}              # VPB_YUV_BT601, VPB_YUV_BT709
+
+
+class VpbFrameNv12(C.Structure):
+    """vpb_frame_nv12: one NV12 frame (Y plane + interleaved half-resolution UV plane) of the _nv12 calls."""
+    _fields_ = [("y", C.c_void_p), ("y_pitch", C.c_int64), ("uv", C.c_void_p), ("uv_pitch", C.c_int64),
+                ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32)]
+
+
+MAX_HEADS = 8                                        # VPB_MAX_HEADS: keypoint heads of one engine
 MAX_SEGMENTS = 64                                     # VPB_MAX_SEGMENTS: runs of one head per multi-head call
 
 
@@ -101,6 +110,21 @@ EXPORTS = {
     "vpb_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p]),
 }
 
+# The NV12 calls: names with a digit, kept apart from EXPORTS, which tests/test_abi.py matches against the header's
+# [a-z_] names; tests/test_nv12_oracle.py checks this table against the header's *_nv12* declarations.
+EXPORTS_NV12 = {
+    "vpb_infer_frames_nv12": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameNv12), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
+    "vpb_infer_frames_nv12_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameNv12), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
+    "vpb_submit_frames_nv12_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameNv12), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_int32]),
+    "vpb_infer_affine_nv12": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameNv12), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine_nv12_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameNv12), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]),
+}
+
 
 def lib():
     """Loads the shared library once.  Raises if it has not been built (python -m easy_vitpose_b200.build)."""
@@ -118,7 +142,7 @@ def lib():
                 import warnings
                 warnings.warn(f"loading a STALE {LIB} (VPB_ALLOW_STALE=1): {exc}")
         handle = C.CDLL(LIB)
-        for name, (res, args) in EXPORTS.items():
+        for name, (res, args) in {**EXPORTS, **EXPORTS_NV12}.items():
             fn = getattr(handle, name)          # AttributeError here = header and library disagree
             fn.restype = res
             fn.argtypes = args

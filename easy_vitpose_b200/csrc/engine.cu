@@ -931,45 +931,57 @@ static int patch_gather(vpb_engine* e, const float* d_crops, int n_src, int B, c
 // (frame_to_patch_rows: crop pre-processing fused with the im2col; it also fills pp_org / pp_offs for the decode).
 // Affine crops (frame_to_patch_rows_affine) take a matrix per box instead of a box, and their keypoints are decoded with
 // centre / scale (decode mode 4) instead of canvas sizes and offsets.
+// NV12 frames come as an Nv12Entry table instead (each entry carries the call's YUV matrix); the gathers then launch the
+// NV12 instantiation of the same kernels, outside the captured graph, so the graph caches need no NV12 key.
 struct Source {
   const float* crops = nullptr;
   const FrameEntry* frames = nullptr;       // num_frames entries, only frames that have boxes
+  const Nv12Entry* nv12 = nullptr;          // instead of frames: NV12 frames
   int num_frames = 0;
   const int32_t* bboxes = nullptr;
   const double* mats = nullptr;             // [n,6] affine matrices (then bboxes is unused)
   const float* cs = nullptr;                // [n,4] centre / scale of the affine decode
 };
-static AffineParams affine_params(const FrameEntry* frames, int num_frames, const double* mats, const float* cs, int n, int* status) {
-  AffineParams q;
+static void set_table(Source& s, const FrameEntry* tab) { s.frames = tab; }
+static void set_table(Source& s, const Nv12Entry* tab) { s.nv12 = tab; }
+template <class Entry>
+static AffineParamsT<Entry> affine_params(const Entry* frames, int num_frames, const double* mats, const float* cs, int n, int* status) {
+  AffineParamsT<Entry> q;
   memset(&q, 0, sizeof(q));
   q.mats = mats; q.cs = cs; q.n = n; q.status = status; q.num_frames = num_frames;
-  memcpy(q.frames, frames, static_cast<size_t>(num_frames) * sizeof(FrameEntry));
+  memcpy(q.frames, frames, static_cast<size_t>(num_frames) * sizeof(Entry));
   return q;
 }
-static int affine_gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
-  AffineParams q = affine_params(src.frames, src.num_frames, src.mats, src.cs, n_src, e->pp_status);
+template <class Entry>
+static int affine_gather(vpb_engine* e, const Source& src, const Entry* tab, int n_src, int B, cudaStream_t st) {
+  AffineParamsT<Entry> q = affine_params(tab, src.num_frames, src.mats, src.cs, n_src, e->pp_status);
   q.rows = e->patch_rows; q.pos_bias = reinterpret_cast<const float4*>(e->pos_bias); q.stream = reinterpret_cast<float4*>(e->x); q.D = e->D;
   e->prof.begin(KC_PREPROCESS, st);
-  CU_TRY(launch_k(frame_to_patch_rows_affine, dim3(B, 16), dim3(384), 0, st, q));
+  CU_TRY(launch_k(frame_to_patch_rows_affine<Entry>, dim3(B, 16), dim3(384), 0, st, q));
   e->prof.end(st);
   return VPB_OK;
 }
-static int frame_gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
-  FramePatchParams q;
+template <class Entry>
+static int frame_gather(vpb_engine* e, const Source& src, const Entry* tab, int n_src, int B, cudaStream_t st) {
+  FramePatchParamsT<Entry> q;
   memset(&q, 0, sizeof(q));
   q.pp.bboxes = src.bboxes;
   q.pp.n = n_src; q.pp.pad = 10; q.pp.crops = nullptr; q.pp.org_wh = e->pp_org; q.pp.offs_yx = e->pp_offs; q.pp.status = e->pp_status;
   q.rows = e->patch_rows; q.pos_bias = reinterpret_cast<const float4*>(e->pos_bias); q.stream = reinterpret_cast<float4*>(e->x); q.D = e->D;
   q.num_frames = src.num_frames;
-  memcpy(q.frames, src.frames, static_cast<size_t>(src.num_frames) * sizeof(FrameEntry));
+  memcpy(q.frames, tab, static_cast<size_t>(src.num_frames) * sizeof(Entry));
   e->prof.begin(KC_PREPROCESS, st);
-  CU_TRY(launch_k(frame_to_patch_rows, dim3(B, 16), dim3(384), 0, st, q));
+  CU_TRY(launch_k(frame_to_patch_rows<Entry>, dim3(B, 16), dim3(384), 0, st, q));
   e->prof.end(st);
   return VPB_OK;
 }
+template <class Entry>
+static int table_gather(vpb_engine* e, const Source& src, const Entry* tab, int n_src, int B, cudaStream_t st) {
+  return src.mats ? affine_gather(e, src, tab, n_src, B, st) : frame_gather(e, src, tab, n_src, B, st);
+}
 static int gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
   if (src.crops) return patch_gather(e, src.crops, n_src, B, st);
-  return src.mats ? affine_gather(e, src, n_src, B, st) : frame_gather(e, src, n_src, B, st);
+  return src.nv12 ? table_gather(e, src, src.nv12, n_src, B, st) : table_gather(e, src, src.frames, n_src, B, st);
 }
 // Chained form of the backbone (chain.cuh): 1 + depth persistent GEMM launches + depth attention launches.
 //   launch 0:        patch embed (+= x) -> LN(norm1 of block 0) -> qkv of block 0
@@ -1667,10 +1679,11 @@ extern "C" int vpb_preprocess(const uint8_t* d_frame, int32_t frame_h, int32_t f
 static_assert(VPB_MAX_FRAMES == FP_MAX_FRAMES, "the header's frame limit is the gather's table size");
 
 // `tab`: num_frames frames with boxes, first_box ascending; d_bboxes holds their n boxes in frame order
-static int infer_frames_enqueue(vpb_engine* e, const FrameEntry* tab, int num_frames, const int32_t* d_bboxes, int32_t n,
+template <class Entry>
+static int infer_frames_enqueue(vpb_engine* e, const Entry* tab, int num_frames, const int32_t* d_bboxes, int32_t n,
                                 float* d_kpts, int32_t* d_idx, cudaStream_t st) {
   Source src;                   // the crops are never materialised: frame_to_patch_rows writes the bf16 patch rows directly
-  src.frames = tab; src.num_frames = num_frames; src.bboxes = d_bboxes;
+  set_table(src, tab); src.num_frames = num_frames; src.bboxes = d_bboxes;
   VPB_TRY(apply_l2_policy(e, st));
   return infer_core(e, src, e->pp_org, e->pp_offs, n, d_kpts, d_idx, nullptr, st);
 }
@@ -1716,6 +1729,44 @@ static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32
   if (!e) return fail(VPB_ERR_ARG, "null engine");
   if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
   VPB_TRY(build_frame_table(fn, fr, num_frames, e->maxB, tab, num_tab, n));
+  return *n ? check_ready_keypoints(e, *n) : VPB_OK;
+}
+// The NV12 counterpart: even height and width >= 2, pitches 0 (packed: width) or >= width, both planes non-NULL, a known
+// matrix (written into every entry).  Frame and box limits as build_frame_table.
+static int build_frame_table_nv12(const char* fn, const vpb_frame_nv12* fr, int32_t num_frames, int32_t matrix, int limit,
+                                  Nv12Entry* tab, int* num_tab, int32_t* n) {
+  if (num_frames < 0 || (num_frames > 0 && !fr)) return fail(VPB_ERR_ARG, "%s: %d frames, frame array %p", fn, num_frames, fr);
+  if (matrix != VPB_YUV_BT601 && matrix != VPB_YUV_BT709)
+    return fail(VPB_ERR_ARG, "%s: unknown YUV matrix %d (VPB_YUV_BT601 or VPB_YUV_BT709 expected)", fn, matrix);
+  long long boxes = 0;
+  int used = 0;
+  for (int j = 0; j < num_frames; ++j) {
+    const vpb_frame_nv12& f = fr[j];
+    if (f.num_boxes < 0) return fail(VPB_ERR_ARG, "%s: frame %d has num_boxes = %d", fn, j, f.num_boxes);
+    if (f.num_boxes == 0) continue;
+    const long long yp = f.y_pitch ? f.y_pitch : f.width, uvp = f.uv_pitch ? f.uv_pitch : f.width;
+    if (!f.y || !f.uv || f.height < 2 || f.width < 2 || (f.height & 1) || (f.width & 1) || yp < f.width || uvp < f.width)
+      return fail(VPB_ERR_ARG, "%s: frame %d: y %p, uv %p, %dx%d (w x h, even and >= 2 expected), pitches %lld / %lld bytes "
+                  "(0 or >= width expected)", fn, j, static_cast<const void*>(f.y), static_cast<const void*>(f.uv), f.width, f.height,
+                  static_cast<long long>(f.y_pitch), static_cast<long long>(f.uv_pitch));
+    if (used == VPB_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than VPB_MAX_FRAMES = %d frames with boxes", fn, VPB_MAX_FRAMES);
+    if (boxes + f.num_boxes > limit)
+      return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, limit, j);
+    Nv12Entry& t = tab[used++];
+    memset(&t, 0, sizeof(t));
+    t.y = f.y; t.uv = f.uv; t.y_pitch = yp; t.uv_pitch = uvp; t.fh = f.height; t.fw = f.width;
+    t.first_box = static_cast<int>(boxes); t.matrix = matrix;
+    boxes += f.num_boxes;
+  }
+  *num_tab = used;
+  *n = static_cast<int32_t>(boxes);
+  return VPB_OK;
+}
+static int frame_table_nv12(const char* fn, vpb_engine* e, const vpb_frame_nv12* fr, int32_t num_frames, int32_t matrix, Nv12Entry* tab,
+                            int* num_tab, int32_t* n) {
+  if (!e) return fail(VPB_ERR_ARG, "null engine");
+  if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
+  VPB_TRY(build_frame_table_nv12(fn, fr, num_frames, matrix, e->maxB, tab, num_tab, n));
   return *n ? check_ready_keypoints(e, *n) : VPB_OK;
 }
 
@@ -1768,7 +1819,8 @@ static int check_boxes_host(const int32_t* bb, int32_t n, int32_t fh, int32_t fw
   }
   return VPB_OK;
 }
-static int check_frames_boxes_host(const vpb_frame* fr, int32_t num_frames, const int32_t* bb) {
+template <class Frame>            // vpb_frame | vpb_frame_nv12
+static int check_frames_boxes_host(const Frame* fr, int32_t num_frames, const int32_t* bb) {
   for (int j = 0, first = 0; j < num_frames; first += fr[j].num_boxes, ++j)
     VPB_TRY(check_boxes_host(bb + 4 * static_cast<size_t>(first), fr[j].num_boxes, fr[j].height, fr[j].width, j));
   return VPB_OK;
@@ -1783,28 +1835,49 @@ static int frame_stage_reserve(vpb_engine* e, int slot, size_t bytes) {
   return VPB_OK;
 }
 
-// Host frames -> staging slot `slot`, enqueued on `st` after the slot's last user: each frame packed (a 2D copy from its pitch),
-// then the boxes of all frames in one copy (none for h_bboxes = NULL: the affine calls stage matrices instead).  Repoints `tab`
-// at the staged frames.
-static int stage_frames_host(vpb_engine* e, int slot, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, cudaStream_t st) {
+// one plane of `rows` rows of `row` bytes, host pitch `pitch` -> packed at dst
+static int stage_plane(uint8_t* dst, const uint8_t* src, long long pitch, size_t row, int rows, cudaStream_t st) {
+  if (static_cast<size_t>(pitch) == row) CU_TRY(cudaMemcpyAsync(dst, src, row * rows, cudaMemcpyHostToDevice, st));
+  else CU_TRY(cudaMemcpy2DAsync(dst, row, src, static_cast<size_t>(pitch), row, rows, cudaMemcpyHostToDevice, st));
+  return VPB_OK;
+}
+static size_t staged_bytes(const FrameEntry& t) { return static_cast<size_t>(t.fh) * t.fw * 3; }
+static size_t staged_bytes(const Nv12Entry& t) { return static_cast<size_t>(t.fh) * t.fw * 3 / 2; }     // Y, then UV
+static int stage_entry(FrameEntry& t, uint8_t* dst, cudaStream_t st) {
+  const size_t row = static_cast<size_t>(t.fw) * 3;
+  VPB_TRY(stage_plane(dst, t.data, t.pitch, row, t.fh, st));
+  t.data = dst; t.pitch = static_cast<long long>(row);
+  return VPB_OK;
+}
+static int stage_entry(Nv12Entry& t, uint8_t* dst, cudaStream_t st) {
+  const size_t row = static_cast<size_t>(t.fw);
+  uint8_t* uv = dst + row * t.fh;
+  VPB_TRY(stage_plane(dst, t.y, t.y_pitch, row, t.fh, st));
+  VPB_TRY(stage_plane(uv, t.uv, t.uv_pitch, row, t.fh / 2, st));
+  t.y = dst; t.uv = uv; t.y_pitch = t.uv_pitch = static_cast<long long>(row);
+  return VPB_OK;
+}
+// Host frames -> staging slot `slot`, enqueued on `st` after the slot's last user: each frame packed (a 2D copy from its pitch;
+// NV12: its Y plane, then its UV plane, 1.5 B per pixel), then the boxes of all frames in one copy (none for h_bboxes = NULL: the
+// affine calls stage matrices instead).  Repoints `tab` at the staged frames.
+template <class Entry>
+static int stage_frames_host(vpb_engine* e, int slot, Entry* tab, int nt, const int32_t* h_bboxes, int32_t n, cudaStream_t st) {
   size_t total = 0;
-  for (int j = 0; j < nt; ++j) total += static_cast<size_t>(tab[j].fh) * tab[j].fw * 3;
+  for (int j = 0; j < nt; ++j) total += staged_bytes(tab[j]);
   VPB_TRY(frame_stage_reserve(e, slot, total));
   CU_TRY(cudaStreamWaitEvent(st, e->ev_done[slot], 0));   // slot 0 is shared with the pipelined path: its last user is done
   size_t off = 0;
   for (int j = 0; j < nt; ++j) {
-    const size_t row = static_cast<size_t>(tab[j].fw) * 3, bytes = row * tab[j].fh;
-    uint8_t* dst = e->frame_stage[slot] + off;
-    if (static_cast<size_t>(tab[j].pitch) == row) CU_TRY(cudaMemcpyAsync(dst, tab[j].data, bytes, cudaMemcpyHostToDevice, st));
-    else CU_TRY(cudaMemcpy2DAsync(dst, row, tab[j].data, static_cast<size_t>(tab[j].pitch), row, tab[j].fh, cudaMemcpyHostToDevice, st));
-    tab[j].data = dst; tab[j].pitch = static_cast<long long>(row);
+    const size_t bytes = staged_bytes(tab[j]);
+    VPB_TRY(stage_entry(tab[j], e->frame_stage[slot] + off, st));
     off += bytes;
   }
   if (h_bboxes) CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   return VPB_OK;
 }
 // synchronous host form on slot 0 and the caller's stream
-static int frames_host_sync(vpb_engine* e, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
+template <class Entry>
+static int frames_host_sync(vpb_engine* e, Entry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
                             cudaStream_t st) {
   VPB_TRY(stage_frames_host(e, 0, tab, nt, h_bboxes, n, st));
   VPB_TRY(infer_frames_enqueue(e, tab, nt, e->bbox_stage[0], n, e->kpts[0], e->idx[0], st));
@@ -1816,7 +1889,8 @@ static int frames_host_sync(vpb_engine* e, FrameEntry* tab, int nt, const int32_
 }
 // Pipelined frames (video): same slots, events and vpb_wait_host as vpb_submit_host; the H2D per step is the uint8 frames and
 // 16 B per box instead of 589 824 B per crop.
-static int frames_host_submit(vpb_engine* e, FrameEntry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
+template <class Entry>
+static int frames_host_submit(vpb_engine* e, Entry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
                               int slot) {
   VPB_TRY(stage_frames_host(e, slot, tab, nt, h_bboxes, n, e->copy_stream));
   CU_TRY(cudaEventRecord(e->ev_h2d[slot], e->copy_stream));
@@ -1876,6 +1950,46 @@ extern "C" int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, 
   return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
 }
 
+// ---- the same three calls on NV12 frames
+extern "C" int vpb_infer_frames_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                                     const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
+  Nv12Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table_nv12("vpb_infer_frames_nv12", e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_nv12: null pointer");
+  return infer_frames_enqueue(e, tab, nt, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                                          const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
+  Nv12Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table_nv12("vpb_infer_frames_nv12_host", e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_nv12_host: null pointer");
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  return frames_host_sync(e, tab, nt, h_bboxes, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_submit_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                                           const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot) {
+  Nv12Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table_nv12("vpb_submit_frames_nv12_host", e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "vpb_submit_frames_nv12_host: slot %d", slot);
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_submit_frames_nv12_host: null pointer");
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
+}
+
 // ------------------------------------------------------------------------------------------------ affine top-down crops
 // host matrices / centre-scale: what the device forms can only flag in the status word is an argument error here
 static int check_affine_host(const double* mats, const float* cs, int32_t n) {
@@ -1904,12 +2018,28 @@ extern "C" int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_fram
   return VPB_OK;
 }
 
-static int infer_affine_enqueue(vpb_engine* e, const FrameEntry* tab, int num_frames, const double* d_mats, const float* d_cs, int32_t n,
+template <class Entry>
+static int infer_affine_enqueue(vpb_engine* e, const Entry* tab, int num_frames, const double* d_mats, const float* d_cs, int32_t n,
                                 float* d_kpts, int32_t* d_idx, cudaStream_t st) {
   Source src;
-  src.frames = tab; src.num_frames = num_frames; src.mats = d_mats; src.cs = d_cs;
+  set_table(src, tab); src.num_frames = num_frames; src.mats = d_mats; src.cs = d_cs;
   VPB_TRY(apply_l2_policy(e, st));
   return infer_core(e, src, nullptr, nullptr, n, d_kpts, d_idx, nullptr, st);
+}
+// the synchronous host form on slot 0: frames, matrices and centre / scale staged, the call, D2H of the keypoints
+template <class Entry>
+static int affine_host_sync(vpb_engine* e, Entry* tab, int nt, const double* h_mats, const float* h_cs, int32_t n, float* h_kpts,
+                            int32_t* h_idx, cudaStream_t st) {
+  VPB_TRY(check_affine_host(h_mats, h_cs, n));
+  VPB_TRY(stage_frames_host(e, 0, tab, nt, nullptr, n, st));         // waits for slot 0's last user
+  CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
+  CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
+  VPB_TRY(infer_affine_enqueue(e, tab, nt, e->mat_stage, e->cs_stage, n, e->kpts[0], e->idx[0], st));
+  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU_TRY(cudaEventRecord(e->ev_done[0], st));
+  CU_TRY(cudaStreamSynchronize(st));
+  return VPB_OK;
 }
 
 extern "C" int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, const float* d_cs,
@@ -1933,17 +2063,31 @@ extern "C" int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, i
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_host: null pointer");
-  VPB_TRY(check_affine_host(h_mats, h_cs, n));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  VPB_TRY(stage_frames_host(e, 0, tab, nt, nullptr, n, st));         // waits for slot 0's last user
-  CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
-  VPB_TRY(infer_affine_enqueue(e, tab, nt, e->mat_stage, e->cs_stage, n, e->kpts[0], e->idx[0], st));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaEventRecord(e->ev_done[0], st));
-  CU_TRY(cudaStreamSynchronize(st));
-  return VPB_OK;
+  return affine_host_sync(e, tab, nt, h_mats, h_cs, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_affine_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                                     const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
+  Nv12Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table_nv12("vpb_infer_affine_nv12", e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_nv12: null pointer");
+  return infer_affine_enqueue(e, tab, nt, d_mats, d_cs, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_affine_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                                          const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
+  Nv12Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table_nv12("vpb_infer_affine_nv12_host", e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_nv12_host: null pointer");
+  return affine_host_sync(e, tab, nt, h_mats, h_cs, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ multi-head calls

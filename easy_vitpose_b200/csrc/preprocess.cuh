@@ -135,8 +135,13 @@ __global__ void __launch_bounds__(PP_W) crop_resize_normalise(const PreprocParam
 // device buffer that two calls in flight could race on.  The entry is picked by a run-time index; __grid_constant__ guarantees
 // that this reads the parameter block in place, where a plain by-value parameter would allow the compiler to copy it to
 // local memory (ptxas reports no stack frame for the kernel either way with CUDA 12.9).
+// NV12 frames (vpb_infer_frames_nv12): the kernels are templated on the table entry; an Nv12Entry tap reads its Y byte and
+// the (U, V) pair of its 2x2 block and converts them to RGB (nv12_rgb) before the unchanged resize / warp arithmetic, so the
+// result is that of cv2.cvtColor(COLOR_YUV2RGB_NV12) followed by the RGB path.  Taps outside the crop or frame still read
+// RGB 0.
 constexpr int FP_MAX_FRAMES = 64;
 struct FrameEntry {
+  static constexpr bool kNv12 = false;
   const uint8_t* data;          // [fh, fw, 3] RGB, row pitch `pitch` bytes
   long long pitch;
   int fh, fw;
@@ -144,17 +149,57 @@ struct FrameEntry {
   int pad_;
 };
 static_assert(sizeof(FrameEntry) == 32, "frame table entry layout");
-struct FramePatchParams {
+constexpr int YUV_BT601 = 0, YUV_BT709 = 1;
+struct Nv12Entry {
+  static constexpr bool kNv12 = true;
+  const uint8_t* y;             // [fh, fw] luma, row pitch y_pitch bytes
+  const uint8_t* uv;            // [fh / 2, fw] interleaved U, V of each 2x2 block, row pitch uv_pitch bytes
+  long long y_pitch, uv_pitch;
+  int fh, fw;                   // both even
+  int first_box;
+  int matrix;                   // YUV_BT601 | YUV_BT709, the same for every entry of a call
+};
+static_assert(sizeof(Nv12Entry) == 48, "NV12 frame table entry layout");
+
+// cv2's fixed-point COLOR_YUV2RGB_NV12 (SHIFT 20, limited range, nearest chroma): oracle/nv12_oracle.py pins the formula.
+// The BT.709 set is round(2^20 x (1.164, 1.793, -0.533, -0.213, 2.112)), the 3-decimal form cv2 uses for BT.601.
+struct YuvCoef { int cy, cvr, cvg, cug, cub; };
+__device__ __forceinline__ YuvCoef yuv_coef(int matrix) {
+  return matrix == YUV_BT709 ? YuvCoef{1220542, 1880097, -558891, -223347, 2214593}
+                             : YuvCoef{1220542, 1673527, -852492, -409993, 2116026};
+}
+// pixel (x, y) of an NV12 frame -> RGB; every intermediate fits in int32 (|sum| < 2^30)
+__device__ __forceinline__ void nv12_rgb(const Nv12Entry& f, const YuvCoef& k, int x, int y, int rgb[3]) {
+  const int Y = f.y[static_cast<size_t>(y) * f.y_pitch + x];
+  const uint8_t* uv = f.uv + static_cast<size_t>(y >> 1) * f.uv_pitch + (x & ~1);
+  const int u = uv[0] - 128, v = uv[1] - 128;
+  const int yy = max(Y - 16, 0) * k.cy + (1 << 19);
+  rgb[0] = min(max((yy + k.cvr * v) >> 20, 0), 255);
+  rgb[1] = min(max((yy + k.cvg * v + k.cug * u) >> 20, 0), 255);
+  rgb[2] = min(max((yy + k.cub * u) >> 20, 0), 255);
+}
+
+__device__ __forceinline__ const uint8_t* first_plane(const FrameEntry& f) { return f.data; }
+__device__ __forceinline__ const uint8_t* first_plane(const Nv12Entry& f) { return f.y; }
+__device__ __forceinline__ long long first_pitch(const FrameEntry& f) { return f.pitch; }
+__device__ __forceinline__ long long first_pitch(const Nv12Entry& f) { return f.y_pitch; }
+
+template <class Entry>
+struct FramePatchParamsT {
   PreprocParams pp;             // frame / pitch / fh / fw / crops unused (the table holds the frames); pp.n = number of boxes
   __nv_bfloat16* rows;          // [n*192, 768]
   const float4* pos_bias;       // [192*D/4]
   float4* stream;               // [n*192*D/4]
   int D;
   int num_frames;               // 1..FP_MAX_FRAMES
-  FrameEntry frames[FP_MAX_FRAMES];
+  Entry frames[FP_MAX_FRAMES];
 };
+using FramePatchParams = FramePatchParamsT<FrameEntry>;
+static_assert(sizeof(FramePatchParamsT<FrameEntry>) <= 4096 && sizeof(FramePatchParamsT<Nv12Entry>) <= 4096,
+              "the frame table travels in the 4 KB parameter block");
 
-__global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant__ FramePatchParams q) {
+template <class Entry>
+__global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant__ FramePatchParamsT<Entry> q) {
   constexpr int FP_PITCH = 208;                               // 2 + 192 + 14 bf16 per tile row: 16-byte aligned rows
   __shared__ uint16_t s_lut[3][256];
   __shared__ PpAxis s_ay[16];
@@ -183,9 +228,9 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
     const int mid = (lo + hi) >> 1;
     if (q.frames[mid].first_box <= box) lo = mid; else hi = mid;
   }
-  const FrameEntry& fr = q.frames[lo];
-  const uint8_t* frame = fr.data;
-  const long long pitch = fr.pitch;
+  const Entry& fr = q.frames[lo];
+  [[maybe_unused]] const uint8_t* frame = first_plane(fr);    // the RGB path's pixels (NV12: the Y plane, read by nv12_rgb)
+  [[maybe_unused]] const long long pitch = first_pitch(fr);
   const int fh = fr.fh, fw = fr.fw;
   const int* bb = p.bboxes + 4 * box;
   const int x0 = min(max(bb[0] - p.pad, 0), fw), x1 = min(max(bb[2] + p.pad, 0), fw);
@@ -225,16 +270,31 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
       const PpAxis ax = s_ax[dx];
       const int cy0 = ay.i0 - top, cy1 = ay.i1 - top, cx0 = ax.i0 - left, cx1 = ax.i1 - left;
       const bool vy0 = cy0 >= 0 && cy0 < h, vy1 = cy1 >= 0 && cy1 < h, vx0 = cx0 >= 0 && cx0 < w, vx1 = cx1 >= 0 && cx1 < w;
-      const uint8_t* r0 = frame + static_cast<size_t>(vy0 ? y0 + cy0 : 0) * pitch;
-      const uint8_t* r1 = frame + static_cast<size_t>(vy1 ? y0 + cy1 : 0) * pitch;
-      const int f0 = (vx0 ? x0 + cx0 : 0) * 3, f1 = (vx1 ? x0 + cx1 : 0) * 3;
+      if constexpr (Entry::kNv12) {
+        const YuvCoef k = yuv_coef(fr.matrix);
+        int t00[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t10[3] = {0, 0, 0}, t11[3] = {0, 0, 0};   // out-of-crop taps: RGB 0
+        if (vy0 && vx0) nv12_rgb(fr, k, x0 + cx0, y0 + cy0, t00);
+        if (vy0 && vx1) nv12_rgb(fr, k, x0 + cx1, y0 + cy0, t01);
+        if (vy1 && vx0) nv12_rgb(fr, k, x0 + cx0, y0 + cy1, t10);
+        if (vy1 && vx1) nv12_rgb(fr, k, x0 + cx1, y0 + cy1, t11);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int p00 = (vy0 && vx0) ? r0[f0 + c] : 0, p01 = (vy0 && vx1) ? r0[f1 + c] : 0;
-        const int p10 = (vy1 && vx0) ? r1[f0 + c] : 0, p11 = (vy1 && vx1) ? r1[f1 + c] : 0;
-        const int s0 = p00 * ax.a0 + p01 * ax.a1, s1 = p10 * ax.a0 + p11 * ax.a1;
-        int v = (((ay.a0 * (s0 >> 4)) >> 16) + ((ay.a1 * (s1 >> 4)) >> 16) + 2) >> 2;
-        v3[c] = s_lut[c][min(max(v, 0), 255)];
+        for (int c = 0; c < 3; ++c) {
+          const int s0 = t00[c] * ax.a0 + t01[c] * ax.a1, s1 = t10[c] * ax.a0 + t11[c] * ax.a1;
+          int v = (((ay.a0 * (s0 >> 4)) >> 16) + ((ay.a1 * (s1 >> 4)) >> 16) + 2) >> 2;
+          v3[c] = s_lut[c][min(max(v, 0), 255)];
+        }
+      } else {
+        const uint8_t* r0 = frame + static_cast<size_t>(vy0 ? y0 + cy0 : 0) * pitch;
+        const uint8_t* r1 = frame + static_cast<size_t>(vy1 ? y0 + cy1 : 0) * pitch;
+        const int f0 = (vx0 ? x0 + cx0 : 0) * 3, f1 = (vx1 ? x0 + cx1 : 0) * 3;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const int p00 = (vy0 && vx0) ? r0[f0 + c] : 0, p01 = (vy0 && vx1) ? r0[f1 + c] : 0;
+          const int p10 = (vy1 && vx0) ? r1[f0 + c] : 0, p11 = (vy1 && vx1) ? r1[f1 + c] : 0;
+          const int s0 = p00 * ax.a0 + p01 * ax.a1, s1 = p10 * ax.a0 + p11 * ax.a1;
+          int v = (((ay.a0 * (s0 >> 4)) >> 16) + ((ay.a1 * (s1 >> 4)) >> 16) + 2) >> 2;
+          v3[c] = s_lut[c][min(max(v, 0), 255)];
+        }
       }
     }
     const int tx = 2 + (mirror ? PP_W - 1 - dx : dx);
@@ -300,6 +360,19 @@ __device__ __forceinline__ void affine_pixel(const uint8_t* frame, long long pit
     v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + (1 << 14)) >> 15;
   }
 }
+// the same from an NV12 frame: each tap converted to RGB first, the constant border is RGB 0
+__device__ __forceinline__ void affine_pixel_nv12(const Nv12Entry& f, const YuvCoef& k, int X, int Y, int v[3]) {
+  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767), fx = X & 31, fy = Y & 31;
+  const bool vx0 = sx >= 0 && sx < f.fw, vx1 = sx + 1 >= 0 && sx + 1 < f.fw, vy0 = sy >= 0 && sy < f.fh, vy1 = sy + 1 >= 0 && sy + 1 < f.fh;
+  const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
+  int t00[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t10[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
+  if (vy0 && vx0) nv12_rgb(f, k, sx, sy, t00);
+  if (vy0 && vx1) nv12_rgb(f, k, sx + 1, sy, t01);
+  if (vy1 && vx0) nv12_rgb(f, k, sx, sy + 1, t10);
+  if (vy1 && vx1) nv12_rgb(f, k, sx + 1, sy + 1, t11);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) v[c] = (t00[c] * w00 + t01[c] * w01 + t10[c] * w10 + t11[c] * w11 + (1 << 14)) >> 15;
+}
 // torchvision ToTensor + Normalize (COCO.py:120-123): float32 throughout, IEEE division
 __device__ __forceinline__ float affine_norm(int c, int v) {
   const float mean = c == 0 ? 0.485f : (c == 1 ? 0.456f : 0.406f), stdv = c == 0 ? 0.229f : (c == 1 ? 0.224f : 0.225f);
@@ -307,7 +380,8 @@ __device__ __forceinline__ float affine_norm(int c, int v) {
 }
 
 // Launch parameters of both affine kernels.  The frame table is frame_to_patch_rows' (same binary search on first_box).
-struct AffineParams {
+template <class Entry>
+struct AffineParamsT {
   const double* mats;           // [n,6] f64: the matrix given to cv2.warpAffine (image -> crop)
   const float* cs;              // [n,4] (cx, cy, sx, sy) of the decode, checked for sx, sy > 0 (may be nullptr)
   int n;
@@ -318,9 +392,13 @@ struct AffineParams {
   float4* stream;
   int D;
   int num_frames;
-  FrameEntry frames[FP_MAX_FRAMES];
+  Entry frames[FP_MAX_FRAMES];
 };
-__device__ __forceinline__ const FrameEntry& affine_frame(const AffineParams& q, int box) {
+using AffineParams = AffineParamsT<FrameEntry>;
+static_assert(sizeof(AffineParamsT<FrameEntry>) <= 4096 && sizeof(AffineParamsT<Nv12Entry>) <= 4096,
+              "the frame table travels in the 4 KB parameter block");
+template <class Entry>
+__device__ __forceinline__ const Entry& affine_frame(const AffineParamsT<Entry>& q, int box) {
   int lo = 0, hi = q.num_frames;                              // the last frame whose first_box <= box
   while (hi - lo > 1) {
     const int mid = (lo + hi) >> 1;
@@ -329,7 +407,8 @@ __device__ __forceinline__ const FrameEntry& affine_frame(const AffineParams& q,
   return q.frames[lo];
 }
 // the device forms cannot return an error for a bad matrix without a sync: flag it (the arithmetic stays in bounds)
-__device__ __forceinline__ void affine_check(const AffineParams& q, int box) {
+template <class Entry>
+__device__ __forceinline__ void affine_check(const AffineParamsT<Entry>& q, int box) {
   bool ok = true;
 #pragma unroll
   for (int i = 0; i < 6; ++i) ok = ok && isfinite(q.mats[6 * box + i]);
@@ -360,7 +439,8 @@ __global__ void __launch_bounds__(PP_W) crop_warp_normalise(const __grid_constan
 // Same grid ((n or 2n) x 16 CTAs, crop c >= n the mirror image of crop c - n), bf16 tile, im2col store and pos_embed + bias
 // seeding; each CTA inverts its matrix once and keeps adelta / bdelta of the 192 columns and X0 / Y0 of its 16 rows in shared
 // memory.  Rows 16 py - 2 < 0 are the conv's zero padding and are never warped.
-__global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_constant__ AffineParams q) {
+template <class Entry>
+__global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_constant__ AffineParamsT<Entry> q) {
   constexpr int FP_PITCH = 208;                               // as frame_to_patch_rows
   __shared__ uint16_t s_lut[3][256];
   __shared__ int2 s_row[16];
@@ -378,7 +458,7 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_c
   for (int i = tid; i < 768; i += 384) s_lut[i >> 8][i & 255] = __bfloat16_as_ushort(__float2bfloat16_rn(affine_norm(i >> 8, i & 255)));
   const bool mirror = crop >= q.n;
   const int box = mirror ? crop - q.n : crop;
-  const FrameEntry& fr = affine_frame(q, box);
+  const Entry& fr = affine_frame(q, box);
   if (tid < PP_W + 16) {
     const AffineInv a = affine_invert(q.mats + 6 * box);
     if (tid < PP_W) s_col[tid] = affine_col(a, tid);
@@ -400,7 +480,8 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_c
     if (dy >= 0) {
       int v[3];
       const int2 r = s_row[ky], c = s_col[dx];
-      affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
+      if constexpr (Entry::kNv12) affine_pixel_nv12(fr, yuv_coef(fr.matrix), (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
+      else affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) v3[ch] = s_lut[ch][v[ch]];
     }

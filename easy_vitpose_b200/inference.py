@@ -97,6 +97,11 @@ class B200PoseBackend:
         return self.model.infer_frames_host(imgs, bboxes_list)[0]
 
     @torch.no_grad()
+    def inference_frames_nv12(self, frames, bboxes_list: "list[np.ndarray]", matrix: str = "bt601") -> "list[np.ndarray]":
+        """inference_frames on NV12 video frames (uint8 [3H/2, W] with the planes stacked, or (y, uv) pairs): no RGB conversion."""
+        return self.model.infer_frames_nv12_host(frames, bboxes_list, matrix)[0]
+
+    @torch.no_grad()
     def inference_frames_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list) -> "list[np.ndarray]":
         """inference_frames on a multi-head engine (ViTPose(..., heads=...)), with a head index per box (heads_list: per frame
         an int array [n_i], e.g. 0 for people and 3 for animals of a ViTPose+ engine) -> one float32 [n_i,K_max,3] (y, x,
@@ -112,6 +117,13 @@ class B200PoseBackend:
         cv2.warpAffine's, and the keypoints are keypoints_from_heatmaps(c, s, use_udp=True)'s -- all on the device."""
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
         return self.model.infer_affine_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args])[0]
+
+    @torch.no_grad()
+    def inference_topdown_nv12(self, frames, bboxes_list: "list[np.ndarray]", padding: float = 1.25, use_udp: bool = True,
+                               matrix: str = "bt601") -> "list[np.ndarray]":
+        """inference_topdown on NV12 video frames (uint8 [3H/2, W] with the planes stacked, or (y, uv) pairs)."""
+        args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
+        return self.model.infer_affine_nv12_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], matrix)[0]
 
     @torch.no_grad()
     def inference_topdown_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list, padding: float = 1.25,

@@ -15,7 +15,7 @@ import torch
 from . import _lib
 from .configs import VITPOSE_PLUS_HEADS
 
-__all__ = ["ViTPose", "plan_frame_chunks", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head", "head_flip_permutations",
+__all__ = ["ViTPose", "plan_frame_chunks", "nv12_planes", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head", "head_flip_permutations",
            "plan_head_calls"]
 
 IMG_H, IMG_W, HM_H, HM_W = 256, 192, 64, 48
@@ -47,14 +47,47 @@ def plan_frame_chunks(counts, limit: int, max_frames: int = _lib.MAX_FRAMES) -> 
     return chunks
 
 
-def _frame_array(frames, chunk):
+def _frame_array(frames, chunk, struct=_lib.VpbFrame):
     """vpb_frame array for one planned call: entries 0..last frame of the call, so that the engine's messages name the
-    caller's frame index; frames outside the call get 0 boxes (skipped).  `frames` holds (data pointer, h, w, pitch)."""
-    arr = (_lib.VpbFrame * (chunk[-1][0] + 1))()
+    caller's frame index; frames outside the call get 0 boxes (skipped).  `frames` holds (data pointer, h, w, pitch), or
+    for struct=VpbFrameNv12 (y pointer, y pitch, uv pointer, uv pitch, h, w)."""
+    arr = (struct * (chunk[-1][0] + 1))()
     for f, s, e in chunk:
-        ptr, h, w, pitch = frames[f]
-        arr[f] = _lib.VpbFrame(ptr, h, w, pitch, e - s)
+        arr[f] = struct(*frames[f], e - s)
     return arr
+
+
+def nv12_planes(frame, what: str = "frame"):
+    """One NV12 frame -> its (y [H,W], uv [H/2,W]) planes as views, for numpy arrays and torch tensors alike.  A frame is
+    either a uint8 [3H/2, W] array with the planes stacked (what cv2 and ffmpeg's `-pix_fmt nv12` produce) or a pair
+    (y, uv) (what a decoder surface is: two planes, any row pitch).  Raises ValueError for odd or mismatched sizes."""
+    if isinstance(frame, (tuple, list)):
+        if len(frame) != 2:
+            raise ValueError(f"{what}: an NV12 (y, uv) pair expected, got {len(frame)} planes")
+        y, uv = frame
+    else:
+        if getattr(frame, "ndim", 0) != 2 or frame.shape[0] % 3:
+            raise ValueError(f"{what}: NV12 [3H/2, W] with the planes stacked expected, got shape {tuple(getattr(frame, 'shape', ()))}")
+        h = frame.shape[0] // 3 * 2
+        y, uv = frame[:h], frame[h:]
+    for p in (y, uv):
+        if getattr(p, "ndim", 0) != 2 or str(p.dtype) not in ("uint8", "torch.uint8"):
+            raise ValueError(f"{what}: NV12 planes must be 2-D uint8, got {getattr(p, 'dtype', type(p))} {tuple(getattr(p, 'shape', ()))}")
+    if type(y) is not type(uv):
+        raise ValueError(f"{what}: the y and uv planes must both be numpy arrays or both tensors")
+    h, w = y.shape
+    if h < 2 or w < 2 or h % 2 or w % 2:
+        raise ValueError(f"{what}: NV12 needs an even height and width >= 2, got {h}x{w} (h x w)")
+    if tuple(uv.shape) != (h // 2, w):
+        raise ValueError(f"{what}: uv plane {tuple(uv.shape)} does not match the {h}x{w} y plane ([H/2, W] expected)")
+    return y, uv
+
+
+def _yuv_matrix(matrix: str) -> int:
+    try:
+        return _lib.YUV_MATRICES[str(matrix).lower()]
+    except KeyError:
+        raise ValueError(f"unknown YUV matrix {matrix!r}: one of {sorted(_lib.YUV_MATRICES)}") from None
 
 
 def group_by_head(heads, num_heads: int) -> "tuple[np.ndarray, list[int]]":
@@ -943,6 +976,173 @@ class ViTPose:
                 arr = _frame_array(table, chunk)
                 _lib.check_value(_lib.lib().vpb_infer_affine_host(
                     self._handle, arr, len(arr), M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
+                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        if not counts:
+            return [], []
+        split = np.cumsum(counts)[:-1]
+        return np.split(kp, split), np.split(idx, split)
+
+    # ---------------------------------------------------------------------------------------- NV12 video frames
+    # Each frame is a uint8 [3H/2, W] array with the planes stacked or a (y [H,W], uv [H/2,W]) pair (nv12_planes); matrix is
+    # "bt601" (cv2's COLOR_YUV2RGB_NV12) or "bt709", both limited range.  Every call is bit-identical to its RGB twin on the
+    # converted frames (oracle/nv12_oracle.py: nv12_to_rgb); only the pixels under the boxes are converted, on the fly.
+    def _device_plane(self, j: int, p) -> torch.Tensor:
+        if not isinstance(p, torch.Tensor):
+            p = torch.from_numpy(np.ascontiguousarray(p))
+        if not p.is_cuda:
+            p = p.to(torch.device("cuda", self._device), non_blocking=True)
+        if p.device.index != self._device:
+            raise ValueError(f"frame {j} lives on {p.device}, the engine on cuda:{self._device}")
+        if p.stride(1) != 1 or p.stride(0) < p.shape[1]:
+            p = p.contiguous()                               # rows of bytes at any pitch are read in place
+        return p
+
+    def _nv12_device_table(self, frames):
+        """-> (the plane tensors to keep alive, [(y ptr, y pitch, uv ptr, uv pitch, h, w)])"""
+        planes = [tuple(self._device_plane(j, p) for p in nv12_planes(f, f"frame {j}")) for j, f in enumerate(frames)]
+        table = [(y.data_ptr(), y.stride(0), uv.data_ptr(), uv.stride(0), y.shape[0], y.shape[1]) for y, uv in planes]
+        return [p for yuv in planes for p in yuv], table
+
+    @staticmethod
+    def _nv12_host_table(frames):
+        planes = []
+        for j, f in enumerate(frames):
+            y, uv = nv12_planes(f, f"frame {j}")
+            if not isinstance(y, np.ndarray):
+                raise ValueError(f"frame {j}: numpy NV12 planes expected")
+            planes.append(tuple(p if p.strides[1] == 1 and p.strides[0] >= p.shape[1] else np.ascontiguousarray(p) for p in (y, uv)))
+        return planes, [(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1]) for y, uv in planes]
+
+    def infer_frames_nv12(self, frames, bboxes, matrix: str = "bt601", check: bool = False):
+        """infer_frames on NV12 frames (vpb_infer_frames_nv12): CUDA (or host, copied over) NV12 frames and per-frame boxes
+        [n_j,4] -> (list of kpts f32 [n_j,K,3], list of idx i32 [n_j,K]).  Chunked, flip test and status word as infer_frames."""
+        self._ensure()
+        mat = _yuv_matrix(matrix)
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        planes, table = self._nv12_device_table(frames)
+        dev = torch.device("cuda", self._device)
+        boxes = []
+        for b in bboxes:
+            b = torch.as_tensor(b)
+            if b.is_floating_point():
+                b = b.round()
+            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
+        counts = [b.shape[0] for b in boxes]
+        bb = torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=dev)
+        n = bb.shape[0]
+        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
+        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
+        s = 0
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+            self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_nv12(
+                self._handle, arr, len(arr), mat, C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
+                C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 1:
+            raise ValueError("a box is empty after padding and clipping to its frame")
+        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+
+    def infer_frames_nv12_host(self, frames, bboxes, matrix: str = "bt601"):
+        """HOST form of infer_frames_nv12 (vpb_infer_frames_nv12_host, synchronous): numpy NV12 frames, per-frame boxes ->
+        numpy (kpts, idx) lists.  Each frame is staged packed at 1.5 B per pixel; an empty box raises ValueError."""
+        self._ensure()
+        mat = _yuv_matrix(matrix)
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        planes, table = self._nv12_host_table(frames)
+        boxes = [self._round_boxes(b) for b in bboxes]
+        counts = [len(b) for b in boxes]
+        bb = np.concatenate(boxes, 0) if boxes else np.zeros((0, 4), np.int32)
+        n = bb.shape[0]
+        kp = np.empty((n, self.num_keypoints, 3), np.float32)
+        idx = np.empty((n, self.num_keypoints), np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, self.batch_limit):
+                arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+                _lib.check_value(_lib.lib().vpb_infer_frames_nv12_host(
+                    self._handle, arr, len(arr), mat, bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
+                    idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        if not counts:
+            return [], []
+        split = np.cumsum(counts)[:-1]
+        return np.split(kp, split), np.split(idx, split)
+
+    def submit_frames_nv12_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int,
+                                matrix: str = "bt601") -> None:
+        """Asynchronous vpb_submit_frames_nv12_host, ONE engine call (wait with wait_host(slot)): the pipelined video form of
+        submit_frames_host for numpy NV12 frames whose rows are contiguous bytes (any row pitch).  Frames, boxes (int32
+        [n_j,4], already rounded) and outputs must stay alive and unmodified until the wait."""
+        self._ensure()
+        mat = _yuv_matrix(matrix)
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        table = []
+        for j, (f, b) in enumerate(zip(frames, bboxes)):
+            y, uv = nv12_planes(f, f"frame {j}")
+            if not isinstance(y, np.ndarray) or y.strides[1] != 1 or uv.strides[1] != 1 or y.strides[0] < y.shape[1] \
+                    or uv.strides[0] < uv.shape[1]:
+                raise ValueError(f"frame {j}: numpy NV12 planes with contiguous bytes in each row expected")
+            if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
+                raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
+            table.append(_lib.VpbFrameNv12(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1], len(b)))
+        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
+        n = bb.shape[0]
+        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
+                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
+            raise ValueError("submit_frames_nv12_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
+        arr = (_lib.VpbFrameNv12 * len(table))(*table)
+        with torch.cuda.device(self._device):
+            _lib.check_value(_lib.lib().vpb_submit_frames_nv12_host(
+                self._handle, arr, len(arr), mat, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
+                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+    def infer_affine_nv12(self, frames, mats, centers, scales, matrix: str = "bt601", check: bool = False):
+        """infer_affine on NV12 frames (vpb_infer_affine_nv12): the warp reads the NV12 planes and converts each tap."""
+        self._ensure()
+        mat = _yuv_matrix(matrix)
+        if not (len(frames) == len(mats) == len(centers) == len(scales)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        planes, table = self._nv12_device_table(frames)
+        dev = torch.device("cuda", self._device)
+        counts, M, CS = self._affine_args(mats, centers, scales)
+        M, CS = M.to(dev), CS.to(dev)
+        n = M.shape[0]
+        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
+        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
+        s = 0
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+            self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_nv12(
+                self._handle, arr, len(arr), mat, C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 2:
+            raise ValueError("a matrix entry is not finite or a scale is <= 0")
+        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+
+    def infer_affine_nv12_host(self, frames, mats, centers, scales, matrix: str = "bt601"):
+        """HOST form of infer_affine_nv12 (vpb_infer_affine_nv12_host, synchronous), checked as infer_affine_host."""
+        self._ensure()
+        mat = _yuv_matrix(matrix)
+        if not (len(frames) == len(mats) == len(centers) == len(scales)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        planes, table = self._nv12_host_table(frames)
+        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
+        M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
+        n = M.shape[0]
+        kp = np.empty((n, self.num_keypoints, 3), np.float32)
+        idx = np.empty((n, self.num_keypoints), np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, self.batch_limit):
+                arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+                _lib.check_value(_lib.lib().vpb_infer_affine_nv12_host(
+                    self._handle, arr, len(arr), mat, M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
                     kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
                 s += sum(e - b for _, b, e in chunk)
         if not counts:

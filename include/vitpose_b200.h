@@ -223,6 +223,41 @@ int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frame
 int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* h_mats, const float* h_cs,
                           float* h_kpts, int32_t* h_idx, void* stream);
 
+/* ---- NV12 video frames (what NVDEC and ffmpeg's `-pix_fmt nv12` produce): the multi-frame and affine calls read decoder
+ * output directly, converting only the pixels the gather taps.  Pixel (x, y) of an even-sized frame takes
+ * Y = y[y * y_pitch + x] and the (U, V) pair uv[(y / 2) * uv_pitch + 2 * (x / 2)], uv[... + 1] (nearest chroma, as cv2), then
+ * with yy = max(Y - 16, 0) * CY (SHIFT 20, half = 1 << 19):
+ *   R = clamp((yy + half + CVR (V - 128)) >> 20), G = clamp((yy + half + CVG (V - 128) + CUG (U - 128)) >> 20),
+ *   B = clamp((yy + half + CUB (U - 128)) >> 20) to 0..255;
+ *   VPB_YUV_BT601: CY 1220542, CVR 1673527, CVG -852492, CUG -409993, CUB 2116026 = cv2 COLOR_YUV2RGB_NV12, bit for bit;
+ *   VPB_YUV_BT709: CY 1220542, CVR 1880097, CVG -558891, CUG -223347, CUB 2214593 (limited-range BT.709, 3-decimal form).
+ * Full-range (JPEG) YUV is not covered.  The converted taps then go through the RGB arithmetic unchanged, and taps outside
+ * the crop or frame read RGB 0, so every call is bit-identical (patch rows, keypoints, argmax, flip test included) to its RGB
+ * counterpart on cv2.cvtColor(frame, COLOR_YUV2RGB_NV12) (BT.601) or the formula above (BT.709).  Arguments, errors, status
+ * bits, limits, staging slots and graph caches are those of the RGB counterparts, plus `matrix`; VPB_ERR_ARG also for an odd
+ * or < 2 height or width, a pitch below width, a NULL plane in a frame with boxes, or an unknown matrix.  The host forms stage
+ * each frame packed at 1.5 B per pixel (Y, then UV). */
+#define VPB_YUV_BT601 0
+#define VPB_YUV_BT709 1
+typedef struct vpb_frame_nv12 {
+  const uint8_t* y;       /* u8 [height, width] luma; device address or host (the _host forms) */
+  int64_t y_pitch;        /* row pitch of y in bytes; 0 = packed (width) */
+  const uint8_t* uv;      /* u8 [height / 2, width]: U, V interleaved, one pair per 2x2 block; may be a separate allocation */
+  int64_t uv_pitch;       /* row pitch of uv in bytes; 0 = packed (width) */
+  int32_t height, width;  /* both even */
+  int32_t num_boxes;      /* as vpb_frame.num_boxes */
+} vpb_frame_nv12;
+int vpb_infer_frames_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                          const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                               const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream);
+int vpb_submit_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
+                                const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot);   /* completes with vpb_wait_host(slot) */
+int vpb_infer_affine_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix, const double* d_mats,
+                          const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_affine_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix, const double* h_mats,
+                               const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream);
+
 /* ---- several keypoint heads (datasets) on one backbone: ViTPose+ (model_split.py) and frozen-backbone fine-tunes
  * (train.py --freeze-backbone).  vpb_create_heads makes an engine with num_heads heads of h_keypoints[j] keypoints each
  * (1 <= num_heads <= VPB_MAX_HEADS, 1..144 keypoints; cfg->num_keypoints is ignored) and an expert width P = expert_rows:
