@@ -131,7 +131,7 @@ struct LnRow {
     for (int i = 0; i < V; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float mean = s * (1.0f / D);
+    const float mean = s / D;                         // divided, as layernorm_f32_to_bf16 (bit-identical to it)
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < V; ++i) {

@@ -226,7 +226,7 @@ __device__ __forceinline__ void ln_row_l2(const float* __restrict__ xrow, const 
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s * (1.0f / D);
+  const float mean = s / D;                           // divided, as layernorm_f32_to_bf16 (bit-identical to it)
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < V; ++i) {

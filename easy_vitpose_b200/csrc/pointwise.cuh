@@ -44,7 +44,10 @@ __global__ void __launch_bounds__(128) layernorm_f32_to_bf16(const float* __rest
     for (int i = 0; i < V; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float mean = s * (1.0f / D);
+    // a correctly rounded division, not s * fl(1/D): fl(1/D) is off by up to 2^-24 for D = 384, 768, 1280, which made the
+    // mean of a constant row differ from its value by an ulp; at variance 0 rstd = eps^-1/2 = 1000 turned that into an
+    // output of beta - 0.12 gamma instead of beta (a row of 1024.0 at D = 384).  ln_row_l2 and chain.cuh's LnRow match it.
+    const float mean = s / D;
     float q = 0.f;
 #pragma unroll
     for (int i = 0; i < V; ++i) {
