@@ -445,18 +445,16 @@ struct vpb_engine {
   bool finalized = false;
   int stop_after = 0;
   Profiler prof;
-  // CUDA-graph replay of the kernel chain behind the patch gather, one graph per batch size: removes ~90 launches of CPU
-  // work per call, which is what bounds small ragged batches (video streams).  The graph only touches engine-owned
-  // memory (the caller's crops are consumed by the eagerly launched patch_im2col; org_wh / keypoints / argmax / heatmaps
-  // move by small device copies), so it is valid for any caller pointers.  Captured on a batch size's second use.
-  // affine = the graph decodes with centre / scale (vpb_infer_affine) instead of canvas sizes / offsets
-  struct GraphEntry { int batch; int seen; cudaGraphExec_t exec; bool affine; };
-  std::vector<GraphEntry> graphs;
-  // multi-head calls: one graph per segment list (heads and counts), at most kMaxMixedGraphs, least recently used out first
-  // affine = the graph decodes with centre / scale (vpb_infer_affine_heads)
-  struct MixedGraph { std::vector<Segment> segs; bool affine; cudaGraphExec_t exec; unsigned long long used; };
-  std::vector<MixedGraph> mixed_graphs;
-  unsigned long long mixed_clock = 0;
+  // CUDA-graph replay of the kernel chain behind the patch gather: removes ~90 launches of CPU work per call, which is what
+  // bounds small ragged batches (video streams).  The graph only touches engine-owned memory (the caller's crops are consumed
+  // by the eagerly launched gather; org_wh / keypoints / argmax / heatmaps move by small device copies), so it is valid for
+  // any caller pointers.  One graph per (mixed, segment list, affine), captured on the key's second use.  mixed = made by a
+  // multi-head call (rows of K_max keypoints; at most kMaxMixedGraphs such graphs, least recently used out first), else by a
+  // single-head call (the one segment {head 0, n}: one graph per batch size and decode kind, unbounded); affine = the graph
+  // decodes with centre / scale instead of canvas sizes / offsets
+  struct CachedGraph { bool mixed; std::vector<Segment> segs; bool affine; cudaGraphExec_t exec; unsigned long long used; };
+  std::vector<CachedGraph> graph_cache;
+  unsigned long long graph_clock = 0;
   bool use_graph = true;
   // L2 residency: the fp32 token stream x (37.7 MB at B=64) is read-modify-written by every residual GEMM and read by every
   // LayerNorm, but the per-layer working set (~220 MB) would evict it from the 50 MB L2 in between; an access-policy window
@@ -662,8 +660,7 @@ extern "C" void vpb_destroy(vpb_engine* e) {
   for (auto& ev : e->prof.pool) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
   for (auto& kv : e->staged) cudaFree(kv.second.first);
   for (void* p : e->allocs) cudaFree(p);
-  for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-  for (auto& g : e->mixed_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+  for (auto& g : e->graph_cache) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (int s = 0; s < 2; ++s) {
     if (e->ev_h2d[s]) cudaEventDestroy(e->ev_h2d[s]);
     if (e->ev_done[s]) cudaEventDestroy(e->ev_done[s]);
@@ -932,7 +929,7 @@ static int patch_gather(vpb_engine* e, const float* d_crops, int n_src, int B, c
 // Affine crops (frame_to_patch_rows_affine) take a matrix per box instead of a box, and their keypoints are decoded with
 // centre / scale (decode mode 4) instead of canvas sizes and offsets.
 // NV12 frames come as an Nv12Entry table instead (each entry carries the call's YUV matrix); the gathers then launch the
-// NV12 instantiation of the same kernels, outside the captured graph, so the graph caches need no NV12 key.
+// NV12 instantiation of the same kernels, outside the captured graph, so the graph cache needs no NV12 key.
 struct Source {
   const float* crops = nullptr;
   const FrameEntry* frames = nullptr;       // num_frames entries, only frames that have boxes
@@ -1549,9 +1546,9 @@ extern "C" int vpb_decode_frame(const float* d_heatmaps, int32_t n, int32_t k, c
 // Crops one keypoint call runs through the model: the batch, and with flip test on its mirror images as well.
 static int model_crops(const vpb_engine* e, int batch) { return e->flip ? 2 * batch : batch; }
 
-// Flip test: `raw` holds the raw maps of one forward, crop c at raw + c * kstride maps (kstride 0 = k) and its mirror image
-// `mirror` crops later; `out` (same layout; may be `raw`) gets the flip-back average of the first `batch` crops, with head
-// permutation `perm` of k keypoints.
+// Flip test: `raw` holds the raw maps of one forward, crop c at raw + c * kstride maps and its mirror image `mirror` crops
+// later; `out` (same layout; may be `raw`) gets the flip-back average of the first `batch` crops, with head permutation `perm`
+// of k keypoints.
 static int flip_average(vpb_engine* e, const float* raw, int batch, int k, const int* perm, int kstride, int mirror, float* out,
                         cudaStream_t st) {
   const long long tot = static_cast<long long>(batch) * k * 3072;
@@ -1560,80 +1557,138 @@ static int flip_average(vpb_engine* e, const float* raw, int batch, int k, const
   e->prof.end(st);
   return VPB_OK;
 }
-// the single-head calls: e->heat holds the 2 * batch raw maps; `out` (batch maps; may be e->heat) gets their average
-static int flip_average(vpb_engine* e, int batch, float* out, cudaStream_t st) {
-  return flip_average(e, e->heat, batch, e->K, e->flip_perm, 0, batch, out, st);
+
+// first entry of head j's permutation in flip_perm (the heads' permutations concatenated in head order)
+static int perm_offset(const vpb_engine* e, int j) {
+  int off = 0;
+  for (int i = 0; i < j; ++i) off += e->hw[i].K;
+  return off;
 }
 
-// The decode of a keypoint call: canvas sizes + frame offsets (VitInference.postprocess, one reference call per crop), or for
-// the affine calls centre / scale (mode 4, one reference call on the whole array, exactly as vpb_decode_modes).
-static int decode_keypoints(vpb_engine* e, const float* heat, int32_t batch, const int32_t* d_org_wh, const int32_t* d_offs_yx,
-                            const float* d_cs, float* d_kpts, int32_t* d_idx, cudaStream_t st) {
-  if (d_cs) return vpb_decode_modes(heat, batch, e->K, DECODE_DARK_UDP, d_cs, nullptr, d_kpts, d_idx, st);
-  return decode_launch(heat, batch, e->K, d_org_wh, d_offs_yx, d_kpts, d_idx, 0, st);
+// The segments the model runs for a call: `segs`, and with flip test on `segs` again for the mirror images (the gathers
+// mirror crop b - n into model crop b >= n), runs of one head merged across the seam.
+static std::vector<Segment> model_segments(const vpb_engine* e, const std::vector<Segment>& segs) {
+  std::vector<Segment> out = segs;
+  if (!e->flip) return out;
+  for (const Segment& sg : segs) {
+    if (out.back().head == sg.head) out.back().count += sg.count;
+    else out.push_back(sg);
+  }
+  return out;
 }
 
-// `heat` receives the batch maps the keypoints are decoded from; with flip test the raw 2 * batch maps go to e->heat first
-static int infer_enqueue(vpb_engine* e, const Source& src, const int32_t* d_org_wh, const int32_t* d_offs_yx, int32_t batch,
-                         float* d_kpts, int32_t* d_idx, float* heat, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int nb = model_crops(e, batch);
-  VPB_TRY(gather(e, src, batch, nb, st));
-  VPB_TRY(backbone(e, nb, st));
+// Keypoint rows per crop in a call's outputs: head 0's K for the single-head calls, K_max for the multi-head calls.
+static int row_stride(const vpb_engine* e, bool mixed) { return mixed ? e->Kmax : e->K; }
+
+// The keypoint pipeline of every call; a single-head call is the one segment {head 0, n} with kstride = head 0's K.
+// Gather (unless done), backbone with the experts of the model segments, then per model segment the head's deconvs + 1x1 conv
+// (crop c at c * kstride maps), and per segment the flip-back average (flip test: raw maps in e->heat, average into `heat`)
+// and the decode of its K_head maps into kpts [n, kstride, 3] / idx [n, kstride].  d_cs (affine calls): centre / scale,
+// decode mode 4 as one reference call per segment; else canvas sizes + offsets, one reference call per crop.  A call whose
+// model crops all use head 0 runs the single-head backbone launches.
+static int heads_enqueue(vpb_engine* e, const Source* src, const std::vector<Segment>& segs, int n, int kstride, const int32_t* d_org_wh,
+                         const int32_t* d_offs_yx, const float* d_cs, float* d_kpts, int32_t* d_idx, float* heat, cudaStream_t st) {
+  const std::vector<Segment> msegs = model_segments(e, segs);
+  const int nb = model_crops(e, n);
+  if (src) VPB_TRY(gather(e, *src, n, nb, st));
+  VPB_TRY(backbone(e, nb, st, (msegs.size() == 1 && msegs[0].head == 0) ? nullptr : &msegs));
   if (e->stop_after && e->stop_after <= 10) return VPB_OK;
-  VPB_TRY(head(e, nb, e->flip ? e->heat : heat, st));
+  float* raw = e->flip ? e->heat : heat;
+  int c0 = 0;
+  for (const Segment& sg : msegs) {
+    VPB_TRY(head(e, sg.count, raw + static_cast<size_t>(c0) * kstride * 3072, st, sg.head, c0, kstride));
+    c0 += sg.count;
+  }
   if (e->stop_after) return VPB_OK;
-  if (e->flip) VPB_TRY(flip_average(e, batch, heat, st));
-  e->prof.begin(KC_DECODE, static_cast<cudaStream_t>(stream));
-  VPB_TRY(decode_keypoints(e, heat, batch, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, st));
-  e->prof.end(static_cast<cudaStream_t>(stream));
+  c0 = 0;
+  for (const Segment& sg : segs) {
+    const size_t m0 = static_cast<size_t>(c0) * kstride * 3072;
+    const int K = e->hw[sg.head].K;
+    if (e->flip) VPB_TRY(flip_average(e, raw + m0, sg.count, K, e->flip_perm + perm_offset(e, sg.head), kstride, n, heat + m0, st));
+    DecodeParams p;
+    p.heatmaps = heat + m0; p.org_wh = d_cs ? nullptr : d_org_wh + 2 * c0; p.offs_yx = (d_offs_yx && !d_cs) ? d_offs_yx + 2 * c0 : nullptr;
+    p.kpts = d_kpts + static_cast<size_t>(c0) * kstride * 3; p.idx = d_idx ? d_idx + static_cast<size_t>(c0) * kstride : nullptr;
+    p.n = sg.count; p.k = K; p.kstride = kstride;
+    p.wrap_batch = d_cs ? 1 : 0;                            // mode 4: keypoints_from_heatmaps on the segment's array
+    p.cs32 = d_cs ? d_cs + 4 * c0 : nullptr;
+    e->prof.begin(KC_DECODE, st);
+    CU_TRY(launch_k(decode_heatmaps<false>, dim3(cdiv(static_cast<long long>(p.n) * p.k, DECODE_WARPS)), dim3(DECODE_WARPS * 32), 0, st, p));
+    e->prof.end(st);
+    c0 += sg.count;
+  }
   return VPB_OK;
 }
 
-// crops -> keypoints; d_offs_yx (nullable) moves the keypoints from crop to frame coordinates inside the decode kernel
-static int infer_core_locked(vpb_engine* e, const Source& src, const int32_t* d_org_wh, const int32_t* d_offs_yx, int32_t batch,
-                             float* d_kpts, int32_t* d_idx, float* d_heatmaps, void* stream);
-static int infer_core(vpb_engine* e, const Source& src, const int32_t* d_org_wh, const int32_t* d_offs_yx, int32_t batch,
-                      float* d_kpts, int32_t* d_idx, float* d_heatmaps, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  VPB_TRY(apply_l2_policy(e, st));
-  WsScope ws(e, st);
-  VPB_TRY(ws.begin(model_crops(e, batch)));
-  VPB_TRY(infer_core_locked(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, d_heatmaps, stream));
-  return ws.end();
+// rows 0 .. K_head-1 of every crop of every segment: [n, kstride, row] -> [n, kstride, row] (rows past K_head are left alone);
+// one contiguous copy for a segment whose head's K is the stride, as in every single-head call
+static int copy_head_rows(const vpb_engine* e, const std::vector<Segment>& segs, int kstride, void* dst, const void* src, size_t row_bytes,
+                          cudaMemcpyKind kind, cudaStream_t st) {
+  const size_t pitch = static_cast<size_t>(kstride) * row_bytes;
+  size_t off = 0;
+  for (const Segment& sg : segs) {
+    char* d = static_cast<char*>(dst) + off;
+    const char* s = static_cast<const char*>(src) + off;
+    const size_t width = e->hw[sg.head].K * row_bytes;
+    if (width == pitch) CU_TRY(cudaMemcpyAsync(d, s, sg.count * pitch, kind, st));
+    else CU_TRY(cudaMemcpy2DAsync(d, pitch, s, pitch, width, sg.count, kind, st));
+    off += sg.count * pitch;
+  }
+  return VPB_OK;
 }
-static int infer_core_locked(vpb_engine* e, const Source& src, const int32_t* d_org_wh, const int32_t* d_offs_yx, int32_t batch,
-                             float* d_kpts, int32_t* d_idx, float* d_heatmaps, void* stream) {
+
+static_assert(2 * VPB_MAX_SEGMENTS <= EXPERT_MAX_SEGMENTS, "a flip-test call's crops and mirror images fit the expert GEMM's table");
+constexpr size_t kMaxMixedGraphs = 16;
+
+static void drop_graphs(vpb_engine* e) {
+  for (auto& g : e->graph_cache) if (g.exec) cudaGraphExecDestroy(g.exec);
+  e->graph_cache.clear();
+}
+
+// Graph replay of everything behind the gather (see vpb_engine::graph_cache): eager on a key's first use, captured on its
+// second.  The gather runs eagerly in front of the replay; the decode inputs move to g_org / g_offs, or for the affine calls
+// the centre / scale to g_cs, and the outputs come back from g_kpts / g_idx / heat.  mixed: a multi-head entry point.
+static int heads_core_locked(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, bool mixed, int n, const int32_t* d_org_wh,
+                             const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
   float* heat = d_heatmaps ? d_heatmaps : e->heat;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int ks = row_stride(e, mixed);
   // eager launches on the legacy default stream (cannot be captured) and when the CALLER is already capturing `st`
   // (a nested cudaStreamBeginCapture would fail): the engine's kernels then simply become nodes of the caller's graph
   if (!e->use_graph || e->prof.on || e->stop_after || st == nullptr || stream_is_capturing(st))
-    return infer_enqueue(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, heat, stream);
+    return heads_enqueue(e, &src, segs, n, ks, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, heat, st);
   const bool affine = src.cs != nullptr;
-  vpb_engine::GraphEntry* g = nullptr;
-  for (auto& c : e->graphs)
-    if (c.batch == batch && c.affine == affine) g = &c;
-  if (!g) {                                                               // first use of this batch size: run eagerly
-    e->graphs.push_back({batch, 1, nullptr, affine});
-    return infer_enqueue(e, src, d_org_wh, d_offs_yx, batch, d_kpts, d_idx, heat, stream);
+  vpb_engine::CachedGraph* g = nullptr;
+  for (auto& c : e->graph_cache)
+    if (c.mixed == mixed && c.segs == segs && c.affine == affine) g = &c;
+  if (!g) {                                                               // first use of this key: run eagerly
+    if (mixed) {
+      auto lru = e->graph_cache.end();
+      size_t count = 0;
+      for (auto it = e->graph_cache.begin(); it != e->graph_cache.end(); ++it)
+        if (it->mixed) {
+          ++count;
+          if (lru == e->graph_cache.end() || it->used < lru->used) lru = it;
+        }
+      if (count == kMaxMixedGraphs) {
+        if (lru->exec) cudaGraphExecDestroy(lru->exec);
+        e->graph_cache.erase(lru);
+      }
+    }
+    e->graph_cache.push_back({mixed, segs, affine, nullptr, ++e->graph_clock});
+    return heads_enqueue(e, &src, segs, n, ks, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, heat, st);
   }
-  const int nb = model_crops(e, batch);
-  VPB_TRY(gather(e, src, batch, nb, st));
+  g->used = ++e->graph_clock;
+  VPB_TRY(gather(e, src, n, model_crops(e, n), st));
   if (affine) {
-    CU_TRY(cudaMemcpyAsync(e->g_cs, src.cs, static_cast<size_t>(batch) * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CU_TRY(cudaMemcpyAsync(e->g_cs, src.cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
   } else {
-    CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(batch) * 2 * sizeof(int32_t), st));
+    CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(n) * 2 * sizeof(int32_t), st));
   }
   if (!g->exec) {                                                         // second use: capture, instantiate
     cudaGraph_t graph = nullptr;
     CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = backbone(e, nb, st);
-    if (rc == VPB_OK) rc = head(e, nb, e->heat, st);
-    if (rc == VPB_OK && e->flip) rc = flip_average(e, batch, e->heat, st);      // in place: the first batch maps
-    if (rc == VPB_OK) rc = decode_keypoints(e, e->heat, batch, e->g_org, e->g_offs, affine ? e->g_cs : nullptr, e->g_kpts, e->g_idx, st);
+    const int rc = heads_enqueue(e, nullptr, segs, n, ks, e->g_org, e->g_offs, affine ? e->g_cs : nullptr, e->g_kpts, e->g_idx, e->heat, st);
     const cudaError_t ce = cudaStreamEndCapture(st, &graph);
     if (rc != VPB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
     if (ce != cudaSuccess) return fail(VPB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
@@ -1642,10 +1697,31 @@ static int infer_core_locked(vpb_engine* e, const Source& src, const int32_t* d_
     if (ie != cudaSuccess) { g->exec = nullptr; return fail(VPB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(ie)); }
   }
   CU_TRY(cudaGraphLaunch(g->exec, st));
-  CU_TRY(cudaMemcpyAsync(d_kpts, e->g_kpts, static_cast<size_t>(batch) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  if (d_idx) CU_TRY(cudaMemcpyAsync(d_idx, e->g_idx, static_cast<size_t>(batch) * e->K * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  if (d_heatmaps)
-    CU_TRY(cudaMemcpyAsync(d_heatmaps, e->heat, static_cast<size_t>(batch) * e->K * 3072 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  VPB_TRY(copy_head_rows(e, segs, ks, d_kpts, e->g_kpts, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (d_idx) VPB_TRY(copy_head_rows(e, segs, ks, d_idx, e->g_idx, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  if (d_heatmaps) VPB_TRY(copy_head_rows(e, segs, ks, d_heatmaps, e->heat, 3072 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return VPB_OK;
+}
+// crops (or frames + boxes, or affine crops: `src`) -> keypoints; d_offs_yx (nullable) moves the keypoints from crop to frame
+// coordinates inside the decode kernel
+static int heads_core(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, bool mixed, int n, const int32_t* d_org_wh,
+                      const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
+  VPB_TRY(apply_l2_policy(e, st));
+  WsScope ws(e, st);
+  VPB_TRY(ws.begin(model_crops(e, n)));
+  VPB_TRY(heads_core_locked(e, src, segs, mixed, n, d_org_wh, d_offs_yx, d_kpts, d_idx, d_heatmaps, st));
+  return ws.end();
+}
+
+// The end of every host call: D2H of the keypoint and argmax rows of staging slot `slot` on `st`, the stream that computed
+// them, then ev_done[slot] for the slot's next user; the synchronous forms (sync) wait for it all.
+static int host_tail(vpb_engine* e, const std::vector<Segment>& segs, bool mixed, int slot, float* h_kpts, int32_t* h_idx, cudaStream_t st,
+                     bool sync) {
+  const int ks = row_stride(e, mixed);
+  VPB_TRY(copy_head_rows(e, segs, ks, h_kpts, e->kpts[slot], 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_idx) VPB_TRY(copy_head_rows(e, segs, ks, h_idx, e->idx[slot], sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CU_TRY(cudaEventRecord(e->ev_done[slot], st));
+  if (sync) CU_TRY(cudaStreamSynchronize(st));
   return VPB_OK;
 }
 
@@ -1656,7 +1732,7 @@ extern "C" int vpb_infer(vpb_engine* e, const float* d_crops, const int32_t* d_o
   if (!d_crops || !d_org_wh || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer: null pointer");
   Source src;
   src.crops = d_crops;
-  return infer_core(e, src, d_org_wh, nullptr, batch, d_kpts, d_idx, d_heatmaps, stream);
+  return heads_core(e, src, {{0, batch}}, false, batch, d_org_wh, nullptr, d_kpts, d_idx, d_heatmaps, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ frame-level entry points
@@ -1678,14 +1754,15 @@ extern "C" int vpb_preprocess(const uint8_t* d_frame, int32_t frame_h, int32_t f
 
 static_assert(VPB_MAX_FRAMES == FP_MAX_FRAMES, "the header's frame limit is the gather's table size");
 
-// `tab`: num_frames frames with boxes, first_box ascending; d_bboxes holds their n boxes in frame order
+// Keypoints of the boxes d_bboxes of a frame table, or with d_mats of its affine crops (centre / scale d_cs for the decode;
+// the canvas sizes and offsets are then unused).  The crops are never materialised: the gathers write the bf16 patch rows
+// directly.  `tab`: num_frames frames with boxes, first_box ascending; the n boxes are in frame order.
 template <class Entry>
-static int infer_frames_enqueue(vpb_engine* e, const Entry* tab, int num_frames, const int32_t* d_bboxes, int32_t n,
-                                float* d_kpts, int32_t* d_idx, cudaStream_t st) {
-  Source src;                   // the crops are never materialised: frame_to_patch_rows writes the bf16 patch rows directly
-  set_table(src, tab); src.num_frames = num_frames; src.bboxes = d_bboxes;
-  VPB_TRY(apply_l2_policy(e, st));
-  return infer_core(e, src, e->pp_org, e->pp_offs, n, d_kpts, d_idx, nullptr, st);
+static int frames_core(vpb_engine* e, const Entry* tab, int num_frames, const int32_t* d_bboxes, const double* d_mats, const float* d_cs,
+                       const std::vector<Segment>& segs, bool mixed, int32_t n, float* d_kpts, int32_t* d_idx, cudaStream_t st) {
+  Source src;
+  set_table(src, tab); src.num_frames = num_frames; src.bboxes = d_bboxes; src.mats = d_mats; src.cs = d_cs;
+  return heads_core(e, src, segs, mixed, n, e->pp_org, e->pp_offs, d_kpts, d_idx, nullptr, st);
 }
 
 // one packed frame that owns every box of the call
@@ -1697,98 +1774,68 @@ static FrameEntry single_frame(const uint8_t* data, int32_t fh, int32_t fw) {
 }
 
 // The caller's frame array -> the gather's table.  Frames without boxes are left out (they do not count towards
-// VPB_MAX_FRAMES); pitch_bytes 0 means packed rows.  *n = the total number of boxes, checked against the batch limit.
-// build_frame_table is the engine-free part (vpb_preprocess_affine): at most `limit` boxes.
-static int build_frame_table(const char* fn, const vpb_frame* fr, int32_t num_frames, int limit, FrameEntry* tab, int* num_tab,
+// VPB_MAX_FRAMES).  *n = the total number of boxes, checked against the batch limit.  build_frame_table is the engine-free
+// part (vpb_preprocess_affine): at most `limit` boxes.  Per frame type, check_call checks what applies to the whole call and
+// table_entry one frame with boxes and its entry (first_box is filled by the caller):
+//   vpb_frame        pitch_bytes 0 (packed rows) or >= 3 * width; `matrix` is unused
+//   vpb_frame_nv12   even height and width >= 2, pitches 0 (packed: width) or >= width, both planes non-NULL, and a known
+//                    matrix, written into every entry
+static int check_call(const char*, const vpb_frame*, int32_t) { return VPB_OK; }
+static int check_call(const char* fn, const vpb_frame_nv12*, int32_t matrix) {
+  if (matrix != VPB_YUV_BT601 && matrix != VPB_YUV_BT709)
+    return fail(VPB_ERR_ARG, "%s: unknown YUV matrix %d (VPB_YUV_BT601 or VPB_YUV_BT709 expected)", fn, matrix);
+  return VPB_OK;
+}
+static int table_entry(const char* fn, int j, const vpb_frame& f, int32_t, FrameEntry* t) {
+  const long long pitch = f.pitch_bytes ? f.pitch_bytes : 3LL * f.width;
+  if (!f.data || f.height < 1 || f.width < 1 || pitch < 3LL * f.width)
+    return fail(VPB_ERR_ARG, "%s: frame %d: data %p, %dx%d (w x h), pitch %lld bytes (0 or >= 3 * width expected)", fn, j,
+                static_cast<const void*>(f.data), f.width, f.height, static_cast<long long>(f.pitch_bytes));
+  memset(t, 0, sizeof(*t));
+  t->data = f.data; t->pitch = pitch; t->fh = f.height; t->fw = f.width;
+  return VPB_OK;
+}
+static int table_entry(const char* fn, int j, const vpb_frame_nv12& f, int32_t matrix, Nv12Entry* t) {
+  const long long yp = f.y_pitch ? f.y_pitch : f.width, uvp = f.uv_pitch ? f.uv_pitch : f.width;
+  if (!f.y || !f.uv || f.height < 2 || f.width < 2 || (f.height & 1) || (f.width & 1) || yp < f.width || uvp < f.width)
+    return fail(VPB_ERR_ARG, "%s: frame %d: y %p, uv %p, %dx%d (w x h, even and >= 2 expected), pitches %lld / %lld bytes "
+                "(0 or >= width expected)", fn, j, static_cast<const void*>(f.y), static_cast<const void*>(f.uv), f.width, f.height,
+                static_cast<long long>(f.y_pitch), static_cast<long long>(f.uv_pitch));
+  memset(t, 0, sizeof(*t));
+  t->y = f.y; t->uv = f.uv; t->y_pitch = yp; t->uv_pitch = uvp; t->fh = f.height; t->fw = f.width; t->matrix = matrix;
+  return VPB_OK;
+}
+template <class Frame, class Entry>
+static int build_frame_table(const char* fn, const Frame* fr, int32_t num_frames, int32_t matrix, int limit, Entry* tab, int* num_tab,
                              int32_t* n) {
   if (num_frames < 0 || (num_frames > 0 && !fr)) return fail(VPB_ERR_ARG, "%s: %d frames, frame array %p", fn, num_frames, fr);
+  VPB_TRY(check_call(fn, fr, matrix));
   long long boxes = 0;
   int used = 0;
   for (int j = 0; j < num_frames; ++j) {
-    const vpb_frame& f = fr[j];
+    const Frame& f = fr[j];
     if (f.num_boxes < 0) return fail(VPB_ERR_ARG, "%s: frame %d has num_boxes = %d", fn, j, f.num_boxes);
     if (f.num_boxes == 0) continue;
-    const long long pitch = f.pitch_bytes ? f.pitch_bytes : 3LL * f.width;
-    if (!f.data || f.height < 1 || f.width < 1 || pitch < 3LL * f.width)
-      return fail(VPB_ERR_ARG, "%s: frame %d: data %p, %dx%d (w x h), pitch %lld bytes (0 or >= 3 * width expected)", fn, j,
-                  static_cast<const void*>(f.data), f.width, f.height, static_cast<long long>(f.pitch_bytes));
+    Entry t;
+    VPB_TRY(table_entry(fn, j, f, matrix, &t));
     if (used == VPB_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than VPB_MAX_FRAMES = %d frames with boxes", fn, VPB_MAX_FRAMES);
     if (boxes + f.num_boxes > limit)
       return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, limit, j);
-    FrameEntry& t = tab[used++];
-    memset(&t, 0, sizeof(t));
-    t.data = f.data; t.pitch = pitch; t.fh = f.height; t.fw = f.width; t.first_box = static_cast<int>(boxes);
+    t.first_box = static_cast<int>(boxes);
+    tab[used++] = t;
     boxes += f.num_boxes;
   }
   *num_tab = used;
   *n = static_cast<int32_t>(boxes);
   return VPB_OK;
 }
-static int frame_table(const char* fn, vpb_engine* e, const vpb_frame* fr, int32_t num_frames, FrameEntry* tab, int* num_tab,
+template <class Frame, class Entry>
+static int frame_table(const char* fn, vpb_engine* e, const Frame* fr, int32_t num_frames, int32_t matrix, Entry* tab, int* num_tab,
                        int32_t* n) {
   if (!e) return fail(VPB_ERR_ARG, "null engine");
   if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
-  VPB_TRY(build_frame_table(fn, fr, num_frames, e->maxB, tab, num_tab, n));
+  VPB_TRY(build_frame_table(fn, fr, num_frames, matrix, e->maxB, tab, num_tab, n));
   return *n ? check_ready_keypoints(e, *n) : VPB_OK;
-}
-// The NV12 counterpart: even height and width >= 2, pitches 0 (packed: width) or >= width, both planes non-NULL, a known
-// matrix (written into every entry).  Frame and box limits as build_frame_table.
-static int build_frame_table_nv12(const char* fn, const vpb_frame_nv12* fr, int32_t num_frames, int32_t matrix, int limit,
-                                  Nv12Entry* tab, int* num_tab, int32_t* n) {
-  if (num_frames < 0 || (num_frames > 0 && !fr)) return fail(VPB_ERR_ARG, "%s: %d frames, frame array %p", fn, num_frames, fr);
-  if (matrix != VPB_YUV_BT601 && matrix != VPB_YUV_BT709)
-    return fail(VPB_ERR_ARG, "%s: unknown YUV matrix %d (VPB_YUV_BT601 or VPB_YUV_BT709 expected)", fn, matrix);
-  long long boxes = 0;
-  int used = 0;
-  for (int j = 0; j < num_frames; ++j) {
-    const vpb_frame_nv12& f = fr[j];
-    if (f.num_boxes < 0) return fail(VPB_ERR_ARG, "%s: frame %d has num_boxes = %d", fn, j, f.num_boxes);
-    if (f.num_boxes == 0) continue;
-    const long long yp = f.y_pitch ? f.y_pitch : f.width, uvp = f.uv_pitch ? f.uv_pitch : f.width;
-    if (!f.y || !f.uv || f.height < 2 || f.width < 2 || (f.height & 1) || (f.width & 1) || yp < f.width || uvp < f.width)
-      return fail(VPB_ERR_ARG, "%s: frame %d: y %p, uv %p, %dx%d (w x h, even and >= 2 expected), pitches %lld / %lld bytes "
-                  "(0 or >= width expected)", fn, j, static_cast<const void*>(f.y), static_cast<const void*>(f.uv), f.width, f.height,
-                  static_cast<long long>(f.y_pitch), static_cast<long long>(f.uv_pitch));
-    if (used == VPB_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than VPB_MAX_FRAMES = %d frames with boxes", fn, VPB_MAX_FRAMES);
-    if (boxes + f.num_boxes > limit)
-      return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, limit, j);
-    Nv12Entry& t = tab[used++];
-    memset(&t, 0, sizeof(t));
-    t.y = f.y; t.uv = f.uv; t.y_pitch = yp; t.uv_pitch = uvp; t.fh = f.height; t.fw = f.width;
-    t.first_box = static_cast<int>(boxes); t.matrix = matrix;
-    boxes += f.num_boxes;
-  }
-  *num_tab = used;
-  *n = static_cast<int32_t>(boxes);
-  return VPB_OK;
-}
-static int frame_table_nv12(const char* fn, vpb_engine* e, const vpb_frame_nv12* fr, int32_t num_frames, int32_t matrix, Nv12Entry* tab,
-                            int* num_tab, int32_t* n) {
-  if (!e) return fail(VPB_ERR_ARG, "null engine");
-  if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
-  VPB_TRY(build_frame_table_nv12(fn, fr, num_frames, matrix, e->maxB, tab, num_tab, n));
-  return *n ? check_ready_keypoints(e, *n) : VPB_OK;
-}
-
-extern "C" int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int32_t frame_w, const int32_t* d_bboxes,
-                               int32_t n, float* d_kpts, int32_t* d_idx, void* stream) {
-  VPB_TRY(check_ready_keypoints(e, n));
-  DeviceGuard dev_guard(e);
-  if (!d_frame || !d_bboxes || !d_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame: bad argument");
-  const FrameEntry f = single_frame(d_frame, frame_h, frame_w);
-  return infer_frames_enqueue(e, &f, 1, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int vpb_infer_frames(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* d_bboxes,
-                                float* d_kpts, int32_t* d_idx, void* stream) {
-  FrameEntry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_frames", e, h_frames, num_frames, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames: null pointer");
-  return infer_frames_enqueue(e, tab, nt, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 
 // Status word of the device-side frame path (bit 0: a box was empty after padding + clipping; such a box is decoded from
@@ -1825,6 +1872,18 @@ static int check_frames_boxes_host(const Frame* fr, int32_t num_frames, const in
     VPB_TRY(check_boxes_host(bb + 4 * static_cast<size_t>(first), fr[j].num_boxes, fr[j].height, fr[j].width, j));
   return VPB_OK;
 }
+// host matrices / centre-scale: what the device forms can only flag in the status word is an argument error here
+static int check_affine_host(const double* mats, const float* cs, int32_t n) {
+  for (int i = 0; i < n; ++i) {
+    for (int j = 0; j < 6; ++j)
+      if (!std::isfinite(mats[6 * i + j])) return fail(VPB_ERR_ARG, "box %d: matrix entry %d is %g (finite expected)", i, j, mats[6 * i + j]);
+    if (!cs) continue;
+    const float* c = cs + 4 * i;
+    if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !(c[2] > 0.f) || !(c[3] > 0.f) || !std::isfinite(c[2]) || !std::isfinite(c[3]))
+      return fail(VPB_ERR_ARG, "box %d: centre (%g, %g), scale (%g, %g): finite centre and scale > 0 expected", i, c[0], c[1], c[2], c[3]);
+  }
+  return VPB_OK;
+}
 static int frame_stage_reserve(vpb_engine* e, int slot, size_t bytes) {
   if (e->frame_cap[slot] >= bytes) return VPB_OK;
   if (e->frame_stage[slot]) { CU_TRY(cudaDeviceSynchronize()); CU_TRY(cudaFree(e->frame_stage[slot])); e->frame_stage[slot] = nullptr; e->frame_cap[slot] = 0; }
@@ -1858,10 +1917,12 @@ static int stage_entry(Nv12Entry& t, uint8_t* dst, cudaStream_t st) {
   return VPB_OK;
 }
 // Host frames -> staging slot `slot`, enqueued on `st` after the slot's last user: each frame packed (a 2D copy from its pitch;
-// NV12: its Y plane, then its UV plane, 1.5 B per pixel), then the boxes of all frames in one copy (none for h_bboxes = NULL: the
-// affine calls stage matrices instead).  Repoints `tab` at the staged frames.
+// NV12: its Y plane, then its UV plane, 1.5 B per pixel), then the boxes of all frames in one copy, or for the affine calls
+// (h_mats) the matrices and the centre / scale (slot 0: the affine calls have no pipelined form).  Repoints `tab` at the
+// staged frames.
 template <class Entry>
-static int stage_frames_host(vpb_engine* e, int slot, Entry* tab, int nt, const int32_t* h_bboxes, int32_t n, cudaStream_t st) {
+static int stage_frames_host(vpb_engine* e, int slot, Entry* tab, int nt, const int32_t* h_bboxes, const double* h_mats, const float* h_cs,
+                             int32_t n, cudaStream_t st) {
   size_t total = 0;
   for (int j = 0; j < nt; ++j) total += staged_bytes(tab[j]);
   VPB_TRY(frame_stage_reserve(e, slot, total));
@@ -1872,34 +1933,44 @@ static int stage_frames_host(vpb_engine* e, int slot, Entry* tab, int nt, const 
     VPB_TRY(stage_entry(tab[j], e->frame_stage[slot] + off, st));
     off += bytes;
   }
-  if (h_bboxes) CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (h_mats) {
+    CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
+  } else {
+    CU_TRY(cudaMemcpyAsync(e->bbox_stage[slot], h_bboxes, static_cast<size_t>(n) * 4 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
   return VPB_OK;
 }
-// synchronous host form on slot 0 and the caller's stream
+// synchronous host form on slot 0 and the caller's stream: the frames with their boxes (or affine matrices) staged, the call,
+// the host tail
 template <class Entry>
-static int frames_host_sync(vpb_engine* e, Entry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
-                            cudaStream_t st) {
-  VPB_TRY(stage_frames_host(e, 0, tab, nt, h_bboxes, n, st));
-  VPB_TRY(infer_frames_enqueue(e, tab, nt, e->bbox_stage[0], n, e->kpts[0], e->idx[0], st));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaEventRecord(e->ev_done[0], st));
-  CU_TRY(cudaStreamSynchronize(st));
-  return VPB_OK;
+static int frames_host_sync(vpb_engine* e, Entry* tab, int nt, const int32_t* h_bboxes, const double* h_mats, const float* h_cs,
+                            const std::vector<Segment>& segs, bool mixed, int32_t n, float* h_kpts, int32_t* h_idx, cudaStream_t st) {
+  VPB_TRY(stage_frames_host(e, 0, tab, nt, h_bboxes, h_mats, h_cs, n, st));
+  VPB_TRY(frames_core(e, tab, nt, e->bbox_stage[0], h_mats ? e->mat_stage : nullptr, h_mats ? e->cs_stage : nullptr, segs, mixed, n,
+                      e->kpts[0], e->idx[0], st));
+  return host_tail(e, segs, mixed, 0, h_kpts, h_idx, st, true);
 }
 // Pipelined frames (video): same slots, events and vpb_wait_host as vpb_submit_host; the H2D per step is the uint8 frames and
 // 16 B per box instead of 589 824 B per crop.
 template <class Entry>
 static int frames_host_submit(vpb_engine* e, Entry* tab, int nt, const int32_t* h_bboxes, int32_t n, float* h_kpts, int32_t* h_idx,
                               int slot) {
-  VPB_TRY(stage_frames_host(e, slot, tab, nt, h_bboxes, n, e->copy_stream));
+  VPB_TRY(stage_frames_host(e, slot, tab, nt, h_bboxes, nullptr, nullptr, n, e->copy_stream));
   CU_TRY(cudaEventRecord(e->ev_h2d[slot], e->copy_stream));
   CU_TRY(cudaStreamWaitEvent(e->compute_stream, e->ev_h2d[slot], 0));
-  VPB_TRY(infer_frames_enqueue(e, tab, nt, e->bbox_stage[slot], n, e->kpts[slot], e->idx[slot], e->compute_stream));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[slot], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->compute_stream));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[slot], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, e->compute_stream));
-  CU_TRY(cudaEventRecord(e->ev_done[slot], e->compute_stream));
-  return VPB_OK;
+  const std::vector<Segment> segs{{0, n}};
+  VPB_TRY(frames_core(e, tab, nt, e->bbox_stage[slot], nullptr, nullptr, segs, false, n, e->kpts[slot], e->idx[slot], e->compute_stream));
+  return host_tail(e, segs, false, slot, h_kpts, h_idx, e->compute_stream, false);
+}
+
+extern "C" int vpb_infer_frame(vpb_engine* e, const uint8_t* d_frame, int32_t frame_h, int32_t frame_w, const int32_t* d_bboxes,
+                               int32_t n, float* d_kpts, int32_t* d_idx, void* stream) {
+  VPB_TRY(check_ready_keypoints(e, n));
+  DeviceGuard dev_guard(e);
+  if (!d_frame || !d_bboxes || !d_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame: bad argument");
+  const FrameEntry f = single_frame(d_frame, frame_h, frame_w);
+  return frames_core(e, &f, 1, d_bboxes, nullptr, nullptr, {{0, n}}, false, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
@@ -1909,7 +1980,7 @@ extern "C" int vpb_infer_frame_host(vpb_engine* e, const uint8_t* h_frame, int32
   if (!h_frame || !h_bboxes || !h_kpts || frame_h < 1 || frame_w < 1) return fail(VPB_ERR_ARG, "vpb_infer_frame_host: bad argument");
   VPB_TRY(check_boxes_host(h_bboxes, n, frame_h, frame_w));
   FrameEntry f = single_frame(h_frame, frame_h, frame_w);
-  return frames_host_sync(e, &f, 1, h_bboxes, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+  return frames_host_sync(e, &f, 1, h_bboxes, nullptr, nullptr, {{0, n}}, false, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h, int32_t frame_w, const int32_t* h_bboxes,
@@ -1923,92 +1994,79 @@ extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int3
   return frames_host_submit(e, &f, 1, h_bboxes, n, h_kpts, h_idx, slot);
 }
 
+// ---- the multi-frame calls: one body per call kind, for RGB frames (vpb_frame -> FrameEntry; `matrix` unused) and NV12 frames
+// (vpb_frame_nv12 -> Nv12Entry); `fn` names the entry point in the messages
+template <class Entry, class Frame>
+static int infer_frames_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix, const int32_t* d_bboxes,
+                          float* d_kpts, int32_t* d_idx, void* stream) {
+  Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
+  return frames_core(e, tab, nt, d_bboxes, nullptr, nullptr, {{0, n}}, false, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+}
+template <class Entry, class Frame>
+static int infer_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix,
+                               const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
+  Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  return frames_host_sync(e, tab, nt, h_bboxes, nullptr, nullptr, {{0, n}}, false, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+}
+template <class Entry, class Frame>
+static int submit_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix,
+                                const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot) {
+  Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "%s: slot %d", fn, slot);
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
+  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
+  return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
+}
+
+extern "C" int vpb_infer_frames(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* d_bboxes,
+                                float* d_kpts, int32_t* d_idx, void* stream) {
+  return infer_frames_t<FrameEntry>("vpb_infer_frames", e, h_frames, num_frames, 0, d_bboxes, d_kpts, d_idx, stream);
+}
 extern "C" int vpb_infer_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
                                      float* h_kpts, int32_t* h_idx, void* stream) {
-  FrameEntry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_frames_host", e, h_frames, num_frames, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_host: null pointer");
-  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
-  return frames_host_sync(e, tab, nt, h_bboxes, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+  return infer_frames_host_t<FrameEntry>("vpb_infer_frames_host", e, h_frames, num_frames, 0, h_bboxes, h_kpts, h_idx, stream);
 }
-
 extern "C" int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
                                       float* h_kpts, int32_t* h_idx, int32_t slot) {
-  FrameEntry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table("vpb_submit_frames_host", e, h_frames, num_frames, tab, &nt, &n));
-  if (slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "vpb_submit_frames_host: slot %d", slot);
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_submit_frames_host: null pointer");
-  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
-  return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
+  return submit_frames_host_t<FrameEntry>("vpb_submit_frames_host", e, h_frames, num_frames, 0, h_bboxes, h_kpts, h_idx, slot);
 }
-
-// ---- the same three calls on NV12 frames
 extern "C" int vpb_infer_frames_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                      const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
-  Nv12Entry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table_nv12("vpb_infer_frames_nv12", e, h_frames, num_frames, matrix, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_nv12: null pointer");
-  return infer_frames_enqueue(e, tab, nt, d_bboxes, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+  return infer_frames_t<Nv12Entry>("vpb_infer_frames_nv12", e, h_frames, num_frames, matrix, d_bboxes, d_kpts, d_idx, stream);
 }
-
 extern "C" int vpb_infer_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                           const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
-  Nv12Entry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table_nv12("vpb_infer_frames_nv12_host", e, h_frames, num_frames, matrix, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_nv12_host: null pointer");
-  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
-  return frames_host_sync(e, tab, nt, h_bboxes, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+  return infer_frames_host_t<Nv12Entry>("vpb_infer_frames_nv12_host", e, h_frames, num_frames, matrix, h_bboxes, h_kpts, h_idx, stream);
 }
-
 extern "C" int vpb_submit_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                            const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot) {
-  Nv12Entry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table_nv12("vpb_submit_frames_nv12_host", e, h_frames, num_frames, matrix, tab, &nt, &n));
-  if (slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "vpb_submit_frames_nv12_host: slot %d", slot);
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_submit_frames_nv12_host: null pointer");
-  VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
-  return frames_host_submit(e, tab, nt, h_bboxes, n, h_kpts, h_idx, slot);
+  return submit_frames_host_t<Nv12Entry>("vpb_submit_frames_nv12_host", e, h_frames, num_frames, matrix, h_bboxes, h_kpts, h_idx, slot);
 }
 
 // ------------------------------------------------------------------------------------------------ affine top-down crops
-// host matrices / centre-scale: what the device forms can only flag in the status word is an argument error here
-static int check_affine_host(const double* mats, const float* cs, int32_t n) {
-  for (int i = 0; i < n; ++i) {
-    for (int j = 0; j < 6; ++j)
-      if (!std::isfinite(mats[6 * i + j])) return fail(VPB_ERR_ARG, "box %d: matrix entry %d is %g (finite expected)", i, j, mats[6 * i + j]);
-    if (!cs) continue;
-    const float* c = cs + 4 * i;
-    if (!std::isfinite(c[0]) || !std::isfinite(c[1]) || !(c[2] > 0.f) || !(c[3] > 0.f) || !std::isfinite(c[2]) || !std::isfinite(c[3]))
-      return fail(VPB_ERR_ARG, "box %d: centre (%g, %g), scale (%g, %g): finite centre and scale > 0 expected", i, c[0], c[1], c[2], c[3]);
-  }
-  return VPB_OK;
-}
-
 extern "C" int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, float* d_crops, void* stream) {
   FrameEntry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(build_frame_table("vpb_preprocess_affine", h_frames, num_frames, 1 << 30, tab, &nt, &n));
+  VPB_TRY(build_frame_table("vpb_preprocess_affine", h_frames, num_frames, 0, 1 << 30, tab, &nt, &n));
   if (n == 0) return VPB_OK;
   if (!d_mats || !d_crops) return fail(VPB_ERR_ARG, "vpb_preprocess_affine: null pointer");
   AffineParams q = affine_params(tab, nt, d_mats, nullptr, n, nullptr);
@@ -2018,101 +2076,57 @@ extern "C" int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_fram
   return VPB_OK;
 }
 
-template <class Entry>
-static int infer_affine_enqueue(vpb_engine* e, const Entry* tab, int num_frames, const double* d_mats, const float* d_cs, int32_t n,
-                                float* d_kpts, int32_t* d_idx, cudaStream_t st) {
-  Source src;
-  set_table(src, tab); src.num_frames = num_frames; src.mats = d_mats; src.cs = d_cs;
-  VPB_TRY(apply_l2_policy(e, st));
-  return infer_core(e, src, nullptr, nullptr, n, d_kpts, d_idx, nullptr, st);
+// RGB and NV12 as the multi-frame calls
+template <class Entry, class Frame>
+static int infer_affine_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix, const double* d_mats,
+                          const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
+  Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
+  return frames_core(e, tab, nt, nullptr, d_mats, d_cs, {{0, n}}, false, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
-// the synchronous host form on slot 0: frames, matrices and centre / scale staged, the call, D2H of the keypoints
-template <class Entry>
-static int affine_host_sync(vpb_engine* e, Entry* tab, int nt, const double* h_mats, const float* h_cs, int32_t n, float* h_kpts,
-                            int32_t* h_idx, cudaStream_t st) {
+template <class Entry, class Frame>
+static int infer_affine_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix,
+                               const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
+  Entry tab[VPB_MAX_FRAMES];
+  int nt = 0;
+  int32_t n = 0;
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  if (n == 0) return VPB_OK;
+  DeviceGuard dev_guard(e);
+  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   VPB_TRY(check_affine_host(h_mats, h_cs, n));
-  VPB_TRY(stage_frames_host(e, 0, tab, nt, nullptr, n, st));         // waits for slot 0's last user
-  CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
-  VPB_TRY(infer_affine_enqueue(e, tab, nt, e->mat_stage, e->cs_stage, n, e->kpts[0], e->idx[0], st));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(n) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(n) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaEventRecord(e->ev_done[0], st));
-  CU_TRY(cudaStreamSynchronize(st));
-  return VPB_OK;
+  return frames_host_sync(e, tab, nt, nullptr, h_mats, h_cs, {{0, n}}, false, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, const float* d_cs,
                                 float* d_kpts, int32_t* d_idx, void* stream) {
-  FrameEntry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_affine", e, h_frames, num_frames, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine: null pointer");
-  return infer_affine_enqueue(e, tab, nt, d_mats, d_cs, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+  return infer_affine_t<FrameEntry>("vpb_infer_affine", e, h_frames, num_frames, 0, d_mats, d_cs, d_kpts, d_idx, stream);
 }
-
 extern "C" int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* h_mats, const float* h_cs,
                                      float* h_kpts, int32_t* h_idx, void* stream) {
-  FrameEntry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_affine_host", e, h_frames, num_frames, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_host: null pointer");
-  return affine_host_sync(e, tab, nt, h_mats, h_cs, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+  return infer_affine_host_t<FrameEntry>("vpb_infer_affine_host", e, h_frames, num_frames, 0, h_mats, h_cs, h_kpts, h_idx, stream);
 }
-
 extern "C" int vpb_infer_affine_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                      const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
-  Nv12Entry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table_nv12("vpb_infer_affine_nv12", e, h_frames, num_frames, matrix, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_nv12: null pointer");
-  return infer_affine_enqueue(e, tab, nt, d_mats, d_cs, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
+  return infer_affine_t<Nv12Entry>("vpb_infer_affine_nv12", e, h_frames, num_frames, matrix, d_mats, d_cs, d_kpts, d_idx, stream);
 }
-
 extern "C" int vpb_infer_affine_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                           const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
-  Nv12Entry tab[VPB_MAX_FRAMES];
-  int nt = 0;
-  int32_t n = 0;
-  VPB_TRY(frame_table_nv12("vpb_infer_affine_nv12_host", e, h_frames, num_frames, matrix, tab, &nt, &n));
-  if (n == 0) return VPB_OK;
-  DeviceGuard dev_guard(e);
-  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_nv12_host: null pointer");
-  return affine_host_sync(e, tab, nt, h_mats, h_cs, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+  return infer_affine_host_t<Nv12Entry>("vpb_infer_affine_nv12_host", e, h_frames, num_frames, matrix, h_mats, h_cs, h_kpts, h_idx, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ multi-head calls
-static_assert(2 * VPB_MAX_SEGMENTS <= EXPERT_MAX_SEGMENTS, "a flip-test call's crops and mirror images fit the expert GEMM's table");
-constexpr size_t kMaxMixedGraphs = 16;
-
-static void drop_graphs(vpb_engine* e) {
-  for (auto& g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-  e->graphs.clear();
-  for (auto& g : e->mixed_graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-  e->mixed_graphs.clear();
-}
-
 static int check_ready_heads(vpb_engine* e, const char* fn) {
   if (!e) return fail(VPB_ERR_ARG, "%s: null engine", fn);
   if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
   if (e->flip && !e->flip_heads)
     return fail(VPB_ERR_STATE, "%s: flip test was set by vpb_set_flip_test; the multi-head calls take vpb_set_flip_test_heads", fn);
   return VPB_OK;
-}
-// first entry of head j's permutation in flip_perm (the heads' permutations concatenated in head order)
-static int perm_offset(const vpb_engine* e, int j) {
-  int off = 0;
-  for (int i = 0; i < j; ++i) off += e->hw[i].K;
-  return off;
 }
 // appends `count` crops of `head` to the runs (runs of one head merge; empty ones vanish)
 static int add_segment(vpb_engine* e, const char* fn, std::vector<Segment>& segs, int item, int head, int count) {
@@ -2122,126 +2136,6 @@ static int add_segment(vpb_engine* e, const char* fn, std::vector<Segment>& segs
   if (!segs.empty() && segs.back().head == head) segs.back().count += count;
   else segs.push_back({head, count});
   return VPB_OK;
-}
-
-// The segments the model runs for a multi-head call: `segs`, and with flip test on `segs` again for the mirror images (the
-// gathers mirror crop b - n into model crop b >= n), runs of one head merged across the seam.
-static std::vector<Segment> model_segments(const vpb_engine* e, const std::vector<Segment>& segs) {
-  std::vector<Segment> out = segs;
-  if (!e->flip) return out;
-  for (const Segment& sg : segs) {
-    if (out.back().head == sg.head) out.back().count += sg.count;
-    else out.push_back(sg);
-  }
-  return out;
-}
-
-// Gather (unless done), backbone with the experts of the model segments, then per model segment the head's deconvs + 1x1
-// conv (crop c at c * K_max maps), and per segment the flip-back average (flip test: raw maps in e->heat, average into
-// `heat`) and the decode of its K_head maps into kpts [n, K_max, 3] / idx [n, K_max].  d_cs (affine calls): centre / scale,
-// decode mode 4 as one reference call per segment; else canvas sizes + offsets, one reference call per crop.  A call whose
-// model crops all use head 0 runs the single-head backbone launches.
-static int heads_enqueue(vpb_engine* e, const Source* src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
-                         const int32_t* d_offs_yx, const float* d_cs, float* d_kpts, int32_t* d_idx, float* heat, cudaStream_t st) {
-  const int Km = e->Kmax;
-  const std::vector<Segment> msegs = model_segments(e, segs);
-  const int nb = model_crops(e, n);
-  if (src) VPB_TRY(gather(e, *src, n, nb, st));
-  VPB_TRY(backbone(e, nb, st, (msegs.size() == 1 && msegs[0].head == 0) ? nullptr : &msegs));
-  if (e->stop_after && e->stop_after <= 10) return VPB_OK;
-  float* raw = e->flip ? e->heat : heat;
-  int c0 = 0;
-  for (const Segment& sg : msegs) {
-    VPB_TRY(head(e, sg.count, raw + static_cast<size_t>(c0) * Km * 3072, st, sg.head, c0, Km));
-    c0 += sg.count;
-  }
-  if (e->stop_after) return VPB_OK;
-  c0 = 0;
-  for (const Segment& sg : segs) {
-    const size_t m0 = static_cast<size_t>(c0) * Km * 3072;
-    const int K = e->hw[sg.head].K;
-    if (e->flip) VPB_TRY(flip_average(e, raw + m0, sg.count, K, e->flip_perm + perm_offset(e, sg.head), Km, n, heat + m0, st));
-    DecodeParams p;
-    p.heatmaps = heat + m0; p.org_wh = d_cs ? nullptr : d_org_wh + 2 * c0; p.offs_yx = (d_offs_yx && !d_cs) ? d_offs_yx + 2 * c0 : nullptr;
-    p.kpts = d_kpts + static_cast<size_t>(c0) * Km * 3; p.idx = d_idx ? d_idx + static_cast<size_t>(c0) * Km : nullptr;
-    p.n = sg.count; p.k = K; p.kstride = Km;
-    p.wrap_batch = d_cs ? 1 : 0;                            // mode 4: keypoints_from_heatmaps on the segment's array
-    p.cs32 = d_cs ? d_cs + 4 * c0 : nullptr;
-    e->prof.begin(KC_DECODE, st);
-    CU_TRY(launch_k(decode_heatmaps<false>, dim3(cdiv(static_cast<long long>(p.n) * p.k, DECODE_WARPS)), dim3(DECODE_WARPS * 32), 0, st, p));
-    e->prof.end(st);
-    c0 += sg.count;
-  }
-  return VPB_OK;
-}
-
-// rows 0 .. K_head-1 of every crop of every segment: [n, K_max, row] -> [n, K_max, row] (rows past K_head are left alone)
-static int copy_head_rows(const vpb_engine* e, const std::vector<Segment>& segs, void* dst, const void* src, size_t row_bytes, cudaMemcpyKind kind,
-                          cudaStream_t st) {
-  const size_t pitch = static_cast<size_t>(e->Kmax) * row_bytes;
-  size_t off = 0;
-  for (const Segment& sg : segs) {
-    CU_TRY(cudaMemcpy2DAsync(static_cast<char*>(dst) + off, pitch, static_cast<const char*>(src) + off, pitch, e->hw[sg.head].K * row_bytes,
-                             sg.count, kind, st));
-    off += sg.count * pitch;
-  }
-  return VPB_OK;
-}
-
-// Graph replay as infer_core_locked, keyed by the segment list and the decode kind: eager on a key's first use, captured on
-// its second.  The affine graphs decode with the centre / scale copied to e->g_cs.
-static int heads_core_locked(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
-                             const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
-  float* heat = d_heatmaps ? d_heatmaps : e->heat;
-  if (!e->use_graph || e->prof.on || e->stop_after || st == nullptr || stream_is_capturing(st))
-    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, heat, st);
-  const bool affine = src.cs != nullptr;
-  vpb_engine::MixedGraph* g = nullptr;
-  for (auto& c : e->mixed_graphs)
-    if (c.segs == segs && c.affine == affine) g = &c;
-  if (!g) {                                                               // first use of this key: run eagerly
-    if (e->mixed_graphs.size() == kMaxMixedGraphs) {
-      auto lru = std::min_element(e->mixed_graphs.begin(), e->mixed_graphs.end(),
-                                  [](const vpb_engine::MixedGraph& a, const vpb_engine::MixedGraph& b) { return a.used < b.used; });
-      if (lru->exec) cudaGraphExecDestroy(lru->exec);
-      e->mixed_graphs.erase(lru);
-    }
-    e->mixed_graphs.push_back({segs, affine, nullptr, ++e->mixed_clock});
-    return heads_enqueue(e, &src, segs, n, d_org_wh, d_offs_yx, src.cs, d_kpts, d_idx, heat, st);
-  }
-  g->used = ++e->mixed_clock;
-  VPB_TRY(gather(e, src, n, model_crops(e, n), st));
-  if (affine) {
-    CU_TRY(cudaMemcpyAsync(e->g_cs, src.cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  } else {
-    CU_TRY(cudaMemcpyAsync(e->g_org, d_org_wh, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    if (d_offs_yx) CU_TRY(cudaMemcpyAsync(e->g_offs, d_offs_yx, static_cast<size_t>(n) * 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    else CU_TRY(cudaMemsetAsync(e->g_offs, 0, static_cast<size_t>(n) * 2 * sizeof(int32_t), st));
-  }
-  if (!g->exec) {
-    cudaGraph_t graph = nullptr;
-    CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int rc = heads_enqueue(e, nullptr, segs, n, e->g_org, e->g_offs, affine ? e->g_cs : nullptr, e->g_kpts, e->g_idx, e->heat, st);
-    const cudaError_t ce = cudaStreamEndCapture(st, &graph);
-    if (rc != VPB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) return fail(VPB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
-    const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ie != cudaSuccess) { g->exec = nullptr; return fail(VPB_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(ie)); }
-  }
-  CU_TRY(cudaGraphLaunch(g->exec, st));
-  VPB_TRY(copy_head_rows(e, segs, d_kpts, e->g_kpts, 3 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  if (d_idx) VPB_TRY(copy_head_rows(e, segs, d_idx, e->g_idx, sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  if (d_heatmaps) VPB_TRY(copy_head_rows(e, segs, d_heatmaps, e->heat, 3072 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return VPB_OK;
-}
-static int heads_core(vpb_engine* e, const Source& src, const std::vector<Segment>& segs, int n, const int32_t* d_org_wh,
-                      const int32_t* d_offs_yx, float* d_kpts, int32_t* d_idx, float* d_heatmaps, cudaStream_t st) {
-  VPB_TRY(apply_l2_policy(e, st));
-  WsScope ws(e, st);
-  VPB_TRY(ws.begin(model_crops(e, n)));
-  VPB_TRY(heads_core_locked(e, src, segs, n, d_org_wh, d_offs_yx, d_kpts, d_idx, d_heatmaps, st));
-  return ws.end();
 }
 
 extern "C" int vpb_infer_heads(vpb_engine* e, const float* d_crops, const int32_t* d_org_wh, const vpb_segment* h_segs, int32_t num_segs,
@@ -2263,7 +2157,7 @@ extern "C" int vpb_infer_heads(vpb_engine* e, const float* d_crops, const int32_
   if (!d_crops || !d_org_wh || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_heads: null pointer");
   Source src;
   src.crops = d_crops;
-  return heads_core(e, src, segs, static_cast<int>(n), d_org_wh, nullptr, d_kpts, d_idx, d_heatmaps, static_cast<cudaStream_t>(stream));
+  return heads_core(e, src, segs, true, static_cast<int>(n), d_org_wh, nullptr, d_kpts, d_idx, d_heatmaps, static_cast<cudaStream_t>(stream));
 }
 
 // the runs of equal head over the frames that have boxes (frame j's boxes all belong to head h_heads[j])
@@ -2281,15 +2175,13 @@ extern "C" int vpb_infer_frames_heads(vpb_engine* e, const vpb_frame* h_frames, 
   FrameEntry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_frames_heads", e, h_frames, num_frames, tab, &nt, &n));
+  VPB_TRY(frame_table("vpb_infer_frames_heads", e, h_frames, num_frames, 0, tab, &nt, &n));
   std::vector<Segment> segs;
   VPB_TRY(frame_segments(e, "vpb_infer_frames_heads", h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_heads: null pointer");
-  Source src;
-  src.frames = tab; src.num_frames = nt; src.bboxes = d_bboxes;
-  return heads_core(e, src, segs, n, e->pp_org, e->pp_offs, d_kpts, d_idx, nullptr, static_cast<cudaStream_t>(stream));
+  return frames_core(e, tab, nt, d_bboxes, nullptr, nullptr, segs, true, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
@@ -2298,23 +2190,14 @@ extern "C" int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_fra
   FrameEntry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_frames_heads_host", e, h_frames, num_frames, tab, &nt, &n));
+  VPB_TRY(frame_table("vpb_infer_frames_heads_host", e, h_frames, num_frames, 0, tab, &nt, &n));
   std::vector<Segment> segs;
   VPB_TRY(frame_segments(e, "vpb_infer_frames_heads_host", h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_heads_host: null pointer");
   VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  VPB_TRY(stage_frames_host(e, 0, tab, nt, h_bboxes, n, st));
-  Source src;
-  src.frames = tab; src.num_frames = nt; src.bboxes = e->bbox_stage[0];
-  VPB_TRY(heads_core(e, src, segs, n, e->pp_org, e->pp_offs, e->kpts[0], e->idx[0], nullptr, st));
-  VPB_TRY(copy_head_rows(e, segs, h_kpts, e->kpts[0], 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (h_idx) VPB_TRY(copy_head_rows(e, segs, h_idx, e->idx[0], sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaEventRecord(e->ev_done[0], st));
-  CU_TRY(cudaStreamSynchronize(st));
-  return VPB_OK;
+  return frames_host_sync(e, tab, nt, h_bboxes, nullptr, nullptr, segs, true, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
@@ -2323,15 +2206,13 @@ extern "C" int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, 
   FrameEntry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_affine_heads", e, h_frames, num_frames, tab, &nt, &n));
+  VPB_TRY(frame_table("vpb_infer_affine_heads", e, h_frames, num_frames, 0, tab, &nt, &n));
   std::vector<Segment> segs;
   VPB_TRY(frame_segments(e, "vpb_infer_affine_heads", h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_heads: null pointer");
-  Source src;
-  src.frames = tab; src.num_frames = nt; src.mats = d_mats; src.cs = d_cs;
-  return heads_core(e, src, segs, n, nullptr, nullptr, d_kpts, d_idx, nullptr, static_cast<cudaStream_t>(stream));
+  return frames_core(e, tab, nt, nullptr, d_mats, d_cs, segs, true, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
@@ -2340,27 +2221,17 @@ extern "C" int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_fra
   FrameEntry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_affine_heads_host", e, h_frames, num_frames, tab, &nt, &n));
+  VPB_TRY(frame_table("vpb_infer_affine_heads_host", e, h_frames, num_frames, 0, tab, &nt, &n));
   std::vector<Segment> segs;
   VPB_TRY(frame_segments(e, "vpb_infer_affine_heads_host", h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_heads_host: null pointer");
   VPB_TRY(check_affine_host(h_mats, h_cs, n));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  VPB_TRY(stage_frames_host(e, 0, tab, nt, nullptr, n, st));         // waits for slot 0's last user
-  CU_TRY(cudaMemcpyAsync(e->mat_stage, h_mats, static_cast<size_t>(n) * 6 * sizeof(double), cudaMemcpyHostToDevice, st));
-  CU_TRY(cudaMemcpyAsync(e->cs_stage, h_cs, static_cast<size_t>(n) * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
-  Source src;
-  src.frames = tab; src.num_frames = nt; src.mats = e->mat_stage; src.cs = e->cs_stage;
-  VPB_TRY(heads_core(e, src, segs, n, nullptr, nullptr, e->kpts[0], e->idx[0], nullptr, st));
-  VPB_TRY(copy_head_rows(e, segs, h_kpts, e->kpts[0], 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (h_idx) VPB_TRY(copy_head_rows(e, segs, h_idx, e->idx[0], sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaEventRecord(e->ev_done[0], st));
-  CU_TRY(cudaStreamSynchronize(st));
-  return VPB_OK;
+  return frames_host_sync(e, tab, nt, nullptr, h_mats, h_cs, segs, true, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
 
+// ------------------------------------------------------------------------------------------------ host crops
 extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t* h_org_wh, int32_t batch, float* h_kpts,
                               int32_t* h_idx, void* stream) {
   VPB_TRY(check_ready_keypoints(e, batch));
@@ -2371,11 +2242,7 @@ extern "C" int vpb_infer_host(vpb_engine* e, const float* h_crops, const int32_t
   CU_TRY(cudaMemcpyAsync(e->crops_stage[0], h_crops, static_cast<size_t>(batch) * 3 * 256 * 192 * sizeof(float), cudaMemcpyHostToDevice, st));
   CU_TRY(cudaMemcpyAsync(e->org_wh[0], h_org_wh, static_cast<size_t>(batch) * 2 * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   VPB_TRY(vpb_infer(e, e->crops_stage[0], e->org_wh[0], batch, e->kpts[0], e->idx[0], nullptr, st));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[0], static_cast<size_t>(batch) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[0], static_cast<size_t>(batch) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  CU_TRY(cudaEventRecord(e->ev_done[0], st));
-  CU_TRY(cudaStreamSynchronize(st));
-  return VPB_OK;
+  return host_tail(e, {{0, batch}}, false, 0, h_kpts, h_idx, st, true);
 }
 
 // Pipelined form of vpb_infer_host: submit(slot) enqueues H2D on the engine's copy stream and the path + D2H on its compute
@@ -2394,10 +2261,7 @@ extern "C" int vpb_submit_host(vpb_engine* e, const float* h_crops, const int32_
   CU_TRY(cudaEventRecord(e->ev_h2d[slot], e->copy_stream));
   CU_TRY(cudaStreamWaitEvent(e->compute_stream, e->ev_h2d[slot], 0));
   VPB_TRY(vpb_infer(e, e->crops_stage[slot], e->org_wh[slot], batch, e->kpts[slot], e->idx[slot], nullptr, e->compute_stream));
-  CU_TRY(cudaMemcpyAsync(h_kpts, e->kpts[slot], static_cast<size_t>(batch) * e->K * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->compute_stream));
-  if (h_idx) CU_TRY(cudaMemcpyAsync(h_idx, e->idx[slot], static_cast<size_t>(batch) * e->K * sizeof(int32_t), cudaMemcpyDeviceToHost, e->compute_stream));
-  CU_TRY(cudaEventRecord(e->ev_done[slot], e->compute_stream));
-  return VPB_OK;
+  return host_tail(e, {{0, batch}}, false, slot, h_kpts, h_idx, e->compute_stream, false);
 }
 extern "C" int vpb_wait_host(vpb_engine* e, int32_t slot) {
   if (!e || slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "vpb_wait_host: bad argument");
@@ -2417,11 +2281,8 @@ extern "C" void vpb_host_free(void* p) {
 extern "C" int vpb_cached_graphs(const vpb_engine* e, int32_t mixed, int32_t* entries, int32_t* captured) {
   if (!e || !entries || !captured) return fail(VPB_ERR_ARG, "vpb_cached_graphs: null argument");
   *entries = *captured = 0;
-  auto count = [&](const auto& list) {
-    for (const auto& g : list) { ++*entries; *captured += g.exec != nullptr; }
-  };
-  if (mixed) count(e->mixed_graphs);
-  else count(e->graphs);
+  for (const auto& g : e->graph_cache)
+    if (g.mixed == (mixed != 0)) { ++*entries; *captured += g.exec != nullptr; }
   return VPB_OK;
 }
 extern "C" int64_t vpb_device_bytes(const vpb_engine* e) {
