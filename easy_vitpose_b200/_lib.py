@@ -45,6 +45,15 @@ class VpbSegment(C.Structure):
     _fields_ = [("head", C.c_int32), ("count", C.c_int32)]
 
 
+DRAW_CHANNEL_ORDERS = {"rgb": 0, "bgr": 1}          # VPB_DRAW_RGB, VPB_DRAW_BGR
+
+
+class VpbCanvas(C.Structure):
+    """vpb_canvas: one frame drawn in place by vpb_draw_poses."""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("pitch_bytes", C.c_int64),
+                ("num_people", C.c_int32)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "vpb_last_error": (C.c_char_p, []),
@@ -108,6 +117,9 @@ EXPORTS = {
     "vpb_attention": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vpb_debug_attention": (C.c_int, [C.c_int32]),
     "vpb_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p]),
+    "vpb_draw_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
+    "vpb_draw_poses": (C.c_int, [C.POINTER(VpbCanvas), C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                 C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p]),
 }
 
 # The NV12 calls: names with a digit, kept apart from EXPORTS, which tests/test_abi.py matches against the header's

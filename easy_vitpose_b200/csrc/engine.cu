@@ -21,6 +21,7 @@
 #include "attention.cuh"
 #include "chain.cuh"
 #include "decode.cuh"
+#include "draw.cuh"
 #include "expert_gemm.cuh"
 #include "gemm.cuh"
 #include "pointwise.cuh"
@@ -2072,6 +2073,77 @@ extern "C" int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_fram
   AffineParams q = affine_params(tab, nt, d_mats, nullptr, n, nullptr);
   q.crops = d_crops;
   crop_warp_normalise<<<dim3(n, PP_H / PP_ROWS), PP_W, 0, static_cast<cudaStream_t>(stream)>>>(q);
+  CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------ pose overlay
+static long long draw_records(long long n, long long k, long long num_limbs) { return n * (num_limbs + k); }
+extern "C" int64_t vpb_draw_workspace_bytes(int32_t n, int32_t k, int32_t num_limbs) {
+  if (n < 0 || k < 1 || num_limbs < 0) return -1;
+  return draw_records(n, k, num_limbs) * (long long)(sizeof(DrawRec) + sizeof(int4));
+}
+extern "C" int vpb_draw_poses(const vpb_canvas* h_frames, int32_t num_frames, int32_t channel_order, const float* d_kpts, int32_t k,
+                              const int32_t* d_person_index, const int32_t* h_limbs, int32_t num_limbs, const uint8_t* h_point_bgr,
+                              int32_t num_point_colors, const uint8_t* h_limb_bgr, int32_t num_limb_colors, int32_t radius,
+                              float threshold, void* d_workspace, void* stream) {
+  const char* fn = "vpb_draw_poses";
+  if (channel_order != VPB_DRAW_RGB && channel_order != VPB_DRAW_BGR) return fail(VPB_ERR_ARG, "%s: unknown channel order %d", fn, channel_order);
+  if (k < 1) return fail(VPB_ERR_ARG, "%s: k=%d", fn, k);
+  if (num_limbs < 0 || num_limbs > DRAW_MAX_LIMBS || (num_limbs > 0 && !h_limbs))
+    return fail(VPB_ERR_ARG, "%s: %d limbs (0..%d and a table)", fn, num_limbs, DRAW_MAX_LIMBS);
+  if (num_point_colors < 1 || num_point_colors > DRAW_MAX_COLORS || num_limb_colors < 1 || num_limb_colors > DRAW_MAX_COLORS ||
+      !h_point_bgr || !h_limb_bgr)
+    return fail(VPB_ERR_ARG, "%s: colour tables of %d and %d entries (1..%d each)", fn, num_point_colors, num_limb_colors, DRAW_MAX_COLORS);
+  if (radius > DRAW_MAX_RADIUS) return fail(VPB_ERR_ARG, "%s: radius %d above %d", fn, radius, DRAW_MAX_RADIUS);
+  if (num_frames < 0 || (num_frames > 0 && !h_frames)) return fail(VPB_ERR_ARG, "%s: %d frames", fn, num_frames);
+  DrawParams q;
+  memset(&q, 0, sizeof(q));
+  for (int e = 0; e < num_limbs; ++e)
+    for (int j = 0; j < 2; ++j) {
+      const int32_t v = h_limbs[2 * e + j];
+      if (v < 0 || v >= k) return fail(VPB_ERR_ARG, "%s: limb %d joins keypoint %d, outside [0, %d)", fn, e, v, k);
+      q.limbs[e][j] = static_cast<uint16_t>(v);
+    }
+  const bool rgb = channel_order == VPB_DRAW_RGB;
+  for (int c = 0; c < 3; ++c) {
+    const int src = rgb ? 2 - c : c;                         // BGR tables, written reversed into RGB frames
+    for (int i = 0; i < num_point_colors; ++i) q.point_rgb[i][c] = h_point_bgr[3 * i + src];
+    for (int i = 0; i < num_limb_colors; ++i) q.limb_rgb[i][c] = h_limb_bgr[3 * i + src];
+  }
+  long long n = 0, tiles = 0;
+  int nt = 0;
+  for (int j = 0; j < num_frames; ++j) {
+    const vpb_canvas& c = h_frames[j];
+    if (c.num_people < 0) return fail(VPB_ERR_ARG, "%s: frame %d has %d people", fn, j, c.num_people);
+    if (c.num_people == 0) continue;
+    if (nt == DRAW_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than %d frames with people", fn, VPB_MAX_FRAMES);
+    if (!c.data) return fail(VPB_ERR_ARG, "%s: frame %d has people and no data", fn, j);
+    if (c.height < 1 || c.width < 1) return fail(VPB_ERR_ARG, "%s: frame %d is %d x %d", fn, j, c.height, c.width);
+    const long long pitch = c.pitch_bytes == 0 ? 3LL * c.width : c.pitch_bytes;
+    if (pitch < 3LL * c.width) return fail(VPB_ERR_ARG, "%s: frame %d pitch %lld below 3 * width %d", fn, j, (long long)c.pitch_bytes, c.width);
+    const int r = radius > 0 ? radius : std::max(1, std::min(c.height, c.width) / 150);
+    if (r > DRAW_MAX_RADIUS) return fail(VPB_ERR_ARG, "%s: frame %d radius %d above %d", fn, j, r, DRAW_MAX_RADIUS);
+    DrawFrame& f = q.frames[nt++];
+    f.data = c.data; f.pitch = pitch; f.h = c.height; f.w = c.width;
+    f.first_person = static_cast<int>(n); f.num_people = c.num_people; f.radius = r; f.first_tile = static_cast<int>(tiles);
+    n += c.num_people;
+    tiles += (long long)((c.width + DRAW_TILE_W - 1) / DRAW_TILE_W) * ((c.height + DRAW_TILE_H - 1) / DRAW_TILE_H);
+    if (draw_records(n, k, num_limbs) > 0x7fffffffLL || tiles > 0x7fffffffLL) return fail(VPB_ERR_ARG, "%s: call too large", fn);
+  }
+  if (n == 0) return VPB_OK;
+  if (!d_kpts || !d_workspace) return fail(VPB_ERR_ARG, "%s: null keypoints or workspace", fn);
+  if (reinterpret_cast<uintptr_t>(d_workspace) % 16 != 0) return fail(VPB_ERR_ARG, "%s: workspace not 16-byte aligned", fn);
+  const long long recs = draw_records(n, k, num_limbs);
+  q.kpts = d_kpts; q.person_index = d_person_index;
+  q.recs = static_cast<DrawRec*>(d_workspace);
+  q.boxes = reinterpret_cast<int4*>(static_cast<char*>(d_workspace) + recs * sizeof(DrawRec));
+  q.n = static_cast<int>(n); q.k = k; q.num_limbs = num_limbs; q.num_point_colors = num_point_colors; q.num_limb_colors = num_limb_colors;
+  q.num_frames = nt; q.total_tiles = static_cast<int>(tiles); q.threshold = threshold;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  draw_setup<<<static_cast<unsigned>(cdiv(recs, DRAW_SETUP_THREADS)), DRAW_SETUP_THREADS, 0, st>>>(q);
+  CU_TRY(cudaGetLastError());
+  draw_raster<<<static_cast<unsigned>(tiles), DRAW_TILE_W * DRAW_TILE_H, 0, st>>>(q);
   CU_TRY(cudaGetLastError());
   return VPB_OK;
 }

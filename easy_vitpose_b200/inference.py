@@ -22,7 +22,7 @@ from .model import ViTPose
 from .top_down_eval import decode_heatmaps
 from .topdown import topdown_args
 
-__all__ = ["B200PoseBackend", "install", "frame_inference", "MEAN", "STD"]
+__all__ = ["B200PoseBackend", "install", "frame_inference", "frame_draw", "MEAN", "STD"]
 
 MEAN = [0.485, 0.456, 0.406]      # easy_ViTPose/inference.py:32
 STD = [0.229, 0.224, 0.225]       # easy_ViTPose/inference.py:33
@@ -134,6 +134,36 @@ class B200PoseBackend:
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
         return self.model.infer_affine_heads_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list)[0]
 
+    def draw_frames(self, imgs: "list[np.ndarray]", kpts_list: "list[np.ndarray]", skeleton, person_index=None,
+                    confidence_threshold: float = 0.5, channel_order: str = "rgb", point_colors=None, limb_colors=None) -> "list[np.ndarray]":
+        """Host form of draw.draw_poses: uint8 [H,W,3] frames + each frame's float32 [n_i,K,3] (y, x, score) keypoints -> new
+        frames with every person's skeleton and keypoints drawn as VitInference.draw() draws them, with one upload, one launch
+        and one download.  person_index: None (position within the frame) or per frame a sequence of n_i colour indices
+        (draw() uses the tracker ids); colours BGR, None = draw.reference_palettes()."""
+        from .draw import draw_poses
+        if len(imgs) != len(kpts_list):
+            raise ValueError(f"{len(imgs)} frames and {len(kpts_list)} keypoint arrays")
+        imgs = [np.ascontiguousarray(im, np.uint8) for im in imgs]
+        if any(im.ndim != 3 or im.shape[2] != 3 for im in imgs):
+            raise ValueError("frames must be uint8 [H, W, 3]")
+        kps = [np.asarray(k, np.float32) for k in kpts_list]
+        if any(k.ndim != 3 or k.shape[2] != 3 for k in kps) or len({k.shape[1] for k in kps}) > 1:
+            raise ValueError("keypoints must be float32 [n_i, K, 3] with one K for all frames")
+        if not imgs:
+            return []
+        counts = [len(k) for k in kps]
+        dev = torch.device("cuda", self.model._device if self.model._device is not None else torch.cuda.current_device())
+        sizes = [im.size for im in imgs]
+        offs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        buf = torch.from_numpy(np.concatenate([im.reshape(-1) for im in imgs])).to(dev)
+        frames = [buf[offs[j]:offs[j + 1]].view(im.shape) for j, im in enumerate(imgs)]
+        kp = torch.from_numpy(np.concatenate(kps, 0))
+        pidx = None if person_index is None else np.concatenate([np.asarray(p, np.int64).reshape(-1) for p in person_index]).astype(np.int32)
+        with torch.cuda.device(dev):
+            draw_poses(frames, kp.to(dev), counts, skeleton, pidx, point_colors, limb_colors, confidence_threshold, channel_order)
+        out = buf.cpu().numpy()
+        return [out[offs[j]:offs[j + 1]].reshape(im.shape) for j, im in enumerate(imgs)]
+
     @torch.no_grad()
     def inference_batch(self, imgs: "list[np.ndarray]") -> np.ndarray:
         """All person crops of a frame in one engine call -> float32 [n,K,3]."""
@@ -194,12 +224,35 @@ def frame_inference(self, img: np.ndarray) -> dict:
     return frame_keypoints
 
 
+def frame_draw(self, show_yolo=True, show_raw_yolo=False, confidence_threshold=0.5) -> np.ndarray:
+    """`VitInference.draw()` (easy_ViTPose/inference.py:283-312) with the pose layer drawn on the device: returns the same
+    RGB array.  The box layers, when requested, run first with the reference's own code (ultralytics' `plot()` and
+    `draw_bboxes`), as draw() orders them; then every person of `self._keypoints`, in its order and with its key as colour
+    index, is drawn with `joints_dict()[self.dataset]['skeleton']` and the palettes draw() passes, in one
+    `B200PoseBackend.draw_frames` call.  Bound onto the reference object by `install(..., batched=True)`."""
+    import importlib
+    img = self._img.copy()
+    bboxes, ids, scores = self._tracker_res
+    if self._yolo_res is not None and (show_raw_yolo or (self.tracker is None and show_yolo)):
+        img = np.array(self._yolo_res.plot())[..., ::-1]
+    if show_yolo and self.tracker is not None:
+        img = importlib.import_module("easy_ViTPose.vit_utils.inference").draw_bboxes(img, bboxes, ids, scores)
+    img = np.ascontiguousarray(img)
+    if not self._keypoints:
+        return img
+    skeleton = importlib.import_module("easy_ViTPose.vit_utils.visualization").joints_dict()[self.dataset]["skeleton"]
+    kpts = np.stack([np.asarray(k, np.float32) for k in self._keypoints.values()], 0)
+    return self._b200.draw_frames([img], [kpts], skeleton, person_index=[list(self._keypoints.keys())],
+                                  confidence_threshold=confidence_threshold)[0]
+
+
 def install(vit_inference, max_batch: int = 64, device=None, batched: bool = False, flip_test: bool = False,
             flip_pairs=None) -> B200PoseBackend:
     """Re-bind a constructed reference `VitInference` (torch .pth backend) to the H100 engine: takes the
     weights out of its `_vit_pose` module, then replaces `_vit_pose` and `_inference` exactly where
     easy_ViTPose/inference.py:156-172 set them.  With `batched=True` the object's `inference` method is re-bound to
-    `frame_inference` as well (one engine call per frame instead of one per person).  With `flip_test=True` every
+    `frame_inference` as well (one engine call per frame instead of one per person), and `draw` to `frame_draw` (the pose
+    layer of every person in one launch on the device).  With `flip_test=True` every
     keypoint call runs the flip test of the reference configs (test_cfg flip_test=True, shift_heatmap=False), with the
     pairs of `flip_pairs_for(vit_inference.dataset, flip_pairs)`; the engine is then built for 2 * max_batch crops, so
     `max_batch` still counts people per call.  Returns the backend (also stored as `._b200`)."""
@@ -223,4 +276,5 @@ def install(vit_inference, max_batch: int = 64, device=None, batched: bool = Fal
     vit_inference._b200 = backend
     if batched:
         vit_inference.inference = types.MethodType(frame_inference, vit_inference)
+        vit_inference.draw = types.MethodType(frame_draw, vit_inference)
     return backend

@@ -311,6 +311,40 @@ int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num
 int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
                                 const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream);
 
+/* ---- pose overlay: the pose layer of VitInference.draw() (easy_ViTPose/inference.py:283-312, vit_utils/visualization.py:360-481)
+ * for the people of up to VPB_MAX_FRAMES frames in two launches, drawn in place, bit-exact with cv2 4.13.  Per person in order
+ * (frame j owns the next h_frames[j].num_people rows of d_kpts, as vpb_infer_frames returns them), the reference's
+ * draw_points_and_skeleton:
+ *   every limb e (a, b) = h_limbs[2e], h_limbs[2e + 1] whose two scores are > threshold (float compare, as numpy does for
+ *   float32 rows): cv2.line(img, (int(x_a), int(y_a)), (int(x_b), int(y_b)), limb colour [idx % num_limb_colors], 2), idx =
+ *   d_person_index[p] or, when NULL, the person's position within its frame;
+ *   then every keypoint i whose score is > threshold: cv2.circle(img, (int(x), int(y)), radius, point colour [i % num_point_colors], -1).
+ * int() truncates toward zero; a coordinate that is not finite or not an int32 is not drawn (the reference raises there).  Later
+ * primitives overwrite earlier ones; pixels no primitive covers are not written.  Colours are BGR triples, as the reference holds
+ * them: channel_order VPB_DRAW_BGR writes them as given, VPB_DRAW_RGB reversed, which equals the reference's flip -> draw -> flip.
+ * radius <= 0 = max(1, min(height, width) / 150) per frame, the reference's rule; at most 1023.
+ * d_kpts f32 [n,k,3] (y, x, score) in frame pixels; d_person_index i32 [n] or NULL; h_limbs i32 [num_limbs,2] (HOST), num_limbs
+ * <= 128, every index in [0, k); h_point_bgr / h_limb_bgr u8 [count,3] (HOST), 1..64 entries each.  d_workspace: device memory of
+ * vpb_draw_workspace_bytes(n, k, num_limbs) bytes, 16-byte aligned, which the call may overwrite until it completes on `stream`.
+ * No host synchronisation; the two launches can be captured in a CUDA graph.  Frames with 0 people are skipped and do not count
+ * towards VPB_MAX_FRAMES; n = 0 returns VPB_OK and launches nothing.  VPB_ERR_ARG: an unknown channel order, k < 1, a limb index
+ * outside [0, k), more than 128 limbs, a colour table of 0 or more than 64 entries, a radius above 1023, more than VPB_MAX_FRAMES
+ * frames with people, a negative num_people, a frame with people whose data is NULL, height or width < 1, or pitch below
+ * 3 * width, a NULL d_kpts or workspace with n > 0. */
+#define VPB_DRAW_RGB 0
+#define VPB_DRAW_BGR 1
+typedef struct vpb_canvas {
+  uint8_t* data;          /* u8 [height, width, 3], device address, drawn in place */
+  int32_t height, width;
+  int64_t pitch_bytes;    /* row pitch; 0 = packed (3 * width) */
+  int32_t num_people;     /* this frame's people are the next num_people rows of d_kpts (0 allowed) */
+} vpb_canvas;
+int64_t vpb_draw_workspace_bytes(int32_t n, int32_t k, int32_t num_limbs);   /* -1 for a negative n or num_limbs, or k < 1 */
+int vpb_draw_poses(const vpb_canvas* h_frames, int32_t num_frames, int32_t channel_order, const float* d_kpts, int32_t k,
+                   const int32_t* d_person_index, const int32_t* h_limbs, int32_t num_limbs, const uint8_t* h_point_bgr,
+                   int32_t num_point_colors, const uint8_t* h_limb_bgr, int32_t num_limb_colors, int32_t radius, float threshold,
+                   void* d_workspace, void* stream);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* The engine's cached CUDA graphs: mixed = 0 the single-head calls' (one per batch size and decode kind), 1 the multi-head
