@@ -27,6 +27,7 @@
 #include "pointwise.cuh"
 #include "preprocess.cuh"
 #include "qkv_attention.cuh"
+#include "track.cuh"
 
 using namespace vpb;
 
@@ -2145,6 +2146,132 @@ extern "C" int vpb_draw_poses(const vpb_canvas* h_frames, int32_t num_frames, in
   CU_TRY(cudaGetLastError());
   draw_raster<<<static_cast<unsigned>(tiles), DRAW_TILE_W * DRAW_TILE_H, 0, st>>>(q);
   CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------ SORT tracker
+struct vpb_tracker {
+  int device = 0;
+  void* mem = nullptr;          // one allocation; TrackParams points into it
+  TrackParams q{};
+};
+
+struct TrackerDevice {          // makes the tracker's device current for one call
+  int prev = -1;
+  explicit TrackerDevice(const vpb_tracker* t) {
+    int cur = -1;
+    if (cudaGetDevice(&cur) == cudaSuccess && cur != t->device && cudaSetDevice(t->device) == cudaSuccess) prev = cur;
+  }
+  ~TrackerDevice() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+extern "C" int vpb_tracker_create(int32_t num_streams, int32_t max_age, int32_t min_hits, double iou_threshold, int32_t device,
+                                  vpb_tracker** out) {
+  const char* fn = "vpb_tracker_create";
+  if (!out) return fail(VPB_ERR_ARG, "%s: null output", fn);
+  *out = nullptr;
+  if (num_streams < 1 || num_streams > 65535) return fail(VPB_ERR_ARG, "%s: %d streams (1..65535)", fn, num_streams);
+  if (max_age < 0 || min_hits < 0) return fail(VPB_ERR_ARG, "%s: max_age %d and min_hits %d must be >= 0", fn, max_age, min_hits);
+  if (!std::isfinite(iou_threshold)) return fail(VPB_ERR_ARG, "%s: iou_threshold is not finite", fn);
+  int ndev = 0;
+  CU_TRY(cudaGetDeviceCount(&ndev));
+  if (device < 0 || device >= ndev) return fail(VPB_ERR_ARG, "%s: device %d of %d", fn, device, ndev);
+  vpb_tracker* t = new vpb_tracker();
+  t->device = device;
+  TrackerDevice guard(t);
+  const size_t S = static_cast<size_t>(num_streams), M = TRACK_MAX;
+  const size_t bytes_state = S * TRACK_FIELDS * M * sizeof(double), bytes_ids = S * M * sizeof(long long);
+  const size_t bytes_i32 = (3 * S * M + 4 * S + 2) * sizeof(int32_t);
+  const size_t total = bytes_state + bytes_ids + 2 * sizeof(long long) + bytes_i32;
+  cudaError_t err = cudaMalloc(&t->mem, total);
+  if (err == cudaSuccess) err = cudaMemset(t->mem, 0, total);
+  if (err == cudaSuccess)
+    err = cudaFuncSetAttribute(track_associate, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(TrackSmem)));
+  if (err != cudaSuccess) {
+    if (t->mem) cudaFree(t->mem);
+    delete t;
+    return fail(VPB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(err));
+  }
+  char* p = static_cast<char*>(t->mem);
+  TrackParams& q = t->q;
+  q.state = reinterpret_cast<double*>(p); p += bytes_state;
+  q.ids = reinterpret_cast<long long*>(p); p += bytes_ids;
+  q.next_id = reinterpret_cast<long long*>(p); p += sizeof(long long);
+  q.id_base = reinterpret_cast<long long*>(p); p += sizeof(long long);
+  int32_t* ip = reinterpret_cast<int32_t*>(p);
+  q.tsu = ip; ip += S * M;
+  q.hits = ip; ip += S * M;
+  q.new_det = ip; ip += S * M;
+  q.num_tracks = ip; ip += S;
+  q.frame_count = ip; ip += S;
+  q.num_new = ip; ip += S;
+  q.status = ip;
+  q.num_streams = num_streams; q.max_age = max_age; q.min_hits = min_hits; q.iou_threshold = iou_threshold;
+  *out = t;
+  return VPB_OK;
+}
+
+extern "C" void vpb_tracker_destroy(vpb_tracker* t) {
+  if (!t) return;
+  TrackerDevice guard(t);
+  cudaDeviceSynchronize();
+  cudaFree(t->mem);
+  delete t;
+}
+
+extern "C" int vpb_tracker_update(vpb_tracker* t, const double* d_dets, const int32_t* d_counts, double* d_rows, int32_t* d_boxes,
+                                  int32_t* d_out_counts, void* stream) {
+  if (!t) return fail(VPB_ERR_ARG, "vpb_tracker_update: null tracker");
+  if (!d_dets || !d_counts || !d_rows || !d_boxes || !d_out_counts) return fail(VPB_ERR_ARG, "vpb_tracker_update: null buffer");
+  TrackerDevice guard(t);
+  TrackParams q = t->q;
+  q.dets = d_dets; q.counts = d_counts; q.rows = d_rows; q.boxes = d_boxes; q.out_counts = d_out_counts;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  track_associate<<<q.num_streams, TRACK_THREADS, sizeof(TrackSmem), st>>>(q);
+  CU_TRY(cudaGetLastError());
+  track_emit<<<q.num_streams, TRACK_THREADS, 0, st>>>(q);
+  CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+extern "C" int vpb_tracker_reset(vpb_tracker* t, int32_t stream_index, void* stream) {
+  if (!t) return fail(VPB_ERR_ARG, "vpb_tracker_reset: null tracker");
+  const int S = t->q.num_streams;
+  if (stream_index < -1 || stream_index >= S) return fail(VPB_ERR_ARG, "vpb_tracker_reset: stream %d of %d", stream_index, S);
+  TrackerDevice guard(t);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int first = stream_index < 0 ? 0 : stream_index, count = stream_index < 0 ? S : 1;
+  CU_TRY(cudaMemsetAsync(t->q.num_tracks + first, 0, count * sizeof(int32_t), st));
+  CU_TRY(cudaMemsetAsync(t->q.frame_count + first, 0, count * sizeof(int32_t), st));
+  return VPB_OK;
+}
+
+extern "C" int vpb_tracker_next_id(vpb_tracker* t, int64_t* out) {
+  if (!t || !out) return fail(VPB_ERR_ARG, "vpb_tracker_next_id: null argument");
+  TrackerDevice guard(t);
+  long long v = 0;
+  CU_TRY(cudaDeviceSynchronize());
+  CU_TRY(cudaMemcpy(&v, t->q.next_id, sizeof(v), cudaMemcpyDeviceToHost));
+  *out = v;
+  return VPB_OK;
+}
+
+extern "C" int vpb_tracker_set_next_id(vpb_tracker* t, int64_t next_id) {
+  if (!t) return fail(VPB_ERR_ARG, "vpb_tracker_set_next_id: null tracker");
+  if (next_id < 0) return fail(VPB_ERR_ARG, "vpb_tracker_set_next_id: negative id %lld", (long long)next_id);
+  TrackerDevice guard(t);
+  const long long v = next_id;
+  CU_TRY(cudaDeviceSynchronize());
+  CU_TRY(cudaMemcpy(t->q.next_id, &v, sizeof(v), cudaMemcpyHostToDevice));
+  return VPB_OK;
+}
+
+extern "C" int vpb_tracker_status(vpb_tracker* t, int32_t* h_status) {
+  if (!t || !h_status) return fail(VPB_ERR_ARG, "vpb_tracker_status: null argument");
+  TrackerDevice guard(t);
+  CU_TRY(cudaDeviceSynchronize());
+  CU_TRY(cudaMemcpy(h_status, t->q.status, sizeof(int32_t), cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemset(t->q.status, 0, sizeof(int32_t)));
   return VPB_OK;
 }
 

@@ -22,7 +22,7 @@ from .model import ViTPose
 from .top_down_eval import decode_heatmaps
 from .topdown import topdown_args
 
-__all__ = ["B200PoseBackend", "install", "frame_inference", "frame_draw", "MEAN", "STD"]
+__all__ = ["B200PoseBackend", "DeviceTracker", "install", "frame_inference", "frame_draw", "MEAN", "STD"]
 
 MEAN = [0.485, 0.456, 0.406]      # easy_ViTPose/inference.py:32
 STD = [0.229, 0.224, 0.225]       # easy_ViTPose/inference.py:33
@@ -165,6 +165,22 @@ class B200PoseBackend:
         return [out[offs[j]:offs[j + 1]].reshape(im.shape) for j, im in enumerate(imgs)]
 
     @torch.no_grad()
+    def inference_frames_tracked(self, imgs: "list[np.ndarray]", dets_list, tracker) -> "list[dict]":
+        """S streams' `frame_inference` after detection: one frame per stream (uint8 RGB [H,W,3], numpy or CUDA) and its
+        detections [n_s, 5] (empty where the detector was skipped, as frame_inference passes them) -> one {id: float32 [K,3]
+        (y, x, score)} per stream.  `tracker` (a track.DeviceSort of S streams on the engine's device) is updated once; its
+        int32 boxes feed infer_frames on the device, and only the row counts and ids come back before the pose call."""
+        if len(imgs) != tracker.num_streams:
+            raise ValueError(f"{len(imgs)} frames for a tracker of {tracker.num_streams} streams")
+        dets, counts = tracker.pack(dets_list)
+        rows, boxes, out_counts = tracker.update_device(dets, counts)
+        n = out_counts.tolist()
+        ids = rows[:, :, 5].long().cpu()                     # the rows' id + 1, the keys frame_inference uses (inference.py:249)
+        frames = [im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(im)) for im in imgs]
+        kps, _ = self.model.infer_frames(frames, [boxes[s, :c] for s, c in enumerate(n)])
+        return [dict(zip(ids[s, :c].tolist(), kp.cpu().numpy())) for s, (c, kp) in enumerate(zip(n, kps))]
+
+    @torch.no_grad()
     def inference_batch(self, imgs: "list[np.ndarray]") -> np.ndarray:
         """All person crops of a frame in one engine call -> float32 [n,K,3]."""
         if not imgs:
@@ -246,8 +262,45 @@ def frame_draw(self, show_yolo=True, show_raw_yolo=False, confidence_threshold=0
                                   confidence_threshold=confidence_threshold)[0]
 
 
+class DeviceTracker:
+    """A one-stream track.DeviceSort behind the reference `Sort` interface: `.update(dets [n, 5])` returns the float64
+    [m, 6] array Sort.update returns.  When the reference's sort module is loaded (`easy_ViTPose.sort`), every update starts
+    from its `KalmanBoxTracker.count` and writes the next id back, so ids interleave with CPU Sort objects of the same
+    process exactly as they do between reference Sorts."""
+
+    def __init__(self, max_age: int = 1, min_hits: int = 3, iou_threshold: float = 0.3, device=None):
+        from .track import DeviceSort
+        self.max_age, self.min_hits, self.iou_threshold = max_age, min_hits, iou_threshold
+        self.sort = DeviceSort(1, max_age, min_hits, iou_threshold, device)
+
+    @staticmethod
+    def _counter():
+        import sys
+        mod = sys.modules.get("easy_ViTPose.sort")
+        return getattr(mod, "KalmanBoxTracker", None)
+
+    def update(self, dets=np.empty((0, 5))) -> np.ndarray:
+        kbt = self._counter()
+        if kbt is not None:
+            self.sort.next_id = int(kbt.count)
+        rows = self.sort.update([dets])[0]
+        self.sort.check()
+        if kbt is not None:
+            kbt.count = self.sort.next_id
+        return rows
+
+
+def _reference_reset(self):
+    """`VitInference.reset()` (easy_ViTPose/inference.py:174-185) with the SORT tracker on the device: the same rule for
+    whether there is a tracker and the same parameters.  Bound by `install(..., batched=True, device_tracker=True)`."""
+    min_hits = 3 if self.yolo_step == 1 else 1
+    use_tracker = self.is_video and not self.single_pose
+    self.tracker = DeviceTracker(self.yolo_step, min_hits, 0.3, self._b200.model._device) if use_tracker else None
+    self.frame_counter = 0
+
+
 def install(vit_inference, max_batch: int = 64, device=None, batched: bool = False, flip_test: bool = False,
-            flip_pairs=None) -> B200PoseBackend:
+            flip_pairs=None, device_tracker: bool = False) -> B200PoseBackend:
     """Re-bind a constructed reference `VitInference` (torch .pth backend) to the H100 engine: takes the
     weights out of its `_vit_pose` module, then replaces `_vit_pose` and `_inference` exactly where
     easy_ViTPose/inference.py:156-172 set them.  With `batched=True` the object's `inference` method is re-bound to
@@ -255,7 +308,11 @@ def install(vit_inference, max_batch: int = 64, device=None, batched: bool = Fal
     layer of every person in one launch on the device).  With `flip_test=True` every
     keypoint call runs the flip test of the reference configs (test_cfg flip_test=True, shift_heatmap=False), with the
     pairs of `flip_pairs_for(vit_inference.dataset, flip_pairs)`; the engine is then built for 2 * max_batch crops, so
-    `max_batch` still counts people per call.  Returns the backend (also stored as `._b200`)."""
+    `max_batch` still counts people per call.  With `batched=True, device_tracker=True` the SORT tracker runs on the device
+    too: `vit_inference.tracker` becomes a `DeviceTracker` with the reference's parameters (only where the reference builds a
+    Sort) and `reset()` is re-bound to rebuild it.  Returns the backend (also stored as `._b200`)."""
+    if device_tracker and not batched:
+        raise ValueError("device_tracker=True needs batched=True")
     pairs = flip_pairs_for(getattr(vit_inference, "dataset", None), flip_pairs) if flip_test else None
     ref = vit_inference._vit_pose
     sd = {k: v.detach().cpu() for k, v in ref.state_dict().items()}
@@ -277,4 +334,9 @@ def install(vit_inference, max_batch: int = 64, device=None, batched: bool = Fal
     if batched:
         vit_inference.inference = types.MethodType(frame_inference, vit_inference)
         vit_inference.draw = types.MethodType(frame_draw, vit_inference)
+    if device_tracker:
+        vit_inference.reset = types.MethodType(_reference_reset, vit_inference)
+        if vit_inference.tracker is not None:
+            vit_inference.tracker = DeviceTracker(vit_inference.tracker.max_age, vit_inference.tracker.min_hits,
+                                                  vit_inference.tracker.iou_threshold, model._device)
     return backend

@@ -345,6 +345,38 @@ int vpb_draw_poses(const vpb_canvas* h_frames, int32_t num_frames, int32_t chann
                    int32_t num_point_colors, const uint8_t* h_limb_bgr, int32_t num_limb_colors, int32_t radius, float threshold,
                    void* d_workspace, void* stream);
 
+/* ---- SORT tracker: easy_ViTPose/sort.py's Sort for num_streams video streams, updated in one step on the device.  Stream s
+ * is one reference Sort(max_age, min_hits, iou_threshold); one update equals calling the S Sort objects round-robin in one
+ * process, and the output equals theirs as float64 values (filterpy 1.4.5's Kalman steps without FMA contraction, scipy's
+ * linear_sum_assignment with its tie rule; `lap`'s lapjv may break ties differently and is not followed).  The id counter
+ * (KalmanBoxTracker.count) is one per tracker: within an update new tracks take ids in stream order, within a stream in
+ * creation order.  Track state stays in device memory between updates.
+ * vpb_tracker_update: d_dets f64 [S,VPB_TRACK_MAX,5] (x1, y1, x2, y2, score), stream s's first d_counts[s] rows (i32 [S], DEVICE);
+ * outputs d_rows f64 [S,VPB_TRACK_MAX,6] (x1, y1, x2, y2, score, id + 1), stream s's first d_out_counts[s] rows in the reference's
+ * order, d_boxes i32 [S,VPB_TRACK_MAX,4] those rows' boxes rounded half to even (the boxes vpb_infer_frames takes, saturated
+ * to int32).  Two launches, no host synchronisation, no data-dependent host work: the call can be captured in a CUDA graph.
+ * A stream whose count is negative or above VPB_TRACK_MAX, or that has a row with a non-finite value or x2 <= x1 or y2 <= y1,
+ * or whose live tracks would exceed VPB_TRACK_MAX, is left unchanged, emits 0 rows and sets a status bit (a reference Sort
+ * raises in scipy or carries NaN state there); the other streams are unaffected.
+ * vpb_tracker_reset: stream_index's tracks and frame count (-1: every stream), enqueued on `stream`; the id counter carries on,
+ * as the reference's VitInference.reset() builds a new Sort but keeps KalmanBoxTracker.count.
+ * vpb_tracker_next_id / vpb_tracker_set_next_id: the counter, SYNCHRONOUS (wait for the device).
+ * vpb_tracker_status: SYNCHRONOUS; the bits VPB_TRACK_* raised since the last query, then clears them.
+ * VPB_ERR_ARG: num_streams outside 1..65535, max_age or min_hits < 0, a non-finite iou_threshold, a bad device, null buffers,
+ * a stream_index outside -1..S-1, a negative next id. */
+#define VPB_TRACK_MAX 128
+#define VPB_TRACK_BAD_ROW 1
+#define VPB_TRACK_OVER_CAPACITY 2
+typedef struct vpb_tracker vpb_tracker;
+int vpb_tracker_create(int32_t num_streams, int32_t max_age, int32_t min_hits, double iou_threshold, int32_t device, vpb_tracker** out);
+void vpb_tracker_destroy(vpb_tracker* t);
+int vpb_tracker_update(vpb_tracker* t, const double* d_dets, const int32_t* d_counts, double* d_rows, int32_t* d_boxes,
+                       int32_t* d_out_counts, void* stream);
+int vpb_tracker_reset(vpb_tracker* t, int32_t stream_index, void* stream);
+int vpb_tracker_next_id(vpb_tracker* t, int64_t* next_id);
+int vpb_tracker_set_next_id(vpb_tracker* t, int64_t next_id);
+int vpb_tracker_status(vpb_tracker* t, int32_t* status);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* The engine's cached CUDA graphs: mixed = 0 the single-head calls' (one per batch size and decode kind), 1 the multi-head
