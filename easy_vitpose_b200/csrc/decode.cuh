@@ -212,7 +212,7 @@ __global__ void __launch_bounds__(DECODE_WARPS * 32) decode_heatmaps(const Decod
     float acc = __fmul_rn(tap(0), rp[R]);
 #pragma unroll
     for (int d = 1; d <= R; ++d) acc = __fmaf_rn(tap(d), __fadd_rn(rp[R + d], rp[R - d]), acc);
-    l = logf(fminf(fmaxf(acc, 1e-3f), 50.0f));
+    l = logf(acc != acc ? acc : fminf(fmaxf(acc, 1e-3f), 50.0f));   // np.clip keeps NaN (fminf / fmaxf alone would not)
   }
   const float i_ = __shfl_sync(0xffffffffu, l, 0), ix1 = __shfl_sync(0xffffffffu, l, 1);
   const float iy1 = __shfl_sync(0xffffffffu, l, 2), ix1y1 = __shfl_sync(0xffffffffu, l, 3);

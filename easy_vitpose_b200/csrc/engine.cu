@@ -2505,9 +2505,30 @@ extern "C" int vpb_kernel_launches(const vpb_engine* e, int32_t batch) {
          (e->ln_fused ? 0 : e->ln_in_gemm ? 1 : 2 * e->depth + 1) + (e->flip ? 1 : 0);
 }
 
+// Debug option "poison": every float and bf16 activation and staging buffer filled with 0xFF bytes (NaN in both types), so a test
+// can tell whether a call uses a value it did not write itself (padding rows of a ragged row block, the unused rows of the 96-position
+// deconv tiles, the maps past a smaller head's K, what an earlier and larger call left behind).  Integer and double buffers,
+// counters and status words (idx, org_wh, g_org, g_offs, pp_*, bbox_stage, mat_stage, flip_perm, chain_counters, ln_counters)
+// are left alone: garbage there would change addressing or the chained-launch protocol, not values.  The cached graphs stay.
+static int poison_workspace(vpb_engine* e) {
+  if (!e->finalized) return fail(VPB_ERR_STATE, "poison: not finalized");
+  DeviceGuard dev_guard(e);
+  CU_TRY(cudaDeviceSynchronize());              // pending calls (submit slots included) finish on the memory they started with
+  const size_t B = e->maxB, M = B * 192, D = e->D, K = e->Kmax, bf = sizeof(__nv_bfloat16), f = sizeof(float);
+  const std::pair<void*, size_t> bufs[] = {
+      {e->patch_rows, M * 768 * bf}, {e->x, M * D * f}, {e->xn, M * D * bf}, {e->qkv, M * 3 * D * bf}, {e->attn, M * D * bf},
+      {e->hid, M * 4 * D * bf}, {e->d1, B * 768 * 256 * bf}, {e->d2, B * 3072 * 256 * bf}, {e->heat, B * K * 3072 * f},
+      {e->g_kpts, B * K * 3 * f}, {e->kpts[0], B * K * 3 * f}, {e->kpts[1], B * K * 3 * f},
+      {e->crops_stage[0], B * 3 * 256 * 192 * f}, {e->crops_stage[1], B * 3 * 256 * 192 * f}, {e->g_cs, B * 4 * f}, {e->cs_stage, B * 4 * f}};
+  for (const auto& b : bufs) CU_TRY(cudaMemset(b.first, 0xFF, b.second));
+  CU_TRY(cudaDeviceSynchronize());
+  return VPB_OK;
+}
+
 extern "C" int vpb_set_option(vpb_engine* e, const char* name, int32_t value) {
   if (!e || !name) return fail(VPB_ERR_ARG, "vpb_set_option: null argument");
   if (!strcmp(name, "stop_after")) e->stop_after = value;
+  else if (!strcmp(name, "poison")) { if (value) VPB_TRY(poison_workspace(e)); }
   else if (!strcmp(name, "profile")) e->prof.on = value != 0;
   else if (!strcmp(name, "pdl")) g_pdl = value != 0;
   else if (!strcmp(name, "graph")) e->use_graph = value != 0;

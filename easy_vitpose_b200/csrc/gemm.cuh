@@ -135,7 +135,7 @@ template <int EPI>
 __device__ __forceinline__ float epi_act(float v) {
   if constexpr (EPI == EPI_BF16_GELU) return gelu_fast(v);
   else if constexpr (EPI == EPI_BF16_GELU_ERF) return gelu_erf_as(v);
-  else if constexpr (EPI == EPI_BF16_RELU_UP) return fmaxf(v, 0.0f);
+  else if constexpr (EPI == EPI_BF16_RELU_UP) return relu_keep_nan(v);
   else return v;
 }
 
@@ -383,7 +383,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmap_a, const __grid_constan
               const int n = 8 * j + cq;
               if (n >= p.N) continue;
               const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-              o[n >> 1] = pack_bf16(fmaxf(acc[4 * j + 2 * h] + b2.x, 0.0f), fmaxf(acc[4 * j + 2 * h + 1] + b2.y, 0.0f));
+              o[n >> 1] = pack_bf16(relu_keep_nan(acc[4 * j + 2 * h] + b2.x), relu_keep_nan(acc[4 * j + 2 * h + 1] + b2.y));
             }
           } else {  // EPI_F32_NCHW
             const int row = m0 + r;

@@ -389,7 +389,10 @@ int64_t vpb_device_bytes(const vpb_engine* e);
  * "ln_in_gemm" (LayerNorm + its consumer GEMM as one launch on the unchained path, default 0), "gelu_erf" (fc1 epilogue with
  * erf instead of the fitted tanh form: rounding-level differences), "ln_ctl" (chained launches: counter polls / publishes of
  * the LayerNorm jobs on a control warp, default 1; VPB_LN_CTL), "ln_job_rows" (8 | 16 rows per LayerNorm job, default 16),
- * "resid_rmw" (residual epilogues as load + add + store instead of TMA reduce-add, default 0; VPB_RESID_RMW). */
+ * "resid_rmw" (residual epilogues as load + add + store instead of TMA reduce-add, default 0; VPB_RESID_RMW).
+ * "poison" (debug; value != 0) is an action, not a setting: SYNCHRONOUSLY fills every float and bf16 activation and staging
+ * buffer with 0xFF bytes (NaN), keeping the cached CUDA graphs, so a test can show that no call uses workspace values it did not
+ * write; integer / double buffers, counters and status words are not touched. */
 int vpb_set_option(vpb_engine* e, const char* name, int32_t value);
 /* Flip test, the test_cfg flip_test=True of every reference config (configs/ViTPose_common.py:91,124,157,190): mmpose's
  * (output + output_flipped) * 0.5, where output_flipped is the model run on flip(crop, dims=[3]) and passed through flip_back
