@@ -36,6 +36,16 @@ class VpbFrameNv12(C.Structure):
                 ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32)]
 
 
+YUV_LAYOUTS = {"nv12": 0, "nv21": 1, "i420": 2, "yv12": 3, "yuyv": 4, "uyvy": 5}    # VPB_YUV_NV12 .. VPB_YUV_UYVY
+YUV_RANGES = {"limited": 0, "full": 1}               # VPB_YUV_LIMITED, VPB_YUV_FULL
+
+
+class VpbFrameYuv(C.Structure):
+    """vpb_frame_yuv: one YUV frame of the _yuv calls, its planes in the layout's storage order."""
+    _fields_ = [("plane", C.c_void_p * 3), ("y_pitch", C.c_int64), ("c_pitch", C.c_int64),
+                ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32)]
+
+
 MAX_HEADS = 8                                        # VPB_MAX_HEADS: keypoint heads of one engine
 MAX_SEGMENTS = 64                                     # VPB_MAX_SEGMENTS: runs of one head per multi-head call
 
@@ -99,6 +109,24 @@ EXPORTS = {
                                          C.c_void_p, C.c_void_p]),
     "vpb_infer_affine_heads_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_frames_yuv": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_frames_yuv_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_submit_frames_yuv_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_int32]),
+    "vpb_infer_affine_yuv": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine_yuv_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_frames_heads_yuv": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_frames_heads_yuv_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine_heads_yuv": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_infer_affine_heads_yuv_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrameYuv), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_host_alloc": (C.c_void_p, [C.c_int64]),
     "vpb_host_free": (None, [C.c_void_p]),
     "vpb_kernel_launches": (C.c_int, [C.c_void_p, C.c_int32]),

@@ -930,19 +930,20 @@ static int patch_gather(vpb_engine* e, const float* d_crops, int n_src, int B, c
 // (frame_to_patch_rows: crop pre-processing fused with the im2col; it also fills pp_org / pp_offs for the decode).
 // Affine crops (frame_to_patch_rows_affine) take a matrix per box instead of a box, and their keypoints are decoded with
 // centre / scale (decode mode 4) instead of canvas sizes and offsets.
-// NV12 frames come as an Nv12Entry table instead (each entry carries the call's YUV matrix); the gathers then launch the
-// NV12 instantiation of the same kernels, outside the captured graph, so the graph cache needs no NV12 key.
+// YUV frames (every layout, NV12 included) come as a YuvEntry table instead (each entry carries the call's matrix and
+// range); the gathers then launch the YUV instantiation of the same kernels, outside the captured graph, so the graph cache
+// needs no YUV key.
 struct Source {
   const float* crops = nullptr;
   const FrameEntry* frames = nullptr;       // num_frames entries, only frames that have boxes
-  const Nv12Entry* nv12 = nullptr;          // instead of frames: NV12 frames
+  const YuvEntry* yuv = nullptr;            // instead of frames: YUV frames
   int num_frames = 0;
   const int32_t* bboxes = nullptr;
   const double* mats = nullptr;             // [n,6] affine matrices (then bboxes is unused)
   const float* cs = nullptr;                // [n,4] centre / scale of the affine decode
 };
 static void set_table(Source& s, const FrameEntry* tab) { s.frames = tab; }
-static void set_table(Source& s, const Nv12Entry* tab) { s.nv12 = tab; }
+static void set_table(Source& s, const YuvEntry* tab) { s.yuv = tab; }
 template <class Entry>
 static AffineParamsT<Entry> affine_params(const Entry* frames, int num_frames, const double* mats, const float* cs, int n, int* status) {
   AffineParamsT<Entry> q;
@@ -980,7 +981,7 @@ static int table_gather(vpb_engine* e, const Source& src, const Entry* tab, int 
 }
 static int gather(vpb_engine* e, const Source& src, int n_src, int B, cudaStream_t st) {
   if (src.crops) return patch_gather(e, src.crops, n_src, B, st);
-  return src.nv12 ? table_gather(e, src, src.nv12, n_src, B, st) : table_gather(e, src, src.frames, n_src, B, st);
+  return src.yuv ? table_gather(e, src, src.yuv, n_src, B, st) : table_gather(e, src, src.frames, n_src, B, st);
 }
 // Chained form of the backbone (chain.cuh): 1 + depth persistent GEMM launches + depth attention launches.
 //   launch 0:        patch embed (+= x) -> LN(norm1 of block 0) -> qkv of block 0
@@ -1779,16 +1780,33 @@ static FrameEntry single_frame(const uint8_t* data, int32_t fh, int32_t fw) {
 // VPB_MAX_FRAMES).  *n = the total number of boxes, checked against the batch limit.  build_frame_table is the engine-free
 // part (vpb_preprocess_affine): at most `limit` boxes.  Per frame type, check_call checks what applies to the whole call and
 // table_entry one frame with boxes and its entry (first_box is filled by the caller):
-//   vpb_frame        pitch_bytes 0 (packed rows) or >= 3 * width; `matrix` is unused
-//   vpb_frame_nv12   even height and width >= 2, pitches 0 (packed: width) or >= width, both planes non-NULL, and a known
-//                    matrix, written into every entry
-static int check_call(const char*, const vpb_frame*, int32_t) { return VPB_OK; }
-static int check_call(const char* fn, const vpb_frame_nv12*, int32_t matrix) {
-  if (matrix != VPB_YUV_BT601 && matrix != VPB_YUV_BT709)
-    return fail(VPB_ERR_ARG, "%s: unknown YUV matrix %d (VPB_YUV_BT601 or VPB_YUV_BT709 expected)", fn, matrix);
+//   vpb_frame        pitch_bytes 0 (packed rows) or >= 3 * width; `fmt` is unused
+//   vpb_frame_yuv    the layout's size rules (even width; even height for 4:2:0), pitches 0 (packed) or >= the row's bytes,
+//                    the planes the layout uses non-NULL, and a known layout, matrix and range, written into every entry
+//   vpb_frame_nv12   the NV12, limited-range vpb_frame_yuv
+static_assert(VPB_YUV_BT601 == YUV_BT601 && VPB_YUV_BT709 == YUV_BT709 && VPB_YUV_LIMITED == YUV_LIMITED && VPB_YUV_FULL == YUV_FULL,
+              "the header's conversion constants are the gather's");
+struct YuvFormat { int32_t layout = VPB_YUV_NV12, matrix = VPB_YUV_BT601, range = VPB_YUV_LIMITED; };
+static YuvFormat yuv_format(int32_t layout, int32_t matrix, int32_t range) {
+  YuvFormat f;
+  f.layout = layout; f.matrix = matrix; f.range = range;
+  return f;
+}
+static YuvFormat nv12_format(int32_t matrix) { return yuv_format(VPB_YUV_NV12, matrix, VPB_YUV_LIMITED); }
+static int check_call(const char*, const vpb_frame*, const YuvFormat&) { return VPB_OK; }
+static int check_call(const char* fn, const vpb_frame_yuv*, const YuvFormat& c) {
+  if (c.layout < VPB_YUV_NV12 || c.layout > VPB_YUV_UYVY)
+    return fail(VPB_ERR_ARG, "%s: unknown YUV layout %d (VPB_YUV_NV12 .. VPB_YUV_UYVY expected)", fn, c.layout);
+  if (c.range != VPB_YUV_LIMITED && c.range != VPB_YUV_FULL)
+    return fail(VPB_ERR_ARG, "%s: unknown YUV range %d (VPB_YUV_LIMITED or VPB_YUV_FULL expected)", fn, c.range);
+  if (c.matrix != VPB_YUV_BT601 && c.matrix != VPB_YUV_BT709)
+    return fail(VPB_ERR_ARG, "%s: unknown YUV matrix %d (VPB_YUV_BT601 or VPB_YUV_BT709 expected)", fn, c.matrix);
   return VPB_OK;
 }
-static int table_entry(const char* fn, int j, const vpb_frame& f, int32_t, FrameEntry* t) {
+static int check_call(const char* fn, const vpb_frame_nv12*, const YuvFormat& c) {
+  return check_call(fn, static_cast<const vpb_frame_yuv*>(nullptr), c);
+}
+static int table_entry(const char* fn, int j, const vpb_frame& f, const YuvFormat&, FrameEntry* t) {
   const long long pitch = f.pitch_bytes ? f.pitch_bytes : 3LL * f.width;
   if (!f.data || f.height < 1 || f.width < 1 || pitch < 3LL * f.width)
     return fail(VPB_ERR_ARG, "%s: frame %d: data %p, %dx%d (w x h), pitch %lld bytes (0 or >= 3 * width expected)", fn, j,
@@ -1797,21 +1815,49 @@ static int table_entry(const char* fn, int j, const vpb_frame& f, int32_t, Frame
   t->data = f.data; t->pitch = pitch; t->fh = f.height; t->fw = f.width;
   return VPB_OK;
 }
-static int table_entry(const char* fn, int j, const vpb_frame_nv12& f, int32_t matrix, Nv12Entry* t) {
-  const long long yp = f.y_pitch ? f.y_pitch : f.width, uvp = f.uv_pitch ? f.uv_pitch : f.width;
-  if (!f.y || !f.uv || f.height < 2 || f.width < 2 || (f.height & 1) || (f.width & 1) || yp < f.width || uvp < f.width)
-    return fail(VPB_ERR_ARG, "%s: frame %d: y %p, uv %p, %dx%d (w x h, even and >= 2 expected), pitches %lld / %lld bytes "
-                "(0 or >= width expected)", fn, j, static_cast<const void*>(f.y), static_cast<const void*>(f.uv), f.width, f.height,
-                static_cast<long long>(f.y_pitch), static_cast<long long>(f.uv_pitch));
+// the pointers and steps of preprocess.cuh's YuvEntry for each layout (the table above YuvEntry)
+static int table_entry(const char* fn, int j, const vpb_frame_yuv& f, const YuvFormat& c, YuvEntry* t) {
+  static const char* const names[] = {"NV12", "NV21", "I420", "YV12", "YUYV", "UYVY"};
+  const bool packed = c.layout == VPB_YUV_YUYV || c.layout == VPB_YUV_UYVY, planar = c.layout == VPB_YUV_I420 || c.layout == VPB_YUV_YV12;
+  const long long yrow = packed ? 2LL * f.width : f.width, crow = planar ? f.width / 2 : f.width;
+  const long long yp = f.y_pitch ? f.y_pitch : yrow, cp = packed ? yp : (f.c_pitch ? f.c_pitch : crow);
+  const int planes = packed ? 1 : planar ? 3 : 2;
+  bool ok = f.height >= 1 && f.width >= 2 && !(f.width & 1) && (packed || !(f.height & 1)) && yp >= yrow && cp >= crow;
+  for (int i = 0; i < planes; ++i) ok = ok && f.plane[i];
+  if (!ok)
+    return fail(VPB_ERR_ARG, "%s: frame %d: %s %dx%d (w x h, even width%s expected), planes %p %p %p (%d used), pitches %lld / %lld "
+                "bytes (0 or >= %lld / %lld expected)", fn, j, names[c.layout], f.width, f.height, packed ? "" : " and height",
+                static_cast<const void*>(f.plane[0]), static_cast<const void*>(f.plane[1]), static_cast<const void*>(f.plane[2]), planes,
+                static_cast<long long>(f.y_pitch), static_cast<long long>(f.c_pitch), yrow, crow);
   memset(t, 0, sizeof(*t));
-  t->y = f.y; t->uv = f.uv; t->y_pitch = yp; t->uv_pitch = uvp; t->fh = f.height; t->fw = f.width; t->matrix = matrix;
+  const uint8_t *p0 = f.plane[0], *p1 = f.plane[1], *p2 = f.plane[2];
+  switch (c.layout) {
+    case VPB_YUV_NV12: t->y = p0; t->u = p1; t->v = p1 + 1; break;
+    case VPB_YUV_NV21: t->y = p0; t->u = p1 + 1; t->v = p1; break;
+    case VPB_YUV_I420: t->y = p0; t->u = p1; t->v = p2; break;
+    case VPB_YUV_YV12: t->y = p0; t->u = p2; t->v = p1; break;
+    case VPB_YUV_YUYV: t->y = p0; t->u = p0 + 1; t->v = p0 + 3; break;
+    default:           t->y = p0 + 1; t->u = p0; t->v = p0 + 2; break;       // UYVY
+  }
+  t->y_step = packed ? 2 : 1;
+  t->c_step = packed ? 4 : planar ? 1 : 2;
+  t->c_vshift = packed ? 0 : 1;
+  t->y_pitch = yp; t->c_pitch = cp; t->fh = f.height; t->fw = f.width;
+  t->conv = static_cast<uint8_t>(c.matrix | c.range << 1);
   return VPB_OK;
 }
+static int table_entry(const char* fn, int j, const vpb_frame_nv12& f, const YuvFormat& c, YuvEntry* t) {
+  vpb_frame_yuv g;
+  memset(&g, 0, sizeof(g));
+  g.plane[0] = f.y; g.plane[1] = f.uv; g.y_pitch = f.y_pitch; g.c_pitch = f.uv_pitch;
+  g.height = f.height; g.width = f.width; g.num_boxes = f.num_boxes;
+  return table_entry(fn, j, g, c, t);
+}
 template <class Frame, class Entry>
-static int build_frame_table(const char* fn, const Frame* fr, int32_t num_frames, int32_t matrix, int limit, Entry* tab, int* num_tab,
+static int build_frame_table(const char* fn, const Frame* fr, int32_t num_frames, const YuvFormat& fmt, int limit, Entry* tab, int* num_tab,
                              int32_t* n) {
   if (num_frames < 0 || (num_frames > 0 && !fr)) return fail(VPB_ERR_ARG, "%s: %d frames, frame array %p", fn, num_frames, fr);
-  VPB_TRY(check_call(fn, fr, matrix));
+  VPB_TRY(check_call(fn, fr, fmt));
   long long boxes = 0;
   int used = 0;
   for (int j = 0; j < num_frames; ++j) {
@@ -1819,7 +1865,7 @@ static int build_frame_table(const char* fn, const Frame* fr, int32_t num_frames
     if (f.num_boxes < 0) return fail(VPB_ERR_ARG, "%s: frame %d has num_boxes = %d", fn, j, f.num_boxes);
     if (f.num_boxes == 0) continue;
     Entry t;
-    VPB_TRY(table_entry(fn, j, f, matrix, &t));
+    VPB_TRY(table_entry(fn, j, f, fmt, &t));
     if (used == VPB_MAX_FRAMES) return fail(VPB_ERR_ARG, "%s: more than VPB_MAX_FRAMES = %d frames with boxes", fn, VPB_MAX_FRAMES);
     if (boxes + f.num_boxes > limit)
       return fail(VPB_ERR_ARG, "%s: more than max_batch = %d boxes (frames 0..%d)", fn, limit, j);
@@ -1832,11 +1878,11 @@ static int build_frame_table(const char* fn, const Frame* fr, int32_t num_frames
   return VPB_OK;
 }
 template <class Frame, class Entry>
-static int frame_table(const char* fn, vpb_engine* e, const Frame* fr, int32_t num_frames, int32_t matrix, Entry* tab, int* num_tab,
+static int frame_table(const char* fn, vpb_engine* e, const Frame* fr, int32_t num_frames, const YuvFormat& fmt, Entry* tab, int* num_tab,
                        int32_t* n) {
   if (!e) return fail(VPB_ERR_ARG, "null engine");
   if (!e->finalized) return fail(VPB_ERR_STATE, "weights not finalized: call vpb_finalize first");
-  VPB_TRY(build_frame_table(fn, fr, num_frames, matrix, e->maxB, tab, num_tab, n));
+  VPB_TRY(build_frame_table(fn, fr, num_frames, fmt, e->maxB, tab, num_tab, n));
   return *n ? check_ready_keypoints(e, *n) : VPB_OK;
 }
 
@@ -1868,7 +1914,7 @@ static int check_boxes_host(const int32_t* bb, int32_t n, int32_t fh, int32_t fw
   }
   return VPB_OK;
 }
-template <class Frame>            // vpb_frame | vpb_frame_nv12
+template <class Frame>            // vpb_frame | vpb_frame_yuv | vpb_frame_nv12
 static int check_frames_boxes_host(const Frame* fr, int32_t num_frames, const int32_t* bb) {
   for (int j = 0, first = 0; j < num_frames; first += fr[j].num_boxes, ++j)
     VPB_TRY(check_boxes_host(bb + 4 * static_cast<size_t>(first), fr[j].num_boxes, fr[j].height, fr[j].width, j));
@@ -1903,23 +1949,44 @@ static int stage_plane(uint8_t* dst, const uint8_t* src, long long pitch, size_t
   return VPB_OK;
 }
 static size_t staged_bytes(const FrameEntry& t) { return static_cast<size_t>(t.fh) * t.fw * 3; }
-static size_t staged_bytes(const Nv12Entry& t) { return static_cast<size_t>(t.fh) * t.fw * 3 / 2; }     // Y, then UV
+static size_t staged_bytes(const YuvEntry& t) {        // 4:2:2: 2 B per pixel; 4:2:0: Y, then the chroma plane(s), 1.5 B per pixel
+  return static_cast<size_t>(t.fh) * t.fw * (t.c_step == 4 ? 4 : 3) / 2;
+}
 static int stage_entry(FrameEntry& t, uint8_t* dst, cudaStream_t st) {
   const size_t row = static_cast<size_t>(t.fw) * 3;
   VPB_TRY(stage_plane(dst, t.data, t.pitch, row, t.fh, st));
   t.data = dst; t.pitch = static_cast<long long>(row);
   return VPB_OK;
 }
-static int stage_entry(Nv12Entry& t, uint8_t* dst, cudaStream_t st) {
-  const size_t row = static_cast<size_t>(t.fw);
-  uint8_t* uv = dst + row * t.fh;
-  VPB_TRY(stage_plane(dst, t.y, t.y_pitch, row, t.fh, st));
-  VPB_TRY(stage_plane(uv, t.uv, t.uv_pitch, row, t.fh / 2, st));
-  t.y = dst; t.uv = uv; t.y_pitch = t.uv_pitch = static_cast<long long>(row);
+// The layout family follows from c_step (table_entry): 4 = packed 4:2:2, 2 = semi-planar (NV12 / NV21), 1 = planar (I420 / YV12).
+// Packed and semi-planar planes are staged whole from their first byte, and y / u / v keep their offsets into them.
+static int stage_entry(YuvEntry& t, uint8_t* dst, cudaStream_t st) {
+  const size_t w = static_cast<size_t>(t.fw), h = static_cast<size_t>(t.fh);
+  if (t.c_step == 4) {
+    const uint8_t* base = std::min({t.y, t.u, t.v});
+    VPB_TRY(stage_plane(dst, base, t.y_pitch, 2 * w, t.fh, st));
+    t.y = dst + (t.y - base); t.u = dst + (t.u - base); t.v = dst + (t.v - base);
+    t.y_pitch = t.c_pitch = static_cast<long long>(2 * w);
+    return VPB_OK;
+  }
+  VPB_TRY(stage_plane(dst, t.y, t.y_pitch, w, t.fh, st));
+  uint8_t* c = dst + w * h;
+  if (t.c_step == 2) {
+    const uint8_t* base = std::min(t.u, t.v);
+    VPB_TRY(stage_plane(c, base, t.c_pitch, w, t.fh / 2, st));
+    t.u = c + (t.u - base); t.v = c + (t.v - base);
+    t.c_pitch = static_cast<long long>(w);
+  } else {
+    VPB_TRY(stage_plane(c, t.u, t.c_pitch, w / 2, t.fh / 2, st));
+    VPB_TRY(stage_plane(c + (w / 2) * (h / 2), t.v, t.c_pitch, w / 2, t.fh / 2, st));
+    t.u = c; t.v = c + (w / 2) * (h / 2);
+    t.c_pitch = static_cast<long long>(w / 2);
+  }
+  t.y = dst; t.y_pitch = static_cast<long long>(w);
   return VPB_OK;
 }
 // Host frames -> staging slot `slot`, enqueued on `st` after the slot's last user: each frame packed (a 2D copy from its pitch;
-// NV12: its Y plane, then its UV plane, 1.5 B per pixel), then the boxes of all frames in one copy, or for the affine calls
+// YUV: stage_entry), then the boxes of all frames in one copy, or for the affine calls
 // (h_mats) the matrices and the centre / scale (slot 0: the affine calls have no pipelined form).  Repoints `tab` at the
 // staged frames.
 template <class Entry>
@@ -1996,27 +2063,27 @@ extern "C" int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int3
   return frames_host_submit(e, &f, 1, h_bboxes, n, h_kpts, h_idx, slot);
 }
 
-// ---- the multi-frame calls: one body per call kind, for RGB frames (vpb_frame -> FrameEntry; `matrix` unused) and NV12 frames
-// (vpb_frame_nv12 -> Nv12Entry); `fn` names the entry point in the messages
+// ---- the multi-frame calls: one body per call kind, for RGB frames (vpb_frame -> FrameEntry; `fmt` unused) and YUV frames
+// (vpb_frame_yuv, vpb_frame_nv12 -> YuvEntry); `fn` names the entry point in the messages
 template <class Entry, class Frame>
-static int infer_frames_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix, const int32_t* d_bboxes,
+static int infer_frames_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt, const int32_t* d_bboxes,
                           float* d_kpts, int32_t* d_idx, void* stream) {
   Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   return frames_core(e, tab, nt, d_bboxes, nullptr, nullptr, {{0, n}}, false, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 template <class Entry, class Frame>
-static int infer_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix,
+static int infer_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
                                const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
   Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
@@ -2024,12 +2091,12 @@ static int infer_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_fra
   return frames_host_sync(e, tab, nt, h_bboxes, nullptr, nullptr, {{0, n}}, false, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
 template <class Entry, class Frame>
-static int submit_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix,
+static int submit_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
                                 const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot) {
   Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   if (slot < 0 || slot > 1) return fail(VPB_ERR_ARG, "%s: slot %d", fn, slot);
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
@@ -2040,27 +2107,42 @@ static int submit_frames_host_t(const char* fn, vpb_engine* e, const Frame* h_fr
 
 extern "C" int vpb_infer_frames(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* d_bboxes,
                                 float* d_kpts, int32_t* d_idx, void* stream) {
-  return infer_frames_t<FrameEntry>("vpb_infer_frames", e, h_frames, num_frames, 0, d_bboxes, d_kpts, d_idx, stream);
+  return infer_frames_t<FrameEntry>("vpb_infer_frames", e, h_frames, num_frames, YuvFormat{}, d_bboxes, d_kpts, d_idx, stream);
 }
 extern "C" int vpb_infer_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
                                      float* h_kpts, int32_t* h_idx, void* stream) {
-  return infer_frames_host_t<FrameEntry>("vpb_infer_frames_host", e, h_frames, num_frames, 0, h_bboxes, h_kpts, h_idx, stream);
+  return infer_frames_host_t<FrameEntry>("vpb_infer_frames_host", e, h_frames, num_frames, YuvFormat{}, h_bboxes, h_kpts, h_idx, stream);
 }
 extern "C" int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
                                       float* h_kpts, int32_t* h_idx, int32_t slot) {
-  return submit_frames_host_t<FrameEntry>("vpb_submit_frames_host", e, h_frames, num_frames, 0, h_bboxes, h_kpts, h_idx, slot);
+  return submit_frames_host_t<FrameEntry>("vpb_submit_frames_host", e, h_frames, num_frames, YuvFormat{}, h_bboxes, h_kpts, h_idx, slot);
 }
 extern "C" int vpb_infer_frames_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                      const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
-  return infer_frames_t<Nv12Entry>("vpb_infer_frames_nv12", e, h_frames, num_frames, matrix, d_bboxes, d_kpts, d_idx, stream);
+  return infer_frames_t<YuvEntry>("vpb_infer_frames_nv12", e, h_frames, num_frames, nv12_format(matrix), d_bboxes, d_kpts, d_idx, stream);
 }
 extern "C" int vpb_infer_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                           const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
-  return infer_frames_host_t<Nv12Entry>("vpb_infer_frames_nv12_host", e, h_frames, num_frames, matrix, h_bboxes, h_kpts, h_idx, stream);
+  return infer_frames_host_t<YuvEntry>("vpb_infer_frames_nv12_host", e, h_frames, num_frames, nv12_format(matrix), h_bboxes, h_kpts, h_idx, stream);
 }
 extern "C" int vpb_submit_frames_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                            const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot) {
-  return submit_frames_host_t<Nv12Entry>("vpb_submit_frames_nv12_host", e, h_frames, num_frames, matrix, h_bboxes, h_kpts, h_idx, slot);
+  return submit_frames_host_t<YuvEntry>("vpb_submit_frames_nv12_host", e, h_frames, num_frames, nv12_format(matrix), h_bboxes, h_kpts, h_idx, slot);
+}
+extern "C" int vpb_infer_frames_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                    int32_t range, const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
+  return infer_frames_t<YuvEntry>("vpb_infer_frames_yuv", e, h_frames, num_frames, yuv_format(layout, matrix, range), d_bboxes, d_kpts,
+                                  d_idx, stream);
+}
+extern "C" int vpb_infer_frames_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                         int32_t range, const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
+  return infer_frames_host_t<YuvEntry>("vpb_infer_frames_yuv_host", e, h_frames, num_frames, yuv_format(layout, matrix, range), h_bboxes,
+                                       h_kpts, h_idx, stream);
+}
+extern "C" int vpb_submit_frames_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                          int32_t range, const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot) {
+  return submit_frames_host_t<YuvEntry>("vpb_submit_frames_yuv_host", e, h_frames, num_frames, yuv_format(layout, matrix, range), h_bboxes,
+                                        h_kpts, h_idx, slot);
 }
 
 // ------------------------------------------------------------------------------------------------ affine top-down crops
@@ -2068,7 +2150,7 @@ extern "C" int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_fram
   FrameEntry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(build_frame_table("vpb_preprocess_affine", h_frames, num_frames, 0, 1 << 30, tab, &nt, &n));
+  VPB_TRY(build_frame_table("vpb_preprocess_affine", h_frames, num_frames, YuvFormat{}, 1 << 30, tab, &nt, &n));
   if (n == 0) return VPB_OK;
   if (!d_mats || !d_crops) return fail(VPB_ERR_ARG, "vpb_preprocess_affine: null pointer");
   AffineParams q = affine_params(tab, nt, d_mats, nullptr, n, nullptr);
@@ -2277,24 +2359,24 @@ extern "C" int vpb_tracker_status(vpb_tracker* t, int32_t* h_status) {
 
 // RGB and NV12 as the multi-frame calls
 template <class Entry, class Frame>
-static int infer_affine_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix, const double* d_mats,
+static int infer_affine_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt, const double* d_mats,
                           const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
   Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   return frames_core(e, tab, nt, nullptr, d_mats, d_cs, {{0, n}}, false, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
 template <class Entry, class Frame>
-static int infer_affine_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, int32_t matrix,
+static int infer_affine_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
                                const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
   Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table(fn, e, h_frames, num_frames, matrix, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
   if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
@@ -2304,19 +2386,29 @@ static int infer_affine_host_t(const char* fn, vpb_engine* e, const Frame* h_fra
 
 extern "C" int vpb_infer_affine(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* d_mats, const float* d_cs,
                                 float* d_kpts, int32_t* d_idx, void* stream) {
-  return infer_affine_t<FrameEntry>("vpb_infer_affine", e, h_frames, num_frames, 0, d_mats, d_cs, d_kpts, d_idx, stream);
+  return infer_affine_t<FrameEntry>("vpb_infer_affine", e, h_frames, num_frames, YuvFormat{}, d_mats, d_cs, d_kpts, d_idx, stream);
 }
 extern "C" int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const double* h_mats, const float* h_cs,
                                      float* h_kpts, int32_t* h_idx, void* stream) {
-  return infer_affine_host_t<FrameEntry>("vpb_infer_affine_host", e, h_frames, num_frames, 0, h_mats, h_cs, h_kpts, h_idx, stream);
+  return infer_affine_host_t<FrameEntry>("vpb_infer_affine_host", e, h_frames, num_frames, YuvFormat{}, h_mats, h_cs, h_kpts, h_idx, stream);
 }
 extern "C" int vpb_infer_affine_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                      const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
-  return infer_affine_t<Nv12Entry>("vpb_infer_affine_nv12", e, h_frames, num_frames, matrix, d_mats, d_cs, d_kpts, d_idx, stream);
+  return infer_affine_t<YuvEntry>("vpb_infer_affine_nv12", e, h_frames, num_frames, nv12_format(matrix), d_mats, d_cs, d_kpts, d_idx, stream);
 }
 extern "C" int vpb_infer_affine_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                                           const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
-  return infer_affine_host_t<Nv12Entry>("vpb_infer_affine_nv12_host", e, h_frames, num_frames, matrix, h_mats, h_cs, h_kpts, h_idx, stream);
+  return infer_affine_host_t<YuvEntry>("vpb_infer_affine_nv12_host", e, h_frames, num_frames, nv12_format(matrix), h_mats, h_cs, h_kpts, h_idx, stream);
+}
+extern "C" int vpb_infer_affine_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                    int32_t range, const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
+  return infer_affine_t<YuvEntry>("vpb_infer_affine_yuv", e, h_frames, num_frames, yuv_format(layout, matrix, range), d_mats, d_cs, d_kpts,
+                                  d_idx, stream);
+}
+extern "C" int vpb_infer_affine_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                         int32_t range, const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
+  return infer_affine_host_t<YuvEntry>("vpb_infer_affine_yuv_host", e, h_frames, num_frames, yuv_format(layout, matrix, range), h_mats, h_cs,
+                                       h_kpts, h_idx, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ multi-head calls
@@ -2360,7 +2452,8 @@ extern "C" int vpb_infer_heads(vpb_engine* e, const float* d_crops, const int32_
 }
 
 // the runs of equal head over the frames that have boxes (frame j's boxes all belong to head h_heads[j])
-static int frame_segments(vpb_engine* e, const char* fn, const vpb_frame* fr, int32_t num_frames, const int32_t* h_heads,
+template <class Frame>
+static int frame_segments(vpb_engine* e, const char* fn, const Frame* fr, int32_t num_frames, const int32_t* h_heads,
                           std::vector<Segment>* segs) {
   if (num_frames > 0 && !h_heads) return fail(VPB_ERR_ARG, "%s: null head array", fn);
   for (int j = 0; j < num_frames; ++j)
@@ -2368,66 +2461,114 @@ static int frame_segments(vpb_engine* e, const char* fn, const vpb_frame* fr, in
   return VPB_OK;
 }
 
-extern "C" int vpb_infer_frames_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
-                                      const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
-  VPB_TRY(check_ready_heads(e, "vpb_infer_frames_heads"));
-  FrameEntry tab[VPB_MAX_FRAMES];
+// one body per multi-head call kind, for RGB frames (FrameEntry) and YUV frames (YuvEntry), as the multi-frame calls
+template <class Entry, class Frame>
+static int infer_frames_heads_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
+                                const int32_t* h_heads, const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, fn));
+  Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_frames_heads", e, h_frames, num_frames, 0, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   std::vector<Segment> segs;
-  VPB_TRY(frame_segments(e, "vpb_infer_frames_heads", h_frames, num_frames, h_heads, &segs));
+  VPB_TRY(frame_segments(e, fn, h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
-  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_heads: null pointer");
+  if (!d_bboxes || !d_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   return frames_core(e, tab, nt, d_bboxes, nullptr, nullptr, segs, true, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
-
-extern "C" int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
-                                           const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
-  VPB_TRY(check_ready_heads(e, "vpb_infer_frames_heads_host"));
-  FrameEntry tab[VPB_MAX_FRAMES];
+template <class Entry, class Frame>
+static int infer_frames_heads_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
+                                     const int32_t* h_heads, const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, fn));
+  Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_frames_heads_host", e, h_frames, num_frames, 0, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   std::vector<Segment> segs;
-  VPB_TRY(frame_segments(e, "vpb_infer_frames_heads_host", h_frames, num_frames, h_heads, &segs));
+  VPB_TRY(frame_segments(e, fn, h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
-  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_frames_heads_host: null pointer");
+  if (!h_bboxes || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   VPB_TRY(check_frames_boxes_host(h_frames, num_frames, h_bboxes));
   return frames_host_sync(e, tab, nt, h_bboxes, nullptr, nullptr, segs, true, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
 }
-
-extern "C" int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
-                                      const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
-  VPB_TRY(check_ready_heads(e, "vpb_infer_affine_heads"));
-  FrameEntry tab[VPB_MAX_FRAMES];
+template <class Entry, class Frame>
+static int infer_affine_heads_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
+                                const int32_t* h_heads, const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
+  VPB_TRY(check_ready_heads(e, fn));
+  Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_affine_heads", e, h_frames, num_frames, 0, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   std::vector<Segment> segs;
-  VPB_TRY(frame_segments(e, "vpb_infer_affine_heads", h_frames, num_frames, h_heads, &segs));
+  VPB_TRY(frame_segments(e, fn, h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
-  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_heads: null pointer");
+  if (!d_mats || !d_cs || !d_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   return frames_core(e, tab, nt, nullptr, d_mats, d_cs, segs, true, n, d_kpts, d_idx, static_cast<cudaStream_t>(stream));
 }
-
-extern "C" int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
-                                           const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
-  VPB_TRY(check_ready_heads(e, "vpb_infer_affine_heads_host"));
-  FrameEntry tab[VPB_MAX_FRAMES];
+template <class Entry, class Frame>
+static int infer_affine_heads_host_t(const char* fn, vpb_engine* e, const Frame* h_frames, int32_t num_frames, const YuvFormat& fmt,
+                                     const int32_t* h_heads, const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx,
+                                     void* stream) {
+  VPB_TRY(check_ready_heads(e, fn));
+  Entry tab[VPB_MAX_FRAMES];
   int nt = 0;
   int32_t n = 0;
-  VPB_TRY(frame_table("vpb_infer_affine_heads_host", e, h_frames, num_frames, 0, tab, &nt, &n));
+  VPB_TRY(frame_table(fn, e, h_frames, num_frames, fmt, tab, &nt, &n));
   std::vector<Segment> segs;
-  VPB_TRY(frame_segments(e, "vpb_infer_affine_heads_host", h_frames, num_frames, h_heads, &segs));
+  VPB_TRY(frame_segments(e, fn, h_frames, num_frames, h_heads, &segs));
   if (n == 0) return VPB_OK;
   DeviceGuard dev_guard(e);
-  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "vpb_infer_affine_heads_host: null pointer");
+  if (!h_mats || !h_cs || !h_kpts) return fail(VPB_ERR_ARG, "%s: null pointer", fn);
   VPB_TRY(check_affine_host(h_mats, h_cs, n));
   return frames_host_sync(e, tab, nt, nullptr, h_mats, h_cs, segs, true, n, h_kpts, h_idx, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_infer_frames_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                      const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream) {
+  return infer_frames_heads_t<FrameEntry>("vpb_infer_frames_heads", e, h_frames, num_frames, YuvFormat{}, h_heads, d_bboxes, d_kpts, d_idx,
+                                          stream);
+}
+extern "C" int vpb_infer_frames_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                           const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream) {
+  return infer_frames_heads_host_t<FrameEntry>("vpb_infer_frames_heads_host", e, h_frames, num_frames, YuvFormat{}, h_heads, h_bboxes,
+                                               h_kpts, h_idx, stream);
+}
+extern "C" int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                      const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream) {
+  return infer_affine_heads_t<FrameEntry>("vpb_infer_affine_heads", e, h_frames, num_frames, YuvFormat{}, h_heads, d_mats, d_cs, d_kpts,
+                                          d_idx, stream);
+}
+extern "C" int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
+                                           const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
+  return infer_affine_heads_host_t<FrameEntry>("vpb_infer_affine_heads_host", e, h_frames, num_frames, YuvFormat{}, h_heads, h_mats, h_cs,
+                                               h_kpts, h_idx, stream);
+}
+extern "C" int vpb_infer_frames_heads_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout,
+                                          int32_t matrix, int32_t range, const int32_t* h_heads, const int32_t* d_bboxes, float* d_kpts,
+                                          int32_t* d_idx, void* stream) {
+  return infer_frames_heads_t<YuvEntry>("vpb_infer_frames_heads_yuv", e, h_frames, num_frames, yuv_format(layout, matrix, range), h_heads,
+                                        d_bboxes, d_kpts, d_idx, stream);
+}
+extern "C" int vpb_infer_frames_heads_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout,
+                                               int32_t matrix, int32_t range, const int32_t* h_heads, const int32_t* h_bboxes,
+                                               float* h_kpts, int32_t* h_idx, void* stream) {
+  return infer_frames_heads_host_t<YuvEntry>("vpb_infer_frames_heads_yuv_host", e, h_frames, num_frames, yuv_format(layout, matrix, range),
+                                             h_heads, h_bboxes, h_kpts, h_idx, stream);
+}
+extern "C" int vpb_infer_affine_heads_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout,
+                                          int32_t matrix, int32_t range, const int32_t* h_heads, const double* d_mats, const float* d_cs,
+                                          float* d_kpts, int32_t* d_idx, void* stream) {
+  return infer_affine_heads_t<YuvEntry>("vpb_infer_affine_heads_yuv", e, h_frames, num_frames, yuv_format(layout, matrix, range), h_heads,
+                                        d_mats, d_cs, d_kpts, d_idx, stream);
+}
+extern "C" int vpb_infer_affine_heads_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout,
+                                               int32_t matrix, int32_t range, const int32_t* h_heads, const double* h_mats,
+                                               const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream) {
+  return infer_affine_heads_host_t<YuvEntry>("vpb_infer_affine_heads_yuv_host", e, h_frames, num_frames, yuv_format(layout, matrix, range),
+                                             h_heads, h_mats, h_cs, h_kpts, h_idx, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ host crops

@@ -135,13 +135,13 @@ __global__ void __launch_bounds__(PP_W) crop_resize_normalise(const PreprocParam
 // device buffer that two calls in flight could race on.  The entry is picked by a run-time index; __grid_constant__ guarantees
 // that this reads the parameter block in place, where a plain by-value parameter would allow the compiler to copy it to
 // local memory (ptxas reports no stack frame for the kernel either way with CUDA 12.9).
-// NV12 frames (vpb_infer_frames_nv12): the kernels are templated on the table entry; an Nv12Entry tap reads its Y byte and
-// the (U, V) pair of its 2x2 block and converts them to RGB (nv12_rgb) before the unchanged resize / warp arithmetic, so the
-// result is that of cv2.cvtColor(COLOR_YUV2RGB_NV12) followed by the RGB path.  Taps outside the crop or frame still read
-// RGB 0.
+// YUV frames (vpb_infer_frames_yuv, vpb_infer_frames_nv12): the kernels are templated on the table entry; a YuvEntry tap
+// reads its Y byte and the (U, V) pair of its chroma block and converts them to RGB (yuv_rgb) before the unchanged resize /
+// warp arithmetic, so the result is that of cv2.cvtColor(COLOR_YUV2RGB_<layout>) (or the full-range conversion) followed
+// by the RGB path.  Taps outside the crop or frame still read RGB 0.
 constexpr int FP_MAX_FRAMES = 64;
 struct FrameEntry {
-  static constexpr bool kNv12 = false;
+  static constexpr bool kYuv = false;
   const uint8_t* data;          // [fh, fw, 3] RGB, row pitch `pitch` bytes
   long long pitch;
   int fh, fw;
@@ -149,40 +149,57 @@ struct FrameEntry {
   int pad_;
 };
 static_assert(sizeof(FrameEntry) == 32, "frame table entry layout");
+// Every 8-bit layout is described by pointers and steps, with no per-layout branch in the kernels:
+//   luma of pixel (x, row)    y[row * y_pitch + x * y_step]
+//   chroma of pixel (x, row)  u[(row >> c_vshift) * c_pitch + (x >> 1) * c_step], and v at the same offset from its pointer
+// The host fills them per layout (engine.cu: yuv_entry):
+//   NV12  Y plane, 1 | uv, uv + 1 | 2 | 1        I420  Y plane, 1 | U plane, V plane | 1 | 1
+//   NV21  Y plane, 1 | vu + 1, vu | 2 | 1        YV12  the same (V is stored first)
+//   YUYV  base, 2 | base + 1, base + 3 | 4 | 0   UYVY  base + 1, 2 | base, base + 2 | 4 | 0
 constexpr int YUV_BT601 = 0, YUV_BT709 = 1;
-struct Nv12Entry {
-  static constexpr bool kNv12 = true;
-  const uint8_t* y;             // [fh, fw] luma, row pitch y_pitch bytes
-  const uint8_t* uv;            // [fh / 2, fw] interleaved U, V of each 2x2 block, row pitch uv_pitch bytes
-  long long y_pitch, uv_pitch;
-  int fh, fw;                   // both even
+constexpr int YUV_LIMITED = 0, YUV_FULL = 1;
+struct YuvEntry {
+  static constexpr bool kYuv = true;
+  const uint8_t* y;
+  const uint8_t* u;
+  const uint8_t* v;
+  long long y_pitch, c_pitch;   // row pitches in bytes; U and V share one
+  int fh, fw;                   // fw even; fh even for 4:2:0
   int first_box;
-  int matrix;                   // YUV_BT601 | YUV_BT709, the same for every entry of a call
+  uint8_t y_step, c_step, c_vshift;
+  uint8_t conv;                 // matrix | range << 1 (YUV_BT601 | YUV_BT709, YUV_LIMITED | YUV_FULL), the same for every entry of a call
 };
-static_assert(sizeof(Nv12Entry) == 48, "NV12 frame table entry layout");
+static_assert(sizeof(YuvEntry) == 56, "YUV frame table entry layout");
 
-// cv2's fixed-point COLOR_YUV2RGB_NV12 (SHIFT 20, limited range, nearest chroma): oracle/nv12_oracle.py pins the formula.
-// The BT.709 set is round(2^20 x (1.164, 1.793, -0.533, -0.213, 2.112)), the 3-decimal form cv2 uses for BT.601.
-struct YuvCoef { int cy, cvr, cvg, cug, cub; };
-__device__ __forceinline__ YuvCoef yuv_coef(int matrix) {
-  return matrix == YUV_BT709 ? YuvCoef{1220542, 1880097, -558891, -223347, 2214593}
-                             : YuvCoef{1220542, 1673527, -852492, -409993, 2116026};
+// Both conversions as one fixed-point form: out = clamp((max(Y - y0, 0) * cy + half + c_v (V - 128) + c_u (U - 128)) >> shift).
+//   limited range: cv2's COLOR_YUV2RGB_NV12 (SHIFT 20, y0 = 16): oracle/nv12_oracle.py pins the formula.  The BT.709 set is
+//                  round(2^20 x (1.164, 1.793, -0.533, -0.213, 2.112)), the 3-decimal form cv2 uses for BT.601.
+//   full range:    cv2's COLOR_YCrCb2RGB (SHIFT 14): Y + ((c (C - 128) + 2^13) >> 14), written with y0 = 0 and cy = 2^14, since
+//                  (Y 2^14 + s) >> 14 = Y + (s >> 14) exactly.  BT.709 is round(2^14 x (1.575, -0.468, -0.187, 1.856)).
+struct YuvCoef { int y0, cy, half, shift, cvr, cvg, cug, cub; };
+__device__ __forceinline__ YuvCoef yuv_coef(int conv) {
+  switch (conv) {
+    case YUV_BT709: return {16, 1220542, 1 << 19, 20, 1880097, -558891, -223347, 2214593};
+    case YUV_BT601 | YUV_FULL << 1: return {0, 1 << 14, 1 << 13, 14, 22987, -11698, -5636, 29049};
+    case YUV_BT709 | YUV_FULL << 1: return {0, 1 << 14, 1 << 13, 14, 25805, -7668, -3064, 30409};
+    default: return {16, 1220542, 1 << 19, 20, 1673527, -852492, -409993, 2116026};
+  }
 }
-// pixel (x, y) of an NV12 frame -> RGB; every intermediate fits in int32 (|sum| < 2^30)
-__device__ __forceinline__ void nv12_rgb(const Nv12Entry& f, const YuvCoef& k, int x, int y, int rgb[3]) {
-  const int Y = f.y[static_cast<size_t>(y) * f.y_pitch + x];
-  const uint8_t* uv = f.uv + static_cast<size_t>(y >> 1) * f.uv_pitch + (x & ~1);
-  const int u = uv[0] - 128, v = uv[1] - 128;
-  const int yy = max(Y - 16, 0) * k.cy + (1 << 19);
-  rgb[0] = min(max((yy + k.cvr * v) >> 20, 0), 255);
-  rgb[1] = min(max((yy + k.cvg * v + k.cug * u) >> 20, 0), 255);
-  rgb[2] = min(max((yy + k.cub * u) >> 20, 0), 255);
+// pixel (x, y) of a YUV frame -> RGB; every intermediate fits in int32 (|sum| < 2^30)
+__device__ __forceinline__ void yuv_rgb(const YuvEntry& f, const YuvCoef& k, int x, int y, int rgb[3]) {
+  const int Y = f.y[static_cast<size_t>(y) * f.y_pitch + x * f.y_step];
+  const size_t c = static_cast<size_t>(y >> f.c_vshift) * f.c_pitch + (x >> 1) * f.c_step;
+  const int u = f.u[c] - 128, v = f.v[c] - 128;
+  const int yy = max(Y - k.y0, 0) * k.cy + k.half;
+  rgb[0] = min(max((yy + k.cvr * v) >> k.shift, 0), 255);
+  rgb[1] = min(max((yy + k.cvg * v + k.cug * u) >> k.shift, 0), 255);
+  rgb[2] = min(max((yy + k.cub * u) >> k.shift, 0), 255);
 }
 
 __device__ __forceinline__ const uint8_t* first_plane(const FrameEntry& f) { return f.data; }
-__device__ __forceinline__ const uint8_t* first_plane(const Nv12Entry& f) { return f.y; }
+__device__ __forceinline__ const uint8_t* first_plane(const YuvEntry& f) { return f.y; }
 __device__ __forceinline__ long long first_pitch(const FrameEntry& f) { return f.pitch; }
-__device__ __forceinline__ long long first_pitch(const Nv12Entry& f) { return f.y_pitch; }
+__device__ __forceinline__ long long first_pitch(const YuvEntry& f) { return f.y_pitch; }
 
 template <class Entry>
 struct FramePatchParamsT {
@@ -195,7 +212,7 @@ struct FramePatchParamsT {
   Entry frames[FP_MAX_FRAMES];
 };
 using FramePatchParams = FramePatchParamsT<FrameEntry>;
-static_assert(sizeof(FramePatchParamsT<FrameEntry>) <= 4096 && sizeof(FramePatchParamsT<Nv12Entry>) <= 4096,
+static_assert(sizeof(FramePatchParamsT<FrameEntry>) <= 4096 && sizeof(FramePatchParamsT<YuvEntry>) <= 4096,
               "the frame table travels in the 4 KB parameter block");
 
 template <class Entry>
@@ -229,7 +246,7 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
     if (q.frames[mid].first_box <= box) lo = mid; else hi = mid;
   }
   const Entry& fr = q.frames[lo];
-  [[maybe_unused]] const uint8_t* frame = first_plane(fr);    // the RGB path's pixels (NV12: the Y plane, read by nv12_rgb)
+  [[maybe_unused]] const uint8_t* frame = first_plane(fr);    // the RGB path's pixels (YUV: the Y plane, read by yuv_rgb)
   [[maybe_unused]] const long long pitch = first_pitch(fr);
   const int fh = fr.fh, fw = fr.fw;
   const int* bb = p.bboxes + 4 * box;
@@ -270,13 +287,13 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
       const PpAxis ax = s_ax[dx];
       const int cy0 = ay.i0 - top, cy1 = ay.i1 - top, cx0 = ax.i0 - left, cx1 = ax.i1 - left;
       const bool vy0 = cy0 >= 0 && cy0 < h, vy1 = cy1 >= 0 && cy1 < h, vx0 = cx0 >= 0 && cx0 < w, vx1 = cx1 >= 0 && cx1 < w;
-      if constexpr (Entry::kNv12) {
-        const YuvCoef k = yuv_coef(fr.matrix);
+      if constexpr (Entry::kYuv) {
+        const YuvCoef k = yuv_coef(fr.conv);
         int t00[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t10[3] = {0, 0, 0}, t11[3] = {0, 0, 0};   // out-of-crop taps: RGB 0
-        if (vy0 && vx0) nv12_rgb(fr, k, x0 + cx0, y0 + cy0, t00);
-        if (vy0 && vx1) nv12_rgb(fr, k, x0 + cx1, y0 + cy0, t01);
-        if (vy1 && vx0) nv12_rgb(fr, k, x0 + cx0, y0 + cy1, t10);
-        if (vy1 && vx1) nv12_rgb(fr, k, x0 + cx1, y0 + cy1, t11);
+        if (vy0 && vx0) yuv_rgb(fr, k, x0 + cx0, y0 + cy0, t00);
+        if (vy0 && vx1) yuv_rgb(fr, k, x0 + cx1, y0 + cy0, t01);
+        if (vy1 && vx0) yuv_rgb(fr, k, x0 + cx0, y0 + cy1, t10);
+        if (vy1 && vx1) yuv_rgb(fr, k, x0 + cx1, y0 + cy1, t11);
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           const int s0 = t00[c] * ax.a0 + t01[c] * ax.a1, s1 = t10[c] * ax.a0 + t11[c] * ax.a1;
@@ -360,16 +377,16 @@ __device__ __forceinline__ void affine_pixel(const uint8_t* frame, long long pit
     v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + (1 << 14)) >> 15;
   }
 }
-// the same from an NV12 frame: each tap converted to RGB first, the constant border is RGB 0
-__device__ __forceinline__ void affine_pixel_nv12(const Nv12Entry& f, const YuvCoef& k, int X, int Y, int v[3]) {
+// the same from a YUV frame: each tap converted to RGB first, the constant border is RGB 0
+__device__ __forceinline__ void affine_pixel_yuv(const YuvEntry& f, const YuvCoef& k, int X, int Y, int v[3]) {
   const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767), fx = X & 31, fy = Y & 31;
   const bool vx0 = sx >= 0 && sx < f.fw, vx1 = sx + 1 >= 0 && sx + 1 < f.fw, vy0 = sy >= 0 && sy < f.fh, vy1 = sy + 1 >= 0 && sy + 1 < f.fh;
   const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
   int t00[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t10[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
-  if (vy0 && vx0) nv12_rgb(f, k, sx, sy, t00);
-  if (vy0 && vx1) nv12_rgb(f, k, sx + 1, sy, t01);
-  if (vy1 && vx0) nv12_rgb(f, k, sx, sy + 1, t10);
-  if (vy1 && vx1) nv12_rgb(f, k, sx + 1, sy + 1, t11);
+  if (vy0 && vx0) yuv_rgb(f, k, sx, sy, t00);
+  if (vy0 && vx1) yuv_rgb(f, k, sx + 1, sy, t01);
+  if (vy1 && vx0) yuv_rgb(f, k, sx, sy + 1, t10);
+  if (vy1 && vx1) yuv_rgb(f, k, sx + 1, sy + 1, t11);
 #pragma unroll
   for (int c = 0; c < 3; ++c) v[c] = (t00[c] * w00 + t01[c] * w01 + t10[c] * w10 + t11[c] * w11 + (1 << 14)) >> 15;
 }
@@ -395,7 +412,7 @@ struct AffineParamsT {
   Entry frames[FP_MAX_FRAMES];
 };
 using AffineParams = AffineParamsT<FrameEntry>;
-static_assert(sizeof(AffineParamsT<FrameEntry>) <= 4096 && sizeof(AffineParamsT<Nv12Entry>) <= 4096,
+static_assert(sizeof(AffineParamsT<FrameEntry>) <= 4096 && sizeof(AffineParamsT<YuvEntry>) <= 4096,
               "the frame table travels in the 4 KB parameter block");
 template <class Entry>
 __device__ __forceinline__ const Entry& affine_frame(const AffineParamsT<Entry>& q, int box) {
@@ -480,7 +497,7 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_c
     if (dy >= 0) {
       int v[3];
       const int2 r = s_row[ky], c = s_col[dx];
-      if constexpr (Entry::kNv12) affine_pixel_nv12(fr, yuv_coef(fr.matrix), (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
+      if constexpr (Entry::kYuv) affine_pixel_yuv(fr, yuv_coef(fr.conv), (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
       else affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) v3[ch] = s_lut[ch][v[ch]];

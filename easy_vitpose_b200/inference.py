@@ -134,6 +134,37 @@ class B200PoseBackend:
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
         return self.model.infer_affine_heads_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list)[0]
 
+    # YUV video frames in any layout ViTPose.infer_frames_yuv takes (layout "i420" | "yv12" | "nv12" | "nv21" | "yuyv" | "uyvy",
+    # e.g. ffmpeg's `-pix_fmt yuv420p` output or a V4L2 webcam's YUYV frame), converted on the device only where the gather taps
+    @torch.no_grad()
+    def inference_frames_yuv(self, frames, bboxes_list: "list[np.ndarray]", layout: str = "i420", matrix: str = "bt601",
+                             full_range: bool = False) -> "list[np.ndarray]":
+        """inference_frames on YUV video frames: no RGB conversion."""
+        return self.model.infer_frames_yuv_host(frames, bboxes_list, layout, matrix, full_range)[0]
+
+    @torch.no_grad()
+    def inference_topdown_yuv(self, frames, bboxes_list: "list[np.ndarray]", padding: float = 1.25, use_udp: bool = True,
+                              layout: str = "i420", matrix: str = "bt601", full_range: bool = False) -> "list[np.ndarray]":
+        """inference_topdown on YUV video frames."""
+        args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
+        return self.model.infer_affine_yuv_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], layout, matrix,
+                                                full_range)[0]
+
+    @torch.no_grad()
+    def inference_frames_heads_yuv(self, frames, bboxes_list: "list[np.ndarray]", heads_list, layout: str = "i420",
+                                   matrix: str = "bt601", full_range: bool = False) -> "list[np.ndarray]":
+        """inference_frames_heads on YUV video frames."""
+        return self.model.infer_frames_heads_yuv_host(frames, bboxes_list, heads_list, layout, matrix, full_range)[0]
+
+    @torch.no_grad()
+    def inference_topdown_heads_yuv(self, frames, bboxes_list: "list[np.ndarray]", heads_list, padding: float = 1.25,
+                                    use_udp: bool = True, layout: str = "i420", matrix: str = "bt601",
+                                    full_range: bool = False) -> "list[np.ndarray]":
+        """inference_topdown_heads on YUV video frames."""
+        args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
+        return self.model.infer_affine_heads_yuv_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list,
+                                                      layout, matrix, full_range)[0]
+
     def draw_frames(self, imgs: "list[np.ndarray]", kpts_list: "list[np.ndarray]", skeleton, person_index=None,
                     confidence_threshold: float = 0.5, channel_order: str = "rgb", point_colors=None, limb_colors=None) -> "list[np.ndarray]":
         """Host form of draw.draw_poses: uint8 [H,W,3] frames + each frame's float32 [n_i,K,3] (y, x, score) keypoints -> new

@@ -15,7 +15,7 @@ import torch
 from . import _lib
 from .configs import VITPOSE_PLUS_HEADS
 
-__all__ = ["ViTPose", "plan_frame_chunks", "nv12_planes", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head", "head_flip_permutations",
+__all__ = ["ViTPose", "plan_frame_chunks", "nv12_planes", "yuv_planes", "split_vitpose_plus", "merge_split_state_dicts", "group_by_head", "head_flip_permutations",
            "plan_head_calls"]
 
 IMG_H, IMG_W, HM_H, HM_W = 256, 192, 64, 48
@@ -50,7 +50,7 @@ def plan_frame_chunks(counts, limit: int, max_frames: int = _lib.MAX_FRAMES) -> 
 def _frame_array(frames, chunk, struct=_lib.VpbFrame):
     """vpb_frame array for one planned call: entries 0..last frame of the call, so that the engine's messages name the
     caller's frame index; frames outside the call get 0 boxes (skipped).  `frames` holds (data pointer, h, w, pitch), or
-    for struct=VpbFrameNv12 (y pointer, y pitch, uv pointer, uv pitch, h, w)."""
+    for struct=VpbFrameNv12 (y pointer, y pitch, uv pointer, uv pitch, h, w), or for struct=VpbFrameYuv ViTPose._yuv_row."""
     arr = (struct * (chunk[-1][0] + 1))()
     for f, s, e in chunk:
         arr[f] = struct(*frames[f], e - s)
@@ -88,6 +88,75 @@ def _yuv_matrix(matrix: str) -> int:
         return _lib.YUV_MATRICES[str(matrix).lower()]
     except KeyError:
         raise ValueError(f"unknown YUV matrix {matrix!r}: one of {sorted(_lib.YUV_MATRICES)}") from None
+
+
+def _yuv_format(layout: str, matrix: str, full_range: bool) -> "tuple[int, int, int]":
+    """(layout, matrix, range) names -> the C constants of the _yuv calls; ValueError for an unknown name."""
+    try:
+        lay = _lib.YUV_LAYOUTS[str(layout).lower()]
+    except KeyError:
+        raise ValueError(f"unknown YUV layout {layout!r}: one of {sorted(_lib.YUV_LAYOUTS)}") from None
+    return lay, _yuv_matrix(matrix), _lib.YUV_RANGES["full" if full_range else "limited"]
+
+
+def _is_u8_2d(p) -> bool:
+    return getattr(p, "ndim", 0) == 2 and str(getattr(p, "dtype", "")) in ("uint8", "torch.uint8")
+
+
+def yuv_planes(frame, layout: str, what: str = "frame") -> "tuple[tuple, int, int]":
+    """One YUV frame -> (its planes in the layout's storage order, as vpb_frame_yuv takes them, height, width), as views
+    where the memory allows, for numpy arrays and torch tensors alike.  Accepted forms:
+      nv12, nv21   uint8 [3H/2, W] with the planes stacked, or a (y [H,W], uv [H/2,W]) pair (uv: vu for nv21)
+      i420, yv12   uint8 [3H/2, W] as cv2 and ffmpeg write it (each chroma plane H/2 x W/2 bytes, packed after the luma), or a
+                   (y [H,W], u [H/2,W/2], v [H/2,W/2]) triple named by content for both layouts
+      yuyv, uyvy   uint8 [H, W, 2] (what cv2.VideoCapture returns with CAP_PROP_CONVERT_RGB = 0) or [H, 2W]
+    Planes may have any row pitch with contiguous rows.  Raises ValueError for unknown layouts, odd or mismatched sizes."""
+    lay = _yuv_format(layout, "bt601", False)[0]
+    name = str(layout).lower()
+    if lay >= _lib.YUV_LAYOUTS["yuyv"]:                      # packed 4:2:2: one [H, 2W] plane
+        if isinstance(frame, (tuple, list)) or getattr(frame, "ndim", 0) not in (2, 3):
+            raise ValueError(f"{what}: {name} [H, W, 2] or [H, 2W] expected, got {type(frame).__name__} "
+                             f"{tuple(getattr(frame, 'shape', ()))}")
+        if frame.ndim == 3:
+            if frame.shape[2] != 2:
+                raise ValueError(f"{what}: {name} [H, W, 2] expected, got shape {tuple(frame.shape)}")
+            frame = frame.reshape(frame.shape[0], 2 * frame.shape[1])
+        if not _is_u8_2d(frame):
+            raise ValueError(f"{what}: {name} frames must be uint8, got {getattr(frame, 'dtype', type(frame))}")
+        h, w = frame.shape[0], frame.shape[1] // 2
+        if h < 1 or w < 2 or frame.shape[1] % 4:
+            raise ValueError(f"{what}: {name} needs an even width >= 2, got {frame.shape[1] / 2:g}x{h} (w x h)")
+        return (frame,), h, w
+    if lay <= _lib.YUV_LAYOUTS["nv21"]:                       # semi-planar: the NV12 forms, for NV21 with the chroma bytes swapped
+        y, c = nv12_planes(frame, what)
+        return (y, c), y.shape[0], y.shape[1]
+    if isinstance(frame, (tuple, list)):                      # planar: (y, u, v) by content
+        if len(frame) != 3:
+            raise ValueError(f"{what}: an {name} (y, u, v) triple expected, got {len(frame)} planes")
+        y, u, v = frame
+    else:
+        if not _is_u8_2d(frame) or frame.shape[0] % 3:
+            raise ValueError(f"{what}: {name} [3H/2, W] with the planes stacked expected, got shape {tuple(getattr(frame, 'shape', ()))}")
+        h, w = frame.shape[0] // 3 * 2, frame.shape[1]
+        if h < 2 or w < 2 or w % 2:
+            raise ValueError(f"{what}: {name} needs an even height and width >= 2, got {h}x{w} (h x w)")
+        y, c = frame[:h], frame[h:]
+        c = c.contiguous() if isinstance(c, torch.Tensor) else np.ascontiguousarray(c)
+        flat, q = c.reshape(-1), (h // 2) * (w // 2)          # each chroma plane is H/2 x W/2 packed bytes
+        first, second = flat[:q].reshape(h // 2, w // 2), flat[q:].reshape(h // 2, w // 2)
+        u, v = (first, second) if name == "i420" else (second, first)
+    for p in (y, u, v):
+        if not _is_u8_2d(p):
+            raise ValueError(f"{what}: {name} planes must be 2-D uint8, got {getattr(p, 'dtype', type(p))} {tuple(getattr(p, 'shape', ()))}")
+    if not (type(y) is type(u) is type(v)):
+        raise ValueError(f"{what}: the planes must all be numpy arrays or all tensors")
+    h, w = y.shape
+    if h < 2 or w < 2 or h % 2 or w % 2:
+        raise ValueError(f"{what}: {name} needs an even height and width >= 2, got {h}x{w} (h x w)")
+    if tuple(u.shape) != (h // 2, w // 2) or tuple(v.shape) != (h // 2, w // 2):
+        raise ValueError(f"{what}: chroma planes {tuple(u.shape)} / {tuple(v.shape)} do not match the {h}x{w} y plane "
+                         "([H/2, W/2] expected)")
+    return ((y, u, v) if name == "i420" else (y, v, u)), h, w
 
 
 def group_by_head(heads, num_heads: int) -> "tuple[np.ndarray, list[int]]":
@@ -1150,6 +1219,195 @@ class ViTPose:
         split = np.cumsum(counts)[:-1]
         return np.split(kp, split), np.split(idx, split)
 
+    # ---------------------------------------------------------------------------------------- YUV video frames
+    # Every call takes layout = "i420" | "yv12" | "nv12" | "nv21" | "yuyv" | "uyvy" (the frame forms of yuv_planes), matrix =
+    # "bt601" | "bt709" and full_range (False: limited range as cv2's COLOR_YUV2RGB_*; True: JPEG range as COLOR_YCrCb2RGB).
+    # Every call is bit-identical to its RGB twin on the converted frames (oracle/yuv_oracle.py: yuv_to_rgb); only the pixels
+    # under the boxes are converted, on the fly.
+    @staticmethod
+    def _yuv_row(planes, h: int, w: int):
+        """-> the vpb_frame_yuv fields before num_boxes: ((plane pointers), y pitch, chroma pitch, h, w)"""
+        dev = isinstance(planes[0], torch.Tensor)
+        ptr = (lambda p: p.data_ptr()) if dev else (lambda p: p.ctypes.data)
+        pitch = (lambda p: p.stride(0)) if dev else (lambda p: p.strides[0])
+        ptrs = tuple(ptr(p) for p in planes) + (None,) * (3 - len(planes))
+        return ptrs, pitch(planes[0]), pitch(planes[1]) if len(planes) > 1 else 0, h, w
+
+    def _yuv_device_table(self, frames, layout: str):
+        """-> (the plane tensors to keep alive, the _yuv_row of every frame)"""
+        keep, table = [], []
+        for j, f in enumerate(frames):
+            planes, h, w = yuv_planes(f, layout, f"frame {j}")
+            planes = [self._device_plane(j, p) for p in planes]
+            if len(planes) == 3 and planes[1].stride(0) != planes[2].stride(0):
+                planes[1:] = [p.contiguous() for p in planes[1:]]    # U and V share one pitch
+            keep += planes
+            table.append(self._yuv_row(planes, h, w))
+        return keep, table
+
+    @staticmethod
+    def _yuv_host_table(frames, layout: str, copy: bool = True):
+        """-> (the numpy planes to keep alive, the _yuv_row of every frame).  Planes whose rows are not contiguous bytes, and
+        U / V planes of different pitches, are copied packed; with copy=False (the pipelined form) they raise ValueError."""
+        keep, table = [], []
+        for j, f in enumerate(frames):
+            planes, h, w = yuv_planes(f, layout, f"frame {j}")
+            if not isinstance(planes[0], np.ndarray):
+                raise ValueError(f"frame {j}: numpy {layout} planes expected")
+            planes = list(planes)
+            for i, p in enumerate(planes):
+                if p.strides[1] != 1 or p.strides[0] < p.shape[1]:
+                    if not copy:
+                        raise ValueError(f"frame {j}: numpy {layout} planes with contiguous bytes in each row expected")
+                    planes[i] = np.ascontiguousarray(p)
+            if len(planes) == 3 and planes[1].strides[0] != planes[2].strides[0]:
+                if not copy:
+                    raise ValueError(f"frame {j}: the U and V planes must share one row pitch")
+                planes[1:] = [np.ascontiguousarray(p) for p in planes[1:]]
+            keep += planes
+            table.append(ViTPose._yuv_row(planes, h, w))
+        return keep, table
+
+    def _device_boxes(self, bboxes) -> "list[torch.Tensor]":
+        dev = torch.device("cuda", self._device)
+        boxes = []
+        for b in bboxes:                                     # rounded as _check_frame does; device boxes stay on the device
+            b = torch.as_tensor(b)
+            if b.is_floating_point():
+                b = b.round()
+            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
+        return boxes
+
+    def infer_frames_yuv(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
+                         check: bool = False):
+        """infer_frames on YUV frames (vpb_infer_frames_yuv): CUDA (or host, copied over) frames and per-frame boxes [n_j,4] ->
+        (list of kpts f32 [n_j,K,3], list of idx i32 [n_j,K]).  Chunked, flip test and status word as infer_frames."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        planes, table = self._yuv_device_table(frames, layout)
+        dev = torch.device("cuda", self._device)
+        boxes = self._device_boxes(bboxes)
+        counts = [b.shape[0] for b in boxes]
+        bb = torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=dev)
+        n = bb.shape[0]
+        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
+        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
+        s = 0
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_yuv(
+                self._handle, arr, len(arr), *fmt, C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
+                C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 1:
+            raise ValueError("a box is empty after padding and clipping to its frame")
+        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+
+    def infer_frames_yuv_host(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False):
+        """HOST form of infer_frames_yuv (vpb_infer_frames_yuv_host, synchronous): numpy frames, per-frame boxes -> numpy
+        (kpts, idx) lists.  Each frame is staged packed (1.5 B per pixel for 4:2:0, 2 B for 4:2:2); an empty box raises
+        ValueError."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        planes, table = self._yuv_host_table(frames, layout)
+        boxes = [self._round_boxes(b) for b in bboxes]
+        counts = [len(b) for b in boxes]
+        bb = np.concatenate(boxes, 0) if boxes else np.zeros((0, 4), np.int32)
+        n = bb.shape[0]
+        kp = np.empty((n, self.num_keypoints, 3), np.float32)
+        idx = np.empty((n, self.num_keypoints), np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, self.batch_limit):
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                _lib.check_value(_lib.lib().vpb_infer_frames_yuv_host(
+                    self._handle, arr, len(arr), *fmt, bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
+                    idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        if not counts:
+            return [], []
+        split = np.cumsum(counts)[:-1]
+        return np.split(kp, split), np.split(idx, split)
+
+    def submit_frames_yuv_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int, layout: str = "i420",
+                               matrix: str = "bt601", full_range: bool = False) -> None:
+        """Asynchronous vpb_submit_frames_yuv_host, ONE engine call (wait with wait_host(slot)): the pipelined video form of
+        submit_frames_host for numpy YUV frames whose planes have contiguous bytes in each row (any row pitch; U and V of one
+        pitch).  Frames, boxes (int32 [n_j,4], already rounded) and outputs must stay alive and unmodified until the wait."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        for j, b in enumerate(bboxes):
+            if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
+                raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
+        planes, table = self._yuv_host_table(frames, layout, copy=False)
+        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
+        n = bb.shape[0]
+        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
+                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
+            raise ValueError("submit_frames_yuv_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
+        arr = (_lib.VpbFrameYuv * len(table))(*[_lib.VpbFrameYuv(*t, len(b)) for t, b in zip(table, bboxes)])
+        with torch.cuda.device(self._device):
+            _lib.check_value(_lib.lib().vpb_submit_frames_yuv_host(
+                self._handle, arr, len(arr), *fmt, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
+                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+    def infer_affine_yuv(self, frames, mats, centers, scales, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
+                         check: bool = False):
+        """infer_affine on YUV frames (vpb_infer_affine_yuv): the warp reads the planes and converts each tap."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if not (len(frames) == len(mats) == len(centers) == len(scales)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        planes, table = self._yuv_device_table(frames, layout)
+        dev = torch.device("cuda", self._device)
+        counts, M, CS = self._affine_args(mats, centers, scales)
+        M, CS = M.to(dev), CS.to(dev)
+        n = M.shape[0]
+        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
+        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
+        s = 0
+        for chunk in plan_frame_chunks(counts, self.batch_limit):
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_yuv(
+                self._handle, arr, len(arr), *fmt, C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 2:
+            raise ValueError("a matrix entry is not finite or a scale is <= 0")
+        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+
+    def infer_affine_yuv_host(self, frames, mats, centers, scales, layout: str = "i420", matrix: str = "bt601",
+                              full_range: bool = False):
+        """HOST form of infer_affine_yuv (vpb_infer_affine_yuv_host, synchronous), checked as infer_affine_host."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if not (len(frames) == len(mats) == len(centers) == len(scales)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        planes, table = self._yuv_host_table(frames, layout)
+        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
+        M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
+        n = M.shape[0]
+        kp = np.empty((n, self.num_keypoints, 3), np.float32)
+        idx = np.empty((n, self.num_keypoints), np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in plan_frame_chunks(counts, self.batch_limit):
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                _lib.check_value(_lib.lib().vpb_infer_affine_yuv_host(
+                    self._handle, arr, len(arr), *fmt, M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
+                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        if not counts:
+            return [], []
+        split = np.cumsum(counts)[:-1]
+        return np.split(kp, split), np.split(idx, split)
+
     # ---------------------------------------------------------------------------------------- several heads (datasets)
     @staticmethod
     def _segments(chunk):
@@ -1327,6 +1585,129 @@ class ViTPose:
                 ha = np.ascontiguousarray(hv[:len(arr)])
                 _lib.check_value(_lib.lib().vpb_infer_affine_heads_host(
                     self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),
+                    CS[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p),
+                    self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        k_t, i_t = self._per_frame(ents, counts, torch.from_numpy(kp), torch.from_numpy(idx))
+        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+
+    # the multi-head calls on YUV frames: frames as the _yuv calls take them, everything else as their RGB twins above
+    def infer_frames_heads_yuv(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
+                               check: bool = False):
+        """infer_frames_heads on YUV frames (vpb_infer_frames_heads_yuv)."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if not (len(frames) == len(bboxes) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        planes, ytab = self._yuv_device_table(frames, layout)
+        dev = torch.device("cuda", self._device)
+        boxes = self._device_boxes(bboxes)
+        ents, _, chunks = plan_head_calls([b.shape[0] for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
+        n = sum(len(sel) for _, sel, _ in ents)
+        bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
+        Km = self.num_keypoints_max
+        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
+        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
+        table = [ytab[j] for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        for chunk in chunks:
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            ha = np.ascontiguousarray(hv[:len(arr)])
+            self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads_yuv(
+                self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), C.c_void_p(bb[s:].data_ptr()),
+                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 1:
+            raise ValueError("a box is empty after padding and clipping to its frame")
+        return self._per_frame(ents, [b.shape[0] for b in boxes], kp, idx)
+
+    def infer_frames_heads_yuv_host(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False):
+        """HOST form of infer_frames_heads_yuv (vpb_infer_frames_heads_yuv_host, synchronous)."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if not (len(frames) == len(bboxes) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        planes, ytab = self._yuv_host_table(frames, layout)
+        boxes = [self._round_boxes(b) for b in bboxes]
+        ents, _, chunks = plan_head_calls([len(b) for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
+        n = sum(len(sel) for _, sel, _ in ents)
+        bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
+        Km = self.num_keypoints_max
+        kp = np.zeros((n, Km, 3), np.float32)
+        idx = np.zeros((n, Km), np.int32)
+        table = [ytab[j] for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in chunks:
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                ha = np.ascontiguousarray(hv[:len(arr)])
+                _lib.check_value(_lib.lib().vpb_infer_frames_heads_yuv_host(
+                    self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), bb[s:].ctypes.data_as(C.c_void_p),
+                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
+                s += sum(e - b for _, b, e in chunk)
+        k_t, i_t = self._per_frame(ents, [len(b) for b in boxes], torch.from_numpy(kp), torch.from_numpy(idx))
+        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+
+    def infer_affine_heads_yuv(self, frames, mats, centers, scales, heads, layout: str = "i420", matrix: str = "bt601",
+                               full_range: bool = False, check: bool = False):
+        """infer_affine_heads on YUV frames (vpb_infer_affine_heads_yuv)."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
+                             f"arrays, {len(heads)} head arrays")
+        planes, ytab = self._yuv_device_table(frames, layout)
+        dev = torch.device("cuda", self._device)
+        counts, M, CS = self._affine_args(mats, centers, scales)
+        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        o = torch.as_tensor(order, device=M.device)
+        M, CS = M.index_select(0, o).contiguous().to(dev), CS.index_select(0, o).contiguous().to(dev)
+        n = M.shape[0]
+        Km = self.num_keypoints_max
+        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
+        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
+        table = [ytab[j] for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        for chunk in chunks:
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            ha = np.ascontiguousarray(hv[:len(arr)])
+            self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_heads_yuv(
+                self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), C.c_void_p(M[s:].data_ptr()),
+                C.c_void_p(CS[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
+            s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & 2:
+            raise ValueError("a matrix entry is not finite or a scale is <= 0")
+        return self._per_frame(ents, counts, kp, idx)
+
+    def infer_affine_heads_yuv_host(self, frames, mats, centers, scales, heads, layout: str = "i420", matrix: str = "bt601",
+                                    full_range: bool = False):
+        """HOST form of infer_affine_heads_yuv (vpb_infer_affine_heads_yuv_host, synchronous)."""
+        self._ensure()
+        fmt = _yuv_format(layout, matrix, full_range)
+        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
+            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
+                             f"arrays, {len(heads)} head arrays")
+        planes, ytab = self._yuv_host_table(frames, layout)
+        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
+        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        M = np.ascontiguousarray(M.cpu().numpy()[order])
+        CS = np.ascontiguousarray(CS.cpu().numpy()[order], np.float32)
+        n = M.shape[0]
+        Km = self.num_keypoints_max
+        kp = np.zeros((n, Km, 3), np.float32)
+        idx = np.zeros((n, Km), np.int32)
+        table = [ytab[j] for j, _, _ in ents]
+        hv = np.array([k for _, _, k in ents], np.int32)
+        s = 0
+        with torch.cuda.device(self._device):
+            for chunk in chunks:
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                ha = np.ascontiguousarray(hv[:len(arr)])
+                _lib.check_value(_lib.lib().vpb_infer_affine_heads_yuv_host(
+                    self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),
                     CS[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p),
                     self._stream()))
                 s += sum(e - b for _, b, e in chunk)

@@ -231,12 +231,13 @@ int vpb_infer_affine_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_
  *   B = clamp((yy + half + CUB (U - 128)) >> 20) to 0..255;
  *   VPB_YUV_BT601: CY 1220542, CVR 1673527, CVG -852492, CUG -409993, CUB 2116026 = cv2 COLOR_YUV2RGB_NV12, bit for bit;
  *   VPB_YUV_BT709: CY 1220542, CVR 1880097, CVG -558891, CUG -223347, CUB 2214593 (limited-range BT.709, 3-decimal form).
- * Full-range (JPEG) YUV is not covered.  The converted taps then go through the RGB arithmetic unchanged, and taps outside
- * the crop or frame read RGB 0, so every call is bit-identical (patch rows, keypoints, argmax, flip test included) to its RGB
- * counterpart on cv2.cvtColor(frame, COLOR_YUV2RGB_NV12) (BT.601) or the formula above (BT.709).  Arguments, errors, status
- * bits, limits, staging slots and graph caches are those of the RGB counterparts, plus `matrix`; VPB_ERR_ARG also for an odd
- * or < 2 height or width, a pitch below width, a NULL plane in a frame with boxes, or an unknown matrix.  The host forms stage
- * each frame packed at 1.5 B per pixel (Y, then UV). */
+ * The converted taps then go through the RGB arithmetic unchanged, and taps outside the crop or frame read RGB 0, so every
+ * call is bit-identical (patch rows, keypoints, argmax, flip test included) to its RGB counterpart on
+ * cv2.cvtColor(frame, COLOR_YUV2RGB_NV12) (BT.601) or the formula above (BT.709).  Arguments, errors, status bits, limits,
+ * staging slots and graph caches are those of the RGB counterparts, plus `matrix`; VPB_ERR_ARG also for an odd or < 2 height
+ * or width, a pitch below width, a NULL plane in a frame with boxes, or an unknown matrix.  The host forms stage each frame
+ * packed at 1.5 B per pixel (Y, then UV).  These calls are the NV12, limited-range case of the _yuv calls below, which also
+ * take NV21, I420, YV12, YUYV and UYVY frames, full-range YUV, and serve the multi-head engines. */
 #define VPB_YUV_BT601 0
 #define VPB_YUV_BT709 1
 typedef struct vpb_frame_nv12 {
@@ -310,6 +311,64 @@ int vpb_infer_affine_heads(vpb_engine* e, const vpb_frame* h_frames, int32_t num
                            const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream);
 int vpb_infer_affine_heads_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_heads,
                                 const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream);
+
+/* ---- YUV video frames in every 8-bit layout a decoder, camera or capture card delivers: the frame, affine and multi-head
+ * calls read them directly and convert only the pixels the gather taps, with nearest chroma as cv2 does.  Each call takes
+ * (layout, matrix, range), the same for all frames of the call.  Pixel (x, row) reads
+ *   Y                    4:2:0 planar and semi-planar: plane[0][row * y_pitch + x];  4:2:2: the Y byte of pixel x of row `row`
+ *   (U, V)               the pair of its chroma block: 2x2 pixels for 4:2:0, 2x1 for 4:2:2
+ * and converts it with
+ *   VPB_YUV_LIMITED:     the NV12 formula above (SHIFT 20, BT.601 = cv2 COLOR_YUV2RGB_*, BT.709 its 3-decimal form);
+ *   VPB_YUV_FULL:        cv2's COLOR_YCrCb2RGB (JPEG range, SHIFT 14, D(s) = (s + 8192) >> 14):
+ *                        R = clamp(Y + D(C0 (V - 128))), G = clamp(Y + D(C2 (U - 128) + C1 (V - 128))), B = clamp(Y + D(C3 (U - 128)));
+ *                        BT.601 C0..C3 = 22987, -11698, -5636, 29049 (cv2 bit for bit); BT.709 25805, -7668, -3064, 30409.
+ * The planes, in the order the layout stores them (unused entries are ignored and may be NULL):
+ *   VPB_YUV_NV12  plane[0] Y [h, w], plane[1] UV [h/2, w] (U first)     VPB_YUV_I420  plane[0] Y, plane[1] U [h/2, w/2], plane[2] V
+ *   VPB_YUV_NV21  plane[0] Y [h, w], plane[1] VU [h/2, w] (V first)     VPB_YUV_YV12  plane[0] Y, plane[1] V [h/2, w/2], plane[2] U
+ *   VPB_YUV_YUYV  plane[0] [h, 2w]: Y0 U Y1 V per pixel pair             VPB_YUV_UYVY  plane[0] [h, 2w]: U Y0 V Y1 per pixel pair
+ * y_pitch is plane[0]'s row pitch (0 = packed: w, or 2w for 4:2:2); c_pitch the chroma planes' (0 = packed: w for NV12 / NV21,
+ * w/2 for I420 / YV12; unused for 4:2:2).  Every call is bit-identical to its RGB counterpart on the converted frame, as the
+ * NV12 calls are, and shares its arguments, errors, status bits, limits, staging slots and graph caches.  VPB_ERR_ARG also for
+ * an odd height or width in 4:2:0, an odd width in 4:2:2, a pitch below the row's bytes, a NULL plane the layout uses in a
+ * frame with boxes, or an unknown layout, matrix or range.  The host forms stage each frame packed: 1.5 B per pixel for 4:2:0
+ * (Y, then the chroma planes), 2 B per pixel for 4:2:2. */
+#define VPB_YUV_NV12 0
+#define VPB_YUV_NV21 1
+#define VPB_YUV_I420 2
+#define VPB_YUV_YV12 3
+#define VPB_YUV_YUYV 4
+#define VPB_YUV_UYVY 5
+#define VPB_YUV_LIMITED 0
+#define VPB_YUV_FULL 1
+typedef struct vpb_frame_yuv {
+  const uint8_t* plane[3];  /* in storage order (above); device addresses or host (the _host forms) */
+  int64_t y_pitch;          /* row pitch of plane[0] in bytes; 0 = packed */
+  int64_t c_pitch;          /* row pitch of the chroma plane(s) in bytes; 0 = packed */
+  int32_t height, width;
+  int32_t num_boxes;        /* as vpb_frame.num_boxes */
+} vpb_frame_yuv;
+int vpb_infer_frames_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                         int32_t range, const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_frames_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                              int32_t range, const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, void* stream);
+int vpb_submit_frames_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                               int32_t range, const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx, int32_t slot);   /* vpb_wait_host(slot) */
+int vpb_infer_affine_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                         int32_t range, const double* d_mats, const float* d_cs, float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_affine_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                              int32_t range, const double* h_mats, const float* h_cs, float* h_kpts, int32_t* h_idx, void* stream);
+/* the multi-head calls on YUV frames (NV12 included): h_heads, outputs and errors as vpb_infer_frames_heads / vpb_infer_affine_heads */
+int vpb_infer_frames_heads_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                               int32_t range, const int32_t* h_heads, const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream);
+int vpb_infer_frames_heads_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                    int32_t range, const int32_t* h_heads, const int32_t* h_bboxes, float* h_kpts, int32_t* h_idx,
+                                    void* stream);
+int vpb_infer_affine_heads_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                               int32_t range, const int32_t* h_heads, const double* d_mats, const float* d_cs, float* d_kpts,
+                               int32_t* d_idx, void* stream);
+int vpb_infer_affine_heads_yuv_host(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
+                                    int32_t range, const int32_t* h_heads, const double* h_mats, const float* h_cs, float* h_kpts,
+                                    int32_t* h_idx, void* stream);
 
 /* ---- pose overlay: the pose layer of VitInference.draw() (easy_ViTPose/inference.py:283-312, vit_utils/visualization.py:360-481)
  * for the people of up to VPB_MAX_FRAMES frames in two launches, drawn in place, bit-exact with cv2 4.13.  Per person in order
