@@ -24,16 +24,17 @@ MAX_FRAMES = 64                                       # VPB_MAX_FRAMES: frames w
 class VpbFrame(C.Structure):
     """vpb_frame: one frame of a multi-frame call (vpb_infer_frames and its host forms)."""
     _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("pitch_bytes", C.c_int64),
-                ("num_boxes", C.c_int32)]
+                ("num_boxes", C.c_int32), ("rotation", C.c_int32)]
 
 
+ROTATIONS = (0, 90, 180, 270)                         # vpb_frame*.rotation: degrees counter-clockwise, stored frame -> view
 YUV_MATRICES = {"bt601": 0, "bt709": 1}              # VPB_YUV_BT601, VPB_YUV_BT709
 
 
 class VpbFrameNv12(C.Structure):
     """vpb_frame_nv12: one NV12 frame (Y plane + interleaved half-resolution UV plane) of the _nv12 calls."""
     _fields_ = [("y", C.c_void_p), ("y_pitch", C.c_int64), ("uv", C.c_void_p), ("uv_pitch", C.c_int64),
-                ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32)]
+                ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32), ("rotation", C.c_int32)]
 
 
 YUV_LAYOUTS = {"nv12": 0, "nv21": 1, "i420": 2, "yv12": 3, "yuyv": 4, "uyvy": 5}    # VPB_YUV_NV12 .. VPB_YUV_UYVY
@@ -43,7 +44,7 @@ YUV_RANGES = {"limited": 0, "full": 1}               # VPB_YUV_LIMITED, VPB_YUV_
 class VpbFrameYuv(C.Structure):
     """vpb_frame_yuv: one YUV frame of the _yuv calls, its planes in the layout's storage order."""
     _fields_ = [("plane", C.c_void_p * 3), ("y_pitch", C.c_int64), ("c_pitch", C.c_int64),
-                ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32)]
+                ("height", C.c_int32), ("width", C.c_int32), ("num_boxes", C.c_int32), ("rotation", C.c_int32)]
 
 
 MAX_HEADS = 8                                        # VPB_MAX_HEADS: keypoint heads of one engine

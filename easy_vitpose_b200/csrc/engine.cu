@@ -1756,6 +1756,13 @@ extern "C" int vpb_preprocess(const uint8_t* d_frame, int32_t frame_h, int32_t f
 }
 
 static_assert(VPB_MAX_FRAMES == FP_MAX_FRAMES, "the header's frame limit is the gather's table size");
+// `rotation` sits in what was the structs' tail padding: sizes and the other offsets are those of the structs without it
+static_assert(sizeof(vpb_frame) == 32 && offsetof(vpb_frame, num_boxes) == 24 && offsetof(vpb_frame, rotation) == 28,
+              "vpb_frame layout");
+static_assert(sizeof(vpb_frame_nv12) == 48 && offsetof(vpb_frame_nv12, num_boxes) == 40 && offsetof(vpb_frame_nv12, rotation) == 44,
+              "vpb_frame_nv12 layout");
+static_assert(sizeof(vpb_frame_yuv) == 56 && offsetof(vpb_frame_yuv, num_boxes) == 48 && offsetof(vpb_frame_yuv, rotation) == 52,
+              "vpb_frame_yuv layout");
 
 // Keypoints of the boxes d_bboxes of a frame table, or with d_mats of its affine crops (centre / scale d_cs for the decode;
 // the canvas sizes and offsets are then unused).  The crops are never materialised: the gathers write the bf16 patch rows
@@ -1784,6 +1791,7 @@ static FrameEntry single_frame(const uint8_t* data, int32_t fh, int32_t fw) {
 //   vpb_frame_yuv    the layout's size rules (even width; even height for 4:2:0), pitches 0 (packed) or >= the row's bytes,
 //                    the planes the layout uses non-NULL, and a known layout, matrix and range, written into every entry
 //   vpb_frame_nv12   the NV12, limited-range vpb_frame_yuv
+// and every frame's rotation is 0, 90, 180 or 270 (the entry's rot code); the entry keeps the stored size.
 static_assert(VPB_YUV_BT601 == YUV_BT601 && VPB_YUV_BT709 == YUV_BT709 && VPB_YUV_LIMITED == YUV_LIMITED && VPB_YUV_FULL == YUV_FULL,
               "the header's conversion constants are the gather's");
 struct YuvFormat { int32_t layout = VPB_YUV_NV12, matrix = VPB_YUV_BT601, range = VPB_YUV_LIMITED; };
@@ -1793,6 +1801,23 @@ static YuvFormat yuv_format(int32_t layout, int32_t matrix, int32_t range) {
   return f;
 }
 static YuvFormat nv12_format(int32_t matrix) { return yuv_format(VPB_YUV_NV12, matrix, VPB_YUV_LIMITED); }
+// vpb_frame*.rotation (degrees counter-clockwise) -> the entries' rot code 0..3, or -1
+static int rotation_code(int32_t degrees) {
+  switch (degrees) {
+    case 0: return 0;
+    case 90: return 1;
+    case 180: return 2;
+    case 270: return 3;
+    default: return -1;
+  }
+}
+// the size of a frame's view: stored (height, width), swapped for 90 and 270 degrees
+template <class Frame>
+static void view_size(const Frame& f, int32_t* h, int32_t* w) {
+  const bool swap = rotation_code(f.rotation) & 1;
+  *h = swap ? f.width : f.height;
+  *w = swap ? f.height : f.width;
+}
 static int check_call(const char*, const vpb_frame*, const YuvFormat&) { return VPB_OK; }
 static int check_call(const char* fn, const vpb_frame_yuv*, const YuvFormat& c) {
   if (c.layout < VPB_YUV_NV12 || c.layout > VPB_YUV_UYVY)
@@ -1812,7 +1837,7 @@ static int table_entry(const char* fn, int j, const vpb_frame& f, const YuvForma
     return fail(VPB_ERR_ARG, "%s: frame %d: data %p, %dx%d (w x h), pitch %lld bytes (0 or >= 3 * width expected)", fn, j,
                 static_cast<const void*>(f.data), f.width, f.height, static_cast<long long>(f.pitch_bytes));
   memset(t, 0, sizeof(*t));
-  t->data = f.data; t->pitch = pitch; t->fh = f.height; t->fw = f.width;
+  t->data = f.data; t->pitch = pitch; t->fh = f.height; t->fw = f.width; t->rot = rotation_code(f.rotation);
   return VPB_OK;
 }
 // the pointers and steps of preprocess.cuh's YuvEntry for each layout (the table above YuvEntry)
@@ -1844,13 +1869,14 @@ static int table_entry(const char* fn, int j, const vpb_frame_yuv& f, const YuvF
   t->c_vshift = packed ? 0 : 1;
   t->y_pitch = yp; t->c_pitch = cp; t->fh = f.height; t->fw = f.width;
   t->conv = static_cast<uint8_t>(c.matrix | c.range << 1);
+  t->rot = static_cast<uint8_t>(rotation_code(f.rotation));
   return VPB_OK;
 }
 static int table_entry(const char* fn, int j, const vpb_frame_nv12& f, const YuvFormat& c, YuvEntry* t) {
   vpb_frame_yuv g;
   memset(&g, 0, sizeof(g));
   g.plane[0] = f.y; g.plane[1] = f.uv; g.y_pitch = f.y_pitch; g.c_pitch = f.uv_pitch;
-  g.height = f.height; g.width = f.width; g.num_boxes = f.num_boxes;
+  g.height = f.height; g.width = f.width; g.num_boxes = f.num_boxes; g.rotation = f.rotation;
   return table_entry(fn, j, g, c, t);
 }
 template <class Frame, class Entry>
@@ -1863,6 +1889,8 @@ static int build_frame_table(const char* fn, const Frame* fr, int32_t num_frames
   for (int j = 0; j < num_frames; ++j) {
     const Frame& f = fr[j];
     if (f.num_boxes < 0) return fail(VPB_ERR_ARG, "%s: frame %d has num_boxes = %d", fn, j, f.num_boxes);
+    if (rotation_code(f.rotation) < 0)
+      return fail(VPB_ERR_ARG, "%s: frame %d has rotation %d (0, 90, 180 or 270 expected)", fn, j, f.rotation);
     if (f.num_boxes == 0) continue;
     Entry t;
     VPB_TRY(table_entry(fn, j, f, fmt, &t));
@@ -1914,10 +1942,13 @@ static int check_boxes_host(const int32_t* bb, int32_t n, int32_t fh, int32_t fw
   }
   return VPB_OK;
 }
-template <class Frame>            // vpb_frame | vpb_frame_yuv | vpb_frame_nv12
+template <class Frame>            // vpb_frame | vpb_frame_yuv | vpb_frame_nv12, after build_frame_table checked the rotations
 static int check_frames_boxes_host(const Frame* fr, int32_t num_frames, const int32_t* bb) {
-  for (int j = 0, first = 0; j < num_frames; first += fr[j].num_boxes, ++j)
-    VPB_TRY(check_boxes_host(bb + 4 * static_cast<size_t>(first), fr[j].num_boxes, fr[j].height, fr[j].width, j));
+  for (int j = 0, first = 0; j < num_frames; first += fr[j].num_boxes, ++j) {
+    int32_t h = 0, w = 0;
+    view_size(fr[j], &h, &w);
+    VPB_TRY(check_boxes_host(bb + 4 * static_cast<size_t>(first), fr[j].num_boxes, h, w, j));
+  }
   return VPB_OK;
 }
 // host matrices / centre-scale: what the device forms can only flag in the status word is an argument error here

@@ -139,6 +139,11 @@ __global__ void __launch_bounds__(PP_W) crop_resize_normalise(const PreprocParam
 // reads its Y byte and the (U, V) pair of its chroma block and converts them to RGB (yuv_rgb) before the unchanged resize /
 // warp arithmetic, so the result is that of cv2.cvtColor(COLOR_YUV2RGB_<layout>) (or the full-range conversion) followed
 // by the RGB path.  Taps outside the crop or frame still read RGB 0.
+// Rotated frames (vpb_frame.rotation): an entry's fh / fw, pitches and planes describe the STORED frame, and `rot` (0..3 =
+// 0, 90, 180, 270 degrees counter-clockwise) turns it into the VIEW the boxes and matrices are given in, the frame that
+// cv2.rotate(stored, ROTATE_90_COUNTERCLOCKWISE | ROTATE_180 | ROTATE_90_CLOCKWISE) would produce.  Clipping, padding and
+// bounds tests use the view's size (view_hw); each tap maps its view pixel to the stored pixel (stored_px) only to address
+// it, so a rotated call reads exactly the bytes an upright call on the rotated copy reads.
 constexpr int FP_MAX_FRAMES = 64;
 struct FrameEntry {
   static constexpr bool kYuv = false;
@@ -146,7 +151,7 @@ struct FrameEntry {
   long long pitch;
   int fh, fw;
   int first_box;
-  int pad_;
+  int rot;                      // 0..3: the view is the stored frame turned by 90 rot degrees counter-clockwise
 };
 static_assert(sizeof(FrameEntry) == 32, "frame table entry layout");
 // Every 8-bit layout is described by pointers and steps, with no per-layout branch in the kernels:
@@ -167,9 +172,27 @@ struct YuvEntry {
   int fh, fw;                   // fw even; fh even for 4:2:0
   int first_box;
   uint8_t y_step, c_step, c_vshift;
-  uint8_t conv;                 // matrix | range << 1 (YUV_BT601 | YUV_BT709, YUV_LIMITED | YUV_FULL), the same for every entry of a call
+  uint8_t conv : 2;             // matrix | range << 1 (YUV_BT601 | YUV_BT709, YUV_LIMITED | YUV_FULL), the same for every entry of a call
+  uint8_t rot : 2;              // as FrameEntry::rot
 };
 static_assert(sizeof(YuvEntry) == 56, "YUV frame table entry layout");
+
+// (view height, view width) of an entry: the stored size, swapped for 90 and 270 degrees
+template <class Entry>
+__device__ __forceinline__ int2 view_hw(const Entry& f) { return f.rot & 1 ? make_int2(f.fw, f.fh) : make_int2(f.fh, f.fw); }
+// view pixel (x, y) -> the stored pixel (sx, sy) it shows, for a view pixel inside the view; np.rot90(stored, rot)[y, x]:
+//   rot 0: (x, y)   1: (fw-1-y, x)   2: (fw-1-x, fh-1-y)   3: (y, fh-1-x)
+// i.e. an axis swap for 90 / 270 and a reflection of stored x (90, 180) and of stored y (180, 270).
+template <class Entry>
+__device__ __forceinline__ int2 stored_px(const Entry& f, int x, int y) {
+  const int rot = f.rot, a = rot & 1 ? y : x, b = rot & 1 ? x : y;
+  return make_int2(rot == 1 || rot == 2 ? f.fw - 1 - a : a, rot & 2 ? f.fh - 1 - b : b);
+}
+// byte offset of view pixel (x, y) in an RGB entry
+__device__ __forceinline__ size_t rgb_offset(const FrameEntry& f, int x, int y) {
+  const int2 s = stored_px(f, x, y);
+  return static_cast<size_t>(s.y) * f.pitch + s.x * 3;
+}
 
 // Both conversions as one fixed-point form: out = clamp((max(Y - y0, 0) * cy + half + c_v (V - 128) + c_u (U - 128)) >> shift).
 //   limited range: cv2's COLOR_YUV2RGB_NV12 (SHIFT 20, y0 = 16): oracle/nv12_oracle.py pins the formula.  The BT.709 set is
@@ -185,8 +208,11 @@ __device__ __forceinline__ YuvCoef yuv_coef(int conv) {
     default: return {16, 1220542, 1 << 19, 20, 1673527, -852492, -409993, 2116026};
   }
 }
-// pixel (x, y) of a YUV frame -> RGB; every intermediate fits in int32 (|sum| < 2^30)
-__device__ __forceinline__ void yuv_rgb(const YuvEntry& f, const YuvCoef& k, int x, int y, int rgb[3]) {
+// view pixel (vx, vy) of a YUV frame -> RGB: the stored pixel's Y and its stored chroma block; every intermediate fits in
+// int32 (|sum| < 2^30)
+__device__ __forceinline__ void yuv_rgb(const YuvEntry& f, const YuvCoef& k, int vx, int vy, int rgb[3]) {
+  const int2 s = stored_px(f, vx, vy);
+  const int x = s.x, y = s.y;
   const int Y = f.y[static_cast<size_t>(y) * f.y_pitch + x * f.y_step];
   const size_t c = static_cast<size_t>(y >> f.c_vshift) * f.c_pitch + (x >> 1) * f.c_step;
   const int u = f.u[c] - 128, v = f.v[c] - 128;
@@ -195,11 +221,6 @@ __device__ __forceinline__ void yuv_rgb(const YuvEntry& f, const YuvCoef& k, int
   rgb[1] = min(max((yy + k.cvg * v + k.cug * u) >> k.shift, 0), 255);
   rgb[2] = min(max((yy + k.cub * u) >> k.shift, 0), 255);
 }
-
-__device__ __forceinline__ const uint8_t* first_plane(const FrameEntry& f) { return f.data; }
-__device__ __forceinline__ const uint8_t* first_plane(const YuvEntry& f) { return f.y; }
-__device__ __forceinline__ long long first_pitch(const FrameEntry& f) { return f.pitch; }
-__device__ __forceinline__ long long first_pitch(const YuvEntry& f) { return f.y_pitch; }
 
 template <class Entry>
 struct FramePatchParamsT {
@@ -246,9 +267,8 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
     if (q.frames[mid].first_box <= box) lo = mid; else hi = mid;
   }
   const Entry& fr = q.frames[lo];
-  [[maybe_unused]] const uint8_t* frame = first_plane(fr);    // the RGB path's pixels (YUV: the Y plane, read by yuv_rgb)
-  [[maybe_unused]] const long long pitch = first_pitch(fr);
-  const int fh = fr.fh, fw = fr.fw;
+  const int2 vhw = view_hw(fr);                               // boxes are clipped to the view
+  const int fh = vhw.x, fw = vhw.y;
   const int* bb = p.bboxes + 4 * box;
   const int x0 = min(max(bb[0] - p.pad, 0), fw), x1 = min(max(bb[2] + p.pad, 0), fw);
   const int y0 = min(max(bb[1] - p.pad, 0), fh), y1 = min(max(bb[3] + p.pad, 0), fh);
@@ -301,13 +321,14 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows(const __grid_constant
           v3[c] = s_lut[c][min(max(v, 0), 255)];
         }
       } else {
-        const uint8_t* r0 = frame + static_cast<size_t>(vy0 ? y0 + cy0 : 0) * pitch;
-        const uint8_t* r1 = frame + static_cast<size_t>(vy1 ? y0 + cy1 : 0) * pitch;
-        const int f0 = (vx0 ? x0 + cx0 : 0) * 3, f1 = (vx1 ? x0 + cx1 : 0) * 3;
+        const int X0 = vx0 ? x0 + cx0 : 0, X1 = vx1 ? x0 + cx1 : 0;           // view pixels, only dereferenced when valid
+        const int Y0 = vy0 ? y0 + cy0 : 0, Y1 = vy1 ? y0 + cy1 : 0;
+        const uint8_t *t00 = fr.data + rgb_offset(fr, X0, Y0), *t01 = fr.data + rgb_offset(fr, X1, Y0);
+        const uint8_t *t10 = fr.data + rgb_offset(fr, X0, Y1), *t11 = fr.data + rgb_offset(fr, X1, Y1);
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-          const int p00 = (vy0 && vx0) ? r0[f0 + c] : 0, p01 = (vy0 && vx1) ? r0[f1 + c] : 0;
-          const int p10 = (vy1 && vx0) ? r1[f0 + c] : 0, p11 = (vy1 && vx1) ? r1[f1 + c] : 0;
+          const int p00 = (vy0 && vx0) ? t00[c] : 0, p01 = (vy0 && vx1) ? t01[c] : 0;
+          const int p10 = (vy1 && vx0) ? t10[c] : 0, p11 = (vy1 && vx1) ? t11[c] : 0;
           const int s0 = p00 * ax.a0 + p01 * ax.a1, s1 = p10 * ax.a0 + p11 * ax.a1;
           int v = (((ay.a0 * (s0 >> 4)) >> 16) + ((ay.a1 * (s1 >> 4)) >> 16) + 2) >> 2;
           v3[c] = s_lut[c][min(max(v, 0), 255)];
@@ -362,25 +383,29 @@ __device__ __forceinline__ int2 affine_row(const AffineInv& a, int y) {
   return make_int2(__double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.m[1], yd), a.m[2]), 1024.0)) + 16,
                    __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(a.m[4], yd), a.m[5]), 1024.0)) + 16);
 }
-// one output pixel from its fixed-point source coordinates: the three warped bytes
-__device__ __forceinline__ void affine_pixel(const uint8_t* frame, long long pitch, int fh, int fw, int X, int Y, int v[3]) {
+// one output pixel from its fixed-point source coordinates (view pixels): the three warped bytes
+__device__ __forceinline__ void affine_pixel(const FrameEntry& f, int X, int Y, int v[3]) {
   const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767), fx = X & 31, fy = Y & 31;
+  const int2 vhw = view_hw(f);
+  const int fh = vhw.x, fw = vhw.y;
   const bool vx0 = sx >= 0 && sx < fw, vx1 = sx + 1 >= 0 && sx + 1 < fw, vy0 = sy >= 0 && sy < fh, vy1 = sy + 1 >= 0 && sy + 1 < fh;
   const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
-  const uint8_t* r0 = frame + static_cast<size_t>(vy0 ? sy : 0) * pitch;     // only dereferenced when valid
-  const uint8_t* r1 = frame + static_cast<size_t>(vy1 ? sy + 1 : 0) * pitch;
-  const int c0 = (vx0 ? sx : 0) * 3, c1 = (vx1 ? sx + 1 : 0) * 3;
+  const int X0 = vx0 ? sx : 0, X1 = vx1 ? sx + 1 : 0, Y0 = vy0 ? sy : 0, Y1 = vy1 ? sy + 1 : 0;   // only dereferenced when valid
+  const uint8_t *t00 = f.data + rgb_offset(f, X0, Y0), *t01 = f.data + rgb_offset(f, X1, Y0);
+  const uint8_t *t10 = f.data + rgb_offset(f, X0, Y1), *t11 = f.data + rgb_offset(f, X1, Y1);
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const int p00 = (vy0 && vx0) ? r0[c0 + c] : 0, p01 = (vy0 && vx1) ? r0[c1 + c] : 0;
-    const int p10 = (vy1 && vx0) ? r1[c0 + c] : 0, p11 = (vy1 && vx1) ? r1[c1 + c] : 0;
+    const int p00 = (vy0 && vx0) ? t00[c] : 0, p01 = (vy0 && vx1) ? t01[c] : 0;
+    const int p10 = (vy1 && vx0) ? t10[c] : 0, p11 = (vy1 && vx1) ? t11[c] : 0;
     v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + (1 << 14)) >> 15;
   }
 }
 // the same from a YUV frame: each tap converted to RGB first, the constant border is RGB 0
 __device__ __forceinline__ void affine_pixel_yuv(const YuvEntry& f, const YuvCoef& k, int X, int Y, int v[3]) {
   const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767), fx = X & 31, fy = Y & 31;
-  const bool vx0 = sx >= 0 && sx < f.fw, vx1 = sx + 1 >= 0 && sx + 1 < f.fw, vy0 = sy >= 0 && sy < f.fh, vy1 = sy + 1 >= 0 && sy + 1 < f.fh;
+  const int2 vhw = view_hw(f);
+  const int fh = vhw.x, fw = vhw.y;
+  const bool vx0 = sx >= 0 && sx < fw, vx1 = sx + 1 >= 0 && sx + 1 < fw, vy0 = sy >= 0 && sy < fh, vy1 = sy + 1 >= 0 && sy + 1 < fh;
   const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
   int t00[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t10[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
   if (vy0 && vx0) yuv_rgb(f, k, sx, sy, t00);
@@ -446,7 +471,7 @@ __global__ void __launch_bounds__(PP_W) crop_warp_normalise(const __grid_constan
   float* out = q.crops + static_cast<size_t>(crop) * 3 * PP_H * PP_W;
   for (int r = 0; r < PP_ROWS; ++r) {
     int v[3];
-    affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (s_row[r].x + col.x) >> 5, (s_row[r].y + col.y) >> 5, v);
+    affine_pixel(fr, (s_row[r].x + col.x) >> 5, (s_row[r].y + col.y) >> 5, v);
 #pragma unroll
     for (int c = 0; c < 3; ++c) out[(c * PP_H + dy0 + r) * PP_W + dx] = affine_norm(c, v[c]);
   }
@@ -498,7 +523,7 @@ __global__ void __launch_bounds__(384) frame_to_patch_rows_affine(const __grid_c
       int v[3];
       const int2 r = s_row[ky], c = s_col[dx];
       if constexpr (Entry::kYuv) affine_pixel_yuv(fr, yuv_coef(fr.conv), (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
-      else affine_pixel(fr.data, fr.pitch, fr.fh, fr.fw, (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
+      else affine_pixel(fr, (r.x + c.x) >> 5, (r.y + c.y) >> 5, v);
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) v3[ch] = s_lut[ch][v[ch]];
     }

@@ -90,80 +90,85 @@ class B200PoseBackend:
         return self.model.infer_frame_host(img, bboxes)[0]
 
     @torch.no_grad()
-    def inference_frames(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]") -> "list[np.ndarray]":
+    def inference_frames(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", rotate=0) -> "list[np.ndarray]":
         """Several uint8 RGB frames (cameras of a rig, frames of a video, several streams) + each frame's boxes -> one
         float32 [n_i,K,3] (y, x, score) per frame, in that frame's pixels: inference_frame for all of them with the people of
-        all frames packed into as few engine calls as max_batch allows."""
-        return self.model.infer_frames_host(imgs, bboxes_list)[0]
+        all frames packed into as few engine calls as max_batch allows.  `rotate` (0 | 90 | 180 | 270 degrees
+        counter-clockwise, one for all frames or one per frame; the reference's `--rotate`): frames are stored sideways and
+        seen as cv2.rotate turns them, boxes and keypoints in the rotated frame's pixels, with no rotated copy made."""
+        return self.model.infer_frames_host(imgs, bboxes_list, rotate)[0]
 
     @torch.no_grad()
-    def inference_frames_nv12(self, frames, bboxes_list: "list[np.ndarray]", matrix: str = "bt601") -> "list[np.ndarray]":
+    def inference_frames_nv12(self, frames, bboxes_list: "list[np.ndarray]", matrix: str = "bt601", rotate=0) -> "list[np.ndarray]":
         """inference_frames on NV12 video frames (uint8 [3H/2, W] with the planes stacked, or (y, uv) pairs): no RGB conversion."""
-        return self.model.infer_frames_nv12_host(frames, bboxes_list, matrix)[0]
+        return self.model.infer_frames_nv12_host(frames, bboxes_list, matrix, rotate=rotate)[0]
 
     @torch.no_grad()
-    def inference_frames_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list) -> "list[np.ndarray]":
+    def inference_frames_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list, rotate=0) -> "list[np.ndarray]":
         """inference_frames on a multi-head engine (ViTPose(..., heads=...)), with a head index per box (heads_list: per frame
         an int array [n_i], e.g. 0 for people and 3 for animals of a ViTPose+ engine) -> one float32 [n_i,K_max,3] (y, x,
         score) per frame; a box of head j fills rows 0..K_j-1."""
-        return self.model.infer_frames_heads_host(imgs, bboxes_list, heads_list)[0]
+        return self.model.infer_frames_heads_host(imgs, bboxes_list, heads_list, rotate)[0]
 
     @torch.no_grad()
     def inference_topdown(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", padding: float = 1.25,
-                          use_udp: bool = True) -> "list[np.ndarray]":
+                          use_udp: bool = True, rotate=0) -> "list[np.ndarray]":
         """mmpose-style top-down inference: uint8 RGB frames + each frame's person boxes [n_i,4] (x, y, w, h) -> one float32
         [n_i,K,3] (y, x, score) per frame in image pixels.  Each box becomes the reference's centre / scale and warp matrix
         (topdown_args: datasets/COCO.py:318-337, the UDP get_warp_matrix of every config's test_cfg), the crop is
-        cv2.warpAffine's, and the keypoints are keypoints_from_heatmaps(c, s, use_udp=True)'s -- all on the device."""
+        cv2.warpAffine's, and the keypoints are keypoints_from_heatmaps(c, s, use_udp=True)'s -- all on the device.  `rotate`
+        as inference_frames: the boxes and keypoints are in the rotated frame's pixels."""
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
-        return self.model.infer_affine_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args])[0]
+        return self.model.infer_affine_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], rotate)[0]
 
     @torch.no_grad()
     def inference_topdown_nv12(self, frames, bboxes_list: "list[np.ndarray]", padding: float = 1.25, use_udp: bool = True,
-                               matrix: str = "bt601") -> "list[np.ndarray]":
+                               matrix: str = "bt601", rotate=0) -> "list[np.ndarray]":
         """inference_topdown on NV12 video frames (uint8 [3H/2, W] with the planes stacked, or (y, uv) pairs)."""
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
-        return self.model.infer_affine_nv12_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], matrix)[0]
+        return self.model.infer_affine_nv12_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], matrix,
+                                                 rotate=rotate)[0]
 
     @torch.no_grad()
     def inference_topdown_heads(self, imgs: "list[np.ndarray]", bboxes_list: "list[np.ndarray]", heads_list, padding: float = 1.25,
-                                use_udp: bool = True) -> "list[np.ndarray]":
+                                use_udp: bool = True, rotate=0) -> "list[np.ndarray]":
         """inference_topdown on a multi-head engine, with a head index per box (heads_list: per frame an int array [n_i]) -> one
         float32 [n_i,K_max,3] (y, x, score) per frame in image pixels; a box of head j fills rows 0..K_j-1.  Flip test, when set
         with ViTPose.set_flip_test_heads, applies with each box's head's pairs."""
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
-        return self.model.infer_affine_heads_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list)[0]
+        return self.model.infer_affine_heads_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list,
+                                                  rotate)[0]
 
     # YUV video frames in any layout ViTPose.infer_frames_yuv takes (layout "i420" | "yv12" | "nv12" | "nv21" | "yuyv" | "uyvy",
     # e.g. ffmpeg's `-pix_fmt yuv420p` output or a V4L2 webcam's YUYV frame), converted on the device only where the gather taps
     @torch.no_grad()
     def inference_frames_yuv(self, frames, bboxes_list: "list[np.ndarray]", layout: str = "i420", matrix: str = "bt601",
-                             full_range: bool = False) -> "list[np.ndarray]":
+                             full_range: bool = False, rotate=0) -> "list[np.ndarray]":
         """inference_frames on YUV video frames: no RGB conversion."""
-        return self.model.infer_frames_yuv_host(frames, bboxes_list, layout, matrix, full_range)[0]
+        return self.model.infer_frames_yuv_host(frames, bboxes_list, layout, matrix, full_range, rotate)[0]
 
     @torch.no_grad()
     def inference_topdown_yuv(self, frames, bboxes_list: "list[np.ndarray]", padding: float = 1.25, use_udp: bool = True,
-                              layout: str = "i420", matrix: str = "bt601", full_range: bool = False) -> "list[np.ndarray]":
+                              layout: str = "i420", matrix: str = "bt601", full_range: bool = False, rotate=0) -> "list[np.ndarray]":
         """inference_topdown on YUV video frames."""
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
         return self.model.infer_affine_yuv_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], layout, matrix,
-                                                full_range)[0]
+                                                full_range, rotate)[0]
 
     @torch.no_grad()
     def inference_frames_heads_yuv(self, frames, bboxes_list: "list[np.ndarray]", heads_list, layout: str = "i420",
-                                   matrix: str = "bt601", full_range: bool = False) -> "list[np.ndarray]":
+                                   matrix: str = "bt601", full_range: bool = False, rotate=0) -> "list[np.ndarray]":
         """inference_frames_heads on YUV video frames."""
-        return self.model.infer_frames_heads_yuv_host(frames, bboxes_list, heads_list, layout, matrix, full_range)[0]
+        return self.model.infer_frames_heads_yuv_host(frames, bboxes_list, heads_list, layout, matrix, full_range, rotate)[0]
 
     @torch.no_grad()
     def inference_topdown_heads_yuv(self, frames, bboxes_list: "list[np.ndarray]", heads_list, padding: float = 1.25,
                                     use_udp: bool = True, layout: str = "i420", matrix: str = "bt601",
-                                    full_range: bool = False) -> "list[np.ndarray]":
+                                    full_range: bool = False, rotate=0) -> "list[np.ndarray]":
         """inference_topdown_heads on YUV video frames."""
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
         return self.model.infer_affine_heads_yuv_host(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list,
-                                                      layout, matrix, full_range)[0]
+                                                      layout, matrix, full_range, rotate)[0]
 
     def draw_frames(self, imgs: "list[np.ndarray]", kpts_list: "list[np.ndarray]", skeleton, person_index=None,
                     confidence_threshold: float = 0.5, channel_order: str = "rgb", point_colors=None, limb_colors=None) -> "list[np.ndarray]":
@@ -196,11 +201,13 @@ class B200PoseBackend:
         return [out[offs[j]:offs[j + 1]].reshape(im.shape) for j, im in enumerate(imgs)]
 
     @torch.no_grad()
-    def inference_frames_tracked(self, imgs: "list[np.ndarray]", dets_list, tracker) -> "list[dict]":
+    def inference_frames_tracked(self, imgs: "list[np.ndarray]", dets_list, tracker, rotate=0) -> "list[dict]":
         """S streams' `frame_inference` after detection: one frame per stream (uint8 RGB [H,W,3], numpy or CUDA) and its
         detections [n_s, 5] (empty where the detector was skipped, as frame_inference passes them) -> one {id: float32 [K,3]
         (y, x, score)} per stream.  `tracker` (a track.DeviceSort of S streams on the engine's device) is updated once; its
-        int32 boxes feed infer_frames on the device, and only the row counts and ids come back before the pose call."""
+        int32 boxes feed infer_frames on the device, and only the row counts and ids come back before the pose call.  `rotate`:
+        each stream's rotation as inference_frames takes it (one for all or one per stream); detections, tracks and keypoints
+        are in the rotated frames' pixels."""
         if len(imgs) != tracker.num_streams:
             raise ValueError(f"{len(imgs)} frames for a tracker of {tracker.num_streams} streams")
         dets, counts = tracker.pack(dets_list)
@@ -208,7 +215,7 @@ class B200PoseBackend:
         n = out_counts.tolist()
         ids = rows[:, :, 5].long().cpu()                     # the rows' id + 1, the keys frame_inference uses (inference.py:249)
         frames = [im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(im)) for im in imgs]
-        kps, _ = self.model.infer_frames(frames, [boxes[s, :c] for s, c in enumerate(n)])
+        kps, _ = self.model.infer_frames(frames, [boxes[s, :c] for s, c in enumerate(n)], rotate=rotate)
         return [dict(zip(ids[s, :c].tolist(), kp.cpu().numpy())) for s, (c, kp) in enumerate(zip(n, kps))]
 
     @torch.no_grad()

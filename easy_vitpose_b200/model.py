@@ -47,13 +47,29 @@ def plan_frame_chunks(counts, limit: int, max_frames: int = _lib.MAX_FRAMES) -> 
     return chunks
 
 
-def _frame_array(frames, chunk, struct=_lib.VpbFrame):
+def _rotations(rotate, num_frames: int) -> "list[int]":
+    """The `rotate` argument of the frame methods -> one rotation per frame.  `rotate` is one int for all frames or a sequence
+    of num_frames ints, each 0, 90, 180 or 270: degrees counter-clockwise, the reference's `--rotate`.  A rotated frame is seen
+    as cv2.rotate(frame, ...) would turn it (its view), and its boxes, matrices and keypoints are in view pixels.  Raises
+    ValueError for anything else, before any launch."""
+    r = np.asarray(rotate.cpu() if isinstance(rotate, torch.Tensor) else rotate)
+    if r.ndim == 0:
+        r = np.full(num_frames, r)
+    if r.ndim != 1 or r.size != num_frames:
+        raise ValueError(f"rotate: one value or one per frame expected ({num_frames} frames), got shape {r.shape}")
+    if r.size and (r.dtype.kind not in "iu" or not np.isin(r, _lib.ROTATIONS).all()):
+        raise ValueError(f"rotate: 0, 90, 180 or 270 (degrees counter-clockwise) expected, got {r.tolist()}")
+    return [int(v) for v in r]
+
+
+def _frame_array(frames, chunk, struct=_lib.VpbFrame, rot=None):
     """vpb_frame array for one planned call: entries 0..last frame of the call, so that the engine's messages name the
     caller's frame index; frames outside the call get 0 boxes (skipped).  `frames` holds (data pointer, h, w, pitch), or
-    for struct=VpbFrameNv12 (y pointer, y pitch, uv pointer, uv pitch, h, w), or for struct=VpbFrameYuv ViTPose._yuv_row."""
+    for struct=VpbFrameNv12 (y pointer, y pitch, uv pointer, uv pitch, h, w), or for struct=VpbFrameYuv ViTPose._yuv_row;
+    rot[f] is frame f's rotation (_rotations; None: all upright)."""
     arr = (struct * (chunk[-1][0] + 1))()
     for f, s, e in chunk:
-        arr[f] = struct(*frames[f], e - s)
+        arr[f] = struct(*frames[f], e - s, 0 if rot is None else rot[f])
     return arr
 
 
@@ -854,15 +870,18 @@ class ViTPose:
             bb = bb.round()                                  # easy_ViTPose/inference.py:253 (round half to even)
         return np.ascontiguousarray(bb.reshape(-1, 4), np.int32)
 
-    def infer_frames(self, frames, bboxes, check: bool = False):
+    def infer_frames(self, frames, bboxes, check: bool = False, rotate=0):
         """The people of several frames in as few engine calls as the limits allow: uint8 RGB frames [H_j,W_j,3] (CUDA) and
         per-frame boxes [n_j,4] -> (list of kpts f32 [n_j,K,3] (y, x, score) in frame j's pixels, list of idx i32 [n_j,K]).
         Bit-identical to one infer_frame per frame.  Calls hold at most batch_limit boxes from at most 64 frames with boxes; a
         frame's boxes may be split over two calls.  A frame whose rows are packed pixels at a larger pitch (a column slice
-        of a wider image) is read in place.  Empty boxes set the status word; `check=True` synchronises and raises."""
+        of a wider image) is read in place.  Empty boxes set the status word; `check=True` synchronises and raises.
+        `rotate` (every frame method takes it): 0, 90, 180 or 270 degrees counter-clockwise for all frames or one per frame
+        (_rotations); frame j is then seen as cv2.rotate turns it, and its boxes and keypoints are in that view's pixels."""
         self._ensure()
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
         dev = torch.device("cuda", self._device)
         boxes = []
@@ -879,7 +898,7 @@ class ViTPose:
         table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
         s = 0                                                # first box of the current call
         for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk)
+            arr = _frame_array(table, chunk, rot=rot)
             self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames(
                 self._handle, arr, len(arr), C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
                 C.c_void_p(idx[s:].data_ptr()), st))
@@ -888,13 +907,14 @@ class ViTPose:
             raise ValueError("a box is empty after padding and clipping to its frame")
         return list(kp.split(counts)) if counts else [], list(idx.split(counts)) if counts else []
 
-    def infer_frames_host(self, frames, bboxes):
+    def infer_frames_host(self, frames, bboxes, rotate=0):
         """HOST form of infer_frames (vpb_infer_frames_host, synchronous): numpy frames [H_j,W_j,3] uint8 and per-frame boxes
         -> (list of kpts [n_j,K,3], list of idx [n_j,K]) numpy arrays, chunked as infer_frames.  A box that is empty after
         padding and clipping raises ValueError naming its frame."""
         self._ensure()
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
         boxes = [self._round_boxes(b) for b in bboxes]
         counts = [len(b) for b in boxes]
@@ -906,7 +926,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk)
+                arr = _frame_array(table, chunk, rot=rot)
                 _lib.check_value(_lib.lib().vpb_infer_frames_host(
                     self._handle, arr, len(arr), bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
                     idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
@@ -916,14 +936,16 @@ class ViTPose:
         split = np.cumsum(counts)[:-1]
         return np.split(kp, split), np.split(idx, split)
 
-    def submit_frames_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int) -> None:
+    def submit_frames_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int, rotate=0) -> None:
         """Asynchronous vpb_submit_frames_host, ONE engine call (wait with wait_host(slot)): uint8 frames [H_j,W_j,3] whose
         rows are packed pixels (any row pitch), per-frame int32 boxes [n_j,4] (already rounded), and the concatenated outputs
         float32 kpts_out [n,K,3] / int32 idx_out [n,K], n = sum n_j <= batch_limit, at most 64 frames with boxes.  Frames and
-        outputs must stay alive and unmodified until the wait (pinned memory: real copy / compute overlap)."""
+        outputs must stay alive and unmodified until the wait (pinned memory: real copy / compute overlap).  `rotate` as
+        infer_frames."""
         self._ensure()
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         for j, (f, b) in enumerate(zip(frames, bboxes)):
             if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
                     or f.strides[2] != 1 or f.strides[1] != 3 or f.strides[0] < 3 * f.shape[1]:
@@ -935,8 +957,8 @@ class ViTPose:
         if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
                 or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
             raise ValueError("submit_frames_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
-        arr = (_lib.VpbFrame * len(frames))(*[_lib.VpbFrame(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0], len(b))
-                                             for f, b in zip(frames, bboxes)])
+        arr = (_lib.VpbFrame * len(frames))(*[_lib.VpbFrame(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0], len(b), r)
+                                             for f, b, r in zip(frames, bboxes, rot)])
         with torch.cuda.device(self._device):
             _lib.check_value(_lib.lib().vpb_submit_frames_host(
                 self._handle, arr, len(arr), bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
@@ -973,13 +995,14 @@ class ViTPose:
             return [], torch.zeros((0, 6), dtype=torch.float64), None if centers is None else torch.zeros((0, 4))
         return counts, torch.cat(ms).contiguous(), None if centers is None else torch.cat(css).contiguous()
 
-    def preprocess_affine(self, frames, mats) -> torch.Tensor:
+    def preprocess_affine(self, frames, mats, rotate=0) -> torch.Tensor:
         """Affine top-down crops: uint8 RGB frames [H_j,W_j,3] and per-frame matrices [n_j,2,3] (what cv2.warpAffine takes,
         image -> 192x256 crop) -> crops f32 [n,3,256,192] on the device, boxes in frame order.  Bit-exact with
         cv2.warpAffine(frame, M, (192, 256), INTER_LINEAR) + torchvision ToTensor / Normalize (datasets/COCO.py:289-302)."""
         self._ensure()
         if len(frames) != len(mats):
             raise ValueError(f"{len(frames)} frames but {len(mats)} matrix arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
         dev = torch.device("cuda", self._device)
         counts, M, _ = self._affine_args(mats)
@@ -990,13 +1013,13 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, max(n, 1)):       # only the 64-frame table limits a call
-                arr = _frame_array(table, chunk)
+                arr = _frame_array(table, chunk, rot=rot)
                 _lib.check(_lib.lib().vpb_preprocess_affine(arr, len(arr), C.c_void_p(M[s:].data_ptr()),
                                                             C.c_void_p(crops[s:].data_ptr()), self._stream()))
                 s += sum(e - b for _, b, e in chunk)
         return crops
 
-    def infer_affine(self, frames, mats, centers, scales, check: bool = False):
+    def infer_affine(self, frames, mats, centers, scales, check: bool = False, rotate=0):
         """The top-down path of mmpose-style evaluation on the device: frames [H_j,W_j,3] uint8 (CUDA), per-frame matrices
         [n_j,2,3], centres [n_j,2] and scales [n_j,2] in PIXELS (topdown_args gives all three) -> (list of kpts f32 [n_j,K,3]
         (y, x, score), list of idx i32 [n_j,K]): the warp fused into the patch gather, the forward and
@@ -1006,6 +1029,7 @@ class ViTPose:
         self._ensure()
         if not (len(frames) == len(mats) == len(centers) == len(scales)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
         dev = torch.device("cuda", self._device)
         counts, M, CS = self._affine_args(mats, centers, scales)
@@ -1016,7 +1040,7 @@ class ViTPose:
         table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
         s = 0
         for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk)
+            arr = _frame_array(table, chunk, rot=rot)
             self._call_on_stream(frames + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine(
                 self._handle, arr, len(arr), C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
                 C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
@@ -1025,13 +1049,14 @@ class ViTPose:
             raise ValueError("a matrix entry is not finite or a scale is <= 0")
         return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
 
-    def infer_affine_host(self, frames, mats, centers, scales):
+    def infer_affine_host(self, frames, mats, centers, scales, rotate=0):
         """HOST form of infer_affine (vpb_infer_affine_host, synchronous): numpy frames and per-frame matrices / centres /
         scales -> (list of kpts [n_j,K,3], list of idx [n_j,K]) numpy arrays.  A non-finite matrix entry or a scale <= 0
         raises ValueError naming the box."""
         self._ensure()
         if not (len(frames) == len(mats) == len(centers) == len(scales)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
         counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
         M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
@@ -1042,7 +1067,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk)
+                arr = _frame_array(table, chunk, rot=rot)
                 _lib.check_value(_lib.lib().vpb_infer_affine_host(
                     self._handle, arr, len(arr), M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
                     kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
@@ -1083,13 +1108,14 @@ class ViTPose:
             planes.append(tuple(p if p.strides[1] == 1 and p.strides[0] >= p.shape[1] else np.ascontiguousarray(p) for p in (y, uv)))
         return planes, [(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1]) for y, uv in planes]
 
-    def infer_frames_nv12(self, frames, bboxes, matrix: str = "bt601", check: bool = False):
+    def infer_frames_nv12(self, frames, bboxes, matrix: str = "bt601", check: bool = False, rotate=0):
         """infer_frames on NV12 frames (vpb_infer_frames_nv12): CUDA (or host, copied over) NV12 frames and per-frame boxes
         [n_j,4] -> (list of kpts f32 [n_j,K,3], list of idx i32 [n_j,K]).  Chunked, flip test and status word as infer_frames."""
         self._ensure()
         mat = _yuv_matrix(matrix)
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._nv12_device_table(frames)
         dev = torch.device("cuda", self._device)
         boxes = []
@@ -1105,7 +1131,7 @@ class ViTPose:
         idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
         s = 0
         for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+            arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
             self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_nv12(
                 self._handle, arr, len(arr), mat, C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
                 C.c_void_p(idx[s:].data_ptr()), st))
@@ -1114,13 +1140,14 @@ class ViTPose:
             raise ValueError("a box is empty after padding and clipping to its frame")
         return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
 
-    def infer_frames_nv12_host(self, frames, bboxes, matrix: str = "bt601"):
+    def infer_frames_nv12_host(self, frames, bboxes, matrix: str = "bt601", rotate=0):
         """HOST form of infer_frames_nv12 (vpb_infer_frames_nv12_host, synchronous): numpy NV12 frames, per-frame boxes ->
         numpy (kpts, idx) lists.  Each frame is staged packed at 1.5 B per pixel; an empty box raises ValueError."""
         self._ensure()
         mat = _yuv_matrix(matrix)
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._nv12_host_table(frames)
         boxes = [self._round_boxes(b) for b in bboxes]
         counts = [len(b) for b in boxes]
@@ -1131,7 +1158,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+                arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
                 _lib.check_value(_lib.lib().vpb_infer_frames_nv12_host(
                     self._handle, arr, len(arr), mat, bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
                     idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
@@ -1142,7 +1169,7 @@ class ViTPose:
         return np.split(kp, split), np.split(idx, split)
 
     def submit_frames_nv12_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int,
-                                matrix: str = "bt601") -> None:
+                                matrix: str = "bt601", rotate=0) -> None:
         """Asynchronous vpb_submit_frames_nv12_host, ONE engine call (wait with wait_host(slot)): the pipelined video form of
         submit_frames_host for numpy NV12 frames whose rows are contiguous bytes (any row pitch).  Frames, boxes (int32
         [n_j,4], already rounded) and outputs must stay alive and unmodified until the wait."""
@@ -1150,6 +1177,7 @@ class ViTPose:
         mat = _yuv_matrix(matrix)
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         table = []
         for j, (f, b) in enumerate(zip(frames, bboxes)):
             y, uv = nv12_planes(f, f"frame {j}")
@@ -1158,7 +1186,8 @@ class ViTPose:
                 raise ValueError(f"frame {j}: numpy NV12 planes with contiguous bytes in each row expected")
             if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
                 raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
-            table.append(_lib.VpbFrameNv12(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1], len(b)))
+            table.append(_lib.VpbFrameNv12(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1], len(b),
+                                           rot[j]))
         bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
         n = bb.shape[0]
         if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
@@ -1170,12 +1199,13 @@ class ViTPose:
                 self._handle, arr, len(arr), mat, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
                 idx_out.ctypes.data_as(C.c_void_p), int(slot)))
 
-    def infer_affine_nv12(self, frames, mats, centers, scales, matrix: str = "bt601", check: bool = False):
+    def infer_affine_nv12(self, frames, mats, centers, scales, matrix: str = "bt601", check: bool = False, rotate=0):
         """infer_affine on NV12 frames (vpb_infer_affine_nv12): the warp reads the NV12 planes and converts each tap."""
         self._ensure()
         mat = _yuv_matrix(matrix)
         if not (len(frames) == len(mats) == len(centers) == len(scales)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._nv12_device_table(frames)
         dev = torch.device("cuda", self._device)
         counts, M, CS = self._affine_args(mats, centers, scales)
@@ -1185,7 +1215,7 @@ class ViTPose:
         idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
         s = 0
         for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+            arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
             self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_nv12(
                 self._handle, arr, len(arr), mat, C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
                 C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
@@ -1194,12 +1224,13 @@ class ViTPose:
             raise ValueError("a matrix entry is not finite or a scale is <= 0")
         return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
 
-    def infer_affine_nv12_host(self, frames, mats, centers, scales, matrix: str = "bt601"):
+    def infer_affine_nv12_host(self, frames, mats, centers, scales, matrix: str = "bt601", rotate=0):
         """HOST form of infer_affine_nv12 (vpb_infer_affine_nv12_host, synchronous), checked as infer_affine_host."""
         self._ensure()
         mat = _yuv_matrix(matrix)
         if not (len(frames) == len(mats) == len(centers) == len(scales)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._nv12_host_table(frames)
         counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
         M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
@@ -1209,7 +1240,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameNv12)
+                arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
                 _lib.check_value(_lib.lib().vpb_infer_affine_nv12_host(
                     self._handle, arr, len(arr), mat, M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
                     kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
@@ -1279,13 +1310,14 @@ class ViTPose:
         return boxes
 
     def infer_frames_yuv(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
-                         check: bool = False):
+                         check: bool = False, rotate=0):
         """infer_frames on YUV frames (vpb_infer_frames_yuv): CUDA (or host, copied over) frames and per-frame boxes [n_j,4] ->
         (list of kpts f32 [n_j,K,3], list of idx i32 [n_j,K]).  Chunked, flip test and status word as infer_frames."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._yuv_device_table(frames, layout)
         dev = torch.device("cuda", self._device)
         boxes = self._device_boxes(bboxes)
@@ -1296,7 +1328,7 @@ class ViTPose:
         idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
         s = 0
         for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
             self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_yuv(
                 self._handle, arr, len(arr), *fmt, C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
                 C.c_void_p(idx[s:].data_ptr()), st))
@@ -1305,7 +1337,7 @@ class ViTPose:
             raise ValueError("a box is empty after padding and clipping to its frame")
         return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
 
-    def infer_frames_yuv_host(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False):
+    def infer_frames_yuv_host(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False, rotate=0):
         """HOST form of infer_frames_yuv (vpb_infer_frames_yuv_host, synchronous): numpy frames, per-frame boxes -> numpy
         (kpts, idx) lists.  Each frame is staged packed (1.5 B per pixel for 4:2:0, 2 B for 4:2:2); an empty box raises
         ValueError."""
@@ -1313,6 +1345,7 @@ class ViTPose:
         fmt = _yuv_format(layout, matrix, full_range)
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._yuv_host_table(frames, layout)
         boxes = [self._round_boxes(b) for b in bboxes]
         counts = [len(b) for b in boxes]
@@ -1323,7 +1356,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
                 _lib.check_value(_lib.lib().vpb_infer_frames_yuv_host(
                     self._handle, arr, len(arr), *fmt, bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
                     idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
@@ -1334,7 +1367,7 @@ class ViTPose:
         return np.split(kp, split), np.split(idx, split)
 
     def submit_frames_yuv_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int, layout: str = "i420",
-                               matrix: str = "bt601", full_range: bool = False) -> None:
+                               matrix: str = "bt601", full_range: bool = False, rotate=0) -> None:
         """Asynchronous vpb_submit_frames_yuv_host, ONE engine call (wait with wait_host(slot)): the pipelined video form of
         submit_frames_host for numpy YUV frames whose planes have contiguous bytes in each row (any row pitch; U and V of one
         pitch).  Frames, boxes (int32 [n_j,4], already rounded) and outputs must stay alive and unmodified until the wait."""
@@ -1342,6 +1375,7 @@ class ViTPose:
         fmt = _yuv_format(layout, matrix, full_range)
         if len(frames) != len(bboxes):
             raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
         for j, b in enumerate(bboxes):
             if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
                 raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
@@ -1351,19 +1385,20 @@ class ViTPose:
         if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
                 or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
             raise ValueError("submit_frames_yuv_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
-        arr = (_lib.VpbFrameYuv * len(table))(*[_lib.VpbFrameYuv(*t, len(b)) for t, b in zip(table, bboxes)])
+        arr = (_lib.VpbFrameYuv * len(table))(*[_lib.VpbFrameYuv(*t, len(b), r) for t, b, r in zip(table, bboxes, rot)])
         with torch.cuda.device(self._device):
             _lib.check_value(_lib.lib().vpb_submit_frames_yuv_host(
                 self._handle, arr, len(arr), *fmt, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
                 idx_out.ctypes.data_as(C.c_void_p), int(slot)))
 
     def infer_affine_yuv(self, frames, mats, centers, scales, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
-                         check: bool = False):
+                         check: bool = False, rotate=0):
         """infer_affine on YUV frames (vpb_infer_affine_yuv): the warp reads the planes and converts each tap."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if not (len(frames) == len(mats) == len(centers) == len(scales)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._yuv_device_table(frames, layout)
         dev = torch.device("cuda", self._device)
         counts, M, CS = self._affine_args(mats, centers, scales)
@@ -1373,7 +1408,7 @@ class ViTPose:
         idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
         s = 0
         for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
             self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_yuv(
                 self._handle, arr, len(arr), *fmt, C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
                 C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
@@ -1383,12 +1418,13 @@ class ViTPose:
         return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
 
     def infer_affine_yuv_host(self, frames, mats, centers, scales, layout: str = "i420", matrix: str = "bt601",
-                              full_range: bool = False):
+                              full_range: bool = False, rotate=0):
         """HOST form of infer_affine_yuv (vpb_infer_affine_yuv_host, synchronous), checked as infer_affine_host."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if not (len(frames) == len(mats) == len(centers) == len(scales)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
+        rot = _rotations(rotate, len(frames))
         planes, table = self._yuv_host_table(frames, layout)
         counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
         M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
@@ -1398,7 +1434,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
                 _lib.check_value(_lib.lib().vpb_infer_affine_yuv_host(
                     self._handle, arr, len(arr), *fmt, M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
                     kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
@@ -1450,7 +1486,7 @@ class ViTPose:
         out = (kp.index_select(0, inv), idx.index_select(0, inv))
         return out + (hm.index_select(0, inv),) if return_heatmaps else out
 
-    def infer_frames_heads(self, frames, bboxes, heads, check: bool = False):
+    def infer_frames_heads(self, frames, bboxes, heads, check: bool = False, rotate=0):
         """infer_frames with a keypoint head per box (heads: per frame an int array [n_j]): the boxes are grouped by head
         (stable; a frame appears once per head it uses) and run through vpb_infer_frames_heads in calls of at most batch_limit
         boxes and 64 entries.  Returns per frame kpts f32 [n_j,K_max,3] (y, x, score) in that frame's pixels and idx i32
@@ -1458,6 +1494,7 @@ class ViTPose:
         self._ensure()
         if not (len(frames) == len(bboxes) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
         dev = torch.device("cuda", self._device)
         boxes = []
@@ -1467,6 +1504,7 @@ class ViTPose:
                 b = b.round()
             boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
         ents, _, chunks = plan_head_calls([b.shape[0] for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         n = sum(len(sel) for _, sel, _ in ents)
         bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
         Km = self.num_keypoints_max
@@ -1476,7 +1514,7 @@ class ViTPose:
         hv = np.array([k for _, _, k in ents], np.int32)
         s = 0
         for chunk in chunks:
-            arr = _frame_array(table, chunk)
+            arr = _frame_array(table, chunk, rot=rot)
             ha = np.ascontiguousarray(hv[:len(arr)])
             self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads(
                 self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), C.c_void_p(bb[s:].data_ptr()),
@@ -1497,15 +1535,17 @@ class ViTPose:
             s += len(sel)
         return outs_k, outs_i
 
-    def infer_frames_heads_host(self, frames, bboxes, heads):
+    def infer_frames_heads_host(self, frames, bboxes, heads, rotate=0):
         """HOST form of infer_frames_heads (vpb_infer_frames_heads_host, synchronous): numpy frames, per-frame boxes and
         head indices -> (list of kpts [n_j,K_max,3], list of idx [n_j,K_max]) numpy arrays.  An empty box raises ValueError."""
         self._ensure()
         if not (len(frames) == len(bboxes) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
         boxes = [self._round_boxes(b) for b in bboxes]
         ents, _, chunks = plan_head_calls([len(b) for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         n = sum(len(sel) for _, sel, _ in ents)
         bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
         Km = self.num_keypoints_max
@@ -1516,7 +1556,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in chunks:
-                arr = _frame_array(table, chunk)
+                arr = _frame_array(table, chunk, rot=rot)
                 ha = np.ascontiguousarray(hv[:len(arr)])
                 _lib.check_value(_lib.lib().vpb_infer_frames_heads_host(
                     self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), bb[s:].ctypes.data_as(C.c_void_p),
@@ -1525,7 +1565,7 @@ class ViTPose:
         k_t, i_t = self._per_frame(ents, [len(b) for b in boxes], torch.from_numpy(kp), torch.from_numpy(idx))
         return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
 
-    def infer_affine_heads(self, frames, mats, centers, scales, heads, check: bool = False):
+    def infer_affine_heads(self, frames, mats, centers, scales, heads, check: bool = False, rotate=0):
         """infer_affine with a keypoint head per box (heads: per frame an int array [n_j]): the boxes are grouped by head (stable;
         a frame appears once per head it uses) and run through vpb_infer_affine_heads in calls of at most batch_limit boxes and
         64 entries (plan_head_calls).  Each call decodes a segment (a run of one head) as one keypoints_from_heatmaps(c, s,
@@ -1535,10 +1575,12 @@ class ViTPose:
         if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
                              f"arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
         dev = torch.device("cuda", self._device)
         counts, M, CS = self._affine_args(mats, centers, scales)
         ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         o = torch.as_tensor(order, device=M.device)
         M, CS = M.index_select(0, o).contiguous().to(dev), CS.index_select(0, o).contiguous().to(dev)
         n = M.shape[0]
@@ -1549,7 +1591,7 @@ class ViTPose:
         hv = np.array([k for _, _, k in ents], np.int32)
         s = 0
         for chunk in chunks:
-            arr = _frame_array(table, chunk)
+            arr = _frame_array(table, chunk, rot=rot)
             ha = np.ascontiguousarray(hv[:len(arr)])
             self._call_on_stream(frames + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_heads(
                 self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
@@ -1559,7 +1601,7 @@ class ViTPose:
             raise ValueError("a matrix entry is not finite or a scale is <= 0")
         return self._per_frame(ents, counts, kp, idx)
 
-    def infer_affine_heads_host(self, frames, mats, centers, scales, heads):
+    def infer_affine_heads_host(self, frames, mats, centers, scales, heads, rotate=0):
         """HOST form of infer_affine_heads (vpb_infer_affine_heads_host, synchronous): numpy frames and per-frame matrices /
         centres / scales / head indices -> (list of kpts [n_j,K_max,3], list of idx [n_j,K_max]) numpy arrays.  A non-finite
         matrix entry or a scale <= 0 raises ValueError."""
@@ -1567,9 +1609,11 @@ class ViTPose:
         if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
                              f"arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
         counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
         ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         M = np.ascontiguousarray(M.cpu().numpy()[order])
         CS = np.ascontiguousarray(CS.cpu().numpy()[order], np.float32)
         n = M.shape[0]
@@ -1581,7 +1625,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in chunks:
-                arr = _frame_array(table, chunk)
+                arr = _frame_array(table, chunk, rot=rot)
                 ha = np.ascontiguousarray(hv[:len(arr)])
                 _lib.check_value(_lib.lib().vpb_infer_affine_heads_host(
                     self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),
@@ -1593,16 +1637,18 @@ class ViTPose:
 
     # the multi-head calls on YUV frames: frames as the _yuv calls take them, everything else as their RGB twins above
     def infer_frames_heads_yuv(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
-                               check: bool = False):
+                               check: bool = False, rotate=0):
         """infer_frames_heads on YUV frames (vpb_infer_frames_heads_yuv)."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if not (len(frames) == len(bboxes) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         planes, ytab = self._yuv_device_table(frames, layout)
         dev = torch.device("cuda", self._device)
         boxes = self._device_boxes(bboxes)
         ents, _, chunks = plan_head_calls([b.shape[0] for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         n = sum(len(sel) for _, sel, _ in ents)
         bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
         Km = self.num_keypoints_max
@@ -1612,7 +1658,7 @@ class ViTPose:
         hv = np.array([k for _, _, k in ents], np.int32)
         s = 0
         for chunk in chunks:
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
             ha = np.ascontiguousarray(hv[:len(arr)])
             self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads_yuv(
                 self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), C.c_void_p(bb[s:].data_ptr()),
@@ -1622,15 +1668,17 @@ class ViTPose:
             raise ValueError("a box is empty after padding and clipping to its frame")
         return self._per_frame(ents, [b.shape[0] for b in boxes], kp, idx)
 
-    def infer_frames_heads_yuv_host(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False):
+    def infer_frames_heads_yuv_host(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False, rotate=0):
         """HOST form of infer_frames_heads_yuv (vpb_infer_frames_heads_yuv_host, synchronous)."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if not (len(frames) == len(bboxes) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         planes, ytab = self._yuv_host_table(frames, layout)
         boxes = [self._round_boxes(b) for b in bboxes]
         ents, _, chunks = plan_head_calls([len(b) for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         n = sum(len(sel) for _, sel, _ in ents)
         bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
         Km = self.num_keypoints_max
@@ -1641,7 +1689,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in chunks:
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
                 ha = np.ascontiguousarray(hv[:len(arr)])
                 _lib.check_value(_lib.lib().vpb_infer_frames_heads_yuv_host(
                     self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), bb[s:].ctypes.data_as(C.c_void_p),
@@ -1651,17 +1699,19 @@ class ViTPose:
         return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
 
     def infer_affine_heads_yuv(self, frames, mats, centers, scales, heads, layout: str = "i420", matrix: str = "bt601",
-                               full_range: bool = False, check: bool = False):
+                               full_range: bool = False, check: bool = False, rotate=0):
         """infer_affine_heads on YUV frames (vpb_infer_affine_heads_yuv)."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
                              f"arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         planes, ytab = self._yuv_device_table(frames, layout)
         dev = torch.device("cuda", self._device)
         counts, M, CS = self._affine_args(mats, centers, scales)
         ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         o = torch.as_tensor(order, device=M.device)
         M, CS = M.index_select(0, o).contiguous().to(dev), CS.index_select(0, o).contiguous().to(dev)
         n = M.shape[0]
@@ -1672,7 +1722,7 @@ class ViTPose:
         hv = np.array([k for _, _, k in ents], np.int32)
         s = 0
         for chunk in chunks:
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
             ha = np.ascontiguousarray(hv[:len(arr)])
             self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_heads_yuv(
                 self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), C.c_void_p(M[s:].data_ptr()),
@@ -1683,16 +1733,18 @@ class ViTPose:
         return self._per_frame(ents, counts, kp, idx)
 
     def infer_affine_heads_yuv_host(self, frames, mats, centers, scales, heads, layout: str = "i420", matrix: str = "bt601",
-                                    full_range: bool = False):
+                                    full_range: bool = False, rotate=0):
         """HOST form of infer_affine_heads_yuv (vpb_infer_affine_heads_yuv_host, synchronous)."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
         if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
             raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
                              f"arrays, {len(heads)} head arrays")
+        rot = _rotations(rotate, len(frames))
         planes, ytab = self._yuv_host_table(frames, layout)
         counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
         ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
         M = np.ascontiguousarray(M.cpu().numpy()[order])
         CS = np.ascontiguousarray(CS.cpu().numpy()[order], np.float32)
         n = M.shape[0]
@@ -1704,7 +1756,7 @@ class ViTPose:
         s = 0
         with torch.cuda.device(self._device):
             for chunk in chunks:
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv)
+                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
                 ha = np.ascontiguousarray(hv[:len(arr)])
                 _lib.check_value(_lib.lib().vpb_infer_affine_heads_yuv_host(
                     self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),

@@ -177,19 +177,34 @@ int vpb_submit_frame_host(vpb_engine* e, const uint8_t* h_frame, int32_t frame_h
  * Frames with 0 boxes are skipped and do not count towards VPB_MAX_FRAMES; n = 0 returns VPB_OK and launches nothing.
  * VPB_ERR_ARG: n above the batch limit (max_batch, max_batch / 2 with flip test on), more than VPB_MAX_FRAMES frames with
  * boxes, a negative num_boxes, a frame with boxes whose data is NULL, height or width < 1, or pitch below 3 * width.
- * Flip test (vpb_set_flip_test) applies as for the single-frame calls. */
+ * Flip test (vpb_set_flip_test) applies as for the single-frame calls.
+ *
+ * Rotated frames (phone footage, portrait-mounted cameras; the reference's `--rotate`, VideoReader's cv2.rotate): every
+ * frame struct (vpb_frame, vpb_frame_nv12, vpb_frame_yuv) ends with `rotation`, 0, 90, 180 or 270 degrees counter-clockwise.
+ * height, width, the pitches and the planes describe the STORED frame (the decoder's output), and the frame the call sees, its
+ * VIEW, is cv2.rotate(stored, code) with code ROTATE_90_COUNTERCLOCKWISE for 90, ROTATE_180 for 180 and ROTATE_90_CLOCKWISE
+ * for 270 (the view is width x height for 90 and 270).  Boxes and affine matrices are given in view pixels, box padding,
+ * clipping, pad_image, the empty-box status bit and the host forms' empty-box check use the view's size, and keypoints come
+ * back in view pixels.  The rotation is folded into the gather's addressing, so a rotated call is bit-identical to the upright
+ * call on the rotated copy; YUV taps read the stored pixel's luma and its stored chroma block, which equals converting the
+ * stored frame and rotating the result.  Size rules (even sizes for 4:2:0, even width for 4:2:2) apply to the stored frame.
+ * Any other value returns VPB_ERR_ARG naming the frame.  Zero-initialise the structs (aggregate initialisation and ctypes
+ * do) so that callers written before the field existed keep rotation 0.  The single-frame calls (vpb_infer_frame*,
+ * vpb_preprocess) take upright frames; a rotated single frame is a one-entry multi-frame call. */
 #define VPB_MAX_FRAMES 64
 typedef struct vpb_frame {
-  const uint8_t* data;    /* u8 [height, width, 3] RGB; device address (vpb_infer_frames) or host (the _host forms) */
+  const uint8_t* data;    /* u8 [height, width, 3] RGB, stored; device address (vpb_infer_frames) or host (the _host forms) */
   int32_t height, width;
   int64_t pitch_bytes;    /* row pitch; 0 = packed (3 * width) */
   int32_t num_boxes;      /* this frame's boxes are the next num_boxes rows of the box array (0 allowed) */
+  int32_t rotation;       /* 0 | 90 | 180 | 270 degrees counter-clockwise, stored -> view (above) */
 } vpb_frame;
-/* Device frames and boxes (d_bboxes i32 [n,4]); empty boxes set bit 0 of the status word, as vpb_infer_frame does. */
+/* Device frames and boxes (d_bboxes i32 [n,4], view pixels); boxes empty after clipping to their view set bit 0 of the status
+ * word, as vpb_infer_frame does. */
 int vpb_infer_frames(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* d_bboxes,
                      float* d_kpts, int32_t* d_idx, void* stream);
-/* HOST frames (any pitch; each is staged packed) and boxes: every box is checked against its own frame and an empty one
- * returns VPB_ERR_ARG naming the frame and the box.  Same staging slots, events, concurrency contract and vpb_wait_host as
+/* HOST frames (any pitch; each is staged packed, as stored) and boxes: every box is checked against its own frame's view and
+ * an empty one returns VPB_ERR_ARG naming the frame and the box.  Same staging slots, events, concurrency contract and vpb_wait_host as
  * vpb_infer_frame_host / vpb_submit_frame_host; the slot's staging buffer grows to the sum of the frame sizes. */
 int vpb_infer_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num_frames, const int32_t* h_bboxes,
                           float* h_kpts, int32_t* h_idx, void* stream);
@@ -198,7 +213,8 @@ int vpb_submit_frames_host(vpb_engine* e, const vpb_frame* h_frames, int32_t num
 
 /* ---- affine top-down crops: the mmpose / HRNet data path of easy_ViTPose/datasets/COCO.py:288-302 (the crop the published
  * COCO AP numbers were measured with) for the people of up to VPB_MAX_FRAMES frames per call.  Frames and their boxes are given
- * as for vpb_infer_frames (vpb_frame.num_boxes = how many of the next matrices belong to that frame).  Per box:
+ * as for vpb_infer_frames (vpb_frame.num_boxes = how many of the next matrices belong to that frame; vpb_frame.rotation as
+ * there: the matrices map view pixels, and taps outside the view read 0).  Per box:
  *   mats f64 [n,6] = the 2x3 matrix handed to cv2.warpAffine (image -> 192x256 crop), e.g. the UDP matrix
  *   get_warp_matrix(rot, 2c, image_size - 1, s * 200) (vit_utils/post_processing/post_transforms.py:312-340) or the HRNet
  *   get_affine_transform (vit_utils/transform.py:46-75);
@@ -210,7 +226,7 @@ int vpb_preprocess_affine(const vpb_frame* h_frames, int32_t num_frames, const d
  * keypoints_from_heatmaps(heatmaps, c, s * 200, use_udp=True) = vpb_decode_modes mode 4 with d_cs f32 [n,4] (cx, cy, sx, sy) in
  * pixels, as keypoints_from_heatmaps takes them (top_down_eval.py:576-579, one reference call on the whole call's array).
  * d_kpts f32 [n,K,3] (y, x, score), d_idx i32 [n,K] or NULL.  The keypoints are in the coordinates transform_preds gives:
- * image pixels for an unrotated matrix.  The reference's decode has no rotation, and neither has this one: for a rotated
+ * view pixels for an unrotated matrix.  The reference's decode has no rotation, and neither has this one: for a rotated
  * matrix they are the reference's values, not the rotated-back positions.  Bit-identical to vpb_preprocess_affine ->
  * vpb_forward -> vpb_decode_modes(mode 4); flip test (vpb_set_flip_test) applies as to the frame calls.
  * VPB_ERR_ARG: n above the batch limit, more than VPB_MAX_FRAMES frames with boxes, a negative num_boxes, a frame with boxes
@@ -245,8 +261,9 @@ typedef struct vpb_frame_nv12 {
   int64_t y_pitch;        /* row pitch of y in bytes; 0 = packed (width) */
   const uint8_t* uv;      /* u8 [height / 2, width]: U, V interleaved, one pair per 2x2 block; may be a separate allocation */
   int64_t uv_pitch;       /* row pitch of uv in bytes; 0 = packed (width) */
-  int32_t height, width;  /* both even */
+  int32_t height, width;  /* both even; the stored frame */
   int32_t num_boxes;      /* as vpb_frame.num_boxes */
+  int32_t rotation;       /* as vpb_frame.rotation */
 } vpb_frame_nv12;
 int vpb_infer_frames_nv12(vpb_engine* e, const vpb_frame_nv12* h_frames, int32_t num_frames, int32_t matrix,
                           const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream);
@@ -344,8 +361,9 @@ typedef struct vpb_frame_yuv {
   const uint8_t* plane[3];  /* in storage order (above); device addresses or host (the _host forms) */
   int64_t y_pitch;          /* row pitch of plane[0] in bytes; 0 = packed */
   int64_t c_pitch;          /* row pitch of the chroma plane(s) in bytes; 0 = packed */
-  int32_t height, width;
+  int32_t height, width;    /* the stored frame */
   int32_t num_boxes;        /* as vpb_frame.num_boxes */
+  int32_t rotation;         /* as vpb_frame.rotation */
 } vpb_frame_yuv;
 int vpb_infer_frames_yuv(vpb_engine* e, const vpb_frame_yuv* h_frames, int32_t num_frames, int32_t layout, int32_t matrix,
                          int32_t range, const int32_t* d_bboxes, float* d_kpts, int32_t* d_idx, void* stream);
