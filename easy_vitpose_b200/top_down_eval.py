@@ -65,7 +65,9 @@ def keypoints_from_heatmaps(heatmaps, center, scale, unbiased=False, post_proces
     for 3 and 5 taps and the scalar tail of its column filter for 5 and 7 are reproduced bit for bit); CombinedTarget blurs the
     response maps with 2*kernel+1, so kernel <= 17 there; kernel = 1 with post_process 'unbiased' / 'megvii' raises ValueError as
     the reference's `_gaussian_blur` does (a zero-width border, :453).  Like the reference, CombinedTarget only accepts N = 1: its
-    index arithmetic (:589) does not broadcast for larger N."""
+    index arithmetic (:589) does not broadcast for larger N.  Also like the reference, use_udp=True on one-keypoint maps
+    [N,1,64,48] raises ValueError for N > 1 (post_dark_udp's squeeze, :414); vpb_decode_modes mode 4 and the engine's affine
+    calls decode that case with the formula's intended shape."""
     # the reference's conflict checks (:548-553) and config normalisation (:556-579), deprecation warnings dropped
     if unbiased:
         assert post_process not in [False, None, "megvii"]
@@ -100,6 +102,9 @@ def keypoints_from_heatmaps(heatmaps, center, scale, unbiased=False, post_proces
             raise ValueError(f"CombinedTarget: operands could not be broadcast together for N={N}, K={K} (reference :589-590)")
         K //= 3
         valid_radius = float(np.float32(valid_radius_factor * heatmaps.shape[2]))
+    elif use_udp and N > 1 and K == 1:
+        # post_dark_udp's `.squeeze()` (:414) drops the K = 1 axis of its [N, 1, 2] offsets, which then do not broadcast
+        raise ValueError(f"use_udp with one keypoint: non-broadcastable output operand for N={N}, K=1 (reference :414)")
     hm = heatmaps if isinstance(heatmaps, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(heatmaps, np.float32))
     if not hm.is_cuda:
         hm = hm.cuda()

@@ -106,7 +106,11 @@ int vpb_flip_back(const float* d_in, int32_t n, int32_t k, const int32_t* d_perm
  *                 (response, offset x, offset y); 2*kernel+1 <= 35; valid_radius = (float)(valid_radius_factor * 64) (:586);
  *                 the (-1,-1) sentinel reads its offsets one row and one pixel before the keypoint's plane, wrapping to the
  *                 last plane of the call for the first keypoint, as numpy's flat index does.  (The reference's own index
- *                 arithmetic (:589) only broadcasts for n = 1; n > 1 here is that formula with the intended shape.) */
+ *                 arithmetic (:589) only broadcasts for n = 1; n > 1 here is that formula with the intended shape.)
+ * Mode 4 with k = 1 and n > 1: the reference raises (post_dark_udp's `.squeeze()`, :414, drops the k axis of its [n,1,2]
+ * offsets); here, as in vpb_decode with wrap_batch = 1 and in the affine calls (a segment of a one-keypoint head), it is the
+ * formula with the intended shape: each crop's DARK offset applied to its own keypoint, the max <= 0 sentinel reading the
+ * previous crop's map as for any k.  The Python keypoints_from_heatmaps raises ValueError there, as the reference does. */
 #define VPB_DECODE_NONE 0
 #define VPB_DECODE_DEFAULT 1
 #define VPB_DECODE_UNBIASED 2
