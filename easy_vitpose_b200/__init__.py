@@ -12,4 +12,5 @@ from .inference import B200PoseBackend, install  # noqa: F401
 from .model import ViTPose, head_flip_permutations, merge_split_state_dicts, plan_head_calls, split_vitpose_plus  # noqa: F401
 from .top_down_eval import decode_heatmaps, decode_topdown, keypoints_from_heatmaps  # noqa: F401
 from .topdown import topdown_args  # noqa: F401
+from .smooth import DeviceOneEuro  # noqa: F401
 from .track import DeviceSort  # noqa: F401

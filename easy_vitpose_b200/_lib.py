@@ -156,6 +156,12 @@ EXPORTS = {
     "vpb_tracker_next_id": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "vpb_tracker_set_next_id": (C.c_int, [C.c_void_p, C.c_int64]),
     "vpb_tracker_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "vpb_smoother_create": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int32,
+                                      C.c_int32, C.POINTER(C.c_void_p)]),
+    "vpb_smoother_destroy": (None, [C.c_void_p]),
+    "vpb_smoother_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_smoother_reset": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "vpb_smoother_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
 }
 
 # The NV12 calls: names with a digit, kept apart from EXPORTS, which tests/test_abi.py matches against the header's

@@ -27,6 +27,7 @@
 #include "pointwise.cuh"
 #include "preprocess.cuh"
 #include "qkv_attention.cuh"
+#include "smooth.cuh"
 #include "track.cuh"
 
 using namespace vpb;
@@ -2385,6 +2386,121 @@ extern "C" int vpb_tracker_status(vpb_tracker* t, int32_t* h_status) {
   CU_TRY(cudaDeviceSynchronize());
   CU_TRY(cudaMemcpy(h_status, t->q.status, sizeof(int32_t), cudaMemcpyDeviceToHost));
   CU_TRY(cudaMemset(t->q.status, 0, sizeof(int32_t)));
+  return VPB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------ One Euro smoother
+struct vpb_smoother {
+  int device = 0;
+  void* mem = nullptr;          // one allocation; SmoothParams points into it
+  SmoothParams q{};
+};
+
+struct SmootherDevice {         // makes the smoother's device current for one call
+  int prev = -1;
+  explicit SmootherDevice(const vpb_smoother* s) {
+    int cur = -1;
+    if (cudaGetDevice(&cur) == cudaSuccess && cur != s->device && cudaSetDevice(s->device) == cudaSuccess) prev = cur;
+  }
+  ~SmootherDevice() { if (prev >= 0) cudaSetDevice(prev); }
+};
+
+extern "C" int vpb_smoother_create(int32_t num_streams, int32_t k, double min_cutoff, double beta, double d_cutoff, double fps,
+                                   double dx0, int32_t max_gap, int32_t device, vpb_smoother** out) {
+  const char* fn = "vpb_smoother_create";
+  if (!out) return fail(VPB_ERR_ARG, "%s: null output", fn);
+  *out = nullptr;
+  if (num_streams < 1 || num_streams > 65535) return fail(VPB_ERR_ARG, "%s: %d streams (1..65535)", fn, num_streams);
+  if (k < 1 || k > SMOOTH_MAX_K) return fail(VPB_ERR_ARG, "%s: %d keypoints (1..%d)", fn, k, SMOOTH_MAX_K);
+  if (!std::isfinite(min_cutoff) || !std::isfinite(beta) || !std::isfinite(d_cutoff) || !std::isfinite(fps) || !std::isfinite(dx0))
+    return fail(VPB_ERR_ARG, "%s: a filter parameter is not finite", fn);
+  if (max_gap < 0) return fail(VPB_ERR_ARG, "%s: max_gap %d must be >= 0", fn, max_gap);
+  int ndev = 0;
+  CU_TRY(cudaGetDeviceCount(&ndev));
+  if (device < 0 || device >= ndev) return fail(VPB_ERR_ARG, "%s: device %d of %d", fn, device, ndev);
+  vpb_smoother* s = new vpb_smoother();
+  s->device = device;
+  SmootherDevice guard(s);
+  const size_t S = static_cast<size_t>(num_streams), M = SMOOTH_MAX;
+  const size_t bytes_state = 2 * S * M * k * 2 * sizeof(double), bytes_f64 = 2 * S * M * sizeof(double);
+  const size_t bytes_i32 = (5 * S * M + 3 * S + 1) * sizeof(int32_t);
+  const size_t total = bytes_state + bytes_f64 + bytes_i32;
+  cudaError_t err = cudaMalloc(&s->mem, total);
+  if (err == cudaSuccess) err = cudaMemset(s->mem, 0, total);
+  SmoothParams& q = s->q;
+  char* p = static_cast<char*>(s->mem);
+  q.x_prev = reinterpret_cast<double*>(p); p += bytes_state / 2;
+  q.dx_prev = reinterpret_cast<double*>(p); p += bytes_state / 2;
+  q.c_last = reinterpret_cast<double*>(p); p += S * M * sizeof(double);
+  q.row_te = reinterpret_cast<double*>(p); p += S * M * sizeof(double);
+  int32_t* ip = reinterpret_cast<int32_t*>(p);
+  q.slot_id = ip; ip += S * M;
+  q.slot_u = ip; ip += S * M;
+  q.slot_first = ip; ip += S * M;
+  q.row_slot = ip; ip += S * M;
+  q.row_mode = ip; ip += S * M;
+  q.updates = ip; ip += S;
+  q.rows = ip; ip += S;
+  q.row0 = ip; ip += S;
+  q.status = ip;
+  if (err == cudaSuccess) err = cudaMemset(q.slot_u, 0xFF, S * M * sizeof(int32_t));      // every slot free (-1)
+  if (err != cudaSuccess) {
+    if (s->mem) cudaFree(s->mem);
+    delete s;
+    return fail(VPB_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(err));
+  }
+  q.num_streams = num_streams; q.k = k; q.max_gap = max_gap; q.realtime = fps <= 0.0;
+  q.min_cutoff = min_cutoff; q.beta = beta; q.d_cutoff = d_cutoff; q.dx0 = dx0;
+  q.deriv_cutoff = fps <= 0.0 ? d_cutoff : fps;
+  *out = s;
+  return VPB_OK;
+}
+
+extern "C" void vpb_smoother_destroy(vpb_smoother* s) {
+  if (!s) return;
+  SmootherDevice guard(s);
+  cudaDeviceSynchronize();
+  cudaFree(s->mem);
+  delete s;
+}
+
+extern "C" int vpb_smoother_update(vpb_smoother* s, float* d_kpts, int32_t n, const int32_t* d_counts, const int32_t* d_ids,
+                                   const double* d_clock, double* d_out, void* stream) {
+  const char* fn = "vpb_smoother_update";
+  if (!s) return fail(VPB_ERR_ARG, "%s: null smoother", fn);
+  if (n < 0) return fail(VPB_ERR_ARG, "%s: %d rows", fn, n);
+  if (!d_counts || (n > 0 && (!d_kpts || !d_ids))) return fail(VPB_ERR_ARG, "%s: null buffer", fn);
+  if (s->q.realtime && !d_clock) return fail(VPB_ERR_ARG, "%s: realtime mode (fps <= 0) needs d_clock", fn);
+  SmootherDevice guard(s);
+  SmoothParams q = s->q;
+  q.kpts = d_kpts; q.n = n; q.counts = d_counts; q.ids = d_ids; q.clock = d_clock; q.out = d_out;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  smooth_assign<<<q.num_streams, SMOOTH_THREADS, 0, st>>>(q);
+  CU_TRY(cudaGetLastError());
+  const dim3 grid(static_cast<unsigned>(cdiv(SMOOTH_MAX * q.k, SMOOTH_APPLY_THREADS)), static_cast<unsigned>(q.num_streams));
+  smooth_apply<<<grid, SMOOTH_APPLY_THREADS, 0, st>>>(q);
+  CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+extern "C" int vpb_smoother_reset(vpb_smoother* s, int32_t stream_index, void* stream) {
+  if (!s) return fail(VPB_ERR_ARG, "vpb_smoother_reset: null smoother");
+  const int S = s->q.num_streams;
+  if (stream_index < -1 || stream_index >= S) return fail(VPB_ERR_ARG, "vpb_smoother_reset: stream %d of %d", stream_index, S);
+  SmootherDevice guard(s);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t first = stream_index < 0 ? 0 : stream_index, count = stream_index < 0 ? S : 1;
+  CU_TRY(cudaMemsetAsync(s->q.slot_u + first * SMOOTH_MAX, 0xFF, count * SMOOTH_MAX * sizeof(int32_t), st));
+  CU_TRY(cudaMemsetAsync(s->q.updates + first, 0, count * sizeof(int32_t), st));
+  return VPB_OK;
+}
+
+extern "C" int vpb_smoother_status(vpb_smoother* s, int32_t* h_status) {
+  if (!s || !h_status) return fail(VPB_ERR_ARG, "vpb_smoother_status: null argument");
+  SmootherDevice guard(s);
+  CU_TRY(cudaDeviceSynchronize());
+  CU_TRY(cudaMemcpy(h_status, s->q.status, sizeof(int32_t), cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemset(s->q.status, 0, sizeof(int32_t)));
   return VPB_OK;
 }
 

@@ -12,6 +12,7 @@ per-person loop of `VitInference.inference` (:258-272) as ONE engine call on the
 """
 from __future__ import annotations
 
+import time
 import types
 
 import numpy as np
@@ -201,21 +202,38 @@ class B200PoseBackend:
         return [out[offs[j]:offs[j + 1]].reshape(im.shape) for j, im in enumerate(imgs)]
 
     @torch.no_grad()
-    def inference_frames_tracked(self, imgs: "list[np.ndarray]", dets_list, tracker, rotate=0) -> "list[dict]":
+    def inference_frames_tracked(self, imgs: "list[np.ndarray]", dets_list, tracker, rotate=0, smoother=None,
+                                 clock=None) -> "list[dict]":
         """S streams' `frame_inference` after detection: one frame per stream (uint8 RGB [H,W,3], numpy or CUDA) and its
         detections [n_s, 5] (empty where the detector was skipped, as frame_inference passes them) -> one {id: float32 [K,3]
         (y, x, score)} per stream.  `tracker` (a track.DeviceSort of S streams on the engine's device) is updated once; its
         int32 boxes feed infer_frames on the device, and only the row counts and ids come back before the pose call.  `rotate`:
         each stream's rotation as inference_frames takes it (one for all or one per stream); detections, tracks and keypoints
-        are in the rotated frames' pixels."""
+        are in the rotated frames' pixels.  `smoother` (a smooth.DeviceOneEuro of S streams and the engine's K) smooths every
+        person's (y, x) by track id on the device before the read-back; the scores stay as the engine gave them.  `clock`:
+        one value per stream for the smoother (realtime mode: seconds, default time.time() for every stream; fps mode:
+        default each stream's update count)."""
         if len(imgs) != tracker.num_streams:
             raise ValueError(f"{len(imgs)} frames for a tracker of {tracker.num_streams} streams")
+        if smoother is not None and (smoother.num_streams != tracker.num_streams or smoother.num_keypoints != self.model.num_keypoints):
+            raise ValueError(f"a smoother of {smoother.num_streams} streams and {smoother.num_keypoints} keypoints for "
+                             f"{tracker.num_streams} streams and {self.model.num_keypoints} keypoints")
         dets, counts = tracker.pack(dets_list)
         rows, boxes, out_counts = tracker.update_device(dets, counts)
         n = out_counts.tolist()
         ids = rows[:, :, 5].long().cpu()                     # the rows' id + 1, the keys frame_inference uses (inference.py:249)
         frames = [im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(im)) for im in imgs]
         kps, _ = self.model.infer_frames(frames, [boxes[s, :c] for s, c in enumerate(n)], rotate=rotate)
+        if smoother is not None:
+            dev = rows.device
+            kp = torch.cat(kps) if kps else torch.zeros((0, self.model.num_keypoints, 3), dtype=torch.float32, device=dev)
+            row_ids = torch.cat([rows[s, :c, 5] for s, c in enumerate(n)]).to(torch.int32)
+            if clock is None and smoother.realtime:
+                clock = [time.time()] * tracker.num_streams
+            clk = None if clock is None else torch.as_tensor(np.asarray(clock, np.float64)).to(dev)
+            with torch.cuda.device(dev):
+                smoother.update_device(kp, out_counts, row_ids, clk)
+            kps = kp.split(n)
         return [dict(zip(ids[s, :c].tolist(), kp.cpu().numpy())) for s, (c, kp) in enumerate(zip(n, kps))]
 
     @torch.no_grad()
@@ -262,6 +280,11 @@ def frame_inference(self, img: np.ndarray) -> dict:
         ids = list(range(len(bboxes)))
 
     kpts, _ = self._b200.model.infer_frame_host(img, bboxes)            # pad/clip, crop, pad_image, pre_img, model, decode, offsets
+    smoother = getattr(self, "_smoother", None)
+    if smoother is not None and self.tracker is not None:               # ids are track ids only where there is a tracker
+        yx = smoother.update([kpts], [ids], clock=[time.time()] if smoother.realtime else None)[0]
+        smoother.check()
+        kpts[:, :, :2] = yx
     frame_keypoints = {i: kpts[n] for n, i in enumerate(ids)}
     scores_bbox = {i: sc for i, sc in zip(ids, scores)}
 
@@ -337,8 +360,17 @@ def _reference_reset(self):
     self.frame_counter = 0
 
 
+SMOOTHING_DEFAULTS = dict(min_cutoff=1.7, beta=0.3, d_cutoff=30.0, fps=None, dx0=0.0, max_gap=30)
+
+
+def _reset_with_smoother(self):
+    """The bound `reset()` followed by forgetting the keypoint filters.  Bound by `install(..., smoothing=...)`."""
+    self._reset_before_smoothing()
+    self._smoother.reset()
+
+
 def install(vit_inference, max_batch: int = 64, device=None, batched: bool = False, flip_test: bool = False,
-            flip_pairs=None, device_tracker: bool = False) -> B200PoseBackend:
+            flip_pairs=None, device_tracker: bool = False, smoothing=None) -> B200PoseBackend:
     """Re-bind a constructed reference `VitInference` (torch .pth backend) to the H100 engine: takes the
     weights out of its `_vit_pose` module, then replaces `_vit_pose` and `_inference` exactly where
     easy_ViTPose/inference.py:156-172 set them.  With `batched=True` the object's `inference` method is re-bound to
@@ -348,9 +380,23 @@ def install(vit_inference, max_batch: int = 64, device=None, batched: bool = Fal
     pairs of `flip_pairs_for(vit_inference.dataset, flip_pairs)`; the engine is then built for 2 * max_batch crops, so
     `max_batch` still counts people per call.  With `batched=True, device_tracker=True` the SORT tracker runs on the device
     too: `vit_inference.tracker` becomes a `DeviceTracker` with the reference's parameters (only where the reference builds a
-    Sort) and `reset()` is re-bound to rebuild it.  Returns the backend (also stored as `._b200`)."""
+    Sort) and `reset()` is re-bound to rebuild it.  With `batched=True, smoothing=dict(...)` every frame's keypoints are
+    smoothed by track id with the reference's OneEuroFilter, one filter per id, on the device (a one-stream
+    `smooth.DeviceOneEuro`; keys min_cutoff, beta, d_cutoff, fps, dx0, max_gap, defaults SMOOTHING_DEFAULTS, `{}` for all of
+    them): the returned dict, `_keypoints` and so `draw()` hold the smoothed (y, x) and the engine's scores, with the CPU
+    `Sort` or `device_tracker=True`.  Smoothing applies only where the reference has a tracker (video, not single_pose):
+    without one the ids are positions in the frame, not people, and the keypoints are left as they are.  With fps=None
+    (realtime) each frame's clock is time.time(), as the reference class reads it.  `reset()` also forgets the filters.
+    Returns the backend (also stored as `._b200`)."""
     if device_tracker and not batched:
         raise ValueError("device_tracker=True needs batched=True")
+    if smoothing is not None:
+        if not batched:
+            raise ValueError("smoothing needs batched=True")
+        unknown = set(smoothing) - set(SMOOTHING_DEFAULTS)
+        if unknown:
+            raise ValueError(f"unknown smoothing parameters {sorted(unknown)}; expected some of {sorted(SMOOTHING_DEFAULTS)}")
+        smoothing = {**SMOOTHING_DEFAULTS, **smoothing}
     pairs = flip_pairs_for(getattr(vit_inference, "dataset", None), flip_pairs) if flip_test else None
     ref = vit_inference._vit_pose
     sd = {k: v.detach().cpu() for k, v in ref.state_dict().items()}
@@ -377,4 +423,9 @@ def install(vit_inference, max_batch: int = 64, device=None, batched: bool = Fal
         if vit_inference.tracker is not None:
             vit_inference.tracker = DeviceTracker(vit_inference.tracker.max_age, vit_inference.tracker.min_hits,
                                                   vit_inference.tracker.iou_threshold, model._device)
+    if smoothing is not None:
+        from .smooth import DeviceOneEuro
+        vit_inference._smoother = DeviceOneEuro(1, K, device=model._device, **smoothing)
+        vit_inference._reset_before_smoothing = vit_inference.reset
+        vit_inference.reset = types.MethodType(_reset_with_smoother, vit_inference)
     return backend

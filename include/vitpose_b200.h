@@ -458,6 +458,41 @@ int vpb_tracker_next_id(vpb_tracker* t, int64_t* next_id);
 int vpb_tracker_set_next_id(vpb_tracker* t, int64_t next_id);
 int vpb_tracker_status(vpb_tracker* t, int32_t* status);
 
+/* ---- One Euro smoother: easy_ViTPose/vit_utils/post_processing/one_euro_filter.py's OneEuroFilter kept per track id, for
+ * num_streams video streams in one step on the device.  Per stream there is a map id -> (filter, c_last, u_last); update u
+ * (the stream's count of accepted updates, from 0) at clock c with rows (id_i, x_i), x_i the (y, x) columns of a [K,3]
+ * keypoint row, does: 1. forget every id absent from more than max_gap updates in a row (max_gap = 0: an id missing once
+ * starts again); 2. a known id outputs filter(x_i, t_e), t_e = c - c_last in fps mode (fps > 0; c defaults to u, so t_e
+ * counts frames) and (c - c_last) * d_cutoff in realtime mode (fps <= 0; c is the caller's timestamp in seconds, standing in
+ * for the reference's time()); 3. a new id builds OneEuroFilter(x_i, dx0, min_cutoff, beta, d_cutoff, fps) and outputs x_i
+ * unchanged; 4. every id of the update takes c_last = c, u_last = u.  Outputs equal that composition of the reference class
+ * as float64 values: numpy's promotion (the first call's float32 x - x_prev), its evaluation order, no FMA contraction, the
+ * x <= 0 mask (-10, NaN not masked), the inf / NaN of t_e = 0.  Filter state stays in device memory between updates.
+ * vpb_smoother_create: k 1..144 keypoints; fps <= 0 selects realtime mode; every parameter finite; max_gap >= 0.
+ * vpb_smoother_update: d_kpts f32 [n,k,3] (y, x, score), the rows of all streams concatenated stream by stream, stream s
+ * holding the next d_counts[s] rows (i32 [S], DEVICE); d_ids i32 [n] each row's track id (frame_inference's keys, the
+ * tracker's id + 1); d_clock f64 [S] each stream's clock, NULL in fps mode = the update count (VPB_ERR_ARG in realtime mode);
+ * n = the rows d_kpts, d_ids and d_out hold.  Writes the smoothed (y, x), rounded to float32, over d_kpts' first two columns
+ * (scores untouched) and, when d_out is not NULL, the float64 result to d_out [n,k,2].  Two launches, no host
+ * synchronisation: the call can be captured in a CUDA graph.  A stream whose count is negative or above VPB_SMOOTH_MAX, whose
+ * rows would run past n, that names an id twice, or that would hold more than VPB_SMOOTH_MAX ids is left unchanged (its rows
+ * are not written, its update count does not advance) and sets a status bit; the other streams are unaffected.
+ * vpb_smoother_reset: forget stream_index's filters and update count (-1: every stream), enqueued on `stream`.
+ * vpb_smoother_status: SYNCHRONOUS; the bits VPB_SMOOTH_* raised since the last query, then clears them.
+ * VPB_ERR_ARG: num_streams outside 1..65535, k outside 1..144, a non-finite parameter, max_gap < 0, a bad device, n < 0, null
+ * buffers, a null d_clock in realtime mode, a stream_index outside -1..S-1. */
+#define VPB_SMOOTH_MAX 128
+#define VPB_SMOOTH_DUPLICATE_ID 1
+#define VPB_SMOOTH_OVER_CAPACITY 2
+typedef struct vpb_smoother vpb_smoother;
+int vpb_smoother_create(int32_t num_streams, int32_t k, double min_cutoff, double beta, double d_cutoff, double fps, double dx0,
+                        int32_t max_gap, int32_t device, vpb_smoother** out);
+void vpb_smoother_destroy(vpb_smoother* s);
+int vpb_smoother_update(vpb_smoother* s, float* d_kpts, int32_t n, const int32_t* d_counts, const int32_t* d_ids,
+                        const double* d_clock, double* d_out, void* stream);
+int vpb_smoother_reset(vpb_smoother* s, int32_t stream_index, void* stream);
+int vpb_smoother_status(vpb_smoother* s, int32_t* status);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* The engine's cached CUDA graphs: mixed = 0 the single-head calls' (one per batch size and decode kind), 1 the multi-head
