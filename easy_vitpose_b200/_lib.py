@@ -56,6 +56,12 @@ class VpbSegment(C.Structure):
     _fields_ = [("head", C.c_int32), ("count", C.c_int32)]
 
 
+class VpbOksNmsParams(C.Structure):
+    """vpb_oks_nms_params: thr, vis_thr (NaN = None), rescore_vis_thr (NaN = off), soft, max_dets."""
+    _fields_ = [("thr", C.c_double), ("vis_thr", C.c_double), ("rescore_vis_thr", C.c_double), ("soft", C.c_int32),
+                ("max_dets", C.c_int32)]
+
+
 DRAW_CHANNEL_ORDERS = {"rgb": 0, "bgr": 1}          # VPB_DRAW_RGB, VPB_DRAW_BGR
 
 
@@ -162,6 +168,10 @@ EXPORTS = {
     "vpb_smoother_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_smoother_reset": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     "vpb_smoother_status": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "vpb_oks_nms": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                              C.POINTER(VpbOksNmsParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_oks_iou": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
+                              C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 # The NV12 calls: names with a digit, kept apart from EXPORTS, which tests/test_abi.py matches against the header's

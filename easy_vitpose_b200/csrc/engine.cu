@@ -26,6 +26,7 @@
 #include "gemm.cuh"
 #include "pointwise.cuh"
 #include "preprocess.cuh"
+#include "oks_nms.cuh"
 #include "qkv_attention.cuh"
 #include "smooth.cuh"
 #include "track.cuh"
@@ -2501,6 +2502,70 @@ extern "C" int vpb_smoother_status(vpb_smoother* s, int32_t* h_status) {
   CU_TRY(cudaDeviceSynchronize());
   CU_TRY(cudaMemcpy(h_status, s->q.status, sizeof(int32_t), cudaMemcpyDeviceToHost));
   CU_TRY(cudaMemset(s->q.status, 0, sizeof(int32_t)));
+  return VPB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- OKS NMS
+// easy_ViTPose/vit_utils/post_processing/nms.py:66-70: the COCO-17 sigmas oks_iou uses when it is given none
+static const double kCocoSigmas[17] = {.26 / 10.0, .25 / 10.0, .25 / 10.0, .35 / 10.0, .35 / 10.0, .79 / 10.0, .79 / 10.0, .72 / 10.0,
+                                       .72 / 10.0, .62 / 10.0, .62 / 10.0, 1.07 / 10.0, 1.07 / 10.0, .87 / 10.0, .87 / 10.0, .89 / 10.0,
+                                       .89 / 10.0};
+
+// the checks and the parameters vpb_oks_nms and vpb_oks_iou share
+static int oks_params(const char* fn, const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d_counts, int32_t num_frames,
+                      const double* d_areas, const double* h_sigmas, double vis_thr, int32_t* d_status, OksNmsParams* q) {
+  if (k < 1 || k > NMS_MAX_K) return fail(VPB_ERR_ARG, "%s: %d keypoints (1..%d)", fn, k, NMS_MAX_K);
+  if (n_rows < 0) return fail(VPB_ERR_ARG, "%s: %d rows", fn, n_rows);
+  if (num_frames < 0 || num_frames > 65535) return fail(VPB_ERR_ARG, "%s: %d frames (0..65535)", fn, num_frames);
+  if (!d_status || (num_frames > 0 && !d_counts) || (n_rows > 0 && (!d_kpts || !d_areas)))
+    return fail(VPB_ERR_ARG, "%s: null buffer", fn);
+  if (!h_sigmas && k != 17) return fail(VPB_ERR_ARG, "%s: %d keypoints need sigmas (the default table has 17)", fn, k);
+  const double* sig = h_sigmas ? h_sigmas : kCocoSigmas;
+  memset(q, 0, sizeof(*q));
+  for (int j = 0; j < k; ++j) {
+    if (!std::isfinite(sig[j])) return fail(VPB_ERR_ARG, "%s: sigma %d is not finite", fn, j);
+    const double v = sig[j] * 2.0;
+    q->vars[j] = v * v;
+  }
+  q->kpts = d_kpts; q->counts = d_counts; q->areas = d_areas; q->status = d_status;
+  q->n_rows = n_rows; q->k = k; q->num_frames = num_frames;
+  q->use_vis = !std::isnan(vis_thr);
+  q->vis_thr = static_cast<float>(vis_thr);
+  return VPB_OK;
+}
+
+extern "C" int vpb_oks_nms(const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d_counts, int32_t num_frames,
+                           const double* d_areas, const double* d_scores, const double* h_sigmas, const vpb_oks_nms_params* params,
+                           int32_t* d_keep, int32_t* d_keep_counts, double* d_scores_out, int32_t* d_status, void* stream) {
+  const char* fn = "vpb_oks_nms";
+  if (!params) return fail(VPB_ERR_ARG, "%s: null params", fn);
+  OksNmsParams q;
+  VPB_TRY(oks_params(fn, d_kpts, n_rows, k, d_counts, num_frames, d_areas, h_sigmas, params->vis_thr, d_status, &q));
+  if (!std::isfinite(params->thr)) return fail(VPB_ERR_ARG, "%s: thr %g is not finite", fn, params->thr);
+  if (params->soft != 0 && params->soft != 1) return fail(VPB_ERR_ARG, "%s: soft %d (0 or 1)", fn, params->soft);
+  if (params->soft && (params->max_dets < 0 || params->max_dets > NMS_MAX_DETS))
+    return fail(VPB_ERR_ARG, "%s: max_dets %d (0..%d)", fn, params->max_dets, NMS_MAX_DETS);
+  if ((num_frames > 0 && !d_keep_counts) || (n_rows > 0 && (!d_scores || !d_keep))) return fail(VPB_ERR_ARG, "%s: null buffer", fn);
+  if (num_frames == 0) return VPB_OK;
+  q.scores = d_scores; q.keep = d_keep; q.keep_counts = d_keep_counts; q.scores_out = d_scores_out;
+  q.soft = params->soft; q.max_dets = params->max_dets; q.thr = static_cast<float>(params->thr);
+  q.rescore = !std::isnan(params->rescore_vis_thr);
+  q.rescore_vis_thr = static_cast<float>(params->rescore_vis_thr);
+  oks_nms_kernel<<<num_frames, NMS_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(q);
+  CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+extern "C" int vpb_oks_iou(const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d_counts, int32_t num_frames,
+                           const double* d_areas, const double* h_sigmas, double vis_thr, float* d_oks, int32_t* d_status, void* stream) {
+  const char* fn = "vpb_oks_iou";
+  OksNmsParams q;
+  VPB_TRY(oks_params(fn, d_kpts, n_rows, k, d_counts, num_frames, d_areas, h_sigmas, vis_thr, d_status, &q));
+  if (n_rows > 0 && !d_oks) return fail(VPB_ERR_ARG, "%s: null buffer", fn);
+  if (num_frames == 0) return VPB_OK;
+  q.oks = d_oks;
+  oks_iou_kernel<<<num_frames, NMS_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(q);
+  CU_TRY(cudaGetLastError());
   return VPB_OK;
 }
 

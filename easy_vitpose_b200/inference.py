@@ -20,8 +20,9 @@ import torch
 
 from .configs import data_cfg, flip_pairs_for, model_cfg
 from .model import ViTPose
+from .nms import check as nms_check, oks_nms_device
 from .top_down_eval import decode_heatmaps
-from .topdown import topdown_args
+from .topdown import topdown_args, xywh2cs
 
 __all__ = ["B200PoseBackend", "DeviceTracker", "install", "frame_inference", "frame_draw", "MEAN", "STD"]
 
@@ -139,6 +140,56 @@ class B200PoseBackend:
         args = [topdown_args(b, padding, use_udp) for b in bboxes_list]
         return self.model.infer_affine_heads_host(imgs, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], heads_list,
                                                   rotate)[0]
+
+    @torch.no_grad()
+    def inference_topdown_eval(self, imgs: "list[np.ndarray]", bboxes_xywh_list: "list[np.ndarray]", box_scores_list,
+                               oks_thr: float = 0.9, in_vis_thr: float = 0.2, soft_nms: bool = False, padding: float = 1.25,
+                               use_udp: bool = True, rotate=0) -> "list[tuple]":
+        """The top-down evaluation with detector boxes (HRNet / mmpose's evaluate, the thresholds of datasets/COCO.py:237-241)
+        on the device: inference_topdown, then each person's score = box score x mean keypoint score above in_vis_thr, then
+        per frame oks_nms (soft_nms: soft_oks_nms, max_dets 20) at oks_thr with the COCO-17 sigmas (the engine must have 17
+        keypoints) and area = s[0] * s[1] * 200 * 200 of the box's scale, all in one read-back.  Returns per frame (kept
+        keypoints float32 [m,K,3] (y, x, score), their rescored scores float64 [m], their box indices int64 [m]), in the
+        reference's order.  Honours the flip test."""
+        if not (len(imgs) == len(bboxes_xywh_list) == len(box_scores_list)):
+            raise ValueError(f"{len(imgs)} frames, {len(bboxes_xywh_list)} box arrays, {len(box_scores_list)} score arrays")
+        K = self.model.num_keypoints
+        boxes = [np.asarray(b, np.float64).reshape(-1, 4) for b in bboxes_xywh_list]
+        scores = [np.asarray(s, np.float64).reshape(-1) for s in box_scores_list]
+        for j, (b, s) in enumerate(zip(boxes, scores)):
+            if len(b) != len(s):
+                raise ValueError(f"frame {j}: {len(b)} boxes and {len(s)} scores")
+        counts = [len(b) for b in boxes]
+        n, F = sum(counts), len(imgs)
+        areas = np.zeros(n, np.float64)
+        for r, box in enumerate(b for bb in boxes for b in bb):
+            s = xywh2cs(box, padding)[1].astype(np.float64)
+            areas[r] = s[0] * s[1] * 200 * 200                   # HRNet's area, from the float64 copy of the scale
+        args = [topdown_args(b, padding, use_udp) for b in boxes]
+        frames = [im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(im)) for im in imgs]
+        kps, _ = self.model.infer_affine(frames, [a[0] for a in args], [a[1] for a in args], [a[2] for a in args], rotate=rotate)
+        dev = torch.device("cuda", self.model._device)
+        kp = torch.cat(kps) if kps else torch.zeros((0, K, 3), dtype=torch.float32, device=dev)
+        host = np.concatenate([areas, np.concatenate(scores) if n else np.zeros(0)])
+        d = torch.from_numpy(host).to(dev)
+        cnt = torch.tensor(counts, dtype=torch.int32).to(dev)
+        # one read-back: scores f64 [n] | kpts f32 [n,K,3] | keep i32 [n] | keep_counts i32 [F] | status i32 [1]
+        nk = n * K * 3
+        back = torch.empty(n + (nk + n + F + 2) // 2, dtype=torch.float64, device=dev)
+        bw = back[n:].view(torch.int32)
+        oks_nms_device(kp, cnt, d[:n], d[n:], oks_thr, soft=soft_nms, rescore_vis_thr=in_vis_thr,
+                             out=(bw[nk:nk + n], bw[nk + n:nk + n + F], back[:n], bw[nk + n + F:nk + n + F + 1].zero_()))
+        bw[:nk].view(torch.float32).view(n, K, 3).copy_(kp)
+        h = back.cpu().numpy()
+        hw = h[n:].view(np.int32)
+        nms_check(hw[nk + n + F])
+        hk = hw[:nk].view(np.float32).reshape(n, K, 3)
+        out, r0 = [], 0
+        for j, c in enumerate(counts):
+            idx = hw[nk + r0:nk + r0 + hw[nk + n + j]].astype(np.int64)
+            out.append((hk[r0 + idx].copy(), h[r0 + idx].copy(), idx))
+            r0 += c
+        return out
 
     # YUV video frames in any layout ViTPose.infer_frames_yuv takes (layout "i420" | "yv12" | "nv12" | "nv21" | "yuyv" | "uyvy",
     # e.g. ffmpeg's `-pix_fmt yuv420p` output or a V4L2 webcam's YUYV frame), converted on the device only where the gather taps

@@ -493,6 +493,49 @@ int vpb_smoother_update(vpb_smoother* s, float* d_kpts, int32_t n, const int32_t
 int vpb_smoother_reset(vpb_smoother* s, int32_t stream_index, void* stream);
 int vpb_smoother_status(vpb_smoother* s, int32_t* status);
 
+/* ---- OKS NMS: easy_ViTPose/vit_utils/post_processing/nms.py's oks_iou, oks_nms and soft_oks_nms, for num_frames frames in
+ * one launch (one CTA per frame), with HRNet's evaluation rescoring as an option.  Frame f holds the next d_counts[f] rows
+ * (i32 [F], DEVICE) of d_kpts f32 [n_rows,k,3] (y, x, score; the OKS is symmetric in the two coordinates, so the
+ * reference's (x, y, score) rows give the same result), d_areas f64 [n_rows] and d_scores f64 [n_rows].  h_sigmas: f64 [k]
+ * (HOST, copied into the launch), NULL = the reference's COCO-17 table (k = 17 only).
+ * Per frame, as the reference computes it (oracle/oks_nms_oracle.py restates it):
+ *   order: scores.argsort()[::-1] with a stable argsort, i.e. descending, NaN above +inf, equal scores later index first;
+ *     soft NMS re-sorts the remaining order by the same rule every round (ties then go to the later position);
+ *   OKS: float32 dx*dx + dy*dy, then / vars / ((a_g + a_d) / 2 + 2^-52) / 2 in float64, exp, numpy's pairwise sum over the
+ *     candidate's keypoints with score > vis_thr (oks_iou's mask quirk keeps the candidate's alone; NaN vis_thr = None, all
+ *     keypoints), / count, rounded to float32; 0 with no keypoint.  exp is CUDA's, so an OKS can differ by one float32 ulp;
+ *   hard (soft = 0): keep the head, drop the rest whose OKS against it is not <= (float)thr, repeat;
+ *   soft (soft = 1): keep the head, scores of the rest *= expf(-(o*o) / (float)thr), re-sort, repeat up to max_dets;
+ *   rescore_vis_thr (NaN = off): each row's score becomes float32(mean of its keypoint scores > (float)rescore_vis_thr, 0
+ *     when none) * float32(d_scores) before the sort, exactly (HRNet's evaluate).
+ * Writes d_keep [n_rows]: over each frame's rows its kept frame-local indices in the reference's order, then -1;
+ * d_keep_counts [F]; d_scores_out [n_rows] (may be NULL) the score each row was sorted by.  Rows outside every frame's range
+ * are not written.  A frame whose count is above VPB_NMS_MAX_PEOPLE (VPB_NMS_TOO_MANY_PEOPLE), negative or running past
+ * n_rows (VPB_NMS_BAD_ROWS) keeps nothing (count 0, -1 over its rows inside the buffer) and ORs its bit into *d_status (i32,
+ * DEVICE; the caller clears it); the other frames are unaffected.  No allocation, no host synchronisation: the call can be
+ * captured in a CUDA graph.
+ * vpb_oks_iou: the OKS matrix of every frame, d_oks f32 [n_rows, VPB_NMS_MAX_PEOPLE]: row r = frame row i, column j < n_f =
+ * oks_iou(g = person i, d = person j); other columns are not written.  Same limits and status bits.
+ * VPB_ERR_ARG: k outside 1..VPB_NMS_MAX_K, n_rows < 0, num_frames outside 0..65535, null buffers or params, NULL h_sigmas
+ * with k != 17, a non-finite sigma or thr, soft not 0 / 1, a soft max_dets outside 0..VPB_NMS_MAX_DETS. */
+#define VPB_NMS_MAX_PEOPLE 256
+#define VPB_NMS_MAX_K 144
+#define VPB_NMS_MAX_DETS 256
+#define VPB_NMS_TOO_MANY_PEOPLE 1
+#define VPB_NMS_BAD_ROWS 2
+typedef struct vpb_oks_nms_params {
+  double thr;               /* oks_nms / soft_oks_nms `thr`, used as float32 */
+  double vis_thr;           /* oks_iou `vis_thr`, NaN = None */
+  double rescore_vis_thr;   /* HRNet's in_vis_thre, NaN = no rescoring */
+  int32_t soft;             /* 0: oks_nms, 1: soft_oks_nms */
+  int32_t max_dets;         /* soft_oks_nms `max_dets` */
+} vpb_oks_nms_params;
+int vpb_oks_nms(const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d_counts, int32_t num_frames, const double* d_areas,
+                const double* d_scores, const double* h_sigmas, const vpb_oks_nms_params* params, int32_t* d_keep,
+                int32_t* d_keep_counts, double* d_scores_out, int32_t* d_status, void* stream);
+int vpb_oks_iou(const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d_counts, int32_t num_frames, const double* d_areas,
+                const double* h_sigmas, double vis_thr, float* d_oks, int32_t* d_status, void* stream);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* The engine's cached CUDA graphs: mixed = 0 the single-head calls' (one per batch size and decode kind), 1 the multi-head
