@@ -7,6 +7,7 @@ csrc/ holds the hand-written CUDA (wgmma GEMM + attention, LayerNorm, gathers, d
 model.ViTPose, top_down_eval.keypoints_from_heatmaps, inference.install / B200PoseBackend.
 """
 from . import distributed  # noqa: F401
+from .coco_eval import DeviceCocoEval, coco_eval_device  # noqa: F401
 from .configs import COCO_FLIP_PAIRS, VITPOSE_PLUS_HEADS, data_cfg, dyn_model_import, flip_pairs_for, model_cfg  # noqa: F401
 from .inference import B200PoseBackend, install  # noqa: F401
 from .nms import oks_iou_device, oks_nms, oks_nms_device, oks_nms_frames, soft_oks_nms  # noqa: F401

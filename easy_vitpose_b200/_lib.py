@@ -62,6 +62,18 @@ class VpbOksNmsParams(C.Structure):
                 ("max_dets", C.c_int32)]
 
 
+class VpbCocoGts(C.Structure):
+    """vpb_coco_gts: the ground truths of vpb_coco_eval, CSR by image (device pointers)."""
+    _fields_ = [("offsets", C.c_void_p), ("kpts", C.c_void_p), ("area", C.c_void_p), ("bbox", C.c_void_p), ("iscrowd", C.c_void_p),
+                ("num_keypoints", C.c_void_p), ("num_images", C.c_int32), ("num_gts", C.c_int32)]
+
+
+class VpbCocoDets(C.Structure):
+    """vpb_coco_dets: the detection frames of vpb_coco_eval (device pointers; keep / keep_counts may be NULL)."""
+    _fields_ = [("kpts", C.c_void_p), ("scores", C.c_void_p), ("counts", C.c_void_p), ("frame_image", C.c_void_p), ("keep", C.c_void_p),
+                ("keep_counts", C.c_void_p), ("n_rows", C.c_int32), ("num_frames", C.c_int32)]
+
+
 DRAW_CHANNEL_ORDERS = {"rgb": 0, "bgr": 1}          # VPB_DRAW_RGB, VPB_DRAW_BGR
 
 
@@ -172,6 +184,9 @@ EXPORTS = {
                               C.POINTER(VpbOksNmsParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vpb_oks_iou": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double,
                               C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vpb_coco_eval_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "vpb_coco_eval": (C.c_int, [C.c_int32, C.c_void_p, C.POINTER(VpbCocoGts), C.POINTER(VpbCocoDets), C.c_void_p, C.c_int64, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 # The NV12 calls: names with a digit, kept apart from EXPORTS, which tests/test_abi.py matches against the header's

@@ -10,7 +10,7 @@ import tempfile
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 LIB = os.path.join(CSRC, "libvitpose_b200.so")
 SOURCES = ["engine.cu"]
-HEADERS = ["ptx.cuh", "wgmma.cuh", "gemm.cuh", "expert_gemm.cuh", "chain.cuh", "attention.cuh", "qkv_attention.cuh", "pointwise.cuh", "decode.cuh", "draw.cuh", "track.cuh", "smooth.cuh", "oks_nms.cuh", "preprocess.cuh",
+HEADERS = ["ptx.cuh", "wgmma.cuh", "gemm.cuh", "expert_gemm.cuh", "chain.cuh", "attention.cuh", "qkv_attention.cuh", "pointwise.cuh", "decode.cuh", "draw.cuh", "track.cuh", "smooth.cuh", "oks_nms.cuh", "pairwise.cuh", "coco_eval.cuh", "preprocess.cuh",
            os.path.join("..", "..", "include", "vitpose_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC"]

@@ -27,6 +27,7 @@
 #include "pointwise.cuh"
 #include "preprocess.cuh"
 #include "oks_nms.cuh"
+#include "coco_eval.cuh"
 #include "qkv_attention.cuh"
 #include "smooth.cuh"
 #include "track.cuh"
@@ -2565,6 +2566,91 @@ extern "C" int vpb_oks_iou(const float* d_kpts, int32_t n_rows, int32_t k, const
   if (num_frames == 0) return VPB_OK;
   q.oks = d_oks;
   oks_iou_kernel<<<num_frames, NMS_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(q);
+  CU_TRY(cudaGetLastError());
+  return VPB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- COCO eval
+// the workspace vpb_coco_eval carves, in this order, each piece aligned to 256 bytes
+struct CocoWorkspace {
+  size_t frame_row0, key0, key1, slot0, slot1, bits, num_dets, npig, summary, total;
+};
+static CocoWorkspace coco_workspace(int64_t num_images, int64_t num_frames) {
+  CocoWorkspace w;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t at = off; off += (bytes + 255) / 256 * 256; return at; };
+  const int64_t slots = num_images * COCO_MAX_DETS;
+  w.frame_row0 = take(num_frames * sizeof(int32_t));
+  w.key0 = take(slots * sizeof(double));
+  w.key1 = take(slots * sizeof(double));
+  w.slot0 = take(slots * sizeof(int32_t));
+  w.slot1 = take(slots * sizeof(int32_t));
+  w.bits = take(slots * sizeof(unsigned long long));
+  w.num_dets = take(num_images * sizeof(int32_t));
+  w.npig = take(COCO_A * num_images * sizeof(int32_t));
+  w.summary = take(10 * COCO_SUMMARY_TERMS * sizeof(double));
+  w.total = off;
+  return w;
+}
+
+extern "C" int64_t vpb_coco_eval_workspace_bytes(int32_t num_images, int32_t num_frames) {
+  if (num_images < 1 || num_images > VPB_COCO_MAX_IMAGES || num_frames < 0) return -1;
+  return static_cast<int64_t>(coco_workspace(num_images, num_frames).total);
+}
+
+extern "C" int vpb_coco_eval(int32_t k, const double* h_sigmas, const vpb_coco_gts* gts, const vpb_coco_dets* dets, void* d_workspace,
+                             int64_t workspace_bytes, double* d_stats, double* d_precision, double* d_recall, int32_t* d_status,
+                             void* stream) {
+  const char* fn = "vpb_coco_eval";
+  if (!gts || !dets) return fail(VPB_ERR_ARG, "%s: null gts or dets", fn);
+  if (k < 1 || k > COCO_MAX_K) return fail(VPB_ERR_ARG, "%s: %d keypoints (1..%d)", fn, k, COCO_MAX_K);
+  const int32_t I = gts->num_images, G = gts->num_gts, F = dets->num_frames, n = dets->n_rows;
+  if (I < 1 || I > VPB_COCO_MAX_IMAGES) return fail(VPB_ERR_ARG, "%s: %d images (1..%d)", fn, I, VPB_COCO_MAX_IMAGES);
+  if (G < 0 || F < 0 || n < 0) return fail(VPB_ERR_ARG, "%s: %d ground truths, %d frames, %d rows", fn, G, F, n);
+  if (!gts->offsets || (G > 0 && (!gts->kpts || !gts->area || !gts->bbox || !gts->iscrowd || !gts->num_keypoints)))
+    return fail(VPB_ERR_ARG, "%s: null ground-truth buffer", fn);
+  if ((F > 0 && (!dets->counts || !dets->frame_image)) || (n > 0 && (!dets->kpts || !dets->scores)))
+    return fail(VPB_ERR_ARG, "%s: null detection buffer", fn);
+  if (dets->keep && F > 0 && !dets->keep_counts) return fail(VPB_ERR_ARG, "%s: a keep list needs keep counts", fn);
+  if (!d_workspace || !d_stats || !d_precision || !d_recall || !d_status) return fail(VPB_ERR_ARG, "%s: null output buffer", fn);
+  const CocoWorkspace w = coco_workspace(I, F);
+  if (workspace_bytes < static_cast<int64_t>(w.total))
+    return fail(VPB_ERR_ARG, "%s: workspace of %lld bytes (%lld needed)", fn, static_cast<long long>(workspace_bytes),
+                static_cast<long long>(w.total));
+  if (!h_sigmas && k != 17) return fail(VPB_ERR_ARG, "%s: %d keypoints need sigmas (the default table has 17)", fn, k);
+  CocoEvalParams q;
+  memset(&q, 0, sizeof(q));
+  const double* sig = h_sigmas ? h_sigmas : kCocoSigmas;
+  for (int j = 0; j < k; ++j) {
+    if (!std::isfinite(sig[j])) return fail(VPB_ERR_ARG, "%s: sigma %d is not finite", fn, j);
+    const double v = sig[j] * 2.0;
+    q.vars[j] = v * v;
+  }
+  char* ws = static_cast<char*>(d_workspace);
+  q.gt_offsets = gts->offsets; q.gt_kpts = gts->kpts; q.gt_area = gts->area; q.gt_bbox = gts->bbox;
+  q.gt_iscrowd = gts->iscrowd; q.gt_num_kpts = gts->num_keypoints;
+  q.dt_kpts = dets->kpts; q.dt_scores = dets->scores; q.counts = dets->counts; q.frame_image = dets->frame_image;
+  q.keep = dets->keep; q.keep_counts = dets->keep_counts;
+  q.frame_row0 = reinterpret_cast<int32_t*>(ws + w.frame_row0);
+  q.key[0] = reinterpret_cast<double*>(ws + w.key0); q.key[1] = reinterpret_cast<double*>(ws + w.key1);
+  q.slot[0] = reinterpret_cast<int32_t*>(ws + w.slot0); q.slot[1] = reinterpret_cast<int32_t*>(ws + w.slot1);
+  q.bits = reinterpret_cast<unsigned long long*>(ws + w.bits);
+  q.num_dets = reinterpret_cast<int32_t*>(ws + w.num_dets);
+  q.npig = reinterpret_cast<int32_t*>(ws + w.npig);
+  q.summary = reinterpret_cast<double*>(ws + w.summary);
+  q.stats = d_stats; q.precision = d_precision; q.recall = d_recall; q.status = d_status;
+  q.k = k; q.num_images = I; q.num_gts = G; q.num_frames = F; q.n_rows = n;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int smem = static_cast<int>(sizeof(CocoImageShared));
+  CU_TRY(cudaFuncSetAttribute(coco_image_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (F > 0) coco_frames_kernel<<<1, 1024, 0, st>>>(q);
+  coco_image_kernel<<<I, COCO_THREADS, smem, st>>>(q);
+  const long long slots = static_cast<long long>(I) * COCO_MAX_DETS;
+  int src = 0;
+  for (long long width = COCO_MAX_DETS; width < slots; width *= 2, src ^= 1)
+    coco_merge_kernel<<<static_cast<unsigned>((slots + COCO_THREADS - 1) / COCO_THREADS), COCO_THREADS, 0, st>>>(q, src, width);
+  coco_accumulate_kernel<<<COCO_A * COCO_T, COCO_ACC_THREADS, 0, st>>>(q, src);
+  coco_summarize_kernel<<<1, 32, 0, st>>>(q);
   CU_TRY(cudaGetLastError());
   return VPB_OK;
 }

@@ -25,6 +25,8 @@
 #pragma once
 #include <cstdint>
 
+#include "pairwise.cuh"
+
 constexpr int NMS_MAX_PEOPLE = 256;              // VPB_NMS_MAX_PEOPLE: one thread per person
 constexpr int NMS_MAX_K = 144;                   // VPB_NMS_MAX_K
 constexpr int NMS_MAX_DETS = 256;                // VPB_NMS_MAX_DETS
@@ -122,35 +124,12 @@ __device__ __forceinline__ double oks_term(const OksNmsParams& q, const float* g
   return exp(-e);
 }
 
-// numpy's pairwise_sum of one block-sized run (8 <= m <= 128): eight strided partial sums, their tree, then the tail
-__device__ __forceinline__ double oks_block(const OksNmsParams& q, const float* g, const float* d, const uint8_t* v, int m, double den) {
-  double r[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) r[j] = oks_term(q, g, d, v[j], den);
-  const int m8 = m - m % 8;
-  for (int i = 8; i < m8; i += 8) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], oks_term(q, g, d, v[i + j], den));
-  }
-  double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])), __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
-  for (int i = m8; i < m; ++i) res = __dadd_rn(res, oks_term(q, g, d, v[i], den));
-  return res;
-}
-
-// oks_iou(g, d): g the kept person, d the candidate, v / m the candidate's visible keypoints
+// oks_iou(g, d): g the kept person, d the candidate, v / m the candidate's visible keypoints (m <= NMS_MAX_K < 256: at most
+// one pairwise split)
 __device__ __forceinline__ float oks_pair(const OksNmsParams& q, const float* g, const float* d, double a_g, double a_d, const uint8_t* v, int m) {
   if (m == 0) return 0.0f;
   const double den = __dadd_rn(__dmul_rn(__dadd_rn(a_g, a_d), 0.5), 2.220446049250313e-16);
-  double sum;
-  if (m < 8) {
-    sum = 0.0;
-    for (int i = 0; i < m; ++i) sum = __dadd_rn(sum, oks_term(q, g, d, v[i], den));
-  } else if (m <= 128) {
-    sum = oks_block(q, g, d, v, m, den);
-  } else {                                       // m <= NMS_MAX_K < 256: one split at n/2 rounded down to a multiple of 8
-    const int h = (m / 2) - (m / 2) % 8;
-    sum = __dadd_rn(oks_block(q, g, d, v, h, den), oks_block(q, g, d, v + h, m - h, den));
-  }
+  const double sum = pairwise_sum<1>([&](int i) { return oks_term(q, g, d, v[i], den); }, 0, m);
   return __double2float_rn(__ddiv_rn(sum, static_cast<double>(m)));
 }
 

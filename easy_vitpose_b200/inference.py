@@ -144,15 +144,20 @@ class B200PoseBackend:
     @torch.no_grad()
     def inference_topdown_eval(self, imgs: "list[np.ndarray]", bboxes_xywh_list: "list[np.ndarray]", box_scores_list,
                                oks_thr: float = 0.9, in_vis_thr: float = 0.2, soft_nms: bool = False, padding: float = 1.25,
-                               use_udp: bool = True, rotate=0) -> "list[tuple]":
+                               use_udp: bool = True, rotate=0, evaluator=None, image_ids=None) -> "list[tuple]":
         """The top-down evaluation with detector boxes (HRNet / mmpose's evaluate, the thresholds of datasets/COCO.py:237-241)
         on the device: inference_topdown, then each person's score = box score x mean keypoint score above in_vis_thr, then
         per frame oks_nms (soft_nms: soft_oks_nms, max_dets 20) at oks_thr with the COCO-17 sigmas (the engine must have 17
         keypoints) and area = s[0] * s[1] * 200 * 200 of the box's scale, all in one read-back.  Returns per frame (kept
         keypoints float32 [m,K,3] (y, x, score), their rescored scores float64 [m], their box indices int64 [m]), in the
-        reference's order.  Honours the flip test."""
+        reference's order.  Honours the flip test.
+        evaluator: a coco_eval.DeviceCocoEval; the kept people and their rescored scores are then appended to it from device
+        memory before the read-back, frame j as image image_ids[j] (one COCO image id per frame), the same detections
+        `evaluator.add` takes from records built from the returned poses."""
         if not (len(imgs) == len(bboxes_xywh_list) == len(box_scores_list)):
             raise ValueError(f"{len(imgs)} frames, {len(bboxes_xywh_list)} box arrays, {len(box_scores_list)} score arrays")
+        if evaluator is not None and (image_ids is None or len(image_ids) != len(imgs)):
+            raise ValueError(f"an evaluator needs one image id per frame ({len(imgs)} frames)")
         K = self.model.num_keypoints
         boxes = [np.asarray(b, np.float64).reshape(-1, 4) for b in bboxes_xywh_list]
         scores = [np.asarray(s, np.float64).reshape(-1) for s in box_scores_list]
@@ -180,6 +185,8 @@ class B200PoseBackend:
         oks_nms_device(kp, cnt, d[:n], d[n:], oks_thr, soft=soft_nms, rescore_vis_thr=in_vis_thr,
                              out=(bw[nk:nk + n], bw[nk + n:nk + n + F], back[:n], bw[nk + n + F:nk + n + F + 1].zero_()))
         bw[:nk].view(torch.float32).view(n, K, 3).copy_(kp)
+        if evaluator is not None:
+            evaluator.add_device(kp, back[:n], cnt, image_ids, keep=bw[nk:nk + n], keep_counts=bw[nk + n:nk + n + F])
         h = back.cpu().numpy()
         hw = h[n:].view(np.int32)
         nms_check(hw[nk + n + F])

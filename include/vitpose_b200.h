@@ -536,6 +536,63 @@ int vpb_oks_nms(const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d
 int vpb_oks_iou(const float* d_kpts, int32_t n_rows, int32_t k, const int32_t* d_counts, int32_t num_frames, const double* d_areas,
                 const double* h_sigmas, double vis_thr, float* d_oks, int32_t* d_status, void* stream);
 
+/* ---- COCO keypoint evaluation: pycocotools' COCOeval(cocoGt, cocoDt, 'keypoints') evaluate(), accumulate() and summarize() for
+ * category 1 with Params.setKpParams (maxDets 20, OKS thresholds .5:.05:.95, recall thresholds 0:.01:1, areas all / medium /
+ * large), over gts->num_images images in one enqueue (oracle/coco_oks_eval.py restates the algorithm).  All buffers DEVICE.
+ * Ground truths, CSR by image in ascending image id (COCOeval's np.unique order): image i holds rows [offsets[i], offsets[i+1])
+ * of kpts f64 [num_gts,k,3] (x, y, v), area f64, bbox f64 [num_gts,4] (x, y, w, h), iscrowd i32 and num_keypoints i32.  _ignore
+ * is iscrowd != 0, num_keypoints == 0, or area outside the range (pycocotools' _prepare overwrites a gt 'ignore' field).
+ * Detections come as frames: frame f holds the next counts[f] rows (the layout vpb_oks_nms reads) of kpts f64 [n_rows,k,2]
+ * (x, y) and scores f64 [n_rows], and belongs to image frame_image[f] (0..num_images-1).  With keep (optional, the d_keep /
+ * d_keep_counts vpb_oks_nms writes) frame f contributes rows keep[first row + j], j < keep_counts[f], in that order; without
+ * it every row.  An image's detections are its frames' rows in frame order, which decides ties among equal scores.  Each
+ * detection's area is loadRes's (max x - min x) * (max y - min y).
+ * Per image: argsort(-score, kind='mergesort') (descending, stable, NaN last), first 20; computeOks in float64 (the bbox
+ * distance for a ground truth with no v > 0); evaluateImg's greedy matching.  accumulate concatenates the images in order and
+ * sorts stably by score; summarize takes np.mean over the entries > -1.  Everything but exp follows numpy's order and rounding
+ * (pairwise sums, no FMA), so the results equal the numpy statement bit for bit unless CUDA's exp moves an OKS by an ulp across
+ * a threshold or another OKS.
+ * Writes d_stats f64 [10] (AP, AP50, AP75, AP_medium, AP_large, AR, AR50, AR75, AR_medium, AR_large), d_precision f64
+ * [3,10,101] (area, threshold, recall threshold; -1 where an area has no non-ignored ground truth) and d_recall f64 [3,10].
+ * An image with more than VPB_COCO_MAX_GTS ground truths (VPB_COCO_TOO_MANY_GTS) or more than VPB_COCO_MAX_ROWS detection rows
+ * (VPB_COCO_TOO_MANY_ROWS), a negative count, rows past n_rows, keep counts or entries outside their frame, a frame_image
+ * outside 0..num_images-1 or offsets out of order (VPB_COCO_BAD_INPUT) ORs its bit into *d_status (i32; the caller clears it),
+ * and every stat is then NaN.  d_workspace: at least vpb_coco_eval_workspace_bytes(num_images, num_frames) bytes (-1 for bad
+ * sizes), 256-byte aligned.  No allocation, no host synchronisation: the call can be captured in a CUDA graph.
+ * h_sigmas f64 [k] (HOST), NULL = the COCO-17 table (k = 17 only).
+ * VPB_ERR_ARG: k outside 1..VPB_COCO_MAX_K, num_images outside 1..VPB_COCO_MAX_IMAGES, a negative size, null buffers, a keep
+ * list without keep counts, a short workspace, NULL h_sigmas with k != 17, a non-finite sigma. */
+#define VPB_COCO_MAX_GTS 256
+#define VPB_COCO_MAX_ROWS 1024
+#define VPB_COCO_MAX_K 144
+#define VPB_COCO_MAX_IMAGES 1000000
+#define VPB_COCO_TOO_MANY_GTS 1
+#define VPB_COCO_TOO_MANY_ROWS 2
+#define VPB_COCO_BAD_INPUT 4
+typedef struct vpb_coco_gts {
+  const int32_t* offsets;        /* [num_images + 1] */
+  const double* kpts;            /* [num_gts, k, 3] */
+  const double* area;            /* [num_gts] */
+  const double* bbox;            /* [num_gts, 4] */
+  const int32_t* iscrowd;        /* [num_gts] */
+  const int32_t* num_keypoints;  /* [num_gts] */
+  int32_t num_images;
+  int32_t num_gts;
+} vpb_coco_gts;
+typedef struct vpb_coco_dets {
+  const double* kpts;            /* [n_rows, k, 2] */
+  const double* scores;          /* [n_rows] */
+  const int32_t* counts;         /* [num_frames] */
+  const int32_t* frame_image;    /* [num_frames] */
+  const int32_t* keep;           /* [n_rows] or NULL */
+  const int32_t* keep_counts;    /* [num_frames] or NULL */
+  int32_t n_rows;
+  int32_t num_frames;
+} vpb_coco_dets;
+int64_t vpb_coco_eval_workspace_bytes(int32_t num_images, int32_t num_frames);
+int vpb_coco_eval(int32_t k, const double* h_sigmas, const vpb_coco_gts* gts, const vpb_coco_dets* dets, void* d_workspace,
+                  int64_t workspace_bytes, double* d_stats, double* d_precision, double* d_recall, int32_t* d_status, void* stream);
+
 /* Introspection used by bench.py / tests. */
 int vpb_kernel_launches(const vpb_engine* e, int32_t batch);          /* kernels one vpb_infer enqueues */
 /* The engine's cached CUDA graphs: mixed = 0 the single-head calls' (one per batch size and decode kind), 1 the multi-head
