@@ -6,6 +6,7 @@ torch is used for what it is good at here: owning device memory and the current 
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from collections import OrderedDict
 
@@ -19,6 +20,8 @@ __all__ = ["ViTPose", "plan_frame_chunks", "nv12_planes", "yuv_planes", "split_v
            "plan_head_calls"]
 
 IMG_H, IMG_W, HM_H, HM_W = 256, 192, 64, 48
+_EMPTY_BOX = "a box is empty after padding and clipping to its frame"     # check=True of the multi-frame calls: status bit 0
+_BAD_AFFINE = "a matrix entry is not finite or a scale is <= 0"             # and of the affine calls: status bit 1
 
 
 def plan_frame_chunks(counts, limit: int, max_frames: int = _lib.MAX_FRAMES) -> "list[list[tuple[int, int, int]]]":
@@ -870,6 +873,124 @@ class ViTPose:
             bb = bb.round()                                  # easy_ViTPose/inference.py:253 (round half to even)
         return np.ascontiguousarray(bb.reshape(-1, 4), np.int32)
 
+    def _device_boxes(self, bboxes) -> "list[torch.Tensor]":
+        dev = torch.device("cuda", self._device)
+        boxes = []
+        for b in bboxes:                                     # rounded as _check_frame does; device boxes stay on the device
+            b = torch.as_tensor(b)
+            if b.is_floating_point():
+                b = b.round()
+            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
+        return boxes
+
+    def _frame_table(self, frames, struct, layout, host: bool):
+        """-> (the frames or planes to keep alive, every frame's `struct` fields before num_boxes), as numpy arrays for the
+        host forms and as device tensors otherwise; `layout` names the layout of VpbFrameYuv frames."""
+        if struct is _lib.VpbFrameYuv:
+            return self._yuv_host_table(frames, layout) if host else self._yuv_device_table(frames, layout)
+        if struct is _lib.VpbFrameNv12:                      # the YUV tables' nv12 planes ("NV12" as the messages spell it)
+            keep, rows = self._yuv_host_table(frames, "NV12") if host else self._yuv_device_table(frames, "NV12")
+            return keep, [(p[0], y_pitch, p[1], uv_pitch, h, w) for p, y_pitch, uv_pitch, h, w in rows]
+        if host:
+            frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
+            return frames, [(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames]
+        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        return frames, [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
+
+    def _frames_call(self, name: str, fmt: tuple, frames, bboxes=None, affine=None, heads=None, *, host: bool, rotate,
+                     check: bool = False, status: int = 0, message: str = "", struct=_lib.VpbFrame, layout=None):
+        """The body of the multi-frame calls: entry point `name` with format ints `fmt` over `struct` frames and per-frame
+        `bboxes` or `affine` = (matrices, centres, scales), grouped by `heads` (plan_head_calls) when given.  The host forms
+        stage numpy arrays and run synchronously; on the device, `check` turns bit `status` into ValueError(message)."""
+        named = [(bboxes, "box arrays")] if affine is None else list(zip(affine, ("matrix arrays", "centre arrays", "scale arrays")))
+        named = [(frames, "frames")] + named + ([] if heads is None else [(heads, "head arrays")])
+        if any(len(a) != len(frames) for a, _ in named):
+            sizes = [f"{len(a)} {what}" for a, what in named]
+            raise ValueError(" but ".join(sizes) if len(sizes) == 2 else ", ".join(sizes))
+        rot = _rotations(rotate, len(frames))
+        keep, table = self._frame_table(frames, struct, layout, host)
+        if affine is not None:
+            counts, M, CS = self._affine_args(*affine, validate=not host)   # the engine checks host values
+            staged = [M.cpu().numpy(), CS.cpu().numpy()] if host else [M, CS]
+        else:
+            boxes = [self._round_boxes(b) for b in bboxes] if host else self._device_boxes(bboxes)
+            counts = [len(b) for b in boxes]
+            staged = [np.concatenate(boxes) if boxes else np.zeros((0, 4), np.int32)] if host else \
+                [torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=torch.device("cuda", self._device))]
+        if heads is None:
+            chunks, K = plan_frame_chunks(counts, self.batch_limit), self.num_keypoints
+        else:
+            ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
+            rot, table = [rot[j] for j, _, _ in ents], [table[j] for j, _, _ in ents]   # one row per entry: its frame's
+            hv, K = np.array([k for _, _, k in ents], np.int32), self.num_keypoints_max
+        n = len(staged[0])
+        if host:
+            staged = [np.ascontiguousarray(a if heads is None else a[order]) for a in staged]
+            new = np.empty if heads is None else np.zeros
+            kp, idx = new((n, K, 3), np.float32), new((n, K), np.int32)
+        else:
+            dev = torch.device("cuda", self._device)
+            staged = [(a if heads is None else a.index_select(0, torch.as_tensor(order, device=a.device))).to(dev) for a in staged]
+            new = torch.empty if heads is None else torch.zeros
+            kp, idx = new((n, K, 3), dtype=torch.float32, device=dev), new((n, K), dtype=torch.int32, device=dev)
+        ptr = (lambda a: a.ctypes.data_as(C.c_void_p)) if host else (lambda t: C.c_void_p(t.data_ptr()))
+        s = 0                                                # first box of the current call
+        with torch.cuda.device(self._device) if host else contextlib.nullcontext():
+            for chunk in chunks:
+                arr = _frame_array(table, chunk, struct, rot)
+                ha = [] if heads is None else [np.ascontiguousarray(hv[:len(arr)])]
+                args = (self._handle, arr, len(arr), *fmt, *(h.ctypes.data_as(C.c_void_p) for h in ha),
+                        *(ptr(a[s:]) for a in staged + [kp, idx]))
+                if host:
+                    _lib.check_value(getattr(_lib.lib(), name)(*args, self._stream()))
+                else:
+                    self._call_on_stream(keep + staged + [kp, idx], lambda st: getattr(_lib.lib(), name)(*args, st))
+                s += sum(e - b for _, b, e in chunk)
+        if check and n and self.frame_status() & status:
+            raise ValueError(message)
+        if heads is not None:
+            if not host:
+                return self._per_frame(ents, counts, kp, idx)
+            k_t, i_t = self._per_frame(ents, counts, torch.from_numpy(kp), torch.from_numpy(idx))
+            return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+        if not counts:
+            return [], []
+        if host:
+            split = np.cumsum(counts)[:-1]
+            return np.split(kp, split), np.split(idx, split)
+        return list(kp.split(counts)), list(idx.split(counts))
+
+    @staticmethod
+    def _per_frame(ents, counts, kp, idx):
+        outs_k = [kp.new_zeros((c,) + tuple(kp.shape[1:])) for c in counts]
+        outs_i = [idx.new_zeros((c,) + tuple(idx.shape[1:])) for c in counts]
+        s = 0
+        for j, sel, _ in ents:
+            outs_k[j][sel] = kp[s:s + len(sel)]
+            outs_i[j][sel] = idx[s:s + len(sel)]
+            s += len(sel)
+        return outs_k, outs_i
+
+    def _submit_frames(self, name: str, fmt: tuple, frames, bboxes, table, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int,
+                       rotate, struct) -> None:
+        """The body of the submit_frames*_host calls: the length and `rotate` checks, table() (the method's own frame and box
+        checks -> (the arrays to keep alive, every frame's `struct` fields before num_boxes)), the outputs check and ONE
+        asynchronous call of engine entry point `name` over all frames, with the format ints `fmt`."""
+        if len(frames) != len(bboxes):
+            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
+        rot = _rotations(rotate, len(frames))
+        keep, rows = table()                                 # keep: what the rows point into, alive over the call
+        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
+        n = bb.shape[0]
+        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
+                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
+            raise ValueError(f"{name[len('vpb_'):]}: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
+        arr = (struct * len(rows))(*[struct(*row, len(b), r) for row, b, r in zip(rows, bboxes, rot)])
+        with torch.cuda.device(self._device):
+            _lib.check_value(getattr(_lib.lib(), name)(
+                self._handle, arr, len(arr), *fmt, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
+                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
     def infer_frames(self, frames, bboxes, check: bool = False, rotate=0):
         """The people of several frames in as few engine calls as the limits allow: uint8 RGB frames [H_j,W_j,3] (CUDA) and
         per-frame boxes [n_j,4] -> (list of kpts f32 [n_j,K,3] (y, x, score) in frame j's pixels, list of idx i32 [n_j,K]).
@@ -879,62 +1000,15 @@ class ViTPose:
         `rotate` (every frame method takes it): 0, 90, 180 or 270 degrees counter-clockwise for all frames or one per frame
         (_rotations); frame j is then seen as cv2.rotate turns it, and its boxes and keypoints are in that view's pixels."""
         self._ensure()
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
-        dev = torch.device("cuda", self._device)
-        boxes = []
-        for b in bboxes:                                     # rounded as _check_frame does; device boxes stay on the device
-            b = torch.as_tensor(b)
-            if b.is_floating_point():
-                b = b.round()
-            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
-        counts = [b.shape[0] for b in boxes]
-        bb = torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=dev)
-        n = bb.shape[0]
-        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
-        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
-        table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
-        s = 0                                                # first box of the current call
-        for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, rot=rot)
-            self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames(
-                self._handle, arr, len(arr), C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
-                C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 1:
-            raise ValueError("a box is empty after padding and clipping to its frame")
-        return list(kp.split(counts)) if counts else [], list(idx.split(counts)) if counts else []
+        return self._frames_call("vpb_infer_frames", (), frames, bboxes, host=False, rotate=rotate, check=check, status=1,
+                                 message=_EMPTY_BOX)
 
     def infer_frames_host(self, frames, bboxes, rotate=0):
         """HOST form of infer_frames (vpb_infer_frames_host, synchronous): numpy frames [H_j,W_j,3] uint8 and per-frame boxes
         -> (list of kpts [n_j,K,3], list of idx [n_j,K]) numpy arrays, chunked as infer_frames.  A box that is empty after
         padding and clipping raises ValueError naming its frame."""
         self._ensure()
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
-        boxes = [self._round_boxes(b) for b in bboxes]
-        counts = [len(b) for b in boxes]
-        bb = np.concatenate(boxes, 0) if boxes else np.zeros((0, 4), np.int32)
-        n = bb.shape[0]
-        kp = np.empty((n, self.num_keypoints, 3), np.float32)
-        idx = np.empty((n, self.num_keypoints), np.int32)
-        table = [(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames]
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, rot=rot)
-                _lib.check_value(_lib.lib().vpb_infer_frames_host(
-                    self._handle, arr, len(arr), bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
-                    idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        if not counts:
-            return [], []
-        split = np.cumsum(counts)[:-1]
-        return np.split(kp, split), np.split(idx, split)
+        return self._frames_call("vpb_infer_frames_host", (), frames, bboxes, host=True, rotate=rotate)
 
     def submit_frames_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int, rotate=0) -> None:
         """Asynchronous vpb_submit_frames_host, ONE engine call (wait with wait_host(slot)): uint8 frames [H_j,W_j,3] whose
@@ -943,26 +1017,16 @@ class ViTPose:
         outputs must stay alive and unmodified until the wait (pinned memory: real copy / compute overlap).  `rotate` as
         infer_frames."""
         self._ensure()
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        for j, (f, b) in enumerate(zip(frames, bboxes)):
-            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
-                    or f.strides[2] != 1 or f.strides[1] != 3 or f.strides[0] < 3 * f.shape[1]:
-                raise ValueError(f"frame {j}: uint8 [H,W,3] with packed pixels in each row expected")
-            if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
-                raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
-        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
-        n = bb.shape[0]
-        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
-                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
-            raise ValueError("submit_frames_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
-        arr = (_lib.VpbFrame * len(frames))(*[_lib.VpbFrame(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0], len(b), r)
-                                             for f, b, r in zip(frames, bboxes, rot)])
-        with torch.cuda.device(self._device):
-            _lib.check_value(_lib.lib().vpb_submit_frames_host(
-                self._handle, arr, len(arr), bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
-                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+        def table():
+            for j, (f, b) in enumerate(zip(frames, bboxes)):
+                if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3 \
+                        or f.strides[2] != 1 or f.strides[1] != 3 or f.strides[0] < 3 * f.shape[1]:
+                    raise ValueError(f"frame {j}: uint8 [H,W,3] with packed pixels in each row expected")
+                if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
+                    raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
+            return frames, [(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames]
+        self._submit_frames("vpb_submit_frames_host", (), frames, bboxes, table, kpts_out, idx_out, slot, rotate, _lib.VpbFrame)
 
     # ---------------------------------------------------------------------------------------- affine top-down crops
     @staticmethod
@@ -1003,13 +1067,12 @@ class ViTPose:
         if len(frames) != len(mats):
             raise ValueError(f"{len(frames)} frames but {len(mats)} matrix arrays")
         rot = _rotations(rotate, len(frames))
-        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
+        frames, table = self._frame_table(frames, _lib.VpbFrame, None, host=False)
         dev = torch.device("cuda", self._device)
         counts, M, _ = self._affine_args(mats)
         M = M.to(dev)
         n = M.shape[0]
         crops = torch.empty((n, 3, IMG_H, IMG_W), dtype=torch.float32, device=dev)
-        table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
         s = 0
         with torch.cuda.device(self._device):
             for chunk in plan_frame_chunks(counts, max(n, 1)):       # only the 64-frame table limits a call
@@ -1027,55 +1090,15 @@ class ViTPose:
         matrices).  Chunked like infer_frames; honours the flip test.  Host-side matrices / scales are checked here; CUDA
         ones set bit 1 of the status word, which `check=True` turns into a ValueError."""
         self._ensure()
-        if not (len(frames) == len(mats) == len(centers) == len(scales)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
-        dev = torch.device("cuda", self._device)
-        counts, M, CS = self._affine_args(mats, centers, scales)
-        M, CS = M.to(dev), CS.to(dev)
-        n = M.shape[0]
-        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
-        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
-        table = [(f.data_ptr(), f.shape[0], f.shape[1], f.stride(0)) for f in frames]
-        s = 0
-        for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, rot=rot)
-            self._call_on_stream(frames + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine(
-                self._handle, arr, len(arr), C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
-                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 2:
-            raise ValueError("a matrix entry is not finite or a scale is <= 0")
-        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+        return self._frames_call("vpb_infer_affine", (), frames, affine=(mats, centers, scales), host=False, rotate=rotate,
+                                 check=check, status=2, message=_BAD_AFFINE)
 
     def infer_affine_host(self, frames, mats, centers, scales, rotate=0):
         """HOST form of infer_affine (vpb_infer_affine_host, synchronous): numpy frames and per-frame matrices / centres /
         scales -> (list of kpts [n_j,K,3], list of idx [n_j,K]) numpy arrays.  A non-finite matrix entry or a scale <= 0
         raises ValueError naming the box."""
         self._ensure()
-        if not (len(frames) == len(mats) == len(centers) == len(scales)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
-        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
-        M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
-        n = M.shape[0]
-        kp = np.empty((n, self.num_keypoints, 3), np.float32)
-        idx = np.empty((n, self.num_keypoints), np.int32)
-        table = [(f.ctypes.data, f.shape[0], f.shape[1], f.strides[0]) for f in frames]
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, rot=rot)
-                _lib.check_value(_lib.lib().vpb_infer_affine_host(
-                    self._handle, arr, len(arr), M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
-                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        if not counts:
-            return [], []
-        split = np.cumsum(counts)[:-1]
-        return np.split(kp, split), np.split(idx, split)
+        return self._frames_call("vpb_infer_affine_host", (), frames, affine=(mats, centers, scales), host=True, rotate=rotate)
 
     # ---------------------------------------------------------------------------------------- NV12 video frames
     # Each frame is a uint8 [3H/2, W] array with the planes stacked or a (y [H,W], uv [H/2,W]) pair (nv12_planes); matrix is
@@ -1092,81 +1115,19 @@ class ViTPose:
             p = p.contiguous()                               # rows of bytes at any pitch are read in place
         return p
 
-    def _nv12_device_table(self, frames):
-        """-> (the plane tensors to keep alive, [(y ptr, y pitch, uv ptr, uv pitch, h, w)])"""
-        planes = [tuple(self._device_plane(j, p) for p in nv12_planes(f, f"frame {j}")) for j, f in enumerate(frames)]
-        table = [(y.data_ptr(), y.stride(0), uv.data_ptr(), uv.stride(0), y.shape[0], y.shape[1]) for y, uv in planes]
-        return [p for yuv in planes for p in yuv], table
-
-    @staticmethod
-    def _nv12_host_table(frames):
-        planes = []
-        for j, f in enumerate(frames):
-            y, uv = nv12_planes(f, f"frame {j}")
-            if not isinstance(y, np.ndarray):
-                raise ValueError(f"frame {j}: numpy NV12 planes expected")
-            planes.append(tuple(p if p.strides[1] == 1 and p.strides[0] >= p.shape[1] else np.ascontiguousarray(p) for p in (y, uv)))
-        return planes, [(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1]) for y, uv in planes]
-
     def infer_frames_nv12(self, frames, bboxes, matrix: str = "bt601", check: bool = False, rotate=0):
         """infer_frames on NV12 frames (vpb_infer_frames_nv12): CUDA (or host, copied over) NV12 frames and per-frame boxes
         [n_j,4] -> (list of kpts f32 [n_j,K,3], list of idx i32 [n_j,K]).  Chunked, flip test and status word as infer_frames."""
         self._ensure()
-        mat = _yuv_matrix(matrix)
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._nv12_device_table(frames)
-        dev = torch.device("cuda", self._device)
-        boxes = []
-        for b in bboxes:
-            b = torch.as_tensor(b)
-            if b.is_floating_point():
-                b = b.round()
-            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
-        counts = [b.shape[0] for b in boxes]
-        bb = torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=dev)
-        n = bb.shape[0]
-        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
-        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
-        s = 0
-        for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
-            self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_nv12(
-                self._handle, arr, len(arr), mat, C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
-                C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 1:
-            raise ValueError("a box is empty after padding and clipping to its frame")
-        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+        return self._frames_call("vpb_infer_frames_nv12", (_yuv_matrix(matrix),), frames, bboxes, host=False, rotate=rotate,
+                                 check=check, status=1, message=_EMPTY_BOX, struct=_lib.VpbFrameNv12)
 
     def infer_frames_nv12_host(self, frames, bboxes, matrix: str = "bt601", rotate=0):
         """HOST form of infer_frames_nv12 (vpb_infer_frames_nv12_host, synchronous): numpy NV12 frames, per-frame boxes ->
         numpy (kpts, idx) lists.  Each frame is staged packed at 1.5 B per pixel; an empty box raises ValueError."""
         self._ensure()
-        mat = _yuv_matrix(matrix)
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._nv12_host_table(frames)
-        boxes = [self._round_boxes(b) for b in bboxes]
-        counts = [len(b) for b in boxes]
-        bb = np.concatenate(boxes, 0) if boxes else np.zeros((0, 4), np.int32)
-        n = bb.shape[0]
-        kp = np.empty((n, self.num_keypoints, 3), np.float32)
-        idx = np.empty((n, self.num_keypoints), np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
-                _lib.check_value(_lib.lib().vpb_infer_frames_nv12_host(
-                    self._handle, arr, len(arr), mat, bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
-                    idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        if not counts:
-            return [], []
-        split = np.cumsum(counts)[:-1]
-        return np.split(kp, split), np.split(idx, split)
+        return self._frames_call("vpb_infer_frames_nv12_host", (_yuv_matrix(matrix),), frames, bboxes, host=True, rotate=rotate,
+                                 struct=_lib.VpbFrameNv12)
 
     def submit_frames_nv12_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int,
                                 matrix: str = "bt601", rotate=0) -> None:
@@ -1175,80 +1136,32 @@ class ViTPose:
         [n_j,4], already rounded) and outputs must stay alive and unmodified until the wait."""
         self._ensure()
         mat = _yuv_matrix(matrix)
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        table = []
-        for j, (f, b) in enumerate(zip(frames, bboxes)):
-            y, uv = nv12_planes(f, f"frame {j}")
-            if not isinstance(y, np.ndarray) or y.strides[1] != 1 or uv.strides[1] != 1 or y.strides[0] < y.shape[1] \
-                    or uv.strides[0] < uv.shape[1]:
-                raise ValueError(f"frame {j}: numpy NV12 planes with contiguous bytes in each row expected")
-            if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
-                raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
-            table.append(_lib.VpbFrameNv12(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1], len(b),
-                                           rot[j]))
-        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
-        n = bb.shape[0]
-        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
-                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
-            raise ValueError("submit_frames_nv12_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
-        arr = (_lib.VpbFrameNv12 * len(table))(*table)
-        with torch.cuda.device(self._device):
-            _lib.check_value(_lib.lib().vpb_submit_frames_nv12_host(
-                self._handle, arr, len(arr), mat, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
-                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+        def table():
+            planes = []
+            for j, (f, b) in enumerate(zip(frames, bboxes)):
+                y, uv = nv12_planes(f, f"frame {j}")
+                if not isinstance(y, np.ndarray) or y.strides[1] != 1 or uv.strides[1] != 1 or y.strides[0] < y.shape[1] \
+                        or uv.strides[0] < uv.shape[1]:
+                    raise ValueError(f"frame {j}: numpy NV12 planes with contiguous bytes in each row expected")
+                if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
+                    raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
+                planes.append((y, uv))
+            return planes, [(y.ctypes.data, y.strides[0], uv.ctypes.data, uv.strides[0], y.shape[0], y.shape[1]) for y, uv in planes]
+        self._submit_frames("vpb_submit_frames_nv12_host", (mat,), frames, bboxes, table, kpts_out, idx_out, slot, rotate,
+                            _lib.VpbFrameNv12)
 
     def infer_affine_nv12(self, frames, mats, centers, scales, matrix: str = "bt601", check: bool = False, rotate=0):
         """infer_affine on NV12 frames (vpb_infer_affine_nv12): the warp reads the NV12 planes and converts each tap."""
         self._ensure()
-        mat = _yuv_matrix(matrix)
-        if not (len(frames) == len(mats) == len(centers) == len(scales)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._nv12_device_table(frames)
-        dev = torch.device("cuda", self._device)
-        counts, M, CS = self._affine_args(mats, centers, scales)
-        M, CS = M.to(dev), CS.to(dev)
-        n = M.shape[0]
-        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
-        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
-        s = 0
-        for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
-            self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_nv12(
-                self._handle, arr, len(arr), mat, C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
-                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 2:
-            raise ValueError("a matrix entry is not finite or a scale is <= 0")
-        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+        return self._frames_call("vpb_infer_affine_nv12", (_yuv_matrix(matrix),), frames, affine=(mats, centers, scales),
+                                 host=False, rotate=rotate, check=check, status=2, message=_BAD_AFFINE, struct=_lib.VpbFrameNv12)
 
     def infer_affine_nv12_host(self, frames, mats, centers, scales, matrix: str = "bt601", rotate=0):
         """HOST form of infer_affine_nv12 (vpb_infer_affine_nv12_host, synchronous), checked as infer_affine_host."""
         self._ensure()
-        mat = _yuv_matrix(matrix)
-        if not (len(frames) == len(mats) == len(centers) == len(scales)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._nv12_host_table(frames)
-        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
-        M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
-        n = M.shape[0]
-        kp = np.empty((n, self.num_keypoints, 3), np.float32)
-        idx = np.empty((n, self.num_keypoints), np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameNv12, rot)
-                _lib.check_value(_lib.lib().vpb_infer_affine_nv12_host(
-                    self._handle, arr, len(arr), mat, M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
-                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        if not counts:
-            return [], []
-        split = np.cumsum(counts)[:-1]
-        return np.split(kp, split), np.split(idx, split)
+        return self._frames_call("vpb_infer_affine_nv12_host", (_yuv_matrix(matrix),), frames, affine=(mats, centers, scales),
+                                 host=True, rotate=rotate, struct=_lib.VpbFrameNv12)
 
     # ---------------------------------------------------------------------------------------- YUV video frames
     # Every call takes layout = "i420" | "yv12" | "nv12" | "nv21" | "yuyv" | "uyvy" (the frame forms of yuv_planes), matrix =
@@ -1299,72 +1212,21 @@ class ViTPose:
             table.append(ViTPose._yuv_row(planes, h, w))
         return keep, table
 
-    def _device_boxes(self, bboxes) -> "list[torch.Tensor]":
-        dev = torch.device("cuda", self._device)
-        boxes = []
-        for b in bboxes:                                     # rounded as _check_frame does; device boxes stay on the device
-            b = torch.as_tensor(b)
-            if b.is_floating_point():
-                b = b.round()
-            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
-        return boxes
-
     def infer_frames_yuv(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
                          check: bool = False, rotate=0):
         """infer_frames on YUV frames (vpb_infer_frames_yuv): CUDA (or host, copied over) frames and per-frame boxes [n_j,4] ->
         (list of kpts f32 [n_j,K,3], list of idx i32 [n_j,K]).  Chunked, flip test and status word as infer_frames."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._yuv_device_table(frames, layout)
-        dev = torch.device("cuda", self._device)
-        boxes = self._device_boxes(bboxes)
-        counts = [b.shape[0] for b in boxes]
-        bb = torch.cat(boxes) if boxes else torch.zeros((0, 4), dtype=torch.int32, device=dev)
-        n = bb.shape[0]
-        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
-        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
-        s = 0
-        for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-            self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_yuv(
-                self._handle, arr, len(arr), *fmt, C.c_void_p(bb[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()),
-                C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 1:
-            raise ValueError("a box is empty after padding and clipping to its frame")
-        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+        return self._frames_call("vpb_infer_frames_yuv", _yuv_format(layout, matrix, full_range), frames, bboxes, host=False,
+                                 rotate=rotate, check=check, status=1, message=_EMPTY_BOX, struct=_lib.VpbFrameYuv, layout=layout)
 
     def infer_frames_yuv_host(self, frames, bboxes, layout: str = "i420", matrix: str = "bt601", full_range: bool = False, rotate=0):
         """HOST form of infer_frames_yuv (vpb_infer_frames_yuv_host, synchronous): numpy frames, per-frame boxes -> numpy
         (kpts, idx) lists.  Each frame is staged packed (1.5 B per pixel for 4:2:0, 2 B for 4:2:2); an empty box raises
         ValueError."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._yuv_host_table(frames, layout)
-        boxes = [self._round_boxes(b) for b in bboxes]
-        counts = [len(b) for b in boxes]
-        bb = np.concatenate(boxes, 0) if boxes else np.zeros((0, 4), np.int32)
-        n = bb.shape[0]
-        kp = np.empty((n, self.num_keypoints, 3), np.float32)
-        idx = np.empty((n, self.num_keypoints), np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-                _lib.check_value(_lib.lib().vpb_infer_frames_yuv_host(
-                    self._handle, arr, len(arr), *fmt, bb[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p),
-                    idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        if not counts:
-            return [], []
-        split = np.cumsum(counts)[:-1]
-        return np.split(kp, split), np.split(idx, split)
+        return self._frames_call("vpb_infer_frames_yuv_host", _yuv_format(layout, matrix, full_range), frames, bboxes, host=True,
+                                 rotate=rotate, struct=_lib.VpbFrameYuv, layout=layout)
 
     def submit_frames_yuv_host(self, frames, bboxes, kpts_out: np.ndarray, idx_out: np.ndarray, slot: int, layout: str = "i420",
                                matrix: str = "bt601", full_range: bool = False, rotate=0) -> None:
@@ -1373,76 +1235,29 @@ class ViTPose:
         pitch).  Frames, boxes (int32 [n_j,4], already rounded) and outputs must stay alive and unmodified until the wait."""
         self._ensure()
         fmt = _yuv_format(layout, matrix, full_range)
-        if len(frames) != len(bboxes):
-            raise ValueError(f"{len(frames)} frames but {len(bboxes)} box arrays")
-        rot = _rotations(rotate, len(frames))
-        for j, b in enumerate(bboxes):
-            if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
-                raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
-        planes, table = self._yuv_host_table(frames, layout, copy=False)
-        bb = np.ascontiguousarray(np.concatenate(bboxes, 0) if len(bboxes) else np.zeros((0, 4), np.int32))
-        n = bb.shape[0]
-        if kpts_out.dtype != np.float32 or idx_out.dtype != np.int32 or kpts_out.shape != (n, self.num_keypoints, 3) \
-                or idx_out.shape != (n, self.num_keypoints) or not (kpts_out.flags.c_contiguous and idx_out.flags.c_contiguous):
-            raise ValueError("submit_frames_yuv_host: outputs must be C-contiguous float32 [n,K,3] and int32 [n,K]")
-        arr = (_lib.VpbFrameYuv * len(table))(*[_lib.VpbFrameYuv(*t, len(b), r) for t, b, r in zip(table, bboxes, rot)])
-        with torch.cuda.device(self._device):
-            _lib.check_value(_lib.lib().vpb_submit_frames_yuv_host(
-                self._handle, arr, len(arr), *fmt, bb.ctypes.data_as(C.c_void_p), kpts_out.ctypes.data_as(C.c_void_p),
-                idx_out.ctypes.data_as(C.c_void_p), int(slot)))
+
+        def table():
+            for j, b in enumerate(bboxes):
+                if b.dtype != np.int32 or b.ndim != 2 or b.shape[1] != 4:
+                    raise TypeError(f"boxes of frame {j}: int32 [n,4] expected")
+            return self._yuv_host_table(frames, layout, copy=False)
+        self._submit_frames("vpb_submit_frames_yuv_host", fmt, frames, bboxes, table, kpts_out, idx_out, slot, rotate,
+                            _lib.VpbFrameYuv)
 
     def infer_affine_yuv(self, frames, mats, centers, scales, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
                          check: bool = False, rotate=0):
         """infer_affine on YUV frames (vpb_infer_affine_yuv): the warp reads the planes and converts each tap."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if not (len(frames) == len(mats) == len(centers) == len(scales)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._yuv_device_table(frames, layout)
-        dev = torch.device("cuda", self._device)
-        counts, M, CS = self._affine_args(mats, centers, scales)
-        M, CS = M.to(dev), CS.to(dev)
-        n = M.shape[0]
-        kp = torch.empty((n, self.num_keypoints, 3), dtype=torch.float32, device=dev)
-        idx = torch.empty((n, self.num_keypoints), dtype=torch.int32, device=dev)
-        s = 0
-        for chunk in plan_frame_chunks(counts, self.batch_limit):
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-            self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_yuv(
-                self._handle, arr, len(arr), *fmt, C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
-                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 2:
-            raise ValueError("a matrix entry is not finite or a scale is <= 0")
-        return (list(kp.split(counts)), list(idx.split(counts))) if counts else ([], [])
+        return self._frames_call("vpb_infer_affine_yuv", _yuv_format(layout, matrix, full_range), frames,
+                                 affine=(mats, centers, scales), host=False, rotate=rotate, check=check, status=2,
+                                 message=_BAD_AFFINE, struct=_lib.VpbFrameYuv, layout=layout)
 
     def infer_affine_yuv_host(self, frames, mats, centers, scales, layout: str = "i420", matrix: str = "bt601",
                               full_range: bool = False, rotate=0):
         """HOST form of infer_affine_yuv (vpb_infer_affine_yuv_host, synchronous), checked as infer_affine_host."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if not (len(frames) == len(mats) == len(centers) == len(scales)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, table = self._yuv_host_table(frames, layout)
-        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
-        M, CS = np.ascontiguousarray(M.cpu().numpy()), np.ascontiguousarray(CS.cpu().numpy(), np.float32)
-        n = M.shape[0]
-        kp = np.empty((n, self.num_keypoints, 3), np.float32)
-        idx = np.empty((n, self.num_keypoints), np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in plan_frame_chunks(counts, self.batch_limit):
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-                _lib.check_value(_lib.lib().vpb_infer_affine_yuv_host(
-                    self._handle, arr, len(arr), *fmt, M[s:].ctypes.data_as(C.c_void_p), CS[s:].ctypes.data_as(C.c_void_p),
-                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        if not counts:
-            return [], []
-        split = np.cumsum(counts)[:-1]
-        return np.split(kp, split), np.split(idx, split)
+        return self._frames_call("vpb_infer_affine_yuv_host", _yuv_format(layout, matrix, full_range), frames,
+                                 affine=(mats, centers, scales), host=True, rotate=rotate, struct=_lib.VpbFrameYuv, layout=layout)
 
     # ---------------------------------------------------------------------------------------- several heads (datasets)
     @staticmethod
@@ -1492,78 +1307,14 @@ class ViTPose:
         boxes and 64 entries.  Returns per frame kpts f32 [n_j,K_max,3] (y, x, score) in that frame's pixels and idx i32
         [n_j,K_max], rows K_j.. of a head-j box zero."""
         self._ensure()
-        if not (len(frames) == len(bboxes) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
-        dev = torch.device("cuda", self._device)
-        boxes = []
-        for b in bboxes:
-            b = torch.as_tensor(b)
-            if b.is_floating_point():
-                b = b.round()
-            boxes.append(b.to(device=dev, dtype=torch.int32).reshape(-1, 4))
-        ents, _, chunks = plan_head_calls([b.shape[0] for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        n = sum(len(sel) for _, sel, _ in ents)
-        bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
-        Km = self.num_keypoints_max
-        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
-        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
-        table = [(frames[j].data_ptr(), frames[j].shape[0], frames[j].shape[1], frames[j].stride(0)) for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        for chunk in chunks:
-            arr = _frame_array(table, chunk, rot=rot)
-            ha = np.ascontiguousarray(hv[:len(arr)])
-            self._call_on_stream(frames + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads(
-                self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), C.c_void_p(bb[s:].data_ptr()),
-                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 1:
-            raise ValueError("a box is empty after padding and clipping to its frame")
-        return self._per_frame(ents, [b.shape[0] for b in boxes], kp, idx)
-
-    @staticmethod
-    def _per_frame(ents, counts, kp, idx):
-        outs_k = [kp.new_zeros((c,) + tuple(kp.shape[1:])) for c in counts]
-        outs_i = [idx.new_zeros((c,) + tuple(idx.shape[1:])) for c in counts]
-        s = 0
-        for j, sel, _ in ents:
-            outs_k[j][sel] = kp[s:s + len(sel)]
-            outs_i[j][sel] = idx[s:s + len(sel)]
-            s += len(sel)
-        return outs_k, outs_i
+        return self._frames_call("vpb_infer_frames_heads", (), frames, bboxes, heads=heads, host=False, rotate=rotate, check=check,
+                                 status=1, message=_EMPTY_BOX)
 
     def infer_frames_heads_host(self, frames, bboxes, heads, rotate=0):
         """HOST form of infer_frames_heads (vpb_infer_frames_heads_host, synchronous): numpy frames, per-frame boxes and
         head indices -> (list of kpts [n_j,K_max,3], list of idx [n_j,K_max]) numpy arrays.  An empty box raises ValueError."""
         self._ensure()
-        if not (len(frames) == len(bboxes) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
-        boxes = [self._round_boxes(b) for b in bboxes]
-        ents, _, chunks = plan_head_calls([len(b) for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        n = sum(len(sel) for _, sel, _ in ents)
-        bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
-        Km = self.num_keypoints_max
-        kp = np.zeros((n, Km, 3), np.float32)
-        idx = np.zeros((n, Km), np.int32)
-        table = [(frames[j].ctypes.data, frames[j].shape[0], frames[j].shape[1], frames[j].strides[0]) for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in chunks:
-                arr = _frame_array(table, chunk, rot=rot)
-                ha = np.ascontiguousarray(hv[:len(arr)])
-                _lib.check_value(_lib.lib().vpb_infer_frames_heads_host(
-                    self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), bb[s:].ctypes.data_as(C.c_void_p),
-                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        k_t, i_t = self._per_frame(ents, [len(b) for b in boxes], torch.from_numpy(kp), torch.from_numpy(idx))
-        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+        return self._frames_call("vpb_infer_frames_heads_host", (), frames, bboxes, heads=heads, host=True, rotate=rotate)
 
     def infer_affine_heads(self, frames, mats, centers, scales, heads, check: bool = False, rotate=0):
         """infer_affine with a keypoint head per box (heads: per frame an int array [n_j]): the boxes are grouped by head (stable;
@@ -1572,199 +1323,47 @@ class ViTPose:
         use_udp=True) call.  Returns per frame kpts f32 [n_j,K_max,3] (y, x, score) and idx i32 [n_j,K_max], rows K_j.. of a
         head-j box zero.  Honours the flip test set by set_flip_test_heads."""
         self._ensure()
-        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
-                             f"arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._device_frame(j, f) for j, f in enumerate(frames)]
-        dev = torch.device("cuda", self._device)
-        counts, M, CS = self._affine_args(mats, centers, scales)
-        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        o = torch.as_tensor(order, device=M.device)
-        M, CS = M.index_select(0, o).contiguous().to(dev), CS.index_select(0, o).contiguous().to(dev)
-        n = M.shape[0]
-        Km = self.num_keypoints_max
-        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
-        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
-        table = [(frames[j].data_ptr(), frames[j].shape[0], frames[j].shape[1], frames[j].stride(0)) for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        for chunk in chunks:
-            arr = _frame_array(table, chunk, rot=rot)
-            ha = np.ascontiguousarray(hv[:len(arr)])
-            self._call_on_stream(frames + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_heads(
-                self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), C.c_void_p(M[s:].data_ptr()), C.c_void_p(CS[s:].data_ptr()),
-                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 2:
-            raise ValueError("a matrix entry is not finite or a scale is <= 0")
-        return self._per_frame(ents, counts, kp, idx)
+        return self._frames_call("vpb_infer_affine_heads", (), frames, affine=(mats, centers, scales), heads=heads, host=False,
+                                 rotate=rotate, check=check, status=2, message=_BAD_AFFINE)
 
     def infer_affine_heads_host(self, frames, mats, centers, scales, heads, rotate=0):
         """HOST form of infer_affine_heads (vpb_infer_affine_heads_host, synchronous): numpy frames and per-frame matrices /
         centres / scales / head indices -> (list of kpts [n_j,K_max,3], list of idx [n_j,K_max]) numpy arrays.  A non-finite
         matrix entry or a scale <= 0 raises ValueError."""
         self._ensure()
-        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
-                             f"arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        frames = [self._host_frame(j, f) for j, f in enumerate(frames)]
-        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
-        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        M = np.ascontiguousarray(M.cpu().numpy()[order])
-        CS = np.ascontiguousarray(CS.cpu().numpy()[order], np.float32)
-        n = M.shape[0]
-        Km = self.num_keypoints_max
-        kp = np.zeros((n, Km, 3), np.float32)
-        idx = np.zeros((n, Km), np.int32)
-        table = [(frames[j].ctypes.data, frames[j].shape[0], frames[j].shape[1], frames[j].strides[0]) for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in chunks:
-                arr = _frame_array(table, chunk, rot=rot)
-                ha = np.ascontiguousarray(hv[:len(arr)])
-                _lib.check_value(_lib.lib().vpb_infer_affine_heads_host(
-                    self._handle, arr, len(arr), ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),
-                    CS[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p),
-                    self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        k_t, i_t = self._per_frame(ents, counts, torch.from_numpy(kp), torch.from_numpy(idx))
-        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+        return self._frames_call("vpb_infer_affine_heads_host", (), frames, affine=(mats, centers, scales), heads=heads, host=True,
+                                 rotate=rotate)
 
     # the multi-head calls on YUV frames: frames as the _yuv calls take them, everything else as their RGB twins above
     def infer_frames_heads_yuv(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False,
                                check: bool = False, rotate=0):
         """infer_frames_heads on YUV frames (vpb_infer_frames_heads_yuv)."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if not (len(frames) == len(bboxes) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, ytab = self._yuv_device_table(frames, layout)
-        dev = torch.device("cuda", self._device)
-        boxes = self._device_boxes(bboxes)
-        ents, _, chunks = plan_head_calls([b.shape[0] for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        n = sum(len(sel) for _, sel, _ in ents)
-        bb = torch.cat([boxes[j][torch.as_tensor(sel, device=dev)] for j, sel, _ in ents]) if ents else torch.zeros((0, 4), dtype=torch.int32, device=dev)
-        Km = self.num_keypoints_max
-        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
-        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
-        table = [ytab[j] for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        for chunk in chunks:
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-            ha = np.ascontiguousarray(hv[:len(arr)])
-            self._call_on_stream(planes + [bb, kp, idx], lambda st: _lib.lib().vpb_infer_frames_heads_yuv(
-                self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), C.c_void_p(bb[s:].data_ptr()),
-                C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 1:
-            raise ValueError("a box is empty after padding and clipping to its frame")
-        return self._per_frame(ents, [b.shape[0] for b in boxes], kp, idx)
+        return self._frames_call("vpb_infer_frames_heads_yuv", _yuv_format(layout, matrix, full_range), frames, bboxes, heads=heads,
+                                 host=False, rotate=rotate, check=check, status=1, message=_EMPTY_BOX, struct=_lib.VpbFrameYuv,
+                                 layout=layout)
 
     def infer_frames_heads_yuv_host(self, frames, bboxes, heads, layout: str = "i420", matrix: str = "bt601", full_range: bool = False, rotate=0):
         """HOST form of infer_frames_heads_yuv (vpb_infer_frames_heads_yuv_host, synchronous)."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if not (len(frames) == len(bboxes) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(bboxes)} box arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, ytab = self._yuv_host_table(frames, layout)
-        boxes = [self._round_boxes(b) for b in bboxes]
-        ents, _, chunks = plan_head_calls([len(b) for b in boxes], heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        n = sum(len(sel) for _, sel, _ in ents)
-        bb = np.ascontiguousarray(np.concatenate([boxes[j][sel] for j, sel, _ in ents], 0) if ents else np.zeros((0, 4), np.int32))
-        Km = self.num_keypoints_max
-        kp = np.zeros((n, Km, 3), np.float32)
-        idx = np.zeros((n, Km), np.int32)
-        table = [ytab[j] for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in chunks:
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-                ha = np.ascontiguousarray(hv[:len(arr)])
-                _lib.check_value(_lib.lib().vpb_infer_frames_heads_yuv_host(
-                    self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), bb[s:].ctypes.data_as(C.c_void_p),
-                    kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p), self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        k_t, i_t = self._per_frame(ents, [len(b) for b in boxes], torch.from_numpy(kp), torch.from_numpy(idx))
-        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+        return self._frames_call("vpb_infer_frames_heads_yuv_host", _yuv_format(layout, matrix, full_range), frames, bboxes, heads=heads,
+                                 host=True, rotate=rotate, struct=_lib.VpbFrameYuv, layout=layout)
 
     def infer_affine_heads_yuv(self, frames, mats, centers, scales, heads, layout: str = "i420", matrix: str = "bt601",
                                full_range: bool = False, check: bool = False, rotate=0):
         """infer_affine_heads on YUV frames (vpb_infer_affine_heads_yuv)."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
-                             f"arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, ytab = self._yuv_device_table(frames, layout)
-        dev = torch.device("cuda", self._device)
-        counts, M, CS = self._affine_args(mats, centers, scales)
-        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        o = torch.as_tensor(order, device=M.device)
-        M, CS = M.index_select(0, o).contiguous().to(dev), CS.index_select(0, o).contiguous().to(dev)
-        n = M.shape[0]
-        Km = self.num_keypoints_max
-        kp = torch.zeros((n, Km, 3), dtype=torch.float32, device=dev)
-        idx = torch.zeros((n, Km), dtype=torch.int32, device=dev)
-        table = [ytab[j] for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        for chunk in chunks:
-            arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-            ha = np.ascontiguousarray(hv[:len(arr)])
-            self._call_on_stream(planes + [M, CS, kp, idx], lambda st: _lib.lib().vpb_infer_affine_heads_yuv(
-                self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), C.c_void_p(M[s:].data_ptr()),
-                C.c_void_p(CS[s:].data_ptr()), C.c_void_p(kp[s:].data_ptr()), C.c_void_p(idx[s:].data_ptr()), st))
-            s += sum(e - b for _, b, e in chunk)
-        if check and n and self.frame_status() & 2:
-            raise ValueError("a matrix entry is not finite or a scale is <= 0")
-        return self._per_frame(ents, counts, kp, idx)
+        return self._frames_call("vpb_infer_affine_heads_yuv", _yuv_format(layout, matrix, full_range), frames,
+                                 affine=(mats, centers, scales), heads=heads, host=False, rotate=rotate, check=check, status=2,
+                                 message=_BAD_AFFINE, struct=_lib.VpbFrameYuv, layout=layout)
 
     def infer_affine_heads_yuv_host(self, frames, mats, centers, scales, heads, layout: str = "i420", matrix: str = "bt601",
                                     full_range: bool = False, rotate=0):
         """HOST form of infer_affine_heads_yuv (vpb_infer_affine_heads_yuv_host, synchronous)."""
         self._ensure()
-        fmt = _yuv_format(layout, matrix, full_range)
-        if not (len(frames) == len(mats) == len(centers) == len(scales) == len(heads)):
-            raise ValueError(f"{len(frames)} frames, {len(mats)} matrix arrays, {len(centers)} centre arrays, {len(scales)} scale "
-                             f"arrays, {len(heads)} head arrays")
-        rot = _rotations(rotate, len(frames))
-        planes, ytab = self._yuv_host_table(frames, layout)
-        counts, M, CS = self._affine_args(mats, centers, scales, validate=False)   # the engine checks host values
-        ents, order, chunks = plan_head_calls(counts, heads, len(self.head_keypoints), self.batch_limit)
-        rot = [rot[j] for j, _, _ in ents]                  # one rotation per entry: its frame's
-        M = np.ascontiguousarray(M.cpu().numpy()[order])
-        CS = np.ascontiguousarray(CS.cpu().numpy()[order], np.float32)
-        n = M.shape[0]
-        Km = self.num_keypoints_max
-        kp = np.zeros((n, Km, 3), np.float32)
-        idx = np.zeros((n, Km), np.int32)
-        table = [ytab[j] for j, _, _ in ents]
-        hv = np.array([k for _, _, k in ents], np.int32)
-        s = 0
-        with torch.cuda.device(self._device):
-            for chunk in chunks:
-                arr = _frame_array(table, chunk, _lib.VpbFrameYuv, rot)
-                ha = np.ascontiguousarray(hv[:len(arr)])
-                _lib.check_value(_lib.lib().vpb_infer_affine_heads_yuv_host(
-                    self._handle, arr, len(arr), *fmt, ha.ctypes.data_as(C.c_void_p), M[s:].ctypes.data_as(C.c_void_p),
-                    CS[s:].ctypes.data_as(C.c_void_p), kp[s:].ctypes.data_as(C.c_void_p), idx[s:].ctypes.data_as(C.c_void_p),
-                    self._stream()))
-                s += sum(e - b for _, b, e in chunk)
-        k_t, i_t = self._per_frame(ents, counts, torch.from_numpy(kp), torch.from_numpy(idx))
-        return [k.numpy() for k in k_t], [i.numpy() for i in i_t]
+        return self._frames_call("vpb_infer_affine_heads_yuv_host", _yuv_format(layout, matrix, full_range), frames,
+                                 affine=(mats, centers, scales), heads=heads, host=True, rotate=rotate, struct=_lib.VpbFrameYuv,
+                                 layout=layout)
 
     def wait_host(self, slot: int) -> None:
         _lib.check(_lib.lib().vpb_wait_host(self._handle, int(slot)))
