@@ -162,6 +162,7 @@ EXPORTS = {
                            C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "vpb_debug_gemm": (C.c_int, [C.c_int32, C.c_void_p]),
     "vpb_attention": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vpb_qkv_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vpb_debug_attention": (C.c_int, [C.c_int32]),
     "vpb_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p]),
     "vpb_draw_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),

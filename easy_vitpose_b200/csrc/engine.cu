@@ -1207,7 +1207,7 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Seg
     e->prof.begin(KC_GEMM_QKV, st);
     if (fused) {                                        // qkv + attention: the profile's gemm_qkv then includes the attention
       QkvAttnParams qp;
-      qp.batch = B; qp.heads = e->heads; qp.dim = D; qp.bias = b.qkv.b; qp.out = e->attn;
+      qp.batch = B; qp.heads = e->heads; qp.dim = D; qp.bias = b.qkv.b; qp.out = e->attn; qp.dbg = nullptr;
       VPB_TRY(qkv_attention_launch(D / e->heads, e->m_xn_att, b.m_qkv_head, qp, st));
     } else {
       int bn;
@@ -3124,6 +3124,21 @@ extern "C" int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, in
   AttnParams ap;
   ap.batch = batch; ap.heads = heads; ap.dim = D; ap.out = reinterpret_cast<__nv_bfloat16*>(d_out); ap.dbg = g_dbg_buf;
   return attention_launch(head_dim, tm, tt, ap, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_qkv_attention(const void* d_xn, const void* d_w, const float* d_bias, int32_t batch, int32_t heads, int32_t head_dim,
+                                 void* d_out, void* stream) {
+  int dev = 0;
+  CU_TRY(cudaGetDevice(&dev));
+  VPB_TRY(device_check(dev));
+  const int D = heads * head_dim;
+  if (!d_xn || !d_w || !d_bias || !d_out || batch < 1 || heads < 1 || D % 64 != 0) return fail(VPB_ERR_ARG, "vpb_qkv_attention: bad argument");
+  CUtensorMap tx, tw;
+  VPB_TRY(make_map(&tx, d_xn, static_cast<uint64_t>(batch) * 192, D, D, 192));
+  VPB_TRY(make_map(&tw, d_w, 3 * static_cast<uint64_t>(D), D, D, head_dim));
+  QkvAttnParams qp;
+  qp.batch = batch; qp.heads = heads; qp.dim = D; qp.bias = d_bias; qp.out = reinterpret_cast<__nv_bfloat16*>(d_out); qp.dbg = g_dbg_buf;
+  return qkv_attention_launch(head_dim, tx, tw, qp, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vpb_layernorm(const float* d_x, const float* d_gamma, const float* d_beta, void* d_y, int32_t rows, int32_t dim, float eps,

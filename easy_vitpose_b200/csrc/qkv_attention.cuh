@@ -44,6 +44,9 @@ struct QkvAttnParams {
   int dim;                // D = heads * head_dim = K of the GEMM (a multiple of 64)
   const float* bias;      // packed qkv bias [3D] (q rows carry head_dim^-0.5 like the weight)
   __nv_bfloat16* out;     // [batch*192, D]
+  long long* dbg;         // debug: per CTA [8], zeroed by the caller, or nullptr.  Cycles of thread 0: 0 GEMM phase, 1 of which
+                          // waiting on the ring's full barriers, 2 hand-off (both CTA barriers), 3..6 the phases of attend_item
+                          // (attention.cuh); 7 items of this CTA
 };
 
 // Producer side (thread 0): load the next `count` k-blocks of the CTA's sequence (item ld_item from k-block ld_kb on, items
@@ -84,6 +87,7 @@ qkv_attention_wgmma(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
   const int lane = threadIdx.x & 31, wq = tid >> 5;
   const int items = p.batch * p.heads;
   const int num_kb = p.dim / GEMM_BK;
+  PhaseClock clk(p.dbg ? p.dbg + blockIdx.x * 8 : nullptr);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_x);
@@ -119,7 +123,9 @@ qkv_attention_wgmma(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
     for (int i = 0; i < Cfg::N / 2; ++i) acc[i] = 0.0f;
     int prev = -1;
     for (int kb = 0; kb < num_kb; ++kb) {
+      const long long w0 = p.dbg ? clock64() : 0;
       mbar_wait(&full[rp.stage], rp.phase);
+      if (p.dbg && threadIdx.x == 0) p.dbg[blockIdx.x * 8 + 1] += clock64() - w0;
       const uint32_t sa = smem_u32(ring + rp.stage * Cfg::STAGE_BYTES) + wg * 64 * 128;
       const uint32_t sb = smem_u32(ring + rp.stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
       const uint64_t ad = wgmma_desc<128>(sa), bd = wgmma_desc<128>(sb);
@@ -139,6 +145,7 @@ qkv_attention_wgmma(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (lane == 0) mbar_arrive(&empty[prev]);
+    clk.mark(0);
 
     // every warpgroup is done with the previous item's Q, K, V and with this item's last ring slot
     __syncthreads();
@@ -169,10 +176,12 @@ qkv_attention_wgmma(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
     }
     fence_proxy_async_smem();                                 // the stores -> visible to wgmma's operand reads
     __syncthreads();
+    clk.mark(2);
 
     // ---- attention over the item's Q, K, V; the barrier above the next hand-off keeps them until every warpgroup is done
-    attend_item<HD, NPOLY>(sQ, sK, sV, p.out, p.dim, b, h, wg, lane, wq, [] {});
+    attend_item<HD, NPOLY>(sQ, sK, sV, p.out, p.dim, b, h, wg, lane, wq, clk, [] {});
   }
+  if (p.dbg && threadIdx.x == 0) p.dbg[blockIdx.x * 8 + 7] = (items - 1 - blockIdx.x) / gridDim.x + 1;
 }
 
 }  // namespace vpb

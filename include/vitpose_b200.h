@@ -651,6 +651,11 @@ int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, void* d_out,
 /* Debug: limit the GEMM smem ring depth and/or collect per-CTA cycle counters (int64 [grid*8]) for following GEMM launches. */
 int vpb_debug_gemm(int32_t stages_limit, void* d_counters);
 int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream);
+/* qkv GEMM + attention in one launch: out = attention(xn[batch*192, D] * W[3D, D]^T + bias[3D]), D = heads * head_dim a multiple
+ * of 64; bit-identical to vpb_gemm (epilogue 0) followed by vpb_attention.  Both attention entry points fill vpb_debug_gemm's
+ * counters when they are set. */
+int vpb_qkv_attention(const void* d_xn, const void* d_w, const float* d_bias, int32_t batch, int32_t heads, int32_t head_dim,
+                      void* d_out, void* stream);
 /* Debug / measurement switch (process-wide) for the attention kernel.  flags < 0: the defaults (every softmax exponential on
  * the MUFU; VPB_ATT_POLY = 1 in the environment evaluates every 4th one by a polynomial on the FMA pipe instead); otherwise
  * bit 0 = polynomial exponentials, bit 1 = run every block's qkv GEMM and attention as one fused launch, bit 2 = as two launches
