@@ -114,6 +114,14 @@ static long long* g_dbg_buf = nullptr;
 // of vpb_debug_gemm force one form for every following launch (kernel-level tests).
 constexpr int kResidRmwDefault = 0;
 constexpr int kLnCtlDefault = 1;      // bit-identical either way (tests/test_gpu_engine.py)
+// Largest L2 access-policy window (and persisting set-aside) over the fp32 token stream x.  The H100 lets 32 MB of its 50 MB L2
+// persist; with all of it held for x, the LayerNorms' bf16 outputs and the GEMMs' operands and outputs share the 18 MB left.  A
+// 24 MB window keeps most of x resident and leaves them 26 MB.  bench.py on an H100 80GB HBM3 (700 W power limit), ms per step,
+// window of 32 MB (the device limit) / 28 / 24 / 20 / 16 MB: b17x64 5.32 / 5.15 / 5.09-5.12 / 5.13 / 5.16; l25x64 16.30 / - /
+// 15.44 / 15.53; h133x32 18.16 / - / 16.41 / 16.45; ap10k-streams (x is 18.9 MB, under the cap) 17.80 / - / 17.78 / 17.76.
+// At b17x64 the LayerNorms went from 0.72 to 0.58 ms per step and fc1 from 1.50 to 1.29; qkv, proj and fc2 gave back 0.07.
+// Where the window lies changes no result.
+constexpr size_t kL2PersistMax = size_t(24) << 20;
 static int resid_rmw_default() {
   static const int v = [] { const char* s = getenv("VPB_RESID_RMW"); return s ? (s[0] != '0') : kResidRmwDefault; }();
   return v;
@@ -465,6 +473,7 @@ struct vpb_engine {
   // LayerNorm, but the per-layer working set (~220 MB) would evict it from the 50 MB L2 in between; an access-policy window
   // (clipped to what the device allows to persist) marks it persisting on every stream the engine launches on.  Measured on an
   // H100 80GB HBM3 (700 W power limit), ViT-B, 64 crops: 9.39 ms per call with the window, 10.52 without (tools/defaults_ab.py).
+  // The window and the persisting set-aside are also capped at kL2PersistMax (see there).
   bool l2_persist = true;
   size_t l2_window_bytes = 0;
   std::vector<cudaStream_t> l2_streams;
@@ -874,6 +883,7 @@ extern "C" int vpb_finalize(vpb_engine* e) {
     size_t want = M * D * sizeof(float);
     if (want > static_cast<size_t>(prop.accessPolicyMaxWindowSize)) want = prop.accessPolicyMaxWindowSize;
     if (want > static_cast<size_t>(prop.persistingL2CacheMaxSize)) want = prop.persistingL2CacheMaxSize;
+    if (want > kL2PersistMax) want = kL2PersistMax;
     if (e->l2_persist && want > 0) {
       CU_TRY(cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want));
       e->l2_window_bytes = want;
