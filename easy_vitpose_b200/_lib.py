@@ -161,6 +161,8 @@ EXPORTS = {
     "vpb_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                            C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "vpb_debug_gemm": (C.c_int, [C.c_int32, C.c_void_p]),
+    "vpb_expert_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                  C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "vpb_attention": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vpb_qkv_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vpb_debug_attention": (C.c_int, [C.c_int32]),

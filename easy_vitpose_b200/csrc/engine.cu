@@ -728,6 +728,18 @@ static int pack_linear(vpb_engine* e, LinearW& L, const std::string& wkey, const
   return VPB_OK;
 }
 
+// The shared rows [0, S) of a stacked fc2 as a linear of S outputs (BlockW::fc2s).  A width serves when it divides S rounded up
+// to 128: the W maps hold S rows, so TMA zero-fills the rows of the last column tile past S, and the output map bounds the
+// stores to the S columns.
+static int make_shared_maps(LinearW& Ls, __nv_bfloat16* w, float* b, int S, int K) {
+  Ls.w = w; Ls.b = b; Ls.n = S; Ls.k = K;
+  for (int i = 0; i < 3; ++i) {
+    Ls.has[i] = (cdiv(S, 128) * 128) % kTileWidths[i] == 0;
+    if (Ls.has[i]) VPB_TRY(make_map(&Ls.tmap[i], w, S, K, K, kTileWidths[i]));
+  }
+  return VPB_OK;
+}
+
 // ViTPose+ fc2 with experts: W / bias stacked [shared; expert 0; ...; expert H-1] (see BlockW).  The first D rows are the fc2
 // that model_split.py gives head 0 (torch.cat([fc2, experts.0]), :56), packed exactly as pack_linear packs it.
 static int pack_fc2_experts(vpb_engine* e, BlockW& b, const std::string& p) {
@@ -747,12 +759,7 @@ static int pack_fc2_experts(vpb_engine* e, BlockW& b, const std::string& p) {
   for (int j = 0; j < e->num_kheads; ++j) VPB_TRY(put(p + "mlp.experts." + std::to_string(j), S + j * P, P));
   VPB_TRY(make_tile_maps(L, L.w, D, K));
   VPB_TRY(make_map(&L.map_c, L.w, D, K, K, e->chain_bn));
-  LinearW& Ls = b.fc2s;
-  Ls.w = L.w; Ls.b = L.b; Ls.n = S; Ls.k = K;
-  for (int i = 0; i < 3; ++i) {
-    Ls.has[i] = (cdiv(S, 128) * 128) % kTileWidths[i] == 0;
-    if (Ls.has[i]) VPB_TRY(make_map(&Ls.tmap[i], L.w, S, K, K, kTileWidths[i]));
-  }
+  VPB_TRY(make_shared_maps(b.fc2s, L.w, L.b, S, K));
   return make_map(&b.m_exp, L.w, rows, K, K, e->expert_bn);
 }
 
@@ -915,6 +922,8 @@ static int layernorm(const float* x, const float* g, const float* b, __nv_bfloat
 }
 
 extern "C" int vpb_debug_gemm(int32_t stages_limit, void* d_counters) {   // counters: int64 [grid*8], see GemmParams::dbg
+  // one stage cannot serve two k-blocks: a slot is released only once the MMAs of the next k-block have been issued
+  if ((stages_limit & 0xff) == 1) return fail(VPB_ERR_ARG, "vpb_debug_gemm: a ring of 1 stage (0 = the compiled depth, else >= 2)");
   g_dbg_flags = stages_limit >> 8;       // bits 8.. carry GemmParams::dbg_flags
   g_dbg_stages = stages_limit & 0xff;
   g_dbg_buf = reinterpret_cast<long long*>(d_counters);
@@ -1101,28 +1110,40 @@ static int pick_tile(const LinearW& L, int M, int* bn, const CUtensorMap** wm) {
 
 // fc2 of a multi-head call on an engine with experts: the shared columns [0, D-P) for all rows (the standalone GEMM, its
 // output map bounded to those columns), then the expert columns of every segment in one grouped launch (expert_gemm.cuh)
-static int fc2_experts(vpb_engine* e, const BlockW& b, int M, const std::vector<Segment>& segs, cudaStream_t st) {
-  const int D = e->D, P = e->P;
-  {
-    GemmParams p = gp(M, D - P, 4 * D, b.fc2s.b, e->x, D);
-    p.rmw = 0;                        // TMA reduce-add: the rmw epilogue bounds columns by ldc, not N (bit-identical either way)
-    int bn;
-    const CUtensorMap* wm;
-    VPB_TRY(pick_tile(b.fc2s, M, &bn, &wm));
-    e->prof.begin(KC_GEMM_FC2, st);
-    VPB_TRY(gemm_launch(bn, EPI_F32_ADD, e->m_hid, *wm, e->o_xs, p, st));
-    e->prof.end(st);
-  }
+// The shared columns: x[:, :S] += A Ws^T + bias over all M rows, `o_xs` = x [M, S] with the row pitch of x (D).
+static int fc2_shared_launch(const LinearW& Ls, int M, int D, float* x, const CUtensorMap& ta, const CUtensorMap& o_xs, cudaStream_t st) {
+  GemmParams p = gp(M, Ls.n, Ls.k, Ls.b, x, D);
+  p.rmw = 0;                          // TMA reduce-add: the rmw epilogue bounds columns by ldc, not N (bit-identical either way)
+  int bn;
+  const CUtensorMap* wm;
+  VPB_TRY(pick_tile(Ls, M, &bn, &wm));
+  return gemm_launch(bn, EPI_F32_ADD, ta, *wm, o_xs, p, st);
+}
+// The grouped expert launch's parameters without segments (add_expert_segment appends them): K = 4D, the P expert columns
+// [D-P, D) of x, W and bias stacked as [shared (D-P rows); expert 0 (P); ...].
+static ExpertParams expert_params(int D, int P, const float* bias, float* x) {
   ExpertParams q;
   memset(&q, 0, sizeof(q));
-  q.K = 4 * D; q.P = P; q.col0 = D - P; q.ldx = D; q.w_row0 = D - P; q.n_tiles = P / e->expert_bn;
-  q.bias = b.fc2.b; q.x = e->x;
+  q.K = 4 * D; q.P = P; q.col0 = D - P; q.ldx = D; q.w_row0 = D - P; q.n_tiles = P / expert_width(P);
+  q.bias = bias; q.x = x; q.stages = g_dbg_stages;
+  return q;
+}
+// rows [row_begin, row_end) use `expert`; first_tile = the prefix sum of the earlier segments' tile counts
+static void add_expert_segment(ExpertParams& q, int row_begin, int row_end, int expert) {
+  ExpertSegment& t = q.seg[q.num_segs++];
+  t.row_begin = row_begin; t.row_end = row_end; t.expert = expert; t.first_tile = q.num_tiles;
+  q.num_tiles += cdiv(row_end - row_begin, GEMM_BM) * q.n_tiles;
+}
+static int fc2_experts(vpb_engine* e, const BlockW& b, int M, const std::vector<Segment>& segs, cudaStream_t st) {
+  const int D = e->D, P = e->P;
+  e->prof.begin(KC_GEMM_FC2, st);
+  VPB_TRY(fc2_shared_launch(b.fc2s, M, D, e->x, e->m_hid, e->o_xs, st));
+  e->prof.end(st);
+  ExpertParams q = expert_params(D, P, b.fc2.b, e->x);
   int row = 0;
   for (const Segment& sg : segs) {
-    ExpertSegment& t = q.seg[q.num_segs++];
-    t.row_begin = row; t.row_end = row + sg.count * 192; t.expert = sg.head; t.first_tile = q.num_tiles;
-    q.num_tiles += cdiv(sg.count * 192, GEMM_BM) * q.n_tiles;
-    row = t.row_end;
+    add_expert_segment(q, row, row + sg.count * 192, sg.head);
+    row += sg.count * 192;
   }
   e->prof.begin(KC_GEMM_FC2, st);
   VPB_TRY(expert_launch(e->expert_bn, e->m_hid, b.m_exp, q, st));
@@ -3084,10 +3105,15 @@ extern "C" int vpb_read_buffer(vpb_engine* e, const char* name, void* host_dst, 
 extern "C" int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, void* d_out, int32_t m, int32_t n, int32_t k,
                         int32_t epilogue, const float* d_resid, int32_t resid_mod, int32_t aux0, int32_t aux1, int32_t aux2,
                         int32_t aux3, void* stream) {
+  if (!d_a || !d_w || !d_out) return fail(VPB_ERR_ARG, "vpb_gemm: null pointer");
+  if (m < 1 || n < 1) return fail(VPB_ERR_ARG, "vpb_gemm: M=%d N=%d must be positive", m, n);
+  if (!d_bias && epilogue != EPI_F32_NCHW) return fail(VPB_ERR_ARG, "vpb_gemm: epilogue %d reads a bias", epilogue);
+  if (epilogue == EPI_F32_NCHW && (aux0 < 1 || aux0 > n || aux1 < 1))
+    return fail(VPB_ERR_ARG, "vpb_gemm: NCHW epilogue with %d channels of %d, %d pixels", aux0, n, aux1);
+  if (epilogue == EPI_BF16_RELU_UP && (aux0 < 1 || aux1 < 1)) return fail(VPB_ERR_ARG, "vpb_gemm: deconv input %d x %d", aux0, aux1);
   int dev = 0;
   CU_TRY(cudaGetDevice(&dev));
   VPB_TRY(device_check(dev));
-  if (!d_a || !d_w || !d_out) return fail(VPB_ERR_ARG, "vpb_gemm: null pointer");
   int bn;
   CUtensorMap ta, tw, tout;
   if (epi_uses_tma(epilogue)) {                  // the engine's width rule and debug overrides (pick_tile)
@@ -3121,6 +3147,37 @@ extern "C" int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, v
   if (epilogue == EPI_F32_NCHW) { p.n_valid = aux0; p.pix = aux1; }
   if (epilogue == EPI_BF16_RELU_UP) { p.up_h = aux0; p.up_w = aux1; p.up_tr = aux2; p.up_tw = aux3 >> 16; p.up_c = aux3 & 0xffff; }
   return gemm_launch(bn, epilogue, ta, tw, tout, p, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vpb_expert_gemm(const void* d_a, const void* d_w, const float* d_bias, float* d_x, int32_t m, int32_t d, int32_t p,
+                               int32_t num_experts, const int32_t* h_segs, int32_t num_segs, int32_t shared, void* stream) {
+  if (!d_a || !d_w || !d_bias || !d_x || !h_segs) return fail(VPB_ERR_ARG, "vpb_expert_gemm: null pointer");
+  if (m < 1 || d < 64 || d % 32 != 0 || p < 32 || p >= d || p % 32 != 0 || num_experts < 1 || num_segs < 1 || num_segs > EXPERT_MAX_SEGMENTS)
+    return fail(VPB_ERR_ARG, "vpb_expert_gemm: M=%d D=%d P=%d experts=%d segments=%d", m, d, p, num_experts, num_segs);
+  ExpertParams q = expert_params(d, p, d_bias, d_x);
+  for (int i = 0, prev_end = 0; i < num_segs; ++i) {
+    const int32_t* sg = h_segs + 3 * i;
+    if (sg[0] < prev_end || sg[1] <= sg[0] || sg[1] > m || sg[2] < 0 || sg[2] >= num_experts)
+      return fail(VPB_ERR_ARG, "vpb_expert_gemm: segment %d = rows [%d, %d) expert %d", i, sg[0], sg[1], sg[2]);
+    add_expert_segment(q, sg[0], sg[1], sg[2]);
+    prev_end = sg[1];
+  }
+  int dev = 0;
+  CU_TRY(cudaGetDevice(&dev));
+  VPB_TRY(device_check(dev));
+  const int S = d - p, K = 4 * d;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUtensorMap ta, tw;
+  VPB_TRY(make_map(&ta, d_a, m, K, K, 128));
+  if (shared) {
+    LinearW Ls;
+    CUtensorMap o_xs;
+    VPB_TRY(make_shared_maps(Ls, static_cast<__nv_bfloat16*>(const_cast<void*>(d_w)), const_cast<float*>(d_bias), S, K));
+    VPB_TRY(make_map(&o_xs, d_x, m, S, d, 64, /*f32=*/true));
+    VPB_TRY(fc2_shared_launch(Ls, m, d, d_x, ta, o_xs, st));
+  }
+  VPB_TRY(make_map(&tw, d_w, S + static_cast<uint64_t>(num_experts) * p, K, K, expert_width(p)));
+  return expert_launch(expert_width(p), ta, tw, q, st);
 }
 
 extern "C" int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream) {

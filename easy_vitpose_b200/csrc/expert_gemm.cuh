@@ -35,6 +35,7 @@ struct ExpertParams {
   int n_tiles;              // column tiles per 128-row block: ceil(P / BN)
   int num_tiles;            // tiles of all segments
   int num_segs;             // 1 .. EXPERT_MAX_SEGMENTS
+  int stages;               // debug: use at most this many ring stages (0 = all), as GemmParams::stages_limit
   const float* bias;        // stacked fc2 bias [D - P + H * P]
   float* x;                 // fp32 residual stream [M, ldx]
   ExpertSegment seg[EXPERT_MAX_SEGMENTS];
@@ -86,6 +87,7 @@ gemm_expert_segments(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
   const int num_kb = p.K / GEMM_BK;
+  const int num_stages = (p.stages > 0 && p.stages < Cfg::STAGES) ? p.stages : Cfg::STAGES;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
@@ -118,7 +120,7 @@ gemm_expert_segments(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
           tma_load_2d(sa + Cfg::A_BYTES, &tmap_w, &full_bar[rp.stage], kb * GEMM_BK, wrow);
         }
         __syncwarp();
-        rp.next(Cfg::STAGES);
+        rp.next(num_stages);
       }
     }
   } else {
@@ -132,7 +134,7 @@ gemm_expert_segments(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
       const int t = tile - sg.first_tile;
       const int m0 = sg.row_begin + (t / p.n_tiles) * GEMM_BM;
       const int n0 = (t % p.n_tiles) * BN;
-      tile_mainloop<BN>(acc, ring, Cfg::STAGE_BYTES, full_bar, empty_bar, num_kb, Cfg::STAGES, rp, wg, lane, nullptr);
+      tile_mainloop<BN>(acc, ring, Cfg::STAGE_BYTES, full_bar, empty_bar, num_kb, num_stages, rp, wg, lane, nullptr);
       epilogue_expert<BN>(acc, n0, m0 + 64 * wg, sg.row_begin, sg.row_end, p, p.bias + p.w_row0 + sg.expert * p.P, tid);
     }
   }

@@ -648,8 +648,20 @@ int vpb_read_buffer(vpb_engine* e, const char* name, void* host_dst, int64_t byt
 int vpb_gemm(const void* d_a, const void* d_w, const float* d_bias, void* d_out, int32_t m, int32_t n, int32_t k,
              int32_t epilogue, const float* d_resid, int32_t resid_mod, int32_t aux0, int32_t aux1, int32_t aux2,
              int32_t aux3, void* stream);
-/* Debug: limit the GEMM smem ring depth and/or collect per-CTA cycle counters (int64 [grid*8]) for following GEMM launches. */
+/* Debug: limit the GEMM smem ring depth and/or collect per-CTA cycle counters (int64 [grid*8]) for following GEMM launches.
+ * Bits 0..7 = the ring depth (0 = the compiled depth; 1 returns VPB_ERR_ARG), bits 8.. = GemmParams::dbg_flags (csrc/gemm.cuh)
+ * and the engine's overrides of tile width and residual form.  The depth applies to vpb_gemm, vpb_expert_gemm and the engine's
+ * standalone and expert GEMM launches. */
 int vpb_debug_gemm(int32_t stages_limit, void* d_counters);
+/* The fc2 of a multi-head call on an engine with experts (ViTPose+), by the engine's own launch code: the grouped expert GEMM
+ * x[r, D-P + n] += A[r, :] * W[D-P + e*P + n, :]^T + bias[D-P + e*P + n] for every row r of a segment with expert e and n < P, and
+ * with shared != 0 first the shared columns x[:, :D-P] += A * W[:D-P]^T + bias[:D-P] over all M rows.  d_a bf16 [M, 4D]; d_w bf16
+ * [D-P + num_experts*P, 4D] and d_bias f32 [D-P + num_experts*P] stacked as [shared; expert 0; ...]; d_x f32 [M, D], updated in
+ * place.  h_segs i32 [num_segs, 3] (HOST): row_begin, row_end, expert; 1..128 segments in ascending, non-overlapping row order.
+ * VPB_ERR_ARG: D not a multiple of 32, P outside 32..D-32 or not a multiple of 32, a segment out of order, empty, past M or with
+ * an expert outside [0, num_experts).  Honours vpb_debug_gemm's ring depth. */
+int vpb_expert_gemm(const void* d_a, const void* d_w, const float* d_bias, float* d_x, int32_t m, int32_t d, int32_t p,
+                    int32_t num_experts, const int32_t* h_segs, int32_t num_segs, int32_t shared, void* stream);
 int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream);
 /* qkv GEMM + attention in one launch: out = attention(xn[batch*192, D] * W[3D, D]^T + bias[3D]), D = heads * head_dim a multiple
  * of 64; bit-identical to vpb_gemm (epilogue 0) followed by vpb_attention.  Both attention entry points fill vpb_debug_gemm's

@@ -147,6 +147,31 @@ def gelu_erf(z: torch.Tensor) -> torch.Tensor:
     return 0.5 * z * (1.0 + torch.erf(z / math.sqrt(2.0)))
 
 
+def gelu_bound(z: torch.Tensor, d_z: torch.Tensor):
+    """The fc1 epilogue on a pre-activation z known to within d_z: the exact erf GELU of z and the bound of the bf16 output."""
+    ref = gelu_erf(z)
+    delta = GELU_SLOPE * d_z + GELU_FIT + (TANH_APPROX + 8 * U) * 0.5 * (z.abs() + d_z)
+    return ref, bf16_bound(ref, delta)
+
+
+def residual(x: torch.Tensor, z: torch.Tensor, delta: torch.Tensor):
+    """The fp32 stream after x += z, z known to within delta: the sum and its bound (one more rounding of the sum)."""
+    ref = x.to(F64) + z
+    return ref, delta + U * ref.abs()
+
+
+def conv_transpose_bound(feat: torch.Tensor, w: torch.Tensor, shift: torch.Tensor, ms: torch.Tensor):
+    """relu(ConvTranspose2d(k4,s2,p1)(feat) + shift) of NHWC feat [B,H,W,Cin] and bf16 w [Cin,Cout,4,4] as one implicit GEMM of
+    K = 4 Cin, NHWC out, and its bound; |ms| = |mean * s| sizes the fp32 roundings of a folded BatchNorm's shift (0: none)."""
+    cin = w.shape[0]
+    a = feat.to(F64).permute(0, 3, 1, 2)
+    z = F.conv_transpose2d(a, w, stride=2, padding=1) + shift[None, :, None, None]
+    s = F.conv_transpose2d(a.abs(), w.abs(), stride=2, padding=1)
+    delta = 4 * cin * UACC * s + U * z.abs() + 2 * U * (shift.abs() + ms)[None, :, None, None]
+    ref = torch.relu(z)
+    return ref.permute(0, 2, 3, 1), bf16_bound(ref, delta).permute(0, 2, 3, 1)
+
+
 # ------------------------------------------------------------------------------------------------ stages
 def patch_rows(crops) -> torch.Tensor:
     """Stage 1: the bf16 im2col of the crops [B,3,256,192] -> [B*192, 768]; bit-exact, no bound."""
@@ -240,27 +265,20 @@ def attention(qkv_buf: torch.Tensor, heads: int):
 def proj(attn: torch.Tensor, x: torch.Tensor, sd: dict, i: int):
     """Stage 6: x += attn Wproj^T + b (fp32 stream, TMA reduce-add)."""
     w, b = linear_weights(sd, f"backbone.blocks.{i}.attn.proj", attn.device)
-    z, delta = _gemm(attn.to(F64), w, b)
-    ref = x.to(F64) + z
-    return ref, delta + U * ref.abs()
+    return residual(x, *_gemm(attn.to(F64), w, b))
 
 
 def fc1(xn: torch.Tensor, sd: dict, i: int):
     """Stage 7: hid = GELU(xn W1^T + b1) -> bf16 [M, 4D], against the exact erf GELU."""
     w, b = linear_weights(sd, f"backbone.blocks.{i}.mlp.fc1", xn.device)
-    z, d_z = _gemm(xn.to(F64), w, b)
-    ref = gelu_erf(z)
-    delta = GELU_SLOPE * d_z + GELU_FIT + (TANH_APPROX + 8 * U) * 0.5 * (z.abs() + d_z)
-    return ref, bf16_bound(ref, delta)
+    return gelu_bound(*_gemm(xn.to(F64), w, b))
 
 
 def fc2(hid: torch.Tensor, x: torch.Tensor, sd: dict, i: int):
     """Stage 8: x += hid W2^T + b2 (fp32 stream).  For an engine with experts pass the head's split state dict
     (split_vitpose_plus), whose fc2 holds the shared rows followed by the head's expert rows."""
     w, b = linear_weights(sd, f"backbone.blocks.{i}.mlp.fc2", hid.device)
-    z, delta = _gemm(hid.to(F64), w, b)
-    ref = x.to(F64) + z
-    return ref, delta + U * ref.abs()
+    return residual(x, *_gemm(hid.to(F64), w, b))
 
 
 def deconv(feat: torch.Tensor, sd: dict, layer: int, prefix: str = "keypoint_head."):
@@ -268,15 +286,9 @@ def deconv(feat: torch.Tensor, sd: dict, layer: int, prefix: str = "keypoint_hea
     and out: ConvTranspose2d(k4,s2,p1) with the BatchNorm folded, + shift, ReLU, -> bf16."""
     dev = feat.device
     w, shift, ms = deconv_weights(sd, prefix, layer, dev)
-    cin = w.shape[0]
     if layer == 0:
-        feat = feat.reshape(-1, 16, 12, cin)
-    a = feat.to(F64).permute(0, 3, 1, 2)
-    z = F.conv_transpose2d(a, w, stride=2, padding=1) + shift[None, :, None, None]
-    s = F.conv_transpose2d(a.abs(), w.abs(), stride=2, padding=1)
-    delta = 4 * cin * UACC * s + U * z.abs() + 2 * U * (shift.abs() + ms)[None, :, None, None]
-    ref = torch.relu(z)
-    return ref.permute(0, 2, 3, 1), bf16_bound(ref, delta).permute(0, 2, 3, 1)
+        feat = feat.reshape(-1, 16, 12, w.shape[0])
+    return conv_transpose_bound(feat, w, shift, ms)
 
 
 def final_layer(d2: torch.Tensor, sd: dict, prefix: str = "keypoint_head."):

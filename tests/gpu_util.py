@@ -6,6 +6,8 @@ import torch
 from easy_vitpose_b200 import _lib
 
 EPI_BF16, EPI_BF16_GELU, EPI_BF16_RELU_UP, EPI_F32_NCHW, EPI_F32_ADD, EPI_BF16_GELU_ERF = 0, 1, 2, 4, 5, 6
+BF16_SENTINEL = 0x7FC1                # a NaN: no GEMM of finite operands stores it
+F32_SENTINEL = -0.70710677            # any add of a value of 1e-7 or more changes its bits
 
 
 def ptr(t):
@@ -36,3 +38,24 @@ def layernorm(x, g, b, eps=1e-6):
     _lib.check(_lib.lib().vpb_layernorm(ptr(x), ptr(g), ptr(b), ptr(y), x.shape[0], x.shape[1], eps, stream()))
     torch.cuda.synchronize()
     return y
+
+
+def f32_bits(v):
+    return int(torch.tensor([v], dtype=torch.float32).view(torch.int32))
+
+
+def bits(t):
+    """the bit patterns of a bf16 or fp32 tensor"""
+    return t.view(torch.int16 if t.dtype == torch.bfloat16 else torch.int32)
+
+
+def sentinel_buffer(n, dtype):
+    """n elements of bf16 or fp32 holding the sentinel bits, and those bits"""
+    b = BF16_SENTINEL if dtype == torch.bfloat16 else f32_bits(F32_SENTINEL)
+    return torch.full((n,), b, dtype=torch.int16 if dtype == torch.bfloat16 else torch.int32, device="cuda").view(dtype), b
+
+
+def untouched(buf, start, stop, sentinel):
+    """buf[:start] and buf[stop:] still hold the sentinel bits"""
+    v = bits(buf)
+    return bool((v[:start] == sentinel).all()) and bool((v[stop:] == sentinel).all())

@@ -121,3 +121,46 @@ def test_decode_api_fails_loudly_without_cuda_and_checks_its_config():
         keypoints_from_heatmaps(hm[:, :15], c, s, use_udp=True, kernel=19, target_type="CombinedTarget")
     with pytest.raises(ValueError):
         keypoints_from_heatmaps(hm, c, s, post_process="fancy")
+
+
+def test_gemm_entry_points_reject_what_the_kernels_cannot_serve():
+    """vpb_gemm, vpb_expert_gemm and vpb_debug_gemm check their arguments before touching the device, so VPB_ERR_ARG (1)
+    comes back with or without a GPU.  The device pointers are misaligned dummies that no tensor map accepts."""
+    import ctypes as C
+
+    from easy_vitpose_b200 import _lib
+    L = _lib.lib()
+    p = C.c_void_p(8)
+    EPI_BF16, EPI_BF16_RELU_UP, EPI_F32_NCHW, EPI_F32_ADD = 0, 2, 4, 5
+
+    def gemm(m, n, k, epi, bias=p, aux=(0, 0, 0, 0)):
+        return L.vpb_gemm(p, p, bias, p, m, n, k, epi, None, 0, *aux, None)
+
+    assert gemm(0, 128, 64, EPI_BF16) == 1                                    # M < 1
+    assert gemm(-5, 128, 64, EPI_F32_ADD) == 1
+    assert gemm(128, 0, 64, EPI_BF16) == 1                                    # N < 1
+    assert gemm(128, 128, 64, EPI_BF16, bias=None) == 1                       # epilogues that read a bias
+    assert gemm(128, 128, 64, EPI_F32_ADD, bias=None) == 1
+    assert gemm(192, 256, 1024, EPI_BF16_RELU_UP, bias=None, aux=(16, 12, 8, (12 << 16) | 256)) == 1
+    assert gemm(192, 256, 1024, EPI_BF16_RELU_UP, aux=(0, 12, 8, (12 << 16) | 256)) == 1      # no input grid (was a host / 0)
+    assert gemm(3072, 32, 256, EPI_F32_NCHW, aux=(0, 3072, 0, 0)) == 1       # no channels
+    assert gemm(3072, 32, 256, EPI_F32_NCHW, aux=(33, 3072, 0, 0)) == 1      # more channels than W rows
+    assert gemm(3072, 32, 256, EPI_F32_NCHW, aux=(17, 0, 0, 0)) == 1         # no pixels
+
+    def experts(segs, M=384, D=384, P=64, H=2):
+        table = (C.c_int32 * max(1, 3 * len(segs)))(*[v for s in segs for v in s])
+        return L.vpb_expert_gemm(p, p, p, p, M, D, P, H, table, len(segs), 1, None)
+
+    for segs in ([(100, 200, 0), (50, 150, 1)], [(10, 10, 0)], [(0, 385, 0)], [(0, 100, 2)], [(0, 100, -1)], [], [(-1, 10, 0)]):
+        assert experts(segs) == 1, segs
+    assert experts([(i, i + 1, 0) for i in range(129)], M=200) == 1          # more than EXPERT_MAX_SEGMENTS
+    for P in (0, 48, 384, 400):
+        assert experts([(0, 100, 0)], P=P) == 1, P
+    assert experts([(0, 100, 0)], D=400, P=64) == 1                          # D % 32
+    assert experts([(0, 100, 0)], H=0) == 1
+    try:
+        assert L.vpb_debug_gemm(1, None) == 1                                 # a one-stage ring cannot hold two k-blocks
+        assert L.vpb_debug_gemm(1 | (4 << 8), None) == 1
+        assert L.vpb_debug_gemm(3 | (4 << 8), None) == 0
+    finally:
+        L.vpb_debug_gemm(0, None)
