@@ -3180,11 +3180,23 @@ extern "C" int vpb_expert_gemm(const void* d_a, const void* d_w, const float* d_
   return expert_launch(expert_width(p), ta, tw, q, st);
 }
 
+// The attention entry points' shape checks, before any device work: a built head_dim, positive counts, and no int overflow of
+// the qkv row width 3 D, the item count batch * heads or the row count batch * 192 (all int in the kernels and TMA coordinates)
+static int attention_shape_check(const char* fn, int32_t batch, int32_t heads, int32_t head_dim) {
+  if (head_dim != 32 && head_dim != 64 && head_dim != 80) return fail(VPB_ERR_ARG, "%s: head_dim %d not built (32, 64, 80)", fn, head_dim);
+  if (batch < 1 || heads < 1) return fail(VPB_ERR_ARG, "%s: batch %d, heads %d must be positive", fn, batch, heads);
+  constexpr int64_t kMax = INT32_MAX;
+  if (3 * static_cast<int64_t>(heads) * head_dim > kMax || static_cast<int64_t>(batch) * heads > kMax || static_cast<int64_t>(batch) * ATT_T > kMax)
+    return fail(VPB_ERR_ARG, "%s: batch %d x heads %d x head_dim %d overflows int", fn, batch, heads, head_dim);
+  return VPB_OK;
+}
+
 extern "C" int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream) {
+  if (!d_qkv || !d_out) return fail(VPB_ERR_ARG, "vpb_attention: null pointer");
+  VPB_TRY(attention_shape_check("vpb_attention", batch, heads, head_dim));
   int dev = 0;
   CU_TRY(cudaGetDevice(&dev));
   VPB_TRY(device_check(dev));
-  if (!d_qkv || !d_out || batch < 1 || heads < 1) return fail(VPB_ERR_ARG, "vpb_attention: bad argument");
   const int D = heads * head_dim;
   CUtensorMap tm, tt;
   VPB_TRY(make_attn_maps(&tm, &tt, d_qkv, static_cast<uint64_t>(batch) * 192, D, head_dim));
@@ -3195,11 +3207,13 @@ extern "C" int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, in
 
 extern "C" int vpb_qkv_attention(const void* d_xn, const void* d_w, const float* d_bias, int32_t batch, int32_t heads, int32_t head_dim,
                                  void* d_out, void* stream) {
+  if (!d_xn || !d_w || !d_bias || !d_out) return fail(VPB_ERR_ARG, "vpb_qkv_attention: null pointer");
+  VPB_TRY(attention_shape_check("vpb_qkv_attention", batch, heads, head_dim));
+  const int D = heads * head_dim;
+  if (D % 64 != 0) return fail(VPB_ERR_ARG, "vpb_qkv_attention: D = %d is not a whole number of 64-wide k-blocks", D);
   int dev = 0;
   CU_TRY(cudaGetDevice(&dev));
   VPB_TRY(device_check(dev));
-  const int D = heads * head_dim;
-  if (!d_xn || !d_w || !d_bias || !d_out || batch < 1 || heads < 1 || D % 64 != 0) return fail(VPB_ERR_ARG, "vpb_qkv_attention: bad argument");
   CUtensorMap tx, tw;
   VPB_TRY(make_map(&tx, d_xn, static_cast<uint64_t>(batch) * 192, D, D, 192));
   VPB_TRY(make_map(&tw, d_w, 3 * static_cast<uint64_t>(D), D, D, head_dim));

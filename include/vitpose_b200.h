@@ -665,7 +665,8 @@ int vpb_expert_gemm(const void* d_a, const void* d_w, const float* d_bias, float
 int vpb_attention(const void* d_qkv, int32_t batch, int32_t heads, int32_t head_dim, void* d_out, void* stream);
 /* qkv GEMM + attention in one launch: out = attention(xn[batch*192, D] * W[3D, D]^T + bias[3D]), D = heads * head_dim a multiple
  * of 64; bit-identical to vpb_gemm (epilogue 0) followed by vpb_attention.  Both attention entry points fill vpb_debug_gemm's
- * counters when they are set. */
+ * counters when they are set.  Both return VPB_ERR_ARG, before any device work, for a null pointer, head_dim other than 32, 64
+ * or 80, batch or heads < 1, or 3 * heads * head_dim, batch * heads or batch * 192 beyond INT32_MAX. */
 int vpb_qkv_attention(const void* d_xn, const void* d_w, const float* d_bias, int32_t batch, int32_t heads, int32_t head_dim,
                       void* d_out, void* stream);
 /* Debug / measurement switch (process-wide) for the attention kernel.  flags < 0: the defaults (every softmax exponential on

@@ -35,7 +35,8 @@ How the bounds are derived (u = 2^-24, the fp32 unit round-off):
             7.5e-5, flush to zero below 2^-126 / clamp at 2^-125), then rounded to bf16 (2^-9).  If every weight p_j
             carries a relative error |e_j| <= eps, the normalised weights shift by w_j (e_j - mean e) / (1 + mean e),
             so the output moves by at most 2 eps / (1 - eps) * sum_j w_j |v_j - o|.  P V is a 192-term fp32 GEMM, the
-            row sum a 192-term fp32 sum, and 1 / sum and the product round twice.
+            row sum a 192-term fp32 sum, and 1 / sum and the product round twice.  Keys more than 1000 below their
+            row's max (masked keys) have weight 0 or 2^-125 p(0) whatever their logit's error, so they stay out of eps.
   Deconv    An implicit GEMM of K = 4 Cin (each output phase reads 2 x 2 taps); the shift beta - mean * s in fp32 adds
             two roundings; ReLU is 1-Lipschitz.
 No constant here was adjusted to make a test pass.
@@ -234,6 +235,39 @@ def qkv(xn: torch.Tensor, sd: dict, i: int, heads: int):
     return z, bf16_bound(z, delta)
 
 
+MASKED = 1000.0                   # a key this far below its row's max logit is masked: exp(s - max) < e^-1000 is 0 in fp64
+
+
+def attention_items(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, guard: bool = True):
+    """softmax(q k^T) v of items [..., 192, hd] (fp64 of bf16 values, q pre-scaled) and the bound of the fp32 value before
+    the bf16 rounding of the output (the Attention paragraph above).
+
+    With `guard`, masked keys (s < max - MASKED) are left out of eps and of the logit error of the max (d_s.amax): the kernel
+    computes their weight as ex2 of an fp32 argument below -1000 log2e, which is 0 (MUFU) or 2^-125 p(0) (ex2_poly's clamp)
+    whatever that argument's error, and the `tiny` term already covers such weights.  Without the guard one key of logit
+    -1e30 (or -inf) makes d_s, and so the bound of its whole row, infinite: a test would pass that row unchecked."""
+    hd = q.shape[-1]
+    s = q @ k.transpose(-1, -2)
+    d_s = hd * UACC * (q.abs() @ k.abs().transpose(-1, -2))
+    m = s.amax(-1, keepdim=True)
+    p = torch.exp(s - m)
+    w = p / p.sum(-1, keepdim=True)
+    o = w @ v
+    if guard:
+        masked = s < m - MASKED
+        d_s = d_s.masked_fill(masked, 0.0)
+    arg = d_s + d_s.amax(-1, keepdim=True) + U * (2 * (s - m).abs() + m.abs())
+    if guard:
+        arg = arg.masked_fill(masked, -math.inf)
+    eps = (torch.exp(arg + math.log1p(P_BF16) + math.log1p(EX2)) - 1).amax(-1, keepdim=True)
+    vo = (v.unsqueeze(-3) - o.unsqueeze(-2)).abs()                              # [..., query, key, hd] = |v_j - o|
+    dev_v = (w.unsqueeze(-1) * vo).sum(-2)
+    tiny = 192 * 2.0 ** -124 * vo.amax(-2)                 # weights flushed to zero or clamped at 2^-125 (sum of p >= 1)
+    delta = (2 * eps / (1 - eps)) * dev_v + 2 * tiny + 192 * UACC * (1 + 2 * eps) * (w @ v.abs()) \
+        + (192 * U + 2 * U) * (o.abs() + dev_v)
+    return o, delta
+
+
 def attention(qkv_buf: torch.Tensor, heads: int):
     """Stage 5: softmax(q k^T) v per (crop, head) from the qkv buffer [B*192, 3D] (q pre-scaled) -> bf16 [B*192, D]."""
     M, D3 = qkv_buf.shape
@@ -242,20 +276,7 @@ def attention(qkv_buf: torch.Tensor, heads: int):
     t = qkv_buf.to(F64).reshape(B, 192, 3, heads, hd).permute(2, 0, 3, 1, 4)      # [3, B, H, 192, hd]
     refs, deltas = [], []
     for c in range(B):                                     # one crop at a time: sum_j w_j |v_j - o| is [H, 192, 192, hd]
-        q, k, v = t[0, c], t[1, c], t[2, c]
-        s = q @ k.transpose(-1, -2)
-        d_s = hd * UACC * (q.abs() @ k.abs().transpose(-1, -2))
-        m = s.amax(-1, keepdim=True)
-        p = torch.exp(s - m)
-        w = p / p.sum(-1, keepdim=True)
-        o = w @ v
-        arg = d_s + d_s.amax(-1, keepdim=True) + U * (2 * (s - m).abs() + m.abs())
-        eps = (torch.exp(arg + math.log1p(P_BF16) + math.log1p(EX2)) - 1).amax(-1, keepdim=True)
-        vo = (v.unsqueeze(-3) - o.unsqueeze(-2)).abs()                          # [H, query, key, hd] = |v_j - o|
-        dev_v = (w.unsqueeze(-1) * vo).sum(-2)
-        tiny = 192 * 2.0 ** -124 * vo.amax(-2)             # weights flushed to zero or clamped at 2^-125 (sum of p >= 1)
-        delta = (2 * eps / (1 - eps)) * dev_v + 2 * tiny + 192 * UACC * (1 + 2 * eps) * (w @ v.abs()) \
-            + (192 * U + 2 * U) * (o.abs() + dev_v)
+        o, delta = attention_items(t[0, c], t[1, c], t[2, c])
         refs.append(o.permute(1, 0, 2).reshape(192, D))
         deltas.append(delta.permute(1, 0, 2).reshape(192, D))
     ref, delta = torch.cat(refs), torch.cat(deltas)

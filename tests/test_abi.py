@@ -124,7 +124,8 @@ def test_decode_api_fails_loudly_without_cuda_and_checks_its_config():
 
 
 def test_gemm_entry_points_reject_what_the_kernels_cannot_serve():
-    """vpb_gemm, vpb_expert_gemm and vpb_debug_gemm check their arguments before touching the device, so VPB_ERR_ARG (1)
+    """vpb_gemm, vpb_expert_gemm, vpb_debug_gemm, vpb_attention and vpb_qkv_attention check their arguments before touching the
+    device, so VPB_ERR_ARG (1)
     comes back with or without a GPU.  The device pointers are misaligned dummies that no tensor map accepts."""
     import ctypes as C
 
@@ -158,6 +159,15 @@ def test_gemm_entry_points_reject_what_the_kernels_cannot_serve():
         assert experts([(0, 100, 0)], P=P) == 1, P
     assert experts([(0, 100, 0)], D=400, P=64) == 1                          # D % 32
     assert experts([(0, 100, 0)], H=0) == 1
+    # the attention entry points: head_dim not built, non-positive counts, int overflow of 3 D, batch * heads or batch * 192
+    big = 2 ** 31 - 1
+    for batch, heads, hd in ((1, 12, 48), (1, 12, 0), (0, 12, 64), (1, 0, 64), (-1, 12, 64), (1, big // 64, 64),
+                             (1, big // 150 + 1, 80), (big // 100, 200, 32), (big // 192 + 1, 1, 64)):
+        assert L.vpb_attention(p, batch, heads, hd, p, None) == 1, (batch, heads, hd)
+        assert L.vpb_qkv_attention(p, p, p, batch, heads, hd, p, None) == 1, (batch, heads, hd)
+    assert L.vpb_attention(None, 1, 12, 64, p, None) == 1
+    assert L.vpb_qkv_attention(p, p, None, 1, 12, 64, p, None) == 1
+    assert L.vpb_qkv_attention(p, p, p, 1, 1, 32, p, None) == 1             # D = 32: not a whole 64-wide k-block
     try:
         assert L.vpb_debug_gemm(1, None) == 1                                 # a one-stage ring cannot hold two k-blocks
         assert L.vpb_debug_gemm(1 | (4 << 8), None) == 1

@@ -84,62 +84,6 @@ def test_decode_nan_and_ties_first_index():
     assert np.array_equal(idx.cpu().numpy()[0], np.argmax(mm.reshape(40, -1), -1))
 
 
-@pytest.mark.parametrize("B,heads,hd", [(1, 2, 64), (1, 12, 64), (3, 12, 64), (7, 16, 64), (40, 16, 64), (64, 12, 64), (1, 2, 32), (5, 12, 32), (64, 12, 32)])
-def test_attention_packed_half_tiles(B, heads, hd):
-    """The shapes that once exercised a packed-pair kernel (the last 64 rows of two heads sharing one pass); on H100 each 64-row
-    tile is one warpgroup's own pass.  Against the fp32 reference, deterministic, and with every 4th softmax exponential on the
-    FMA pipe (ex2_poly) instead of the MUFU within tolerance of both."""
-    from easy_vitpose_b200 import _lib
-    from gpu_util import attention
-    torch.manual_seed(B * 100 + heads + hd + 1)
-    D = heads * hd
-    qkv = torch.randn(B * 192, 3 * D, device=_dev())
-    qkv[:, :D] *= (hd ** -0.5) * 2.0
-    qkv = qkv.bfloat16()
-    try:
-        _lib.lib().vpb_debug_attention(0)                            # all exponentials on the MUFU
-        out = attention(qkv, B, heads, hd).float()
-        again = attention(qkv, B, heads, hd).float()
-        _lib.lib().vpb_debug_attention(1)                            # every 4th exponential as a polynomial
-        fast = attention(qkv, B, heads, hd).float()
-    finally:
-        _lib.lib().vpb_debug_attention(-1)
-    q, k, v = (qkv.float().reshape(B, 192, 3, heads, hd)[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-    ref = (torch.softmax(q @ k.transpose(-1, -2), -1) @ v).permute(0, 2, 1, 3).reshape(B * 192, D)
-    r = _rel(out, ref)
-    print("attention rel err", r, "hd", hd, "| max |poly - mufu|", float((fast - out).abs().max()))
-    assert torch.equal(out, again)                                   # deterministic
-    assert r < 2e-2
-    assert _rel(fast, ref) < 2e-2 and (fast - out).abs().max() < 2e-2
-
-
-@pytest.mark.parametrize("B,heads,cap", [(1, 8, 7), (1, 10, 9), (1, 16, 11), (1, 6, 5), (2, 10, 19), (2, 11, 17), (3, 12, 1), (6, 12, 5)])
-def test_attention_packed_other_grids(B, heads, cap):
-    """The attention kernel with fewer CTAs than SMs (what a smaller / partitioned device would launch): a CTA then walks several
-    items through its two operand stages, including odd counts and a single CTA for the whole launch.  Every item is computed
-    by the same arithmetic, so the result must not change by a bit."""
-    from easy_vitpose_b200 import _lib
-    from gpu_util import attention
-    hd = 64
-    torch.manual_seed(B * 1000 + heads * 10 + cap)
-    D = heads * hd
-    qkv = torch.randn(B * 192, 3 * D, device=_dev())
-    qkv[:, :D] *= (hd ** -0.5) * 2.0
-    qkv = qkv.bfloat16()
-    try:
-        _lib.lib().vpb_debug_attention(0)
-        plain = attention(qkv, B, heads, hd)
-        _lib.lib().vpb_debug_attention(1)
-        poly = attention(qkv, B, heads, hd)
-        _lib.lib().vpb_debug_attention(1 | (cap << 8))
-        poly_capped = attention(qkv, B, heads, hd)
-        _lib.lib().vpb_debug_attention(0 | (cap << 8))
-        plain_capped = attention(qkv, B, heads, hd)
-    finally:
-        _lib.lib().vpb_debug_attention(-1)
-    assert torch.equal(plain_capped, plain) and torch.equal(poly_capped, poly)
-
-
 # ------------------------------------------------------------------------------------------------ LayerNorm
 @pytest.mark.parametrize("D", [384, 768, 1024, 1280])
 def test_layernorm(D):
@@ -351,22 +295,3 @@ def test_gemm_heatmap_nchw(Kk, Npad):
     r = S.worst_ratio(out, ref, bound)
     print("1x1 conv worst |err| / bound", r)
     assert r <= 1
-
-
-# ------------------------------------------------------------------------------------------------ attention
-@pytest.mark.parametrize("B,heads,hd", [(1, 1, 64), (3, 12, 64), (40, 16, 64), (64, 12, 64),
-                                        (1, 1, 32), (5, 12, 32), (1, 1, 80), (4, 16, 80), (33, 16, 80)])
-def test_attention(B, heads, hd):
-    from gpu_util import attention
-    torch.manual_seed(B * 100 + heads + hd)
-    D = heads * hd
-    qkv = torch.randn(B * 192, 3 * D, device=_dev())
-    qkv[:, :D] *= (hd ** -0.5) * 2.0                                 # q arrives pre-scaled; keep logits O(few)
-    qkv = qkv.bfloat16()
-    out = attention(qkv, B, heads, hd).float()
-    q, k, v = (qkv.float().reshape(B, 192, 3, heads, hd)[:, :, i].permute(0, 2, 1, 3) for i in range(3))
-    p = torch.softmax(q @ k.transpose(-1, -2), -1)
-    ref = (p @ v).permute(0, 2, 1, 3).reshape(B * 192, D)
-    r = _rel(out, ref)
-    print("attention rel err", r, "hd", hd)
-    assert r < 2e-2
