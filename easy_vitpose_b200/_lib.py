@@ -49,6 +49,7 @@ class VpbFrameYuv(C.Structure):
 
 MAX_HEADS = 8                                        # VPB_MAX_HEADS: keypoint heads of one engine
 MAX_SEGMENTS = 64                                     # VPB_MAX_SEGMENTS: runs of one head per multi-head call
+DECODERS = {"classic": 0, "simple": 1}                # VPB_DECODER_CLASSIC, VPB_DECODER_SIMPLE (vpb_create_ex)
 
 
 class VpbSegment(C.Structure):
@@ -118,6 +119,7 @@ EXPORTS = {
     "vpb_infer_affine_host": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]),
     "vpb_create_heads": (C.c_int, [C.POINTER(VpbConfig), C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+    "vpb_create_ex": (C.c_int, [C.POINTER(VpbConfig), C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
     "vpb_infer_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(VpbSegment), C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p]),
     "vpb_infer_frames_heads": (C.c_int, [C.c_void_p, C.POINTER(VpbFrame), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -36,25 +36,34 @@ def flip_pairs_for(dataset: str, flip_pairs=None) -> "list[tuple[int, int]]":
     raise ValueError(f"no flip pairs known for dataset {dataset!r}: pass flip_pairs explicitly")
 
 
-def model_cfg(size: str, num_keypoints: int) -> dict:
+def model_cfg(size: str, num_keypoints: int, decoder: str = "classic") -> dict:
+    """The reference's model dict for ViT-`size` with a K-keypoint head: decoder "classic" = the configs' 2x deconv + 1x1 conv
+    head (configs/ViTPose_common.py), "simple" = the paper's simple decoder of the reference's training configs
+    (train_configs/ViTPose_{base,large,huge}_simple_coco_256x192.py:60-68: relu, 4x bilinear upsample, 3x3 conv)."""
     name = MODEL_ABBR.get(size, size)
     if name not in _DIMS:
         raise KeyError(f"unknown model size {size!r}")
+    if decoder not in ("classic", "simple"):
+        raise ValueError(f"decoder {decoder!r}: 'classic' or 'simple'")
     D, depth, heads = _DIMS[name]
+    if decoder == "simple":
+        head = dict(type="TopdownHeatmapSimpleHead", in_channels=D, num_deconv_layers=0, num_deconv_filters=[],
+                    num_deconv_kernels=[], upsample=4, extra=dict(final_conv_kernel=3), out_channels=num_keypoints)
+    else:
+        head = dict(type="TopdownHeatmapSimpleHead", in_channels=D, num_deconv_layers=2, num_deconv_filters=(256, 256),
+                    num_deconv_kernels=(4, 4), extra=dict(final_conv_kernel=1), out_channels=num_keypoints)
     return dict(
         type="TopDown", pretrained=None,
         backbone=dict(type="ViT", img_size=(256, 192), patch_size=16, embed_dim=D, depth=depth, num_heads=heads,
                       ratio=1, use_checkpoint=False, mlp_ratio=4, qkv_bias=True, drop_path_rate=_DROP_PATH[name]),
-        keypoint_head=dict(type="TopdownHeatmapSimpleHead", in_channels=D, num_deconv_layers=2,
-                           num_deconv_filters=(256, 256), num_deconv_kernels=(4, 4),
-                           extra=dict(final_conv_kernel=1), out_channels=num_keypoints),
+        keypoint_head=head,
         train_cfg=dict(),
         test_cfg=dict(flip_test=True, post_process="default", shift_heatmap=False,
                       target_type="GaussianHeatmap", modulate_kernel=11, use_udp=True))
 
 
-def dyn_model_import(dataset: str, model: str) -> dict:
-    """Same call shape as the reference helper: dataset name + size letter -> model cfg dict."""
+def dyn_model_import(dataset: str, model: str, decoder: str = "classic") -> dict:
+    """Same call shape as the reference helper: dataset name + size letter -> model cfg dict (decoder: see model_cfg)."""
     if dataset not in DATASET_KEYPOINTS:
         raise KeyError(f"dataset {dataset!r} has no fixed keypoint count here; use model_cfg(size, K)")
-    return copy.deepcopy(model_cfg(model, DATASET_KEYPOINTS[dataset]))
+    return copy.deepcopy(model_cfg(model, DATASET_KEYPOINTS[dataset], decoder))

@@ -29,6 +29,7 @@
 #include "oks_nms.cuh"
 #include "coco_eval.cuh"
 #include "qkv_attention.cuh"
+#include "simple_head.cuh"
 #include "smooth.cuh"
 #include "track.cuh"
 
@@ -152,6 +153,7 @@ struct DeviceState {
   bool attn_attr = false;
   unsigned gemm_attr = 0;           // bit per gemm instantiation (see gemm_slot)
   unsigned expert_attr = 0;         // bit per expert GEMM tile width (expert_launch)
+  unsigned simple_head_attr = 0;    // bit per last-group width of the simple head (simple_head_t)
 };
 static DeviceState g_devs[kMaxDevices];
 static DeviceState* cur_dev() {
@@ -386,9 +388,10 @@ static int qkv_attention_launch(int hd, const CUtensorMap& tx, const CUtensorMap
 // Optional ("profile" option): a CUDA-event pair around every launch, on the launch stream, summed per kernel
 // class by vpb_profile_collect.  bench.py uses it to report the dominant kernel's achieved FLOP/s live.
 enum KClass : int { KC_PATCH_IM2COL, KC_GEMM_PATCH, KC_LN, KC_GEMM_QKV, KC_ATTN, KC_GEMM_PROJ, KC_GEMM_FC1, KC_GEMM_FC2,
-                    KC_GEMM_DECONV, KC_GEMM_FINAL, KC_DECODE, KC_PREPROCESS, KC_CHAIN, KC_COUNT };
+                    KC_GEMM_DECONV, KC_GEMM_FINAL, KC_DECODE, KC_PREPROCESS, KC_CHAIN, KC_SIMPLE_HEAD, KC_COUNT };
 static const char* kclass_names[KC_COUNT] = {"patch_im2col", "gemm_patch_embed", "layernorm", "gemm_qkv", "attention", "gemm_proj",
-                                             "gemm_fc1_gelu", "gemm_fc2", "gemm_deconv", "gemm_final_conv", "decode", "crop_preprocess", "gemm_chain"};
+                                             "gemm_fc1_gelu", "gemm_fc2", "gemm_deconv", "gemm_final_conv", "decode", "crop_preprocess", "gemm_chain",
+                                             "simple_head"};
 struct ProfRec { int cls; cudaEvent_t a, b; };
 struct Profiler {
   bool on = false;
@@ -445,6 +448,11 @@ struct HeadW {
   int K = 0, n_final = 0;           // n_final = padded channel count of the 1x1 conv GEMM
   LinearW dc1, dc2, fin;            // dc*: the 4 phase matrices stacked [4*256, 4*Cin]
   CUtensorMap m_fin_w;              // final 1x1 conv W: boxes of n_final rows (one column tile)
+  // simple decoder (VPB_DECODER_SIMPLE): the 3x3 conv's taps packed as simple_head.cuh lays them out, in boxes of 144 rows (a
+  // full group of 16 keypoints) and of the last group's width
+  __nv_bfloat16* tap_w = nullptr;
+  float* tap_b = nullptr;
+  CUtensorMap m_tap_full, m_tap_rem;
 };
 // A run of consecutive crops of one head in a multi-head call
 struct Segment { int head, count; };
@@ -454,6 +462,7 @@ struct vpb_engine {
   int D, depth, heads, K, maxB;    // K = head 0's keypoints: what the single-head calls return per crop
   // keypoint heads (vpb_create_heads; vpb_create: one head, P = 0) and the expert width P of each block's fc2
   int num_kheads = 1, P = 0, Kmax = 0, expert_bn = 0;
+  int decoder = VPB_DECODER_CLASSIC;   // every head of the engine: classic (2 deconvs + 1x1 conv) or simple (relu, 4x up, 3x3 conv)
   std::vector<HeadW> hw;
   bool finalized = false;
   int stop_after = 0;
@@ -586,6 +595,11 @@ static std::vector<std::pair<std::string, int64_t>> expected_keys(const vpb_engi
   v.push_back({"backbone.last_norm.weight", D}); v.push_back({"backbone.last_norm.bias", D});
   for (int j = 0; j < e->num_kheads; ++j) {
     const std::string hp = head_prefix(j);
+    if (e->decoder == VPB_DECODER_SIMPLE) {
+      v.push_back({hp + "final_layer.weight", static_cast<int64_t>(e->hw[j].K) * D * 9});
+      v.push_back({hp + "final_layer.bias", e->hw[j].K});
+      continue;
+    }
     int64_t cin = D;
     for (int li : {0, 3}) {
       const std::string p = hp + "deconv_layers.";
@@ -662,6 +676,17 @@ extern "C" int vpb_create_heads(const vpb_config* cfg, int32_t num_heads, const 
     e->hw[j].n_final = h_keypoints[j] <= 32 ? 32 : 144;
     e->Kmax = std::max(e->Kmax, static_cast<int>(h_keypoints[j]));
   }
+  return VPB_OK;
+}
+
+extern "C" int vpb_create_ex(const vpb_config* cfg, int32_t num_heads, const int32_t* h_keypoints, int32_t expert_rows, int32_t decoder,
+                             vpb_engine** out) {
+  if (!out) return fail(VPB_ERR_ARG, "vpb_create_ex: null argument");
+  *out = nullptr;
+  if (decoder != VPB_DECODER_CLASSIC && decoder != VPB_DECODER_SIMPLE)
+    return fail(VPB_ERR_ARG, "vpb_create_ex: decoder %d (VPB_DECODER_CLASSIC 0 or VPB_DECODER_SIMPLE 1)", decoder);
+  VPB_TRY(vpb_create_heads(cfg, num_heads, h_keypoints, expert_rows, out));
+  (*out)->decoder = decoder;
   return VPB_OK;
 }
 
@@ -803,6 +828,17 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   for (int j = 0; j < e->num_kheads; ++j) {
     HeadW& h = e->hw[j];
     const std::string hp = head_prefix(j);
+    if (e->decoder == VPB_DECODER_SIMPLE) {   // 3x3 conv taps as bf16 rows [ceil(K / 16) * 144, D], bias as is
+      const int rows = cdiv(h.K, SH_GROUP) * SH_NFULL;
+      VPB_TRY(dev_alloc(e, &h.tap_w, static_cast<size_t>(rows) * D));
+      pack_simple_head<<<cdiv(static_cast<long long>(rows) * D, 256), 256>>>(e->staged[hp + "final_layer.weight"].first, h.tap_w, h.K, D);
+      CU_TRY(cudaGetLastError());
+      VPB_TRY(copy_vec(e, &h.tap_b, hp + "final_layer.bias"));
+      const int kr = h.K % SH_GROUP;
+      VPB_TRY(make_map(&h.m_tap_full, h.tap_w, rows, D, D, SH_NFULL));
+      VPB_TRY(make_map(&h.m_tap_rem, h.tap_w, rows, D, D, kr ? sh_width(9 * kr) : SH_NFULL));
+      continue;
+    }
     int cin = D;
     for (int layer = 0; layer < 2; ++layer) {
       LinearW& dc = layer == 0 ? h.dc1 : h.dc2;
@@ -833,8 +869,10 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(dev_alloc(e, &e->qkv, M * 3 * D));
   VPB_TRY(dev_alloc(e, &e->attn, M * D));
   VPB_TRY(dev_alloc(e, &e->hid, M * 4 * D));
-  VPB_TRY(dev_alloc(e, &e->d1, B * 768 * 256));
-  VPB_TRY(dev_alloc(e, &e->d2, B * 3072 * 256));
+  if (e->decoder == VPB_DECODER_CLASSIC) {   // the deconvs' outputs; the simple head keeps its maps on chip
+    VPB_TRY(dev_alloc(e, &e->d1, B * 768 * 256));
+    VPB_TRY(dev_alloc(e, &e->d2, B * 3072 * 256));
+  }
   VPB_TRY(dev_alloc(e, &e->heat, B * e->Kmax * 3072));
   for (int s = 0; s < 2; ++s) {
     VPB_TRY(dev_alloc(e, &e->kpts[s], B * e->Kmax * 3));
@@ -874,9 +912,11 @@ extern "C" int vpb_finalize(vpb_engine* e) {
   VPB_TRY(make_map(&e->m_xn_att, e->xn, M, D, D, 192));
   VPB_TRY(make_map(&e->m_attn, e->attn, M, D, D, 128));
   VPB_TRY(make_map(&e->m_hid, e->hid, M, 4 * D, 4 * D, 128));
-  VPB_TRY(make_map_nhwc(&e->m_feat_nhwc, e->xn, B, 16, 12, D, 8, 12));   // 8 x 12 = 96 positions per M tile (12 is not a multiple of 8)
-  VPB_TRY(make_map_nhwc(&e->m_d1_nhwc, e->d1, B, 32, 24, 256, 16, 8));  // 16 x 8 = 128 positions per M tile: full tiles
-  VPB_TRY(make_map(&e->m_d2, e->d2, B * 3072, 256, 256, 128));
+  if (e->decoder == VPB_DECODER_CLASSIC) {
+    VPB_TRY(make_map_nhwc(&e->m_feat_nhwc, e->xn, B, 16, 12, D, 8, 12));   // 8 x 12 = 96 positions per M tile (12 is not a multiple of 8)
+    VPB_TRY(make_map_nhwc(&e->m_d1_nhwc, e->d1, B, 32, 24, 256, 16, 8));  // 16 x 8 = 128 positions per M tile: full tiles
+    VPB_TRY(make_map(&e->m_d2, e->d2, B * 3072, 256, 256, 128));
+  }
   VPB_TRY(make_attn_maps(&e->m_qkv_att, &e->m_qkv_att_tail, e->qkv, M, D, D / e->heads));
   VPB_TRY(make_map(&e->o_qkv, e->qkv, M, 3 * D, 3 * D, 64));
   VPB_TRY(make_map(&e->o_hid, e->hid, M, 4 * D, 4 * D, 64));
@@ -1309,6 +1349,39 @@ static int backbone(vpb_engine* e, int B, cudaStream_t st, const std::vector<Seg
   return standalone_ln(e->lnf_g, e->lnf_b);
 }
 
+// The simple decoder of head h on crops c0 .. c0+B-1 of the workspace (same outputs as head() below): one launch, grid (crop,
+// group of 16 keypoints), the last group at the narrowest wgmma width that holds its taps
+template <int NT_REM>
+static int simple_head_t(const vpb_engine* e, int B, const HeadW& h, const SimpleHeadParams& p, cudaStream_t st) {
+  auto kern = simple_head_kernel<NT_REM>;
+  DeviceState* ds = cur_dev();
+  if (ds->sms == 0) return fail(VPB_ERR_STATE, "simple head: device not initialised (device_check)");
+  constexpr unsigned slot = 1u << (NT_REM == 32 ? 0 : NT_REM == 64 ? 1 : NT_REM == 96 ? 2 : NT_REM == 128 ? 3 : 4);
+  if (!(ds->simple_head_attr & slot)) {
+    CU_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
+    ds->simple_head_attr |= slot;
+  }
+  CU_TRY(launch_k(kern, dim3(B, cdiv(h.K, SH_GROUP)), dim3(SH_THREADS), SH_SMEM, st, e->m_xn_att, h.m_tap_full, h.m_tap_rem, p));
+  return VPB_OK;
+}
+static int simple_head(vpb_engine* e, int B, float* d_heat, cudaStream_t st, const HeadW& h, int c0, int ch_stride) {
+  if (e->D % SH_BK != 0) return fail(VPB_ERR_ARG, "simple head: D=%d is not a multiple of %d", e->D, SH_BK);
+  SimpleHeadParams p;
+  p.bias = h.tap_b; p.out = d_heat; p.D = e->D; p.K = h.K; p.c0 = c0; p.ch_stride = ch_stride ? ch_stride : h.K;
+  const int kr = h.K % SH_GROUP;
+  e->prof.begin(KC_SIMPLE_HEAD, st);
+  int rc;
+  switch (kr ? sh_width(9 * kr) : SH_NFULL) {
+    case 32: rc = simple_head_t<32>(e, B, h, p, st); break;
+    case 64: rc = simple_head_t<64>(e, B, h, p, st); break;
+    case 96: rc = simple_head_t<96>(e, B, h, p, st); break;
+    case 128: rc = simple_head_t<128>(e, B, h, p, st); break;
+    default: rc = simple_head_t<144>(e, B, h, p, st); break;
+  }
+  e->prof.end(st);
+  return rc;
+}
+
 // Head j on crops c0 .. c0+B-1 of the workspace -> heatmaps of crop c at d_heat + c * ch_stride maps (ch_stride = the head's K
 // for the single-head calls, K_max for a multi-head call).  A deconv tile never straddles a crop, so a segment of crops is the
 // same launches on A maps and outputs that start at crop c0; the crop-0 maps are the engine's own.
@@ -1316,6 +1389,7 @@ static int head(vpb_engine* e, int B, float* d_heat, cudaStream_t st, int j = 0,
   const int D = e->D;
   const int stop = e->stop_after;
   const HeadW& h = e->hw[j];
+  if (e->decoder == VPB_DECODER_SIMPLE) return simple_head(e, B, d_heat, st, h, c0, ch_stride);
   CUtensorMap feat = e->m_feat_nhwc, d1 = e->m_d1_nhwc, d2 = e->m_d2;
   if (c0 > 0) {
     VPB_TRY(make_map_nhwc(&feat, e->xn + static_cast<size_t>(c0) * 192 * D, B, 16, 12, D, 8, 12));
@@ -2966,12 +3040,14 @@ extern "C" int vpb_kernel_launches(const vpb_engine* e, int32_t batch) {
   // patch im2col + patch GEMM + depth*(qkv, attention, proj, fc1, fc2) + 2 deconv GEMMs + 1x1 GEMM + decode; the 2*depth+1
   // LayerNorms ride in the tails of the patch / proj / fc2 GEMMs unless ln_fused is switched off
   // flip test adds the flip-back average in front of the decode; the chains then see 2 * batch crops
+  // the simple decoder is one launch where the classic one is three (2 deconvs + 1x1)
+  const int head_launches = e->decoder == VPB_DECODER_SIMPLE ? 1 : 2 + 1;
   if (e->use_chain && model_crops(e, batch) >= e->chain_min_batch && !e->ln_fused)
-    return 1 + (1 + e->depth) + e->depth + 2 + 1 + 1 + (e->flip ? 1 : 0);   // gather, chains, attention, deconvs, 1x1, decode
+    return 1 + (1 + e->depth) + e->depth + head_launches + 1 + (e->flip ? 1 : 0);   // gather, chains, attention, head, decode
   // one kernel per GEMM: gather, patch GEMM, depth x (qkv, attention, proj, fc1, fc2), 2 deconvs, 1x1, decode; the LayerNorms are
   // launches of their own (2 * depth + 1), or ride in front of qkv / fc1 (ln_in_gemm: only last_norm is left), or in the tails.
   // qkv and attention are one launch per block where fuse_qkv_attention says so (large batches)
-  return 2 + e->depth * (fuse_qkv_attention(e, model_crops(e, batch)) ? 4 : 5) + 2 + 1 + 1 +
+  return 2 + e->depth * (fuse_qkv_attention(e, model_crops(e, batch)) ? 4 : 5) + head_launches + 1 +
          (e->ln_fused ? 0 : e->ln_in_gemm ? 1 : 2 * e->depth + 1) + (e->flip ? 1 : 0);
 }
 
@@ -2990,7 +3066,8 @@ static int poison_workspace(vpb_engine* e) {
       {e->hid, M * 4 * D * bf}, {e->d1, B * 768 * 256 * bf}, {e->d2, B * 3072 * 256 * bf}, {e->heat, B * K * 3072 * f},
       {e->g_kpts, B * K * 3 * f}, {e->kpts[0], B * K * 3 * f}, {e->kpts[1], B * K * 3 * f},
       {e->crops_stage[0], B * 3 * 256 * 192 * f}, {e->crops_stage[1], B * 3 * 256 * 192 * f}, {e->g_cs, B * 4 * f}, {e->cs_stage, B * 4 * f}};
-  for (const auto& b : bufs) CU_TRY(cudaMemset(b.first, 0xFF, b.second));
+  for (const auto& b : bufs)
+    if (b.first) CU_TRY(cudaMemset(b.first, 0xFF, b.second));   // d1 / d2 exist only for the classic decoder
   CU_TRY(cudaDeviceSynchronize());
   return VPB_OK;
 }
@@ -3096,6 +3173,7 @@ extern "C" int vpb_read_buffer(vpb_engine* e, const char* name, void* host_dst, 
   else if (n == "d2") src = e->d2;
   else if (n == "heat") src = e->heat;
   else return fail(VPB_ERR_ARG, "unknown buffer %s", name);
+  if (!src) return fail(VPB_ERR_ARG, "buffer %s: not allocated by this engine (the simple decoder has no deconv maps)", name);
   CU_TRY(cudaDeviceSynchronize());
   CU_TRY(cudaMemcpy(host_dst, src, bytes, cudaMemcpyDeviceToHost));
   return VPB_OK;

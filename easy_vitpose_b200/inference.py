@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from .configs import data_cfg, flip_pairs_for, model_cfg
-from .model import ViTPose
+from .model import ViTPose, _unwrap, state_dict_decoder
 from .nms import check as nms_check, oks_nms_device
 from .top_down_eval import decode_heatmaps
 from .topdown import topdown_args, xywh2cs
@@ -52,7 +52,11 @@ class B200PoseBackend:
 
     @classmethod
     def from_state_dict(cls, state_dict: dict, size: str, num_keypoints: int, max_batch: int = 64, device=None):
-        m = ViTPose(model_cfg(size, num_keypoints), max_batch=max_batch)
+        """A backend for a reference checkpoint ({'state_dict': ...} or the bare dict).  The decoder comes from the keys: a 3x3
+        keypoint_head.final_layer.weight and no deconv_layers.* is the simple decoder, anything else the classic head (the
+        strict load then reports what does not fit)."""
+        state_dict = _unwrap(state_dict)
+        m = ViTPose(model_cfg(size, num_keypoints, state_dict_decoder(state_dict)), max_batch=max_batch)
         m.load_state_dict(state_dict)
         return cls(m, device if device is not None else "cuda")
 

@@ -235,7 +235,7 @@ def _inverse(order: np.ndarray) -> np.ndarray:
     return inv
 
 
-# the head tensors model_split.py moves (:35-48), relative to the head's prefix
+# the head tensors model_split.py moves (:35-48), relative to the head's prefix (a simple-decoder head has final_layer.* only)
 _HEAD_PARTS = ("deconv_layers.0.weight", "deconv_layers.1.weight", "deconv_layers.1.bias", "deconv_layers.1.running_mean",
                "deconv_layers.1.running_var", "deconv_layers.1.num_batches_tracked", "deconv_layers.3.weight",
                "deconv_layers.4.weight", "deconv_layers.4.bias", "deconv_layers.4.running_mean", "deconv_layers.4.running_var",
@@ -276,11 +276,12 @@ def split_vitpose_plus(sd, names=None, keypoints=None) -> "OrderedDict[str, Orde
                 v = torch.cat([torch.as_tensor(v), torch.as_tensor(sd[ek])], 0)
             d[k] = v
         if i > 0:
+            simple = _head_prefix(i) + "deconv_layers.0.weight" not in sd and _head_prefix(i) + "final_layer.weight" in sd
             for part in _HEAD_PARTS:
                 src = _head_prefix(i) + part
                 if src in sd:
                     d["keypoint_head." + part] = sd[src]
-                elif not part.endswith("num_batches_tracked"):
+                elif not part.endswith("num_batches_tracked") and not (simple and part.startswith("deconv_layers.")):
                     raise KeyError(f"{src} missing")
             for part in ("final_layer.weight", "final_layer.bias"):
                 d["keypoint_head." + part] = d["keypoint_head." + part][:K]
@@ -325,9 +326,35 @@ def merge_split_state_dicts(sds, part_features: int) -> "OrderedDict[str, torch.
     return out
 
 
-def _expected_shapes(D: int, depth: int, K: int, head_keypoints=None, P: int = 0) -> "OrderedDict[str, tuple]":
+def head_decoder(hd: dict) -> str:
+    """The decoder a reference keypoint_head dict describes: "classic" (2x deconv(256, 4x4) + 1x1 conv, the configs) or "simple"
+    (num_deconv_layers=0, upsample=4, final_conv_kernel=3, align_corners false: the training configs' simple decoder).
+    ValueError for every other head."""
+    hd = {k: v for k, v in hd.items() if k != "type"}
+    final = (hd.get("extra") or {}).get("final_conv_kernel", 1)
+    if hd.get("num_deconv_layers", 3) == 2 and tuple(hd.get("num_deconv_filters", ())) == (256, 256) \
+            and tuple(hd.get("num_deconv_kernels", ())) == (4, 4) and final == 1:
+        return "classic"
+    if hd.get("num_deconv_layers", 3) == 0 and not tuple(hd.get("num_deconv_filters", ())) \
+            and not tuple(hd.get("num_deconv_kernels", ())) and hd.get("upsample", 0) == 4 and final == 3 \
+            and "num_conv_layers" not in (hd.get("extra") or {}) and not hd.get("align_corners", False):
+        return "simple"
+    raise ValueError("only the 2x deconv(256,4x4) + 1x1 conv head of the reference's configs, or the simple decoder of its "
+                     "training configs (num_deconv_layers=0, upsample=4, final_conv_kernel=3) is built")
+
+
+def state_dict_decoder(sd) -> str:
+    """The decoder a reference state_dict was trained with: "simple" when keypoint_head.final_layer.weight is a 3x3 conv and
+    there is no keypoint_head.deconv_layers.* key, else "classic"."""
+    sd = _unwrap(sd)
+    w = sd.get("keypoint_head.final_layer.weight")
+    deconv = any(k.startswith("keypoint_head.deconv_layers.") for k in sd)
+    return "simple" if w is not None and tuple(w.shape[-2:]) == (3, 3) and not deconv else "classic"
+
+
+def _expected_shapes(D: int, depth: int, K: int, head_keypoints=None, P: int = 0, decoder: str = "classic") -> "OrderedDict[str, tuple]":
     """state_dict contract of the reference ViTPose (SURVEY.md section 8b); with head_keypoints / P the ViTPose+ key set of a
-    multi-head engine (vpb_create_heads)."""
+    multi-head engine (vpb_create_heads); decoder "simple": every head is final_layer [K,D,3,3] + bias alone."""
     s: "OrderedDict[str, tuple]" = OrderedDict()
     s["backbone.pos_embed"] = (1, 193, D)
     s["backbone.patch_embed.proj.weight"] = (D, 3, 16, 16)
@@ -345,6 +372,10 @@ def _expected_shapes(D: int, depth: int, K: int, head_keypoints=None, P: int = 0
     s["backbone.last_norm.weight"] = (D,); s["backbone.last_norm.bias"] = (D,)
     for j, Kj in enumerate(head_keypoints or [K]):
         hp = _head_prefix(j)
+        if decoder == "simple":
+            s[hp + "final_layer.weight"] = (Kj, D, 3, 3)
+            s[hp + "final_layer.bias"] = (Kj,)
+            continue
         cin = D
         for li in (0, 3):
             s[f"{hp}deconv_layers.{li}.weight"] = (cin, 256, 4, 4)
@@ -397,7 +428,9 @@ class ViTPose:
 
     cfg is the reference's model dict (cfg['backbone'], cfg['keypoint_head']; 'type' keys ignored,
     model.py:14-15).  Only the configurations the reference ships are accepted: patch 16, 256x192,
-    mlp_ratio 4, qkv_bias, two 4x4 deconvs of 256 filters and a 1x1 final conv.
+    mlp_ratio 4, qkv_bias, and either two 4x4 deconvs of 256 filters and a 1x1 final conv (`decoder` "classic") or the
+    simple decoder of the reference's training configs (`decoder` "simple": relu, 4x bilinear upsample, 3x3 conv;
+    train_configs/ViTPose_{base,large,huge}_simple_coco_256x192.py:60-68).
     """
 
     def __init__(self, cfg: dict, max_batch: int = 64, device: "int | str | torch.device | None" = None, *, heads=None,
@@ -408,9 +441,7 @@ class ViTPose:
             raise ValueError("only img_size=(256,192), patch_size=16, ratio=1 (the reference's configs) are built")
         if bb.get("mlp_ratio", 4) != 4 or not bb.get("qkv_bias", False):
             raise ValueError("only mlp_ratio=4, qkv_bias=True (the reference's configs) are built")
-        if hd.get("num_deconv_layers", 3) != 2 or tuple(hd.get("num_deconv_filters", ())) != (256, 256) \
-                or tuple(hd.get("num_deconv_kernels", ())) != (4, 4) or (hd.get("extra") or {}).get("final_conv_kernel", 1) != 1:
-            raise ValueError("only the 2x deconv(256,4x4) + 1x1 conv head of the reference's configs is built")
+        self.decoder = head_decoder(hd)
         self.embed_dim = int(bb["embed_dim"]); self.depth = int(bb["depth"]); self.num_heads = int(bb["num_heads"])
         self.num_keypoints = int(hd["out_channels"])
         # several keypoint heads on one backbone (ViTPose+ / frozen-backbone fine-tunes): `heads` = keypoint counts or
@@ -487,7 +518,7 @@ class ViTPose:
         if "state_dict" in state_dict and not any(k.startswith("backbone.") for k in state_dict):
             state_dict = state_dict["state_dict"]
         exp = _expected_shapes(self.embed_dim, self.depth, self.num_keypoints, self.head_keypoints if self._multi else None,
-                               self.expert_rows)
+                               self.expert_rows, self.decoder)
         missing = [k for k in exp if k not in state_dict and not k.endswith("num_batches_tracked")]
         unexpected = [k for k in state_dict if k not in exp]
         if strict and (missing or unexpected):
@@ -526,7 +557,11 @@ class ViTPose:
         L = _lib.lib()
         cfg = _lib.VpbConfig(self.embed_dim, self.depth, self.num_heads, self.num_keypoints, self.max_batch, self._device)
         with torch.cuda.device(self._device):
-            if self._multi:
+            if self.decoder != "classic":
+                ks = (C.c_int32 * len(self.head_keypoints))(*self.head_keypoints)
+                _lib.check(L.vpb_create_ex(C.byref(cfg), len(ks), ks, self.expert_rows, _lib.DECODERS[self.decoder],
+                                           C.byref(self._handle)))
+            elif self._multi:
                 ks = (C.c_int32 * len(self.head_keypoints))(*self.head_keypoints)
                 _lib.check(L.vpb_create_heads(C.byref(cfg), len(ks), ks, self.expert_rows, C.byref(self._handle)))
             else:

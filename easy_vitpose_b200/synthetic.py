@@ -16,8 +16,10 @@ __all__ = ["random_state_dict", "random_crops"]
 _DIMS = {"s": (384, 12, 12), "b": (768, 12, 12), "l": (1024, 24, 16), "h": (1280, 32, 16)}
 
 
-def random_state_dict(size: str, num_keypoints: int, seed: int = 0, peaks: bool = True) -> "dict[str, np.ndarray]":
-    """float32 arrays under the reference key names for ViT-`size` ('s' | 'b' | 'l' | 'h') with a K-keypoint simple head."""
+def random_state_dict(size: str, num_keypoints: int, seed: int = 0, peaks: bool = True, decoder: str = "classic") -> "dict[str, np.ndarray]":
+    """float32 arrays under the reference key names for ViT-`size` ('s' | 'b' | 'l' | 'h') with a K-keypoint head: decoder
+    "classic" (2 deconvs + 1x1 conv) or "simple" (final_layer [K, D, 3, 3]; its peak pathway reads the hot channel through the
+    centre tap)."""
     D, depth, _ = _DIMS[size]
     F, K = 256, int(num_keypoints)
     rs = np.random.RandomState(seed)
@@ -39,6 +41,16 @@ def random_state_dict(size: str, num_keypoints: int, seed: int = 0, peaks: bool 
             sd[p + name] = n(*shape, std=std, mean=mean)
     sd["backbone.last_norm.weight"] = n(D, std=0.05, mean=1.0)
     sd["backbone.last_norm.bias"] = n(D, std=0.02)
+    if decoder == "simple":
+        sd["keypoint_head.final_layer.weight"] = n(K, D, 3, 3, std=(0.002 if peaks else 0.02) / math.sqrt(9 * D / F))
+        sd["keypoint_head.final_layer.bias"] = n(K, std=0.01)
+        for k in range(K if peaks else 0):
+            c, t = k % D, int(rs.randint(0, 192))
+            sd["backbone.pos_embed"][0, 1 + t, c] += np.float32(depth)
+            sd["keypoint_head.final_layer.weight"][k, c, 1, 1] += np.float32(0.2)
+        return sd
+    if decoder != "classic":
+        raise ValueError(f"decoder {decoder!r}: 'classic' or 'simple'")
     cin = D
     for li in (0, 3):
         sd[f"keypoint_head.deconv_layers.{li}.weight"] = n(cin, F, 4, 4, std=(0.15 if peaks else 1.0) / math.sqrt(cin))

@@ -45,8 +45,8 @@ extern "C" {
 typedef struct vpb_engine vpb_engine;
 
 /* Model hyper-parameters: easy_ViTPose/configs/ViTPose_common.py:65-195 (embed_dim, depth, num_heads;
- * mlp_ratio 4, qkv_bias, patch 16, img 256x192, 2 deconv layers of 256 filters, 1x1 final conv are fixed
- * on this path) and the per-dataset out_channels (e.g. configs/ViTPose_coco.py:16-18). */
+ * mlp_ratio 4, qkv_bias, patch 16, img 256x192 are fixed on this path; the head is 2 deconv layers of 256 filters and a
+ * 1x1 final conv, or the simple decoder of vpb_create_ex) and the per-dataset out_channels (e.g. configs/ViTPose_coco.py:16-18). */
 typedef struct vpb_config {
   int32_t embed_dim;      /* 384 / 768 / 1024 / 1280 */
   int32_t depth;          /* 12 / 12 / 24 / 32 */
@@ -300,6 +300,18 @@ int vpb_infer_affine_nv12_host(vpb_engine* e, const vpb_frame_nv12* h_frames, in
 #define VPB_MAX_HEADS 8
 #define VPB_MAX_SEGMENTS 64
 int vpb_create_heads(const vpb_config* cfg, int32_t num_heads, const int32_t* h_keypoints, int32_t expert_rows, vpb_engine** out);
+/* The decoder of every head of an engine.  VPB_DECODER_CLASSIC: 2x (deconv 4x4 of 256 filters -> BN -> ReLU), 1x1 conv (the
+ * reference's configs, ViTPose_common.py).  VPB_DECODER_SIMPLE: the ViTPose paper's simple decoder (train_configs/
+ * ViTPose_{base,large,huge}_simple_coco_256x192.py: num_deconv_layers=0, upsample=4, final_conv_kernel=3):
+ *     relu(features) -> bilinear 4x upsample, align_corners=False -> 3x3 conv, padding 1 -> [K,64,48]
+ * (relu before the upsample, as the upstream head's _transform_inputs does it).  Its heads load final_layer.{weight,bias} of
+ * shapes [K,D,3,3], [K] and no deconv_layers.* key (strict as for vpb_create: those keys are unexpected); vpb_forward, vpb_head
+ * and every keypoint call run it in one launch (simple_head.cuh), and the engine allocates no deconv workspace.
+ * vpb_create_ex is vpb_create_heads with a decoder; vpb_create and vpb_create_heads are its VPB_DECODER_CLASSIC forms. */
+#define VPB_DECODER_CLASSIC 0
+#define VPB_DECODER_SIMPLE 1
+int vpb_create_ex(const vpb_config* cfg, int32_t num_heads, const int32_t* h_keypoints, int32_t expert_rows, int32_t decoder,
+                  vpb_engine** out);
 /* A run of `count` consecutive crops of head `head`. */
 typedef struct vpb_segment {
   int32_t head, count;
